@@ -1,14 +1,17 @@
 #!/usr/bin/env python
 """bench.py -- decode tokens/s for Llama-3.1-8B at P=98K, K=10, L=150 (BASELINE.json configs[1]).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W]                 # this repo's CUDA path
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--dump-outputs DIR]   # this repo's CUDA path
     python bench.py --impl reference [--gpus N] [--steps K] [--warmup W] # the reference's CPU path
     torchrun --nproc-per-node N ... bench.py --gpus N ...               # one rank per GPU
 
 One "step" = one decode token for the whole batch through all 32 layers of a random-init
 Llama-3.1-8B (library GEMMs for the projections/MLP; the 30 sparse layers run this repo's three
-sm_100a kernels; the 2 dense layers run the same gather-attention kernel over the full context).
+sm_90a kernels; the 2 dense layers run the same gather-attention kernel over the full context).
 The context is synthetic (seeded random K/V pushed through the server's own fill()/build_table()).
+Weights, context and token ids are seeded, so the same arguments give the same inputs on every run;
+--dump-outputs DIR writes the logits of the last timed step to DIR/logits.npy (float32, (B, vocab)); above 64 MB
+(B > 130 at Llama's vocabulary) it keeps a fixed seeded sample of the batch rows, in ascending row order.
 
 The JSON line carries, besides the base contract:
   roofline     the dominant kernel (attend_kernel, the fused gather attention): algorithmic bytes
@@ -71,7 +74,25 @@ def parse_args():
     ap.add_argument("--no-graph", action="store_true")
     ap.add_argument("--profile-step", action="store_true",
                     help="bracket ONE extra decode step with cudaProfilerStart/Stop (for `ncu --profile-from-start off`)")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the logits of the last timed step to DIR/logits.npy (float32, at most 64 MB: a fixed seeded sample "
+                         "of the batch rows above that) for output-to-output comparisons")
+    args = ap.parse_args()
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs needs --impl ours: the reference arm times the CPU operators and computes no logits")
+    return args
+
+
+DUMP_CAP_BYTES = 64 << 20
+
+
+def dump_rows(logits):
+    """The rows of (B, vocab) float32 logits that fit DUMP_CAP_BYTES: all of them, or a sample fixed by a seed and B."""
+    import numpy as np
+    keep = DUMP_CAP_BYTES // (logits.shape[1] * logits.dtype.itemsize)
+    if logits.shape[0] <= keep:
+        return logits
+    return logits[np.sort(np.random.default_rng(0).choice(logits.shape[0], keep, replace=False))]
 
 
 # ------------------------------------------------------------------------------------------------
@@ -119,25 +140,19 @@ class ClockSampler:
                 "reasons": sorted(reasons), "samples": len(sm)}
 
 
-def profiled_traffic(kernel_substr: str):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel from the committed
-    `ncu --set full` capture (profiles/r2_dram_traffic_per_launch.json, written by scripts/summarize_ncu.py)."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "r2_dram_traffic_per_launch.json")) as f:
-            for k, v in json.load(f).items():
-                if kernel_substr in k:
-                    return float(v)
-    except Exception:
-        pass
-    return None
+# NVIDIA H100 SXM data sheet: 3.35 TB/s of HBM3 (a bound, not a figure this benchmark reached)
+HBM_PEAK_GBS = 3350.0
 
 
-def measured_peak_gbs():
+def gpu_identity(index: int):
+    """The card the numbers were measured on and the power limit it ran under (both are part of every number)."""
     try:
-        with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
-            return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
+        name, limit = subprocess.check_output(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader,nounits", "-i",
+                                               str(index)], text=True).strip().split(", ")
+        return {"name": name, "power_limit_w": float(limit)}
     except Exception:
-        return 6650.0, "fallback 6.65 TB/s (B200_PROFILING.md)"
+        import torch
+        return {"name": torch.cuda.get_device_name(index), "power_limit_w": None}
 
 
 # ------------------------------------------------------------------------------------------------
@@ -383,7 +398,7 @@ def workload_config(args):
                         f"({layers}; random-init weights; synthetic {args.dist} KV context)",
             "global_batch": args.B * (args.gpus if args.parallel == "dp" else 1), "seq_len": args.P,
             "parallelism": (f"dp{args.gpus}" if args.parallel == "dp" else f"kv-head-tp{args.gpus}") if args.gpus > 1 else "single",
-            "l2_policy": "working set per step (16 GB weights + 30 distinct layers of tables/KV) >> 126 MB L2; no explicit flush"}
+            "l2_policy": "working set per step (16 GB weights + 30 distinct layers of tables/KV) >> 50 MB L2; no explicit flush"}
 
 
 # ------------------------------------------------------------------------------------------------
@@ -467,7 +482,7 @@ def graph_us_per_call(fn, calls_per_replay: int, reps: int = 5):
     return us, reps * calls_per_replay
 
 
-def measure_hot_path(args, runner, dev, default_workload):
+def measure_hot_path(args, runner, dev):
     """The sparse-attention path alone on this rank's heads: fused single-launch decode (the product path), the three-launch
     variant with per-stage CUDA events, the host-buffer entry point, and the roofline of the dominant kernel."""
     import ctypes
@@ -543,12 +558,13 @@ def measure_hot_path(args, runner, dev, default_workload):
                 mhz = float(subprocess.check_output(["nvidia-smi", "--query-gpu=clocks.sm", "--format=csv,noheader,nounits", "-i",
                                                      str(torch.cuda.current_device())]).decode().split()[0])
             except Exception:
-                mhz = 1965.0
+                mhz = 1980.0   # H100 SXM maximum SM clock
             recs = []
+            n_sms = torch.cuda.get_device_properties(dev).multi_processor_count
             ctx.plan()
             for li, l in enumerate(sparse_layers):
                 ctx.decode(l, qs[0, li], ks[0, li], vs[0, li], out_tmp)
-                recs += [r for r in ctx.fused_debug_read(min(H_loc * 8, 8 * 148)) if r[0] and r[6] and r[8]]
+                recs += [r for r in ctx.fused_debug_read(min(H_loc * 8, 8 * n_sms)) if r[0] and r[6] and r[8]]
             if recs:
                 gather_us = statistics.median((r[8] - r[6]) / mhz for r in recs)
         except Exception:
@@ -567,15 +583,13 @@ def measure_hot_path(args, runner, dev, default_workload):
         nnz_fracs.append(tot / (H_loc * n))
     s1_bytes = args.K * args.L * d * 2
     layer_bytes = (statistics.mean(attend_bytes) + statistics.mean(probe_bytes) + s1_bytes) if attend_bytes else float("nan")
-    peak, peak_src = measured_peak_gbs()
+    peak, peak_src = HBM_PEAK_GBS, "NVIDIA H100 SXM data sheet (3.35 TB/s HBM3)"
     gbs = (layer_bytes / 1e9) / (us_graph / 1e6) if nS else float("nan")
     three = {"simhash": 1e3 * statistics.mean(stage_ms[0]), "probe": 1e3 * statistics.mean(stage_ms[1]),
              "attend": 1e3 * statistics.mean(stage_ms[2])} if stage_ms[2] else None
     kname = ("fused_decode_kernel (one launch per sparse layer: SimHash -> probe -> gather attention + window, LSE merge folded in)"
              if fused else "three launches: simhash_kernel | probe_kernel | attend_mma_kernel")
     roofline = {"kernel": kname, "bound": "hbm", "achieved": gbs, "peak": peak, "unit": "GB/s", "frac": gbs / peak, "peak_source": peak_src,
-                "traffic": profiled_traffic("fused_decode_kernel") if (default_workload and fused) else None,
-                "traffic_source": ("profiles/r2_dram_traffic_per_launch.json (ncu --set full, same workload)" if (default_workload and fused) else None),
                 "bytes_per_launch": layer_bytes,
                 "bytes_breakdown": {"S1_hash_func": s1_bytes, "S2_probe": statistics.mean(probe_bytes) if probe_bytes else None,
                                     "S3_gather": statistics.mean(attend_bytes) if attend_bytes else None},
@@ -583,13 +597,14 @@ def measure_hot_path(args, runner, dev, default_workload):
                                   "frac": statistics.mean(attend_bytes) / (gather_us * 1e-6) / 1e9 / peak, "unit": "GB/s",
                                   "note": "S3 bytes of a launch / median over CTAs of (first row requested -> all tiles consumed and merged), clock64 "
                                           "stamps of the kernel's debug instantiation in a separate untimed pass; the same fetch with nothing else "
-                                          "in the kernel: profiles/r2_gather_microbench.txt"} if (gather_us and attend_bytes) else None),
+                                          "in the kernel: scripts/micro/gather_bw.cu"} if (gather_us and attend_bytes) else None),
                 "us_per_launch": us_graph, "launches_timed": launches_timed,
                 "timing": "one launch per sparse layer (30 distinct layers => cold L2), all captured in ONE CUDA graph like the step, CUDA "
                           "events around the replays; achieved = algorithmic (S1+S2+S3) bytes / that duration",
                 "three_launch_us_per_layer": three}
     hot = {"ms_per_token": hot_ms_token, "tokens_per_s": args.B * 1e3 / hot_ms_token if hot_ms_token else None,
            "ms_per_token_graph": us_graph * nS / 1e3, "us_per_layer_graph": us_graph, "fused_single_launch": fused,
+           "fused_cluster_waves": ctx.get_info("fused_cluster_waves"),
            "host_buffers_ms_per_token": hot_host_ms_token, "three_launch_us_per_layer": three,
            "sample_fraction": statistics.mean(nnz_fracs) if nnz_fracs else None,
            "note": "ms_per_token: the sparse layers enqueued back to back from the host, CUDA events around whole tokens; "
@@ -611,7 +626,8 @@ def measure_step(args, runner, dev, rank, world, local_rank, replicas, sample_cl
         used = runner.capture(warm=3)
         launches_per_step = (ctx.launch_count - launches_before) // used
     step_fn = runner.step if args.no_graph else runner.replay
-    ids_host = torch.randint(0, vocab, (args.steps + args.warmup + 8, args.B, 1), dtype=torch.long).pin_memory()
+    ids_host = torch.randint(0, vocab, (args.steps + args.warmup + 8, args.B, 1), dtype=torch.long,
+                             generator=torch.Generator().manual_seed(11)).pin_memory()
     logits_host = torch.empty((args.B, vocab), dtype=torch.float32).pin_memory()
     runner.ids.copy_(ids_host[0])
     for _ in range(args.warmup):
@@ -627,6 +643,7 @@ def measure_step(args, runner, dev, rank, world, local_rank, replicas, sample_cl
         sampler.start()
     ms_total = timed(step_fn, args.steps)
     clocks = sampler.stop() if (rank == 0 and sample_clocks) else None
+    last_logits = runner.logits.float().cpu().numpy()   # what the last timed step returned (the e2e steps below overwrite it)
     tokens = args.B * args.steps * replicas
     value = tokens / (ms_total / 1e3)
     it = {"i": 0}
@@ -642,7 +659,7 @@ def measure_step(args, runner, dev, rank, world, local_rank, replicas, sample_cl
         e2e_step()
     ms_e2e = timed(e2e_step, args.steps)
     return dict(value=value, ms_per_step=ms_total / args.steps, e2e_value=tokens / (ms_e2e / 1e3), e2e_ms_per_step=ms_e2e / args.steps,
-                clocks=clocks, launches_per_step=launches_per_step, h2d=args.B * 8, d2h=args.B * vocab * 4)
+                clocks=clocks, launches_per_step=launches_per_step, h2d=args.B * 8, d2h=args.B * vocab * 4, logits=last_logits)
 
 
 def release_runner(runner):
@@ -750,14 +767,17 @@ def main():
 
     tp = args.parallel == "tp" and world > 1
     shape = model_shape(args.model)
-    default_workload = (args.B, args.P, args.M, args.K, args.L, args.layers, args.dist, args.model) == (1, 98000, 98304, 10, 150, 0, "gauss", "8b") and not tp
     runner, prefill_s = build_runner(args, shape, dev, rank, world, tp, args.tp_mode, args.tp_transport)
     ctx = runner.server.ctx
     n_layers = runner.n_layers
     n_sparse = len([l for l in range(n_layers) if l not in runner.server.dense_layers])
-    hot, roofline, _ = measure_hot_path(args, runner, dev, default_workload)
+    hot, roofline, _ = measure_hot_path(args, runner, dev)
     replicas = world if (world > 1 and not tp) else 1
     r = measure_step(args, runner, dev, rank, world, local_rank, replicas)
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "logits.npy"), dump_rows(r["logits"]))
 
     line = None
     if rank == 0:
@@ -773,6 +793,7 @@ def main():
             "dtype": "bf16", "data": "synthetic",
             "config": workload_config(args),
             "where": "gpu",
+            "gpu": gpu_identity(local_rank),
             "clocks": r["clocks"],
             "e2e": {"value": r["e2e_value"], "unit": UNIT, "h2d_bytes_per_step": r["h2d"], "d2h_bytes_per_step": r["d2h"],
                     "ms_per_step": r["e2e_ms_per_step"]},

@@ -1,5 +1,5 @@
 /*
- * magicpig_b200.h -- C ABI of the B200-native LSH-sampled sparse-attention decode path.
+ * magicpig_b200.h -- C ABI of the H100-native (sm_90a) LSH-sampled sparse-attention decode path.
  *
  * This is the drop-in boundary for ONE hot path of Infini-AI-Lab/MagicPIG: everything that
  * `models/attnserver.py::LSHSparseAttnServer.decode` (attnserver.py:228-312) does for a sparse
@@ -106,14 +106,16 @@ size_t mpig_device_bytes(const mpig_ctx *ctx);
  *   "attend_ctas" / "attend_warps"   grid / CTA shape of the stand-alone gather kernel (0 = automatic)
  *   "attend_impl"     only 1 (tensor-core tile math) exists; anything else returns MPIG_EUNSUPPORTED
  *   "dense_impl"      1 = GQA-shared dense kernel (default), 0 = the gather kernel in range mode
- *   "keyhash_impl"    1 = persistent warp-specialised tcgen05 pipeline (default), 0 = one tile per CTA
- *   "keyhash_stages"  B-tile ring depth of that pipeline (2..4, default 2)
+ *   "keyhash_impl"    1 = persistent warp-specialised wgmma pipeline (default), 0 = one tile per CTA
+ *   "keyhash_stages"  B-tile ring depth of that pipeline (2..4, default 2; capped at what fits in shared memory beside
+ *                     the two key tiles, which is 2 on sm_90a)
  *   "pdl_first"       1 = launch the first kernel of mpig_decode with programmatic stream serialization too (default)
  *   "attend_skip" / "attend_debug" / "fused_debug" / "keyhash_skip"   timing-only elimination switches and clock stamps
  *                     (results are WRONG while a skip bit is set; used by scripts/kernel_bench.py and scripts/keyhash_bench.py) */
 int mpig_set_option(mpig_ctx *ctx, const char *key, int64_t value);
 /* Read-only facts: "last_decode_fused" (1 if the last mpig_decode ran the fused kernel), "fused_applicable",
- * "window_capacity" (sink + local + generation_buffer rows). */
+ * "fused_cluster_waves" (waves of thread-block clusters one fused launch takes on this device; 1 = all resident at once,
+ * 0 = fused decode not applicable), "window_capacity" (sink + local + generation_buffer rows). */
 int mpig_get_info(mpig_ctx *ctx, const char *key, int64_t *value);
 /* Capacity errors the DEVICE detected (the lengths saturate there): bit 0 = a sparse window is full (generation_buffer
  * exhausted: each further token overwrites the previous one's K/V), bit 1 = a dense cache reached max_length.  mpig_plan
@@ -134,7 +136,7 @@ int mpig_set_hash_func(mpig_ctx *ctx, const void *hash_func_bf16, void *stream);
 int mpig_lsh_fill(mpig_ctx *ctx, int layer, int request, const int16_t *sorted_codes,
                   const int32_t *sorted_indices, int n, void *stream);
 /* Key-side SimHash (attnserver.py:159-168): codes int16 (Hkv, L, n) of keys bf16 (Hkv, n, d) [already centred], with the
- * context's hash_func.  tcgen05 tensor-core GEMM whose epilogue keeps only the sign bits. */
+ * context's hash_func.  wgmma tensor-core GEMM whose epilogue keeps only the sign bits. */
 int mpig_hash_keys(mpig_ctx *ctx, const void *keys_bf16, int n, int16_t *codes_out, void *stream);
 /* Device-side replacement of `sort()` + LSH::fill (attnserver.py:186-193 + lsh.cc:143-201):
  * counting-sort the UNSORTED key codes int16 (Hkv, L, n) straight into the CSR tables. */

@@ -1,7 +1,7 @@
-"""magicpig_b200 -- B200-native LSH-sampled sparse-attention decode path (drop-in for MagicPIG's
+"""magicpig_b200 -- H100-native LSH-sampled sparse-attention decode path (drop-in for MagicPIG's
 `models/attnserver.py` operator surface).  See DESIGN.md and include/magicpig_b200.h.
 
-Layout:  csrc/ (sm_100a kernels + C ABI)  _native.py (ctypes)  ops.py (Context, LSH,
+Layout:  csrc/ (sm_90a kernels + C ABI)  _native.py (ctypes)  ops.py (Context, LSH,
 SparseAttentionServer mirrors)  attnserver.py (LSHSparseAttnServer)  synth.py (seeded inputs)
 """
 __version__ = "0.1.0"

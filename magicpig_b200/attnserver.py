@@ -9,7 +9,7 @@ unchanged (`llama.py:91-93, 208, 264, 282-284, 292, 315, 357`):
 
 What changes is where things live and run: the offloaded KV cache, the L hash tables and the
 sink/local/generated window are resident in HBM inside a `magicpig_b200.ops.Context`, and a sparse
-layer's decode is three hand-written sm_100a kernels (SimHash -> probe -> gather attention with the
+layer's decode is three hand-written sm_90a kernels (SimHash -> probe -> gather attention with the
 window merge folded in) instead of a GPU->CPU->GPU round trip through OpenMP/AVX-512 operators.
 There is no FlashInfer dependency and no CPU fallback.
 """
@@ -45,7 +45,8 @@ class LSHSparseAttnServer:
         hash_func   inject the (d, K*L) bf16 projection (the reference draws it unseeded, :55);
         table_build "device" = counting sort on the GPU (mpig_lsh_build); "sorted" = the reference's
                     `sort()` + LSH.fill route (attnserver.py:186-193) with the fill done on the GPU;
-        key_hash    "tcgen05" = key-side SimHash GEMM + sign pack in one tensor-core kernel (mpig_hash_keys);
+        key_hash    "tcgen05" (the name of the first target's tensor cores, kept for compatibility) = key-side SimHash GEMM +
+                    sign pack in one tensor-core kernel (mpig_hash_keys, wgmma on sm_90a);
                     "torch" = the reference's chunked `matmul(...).gt(0)` + pack glue (attnserver.py:159-168);
         num_*_heads per-rank head counts under KV-head tensor parallelism (attnserver_dist.py:252-254).
         """
@@ -109,7 +110,7 @@ class LSHSparseAttnServer:
         kn = offload_key.norm(p=2, dim=-1).float()                                   # attnserver.py:146 (bf16-rounded)
         self.avg_k[layer_idx][request_id] = avg_k
         n = offload_key.shape[1]
-        # key-side SimHash (attnserver.py:159-168): tcgen05 GEMM with the sign-pack epilogue (csrc/keyhash.cu); the torch
+        # key-side SimHash (attnserver.py:159-168): tensor-core GEMM with the sign-pack epilogue (csrc/keyhash.cu); the torch
         # GEMM + pack glue stays selectable (key_hash="torch") as the cross-check the tests use
         if self.key_hash == "tcgen05":
             self.hash_code_buffer[:, :, :n].copy_(self.ctx.hash_keys(offload_key.contiguous()))

@@ -1,6 +1,6 @@
-"""Build the sm_100a CUDA library in-tree:  magicpig_b200/lib/libmagicpig_b200.so
+"""Build the sm_90a (H100) CUDA library in-tree:  magicpig_b200/lib/libmagicpig_b200.so
 
-nvcc cross-compiles without a GPU.  The .so is git-ignored but travels with the gpurun snapshot.
+nvcc cross-compiles without a GPU.  The .so and its objects are build products (git-ignored).
 """
 from __future__ import annotations
 
@@ -15,12 +15,12 @@ LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libmagicpig_b200.so")
 SOURCES = ["context.cu", "tables.cu", "store.cu", "fused.cu", "attend_mma.cu", "attend_dense.cu", "simhash.cu", "decode.cu", "peer.cu", "aux_ops.cu", "aux_gemv.cu", "keyhash.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
          "-ccbin", "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"]
 
 
 def _newest_input() -> float:
-    t = 0.0
+    t = os.path.getmtime(os.path.abspath(__file__))   # the flags (target architecture) live here
     for root in (CSRC, os.path.join(HERE, "..", "include")):
         for f in os.listdir(root):
             t = max(t, os.path.getmtime(os.path.join(root, f)))

@@ -125,7 +125,7 @@ __device__ __forceinline__ void merge_states(SlotFn slot_ptr, int n, int lane, f
             m_i = GLOBAL ? __ldcg(pp) : pp[0];
             l_i = GLOBAL ? __ldcg(pp + 1) : pp[1];
         }
-        const float mn = fmaxf(M_, warp_max_redux(m_i));
+        const float mn = fmaxf(M_, warp_max(m_i));
         const float f_old = (M_ == -CUDART_INF_F) ? 0.f : exp2f((M_ - mn) * LOG2E_F);
         const float f_i = (m_i == -CUDART_INF_F) ? 0.f : exp2f((m_i - mn) * LOG2E_F);
         L_ = L_ * f_old + warp_sum(l_i * f_i);

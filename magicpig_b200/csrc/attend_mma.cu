@@ -82,7 +82,7 @@ __device__ __forceinline__ int atom_add_acq_rel_cta_shared(int *addr, int v) {
 template <bool USE_TMA, bool DBG>
 __global__ void __launch_bounds__(384, 1) attend_mma_kernel(const __grid_constant__ AttendParams gp) {
     extern __shared__ __align__(128) uint8_t smem[];
-    // Kernel parameters live in the constant bank; on sm_100 every use is a separate LDC and the first touch of each
+    // Kernel parameters live in the constant bank; every use is a separate LDC and the first touch of each
     // constant line after a launch is a long miss, which serialised into several microseconds on each warp's critical
     // path.  They are staged ONCE into shared memory (one parallel burst of LDCs) and read from there afterwards.
     __shared__ AttendParams p_smem;

@@ -66,11 +66,10 @@ __global__ void __launch_bounds__(GV_THREADS) gemv_kernel(const __grid_constant_
     const int kv = K >> 3;                            // 16-B vectors per row
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     // Programmatic dependent launch only on the two edges around the attention kernel, and only on request (mpig_aux_set_pdl).
-    // Round 1 measured PDL on EVERY GEMV at -25 % and a trigger in front of the small SimHash kernel at -2.5 %: grids parked at
-    // griddepcontrol.wait held registers / shared memory the running weight stream needed.  The fused attention kernel takes a
-    // whole SM per CTA, so it cannot squat beside running GEMV CTAs: triggering it early only hides its launch latency and
-    // constant-data prologue behind this kernel's tail; and the o-projection that follows it parks on SMs the attention grid does
-    // not use (20 of 148 at C2) or has already left.
+    // PDL on EVERY GEMV is slower: grids parked at griddepcontrol.wait hold registers / shared memory the running weight
+    // stream needs.  The fused attention kernel takes a whole SM per CTA, so it cannot squat beside running GEMV CTAs:
+    // triggering it early only hides its launch latency and constant-data prologue behind this kernel's tail; and the
+    // o-projection that follows it parks on SMs the attention grid does not use or has already left.
     if (MODE == GV_ROPE && (a.pdl & 1)) pdl_launch_dependents();
     if (MODE == GV_PLAIN && !PRE && (a.pdl & 2)) pdl_wait();
     // the warp's output rows

@@ -138,7 +138,10 @@ int mpig_aux_rope_split(const void *qkv, const void *cos_tab, const void *sin_ta
 int mpig_aux_silu_mul(const void *gate_up, void *out, int rows, int inter, void *stream) {
     MPIG_REQUIRE(gate_up && out && rows > 0 && inter > 0 && inter % 8 == 0, MPIG_EINVAL, "mpig_aux_silu_mul: bad arguments");
     const size_t total = (size_t)rows * inter / 8;
-    const int blocks = (int)std::min<size_t>((total + 255) / 256, 148 * 8);
+    int dev = 0, sms = 0;
+    MPIG_CUDA(cudaGetDevice(&dev));
+    MPIG_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    const int blocks = (int)std::min<size_t>((total + 255) / 256, (size_t)sms * 8);   // grid-stride: 8 blocks per SM
     silu_mul_kernel<<<blocks, 256, 0, as_stream(stream)>>>((const uint4 *)gate_up, (uint4 *)out, rows, inter);
     MPIG_CUDA(cudaGetLastError());
     return MPIG_OK;

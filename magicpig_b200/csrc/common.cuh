@@ -1,4 +1,4 @@
-// common.cuh -- context layout, error plumbing and PTX wrappers shared by the sm_100a kernels.
+// common.cuh -- context layout, error plumbing and PTX wrappers shared by the sm_90a kernels.
 //
 // HBM layout owned by a context (all per SPARSE layer unless noted; B requests, Hkv kv-heads,
 // M = max_length rows of capacity, d = head_dim, REC = 2*d bf16 = 512 B at d = 128):
@@ -92,6 +92,7 @@ struct mpig_ctx {
     int NB = 0, Wcap = 0, G = 0, H = 0 /* B*Hq */, BG = 0 /* B*Hkv */, rec_bytes = 0, num_sms = 0;
     int bitmap_words = 0;  // ceil(M/32)
     int cta_per_sm = 1;    // probing / fused CTAs per SM the geometry is planned for (mpig_config.reserved[0] == 2 -> 2)
+    int max_cluster = 8;   // largest probing / fused cluster whose B*Hq copies are all resident at once (mpig_create)
     std::vector<mpig::LayerStore> layers;
     std::vector<std::vector<int>> n_off;  // [layer][request] offloaded key count (host bookkeeping)
     // global state
@@ -122,7 +123,7 @@ struct mpig_ctx {
     int dense_impl = 1;  // 1 = GQA-shared dense kernel (attend_dense.cu), 0 = the gather kernel (attend_mma.cu) in range mode
     bool hash_func_set = false;  // mpig_set_hash_func has been called (hashing with the zero projection is refused)
     int pdl_first = 1;     // launch the first kernel of a decode (simhash) with programmatic stream serialization as well
-    int keyhash_skip = 0;  // debug/timing only: 1 = no stores, 2 = no TMEM reads, 4 = no MMAs (results are wrong)
+    int keyhash_skip = 0;  // debug/timing only: 1 = no stores, 2 = no sign pack, 4 = no MMAs (results are wrong)
     int keyhash_stages = 2;  // B-tile ring depth of the pipelined key-hash kernel (2..4)
     int keyhash_impl = 1;  // 1 = persistent warp-specialised pipeline (keyhash.cu), 0 = one tile per CTA
     std::vector<cudaEvent_t> timing_events;  // 4 per timed decode call
@@ -248,22 +249,13 @@ __device__ __forceinline__ uint64_t policy_evict_first() {
     return p;
 }
 
-// warp-wide max in ONE instruction (sm_100a: redux.sync on f32 -> CREDUX.MAX.F32); -inf lanes are neutral, no NaN inputs expected
-__device__ __forceinline__ float warp_max_redux(float v) {
-    float r;
-    asm volatile("redux.sync.max.f32 %0, %1, 0xffffffff;" : "=f"(r) : "f"(v));
-    return r;
-}
 __device__ __forceinline__ void prefetch_l2(const void *p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
-// {a0, a1} += p * {v0, v1}: ONE instruction for two fp32 FMAs (sm_100a fma.rn.f32x2 -> FFMA2), each component the same IEEE fma
+// {a0, a1} += p * {v0, v1}: two IEEE fp32 fmas
 __device__ __forceinline__ void ffma2(float &a0, float &a1, float p, float v0, float v1) {
-    unsigned long long A, P, V;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(A) : "f"(a0), "f"(a1));
-    asm("mov.b64 %0, {%1, %1};" : "=l"(P) : "f"(p));
-    asm("mov.b64 %0, {%1, %2};" : "=l"(V) : "f"(v0), "f"(v1));
-    asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(A) : "l"(P), "l"(V));
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(a0), "=f"(a1) : "l"(A));
+    a0 = fmaf(p, v0, a0);
+    a1 = fmaf(p, v1, a1);
 }
+// warp-wide max by butterfly shuffles (sm_90 has no f32 redux.sync); -inf lanes are neutral, no NaN inputs expected
 __device__ __forceinline__ float warp_max(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
@@ -319,6 +311,9 @@ int launch_fused(mpig_ctx *ctx, int layer, const void *q, const void *k, const v
                  const mpig_peer *peer = nullptr, int peer_rank = 0, int peer_world = 1, volatile uint32_t *host_flags = nullptr,
                  uint32_t host_epoch = 0);
 bool fused_applicable(const mpig_ctx *ctx);
+// clusters of C fused-kernel CTAs of `threads` threads (at the full shared-memory carve-up) the current device keeps resident
+int fused_resident_clusters(int C, int threads);
+int fused_cluster_waves(const mpig_ctx *ctx);   // waves of clusters one fused launch takes (0 = not applicable / unknown)
 int launch_pack_nhd(mpig_ctx *ctx, const void *k, const void *v, uint8_t *rec, int Hkv, int n, int rows_cap, cudaStream_t s);
 
 // ---- host helpers --------------------------------------------------------------------------

@@ -101,10 +101,11 @@ int mpig_create(const mpig_config *cfg, mpig_ctx **out) {
     MPIG_CUDA(cudaSetDevice(cfg->device));
     cudaDeviceProp prop;
     MPIG_CUDA(cudaGetDeviceProperties(&prop, cfg->device));
-    MPIG_REQUIRE(prop.major == 10, MPIG_EUNSUPPORTED,
-                 "mpig_create: device %d is sm_%d%d; this library is built for sm_100a (B200) only and has no fallback",
+    MPIG_REQUIRE(prop.major == 9 && prop.minor == 0, MPIG_EUNSUPPORTED,
+                 "mpig_create: device %d is sm_%d%d; this library is built for sm_90a (H100) only and has no fallback",
                  cfg->device, prop.major, prop.minor);
 
+    int ctx_max_cluster = 8;
     mpig_ctx *ctx = new mpig_ctx();
     ctx->cfg = *cfg;
     ctx->NB = 1 << cfg->K;
@@ -116,8 +117,15 @@ int mpig_create(const mpig_config *cfg, mpig_ctx **out) {
         // `occ` CTAs of the probing / fused kernels share an SM (reserved[0]; default 1: one 1024-thread CTA per SM; 2: clusters
         // twice as large made of 512-thread CTAs, two per SM, whose latency phases overlap each other)
         const int occ = (cfg->reserved[0] == 2) ? 2 : 1;
-        while (c_target * 2 <= 8 && (long long)cfg->batch_size * cfg->num_attention_heads * c_target * 2 <= (long long)occ * prop.multiProcessorCount)
+        // ... and only while all B*Hq clusters stay resident at once: a cluster occupies SMs of ONE GPC and the H100's GPCs have
+        // unequal SM counts, so fewer clusters of 4 fit than #SMs / 4 (a second wave of clusters doubles the launch)
+        const long long heads = (long long)cfg->batch_size * cfg->num_attention_heads;
+        while (c_target * 2 <= 8 && heads * c_target * 2 <= (long long)occ * prop.multiProcessorCount) {
+            const int resident = fused_resident_clusters(c_target * 2, heads * c_target * 2 > prop.multiProcessorCount ? 512 : 1024);
+            if (resident > 0 && heads > resident) break;
             c_target *= 2;
+        }
+        ctx_max_cluster = c_target;
         const int min_seg = (cfg->max_length + SEG - 1) / SEG;
         int nseg = std::max(min_seg, std::min(c_target, (cfg->max_length + 1023) / 1024));   // segments of < 1024 keys are not worth it
         int seg_len = (((cfg->max_length + nseg - 1) / nseg) + 63) & ~63;
@@ -132,6 +140,7 @@ int mpig_create(const mpig_config *cfg, mpig_ctx **out) {
     ctx->rec_bytes = 2 * cfg->head_dim * 2;
     ctx->num_sms = prop.multiProcessorCount;
     ctx->cta_per_sm = (cfg->reserved[0] == 2) ? 2 : 1;
+    ctx->max_cluster = ctx_max_cluster;
     ctx->bitmap_words = (cfg->max_length + 31) / 32;
     ctx->layers.resize(cfg->num_layers);
     ctx->n_off.assign(cfg->num_layers, std::vector<int>(cfg->batch_size, 0));
@@ -378,6 +387,7 @@ int mpig_get_info(mpig_ctx *ctx, const char *key, int64_t *value) {
     std::string k(key);
     if (k == "last_decode_fused") *value = ctx->last_decode_fused;
     else if (k == "fused_applicable") *value = fused_applicable(ctx) ? 1 : 0;
+    else if (k == "fused_cluster_waves") *value = fused_cluster_waves(ctx);
     else if (k == "window_capacity") *value = ctx->Wcap;
     else {
         set_error("mpig_get_info: unknown key '%s'", key);

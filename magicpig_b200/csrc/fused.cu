@@ -24,7 +24,7 @@
 //   ATTEND  consumer warps take 16-row tiles of that list: ONE elected lane issues the 16 512-byte cp.async.bulk (TMA engine)
 //           of a tile in a warp-uniform sequence, 8 warps at a time in warp order (issue window), completion counted in bytes
 //           on the warp's mbarrier; scores on the tensor cores (ldmatrix + mma.m16n8k16, q in column 0), the LSH re-weighting
-//           lane-per-row, online softmax in base 2 (CREDUX max), PV as FFMA2.  Window tiles (round-robin over the cluster)
+//           lane-per-row, online softmax in base 2 (shuffle max), PV as fp32 FMAs.  Window tiles (round-robin over the cluster)
 //           take the same path; the token being decoded is built in place from k_new - avg_k / v_new: no CTA waits for an append.
 //   MERGE   warp states -> CTA state (four warps, a dimension per lane) -> rank 0 (DSMEM, one cluster barrier) -> output.
 // The index list and nnz are written to HBM only for mpig_last_probe (nnz always: one int per head; the list on request).
@@ -773,7 +773,7 @@ __global__ void __launch_bounds__(THREADS, (THREADS == 1024) ? 1 : 2) fused_deco
                 }
                 if (DBG && wrec) wrec[11] = clk64() + (unsigned long long)(z == 123.456f);
                 // online softmax (base 2)
-                const float m_new = fmaxf(m_run, warp_max_redux(z));
+                const float m_new = fmaxf(m_run, warp_max(z));
                 const float corr = (m_run == -CUDART_INF_F) ? 0.f : exp2f((m_run - m_new) * LOG2E_F);
                 const float pj = (lane < nrows) ? exp2f((z - m_new) * LOG2E_F) : 0.f;
                 l_run = l_run * corr + pj;   // per-LANE partial sum (corr is warp-uniform): reduced once, before the state is stored
@@ -837,7 +837,7 @@ __global__ void __launch_bounds__(THREADS, (THREADS == 1024) ? 1 : 2) fused_deco
             l_i = pp[1];
         }
         if (DBG) t_rel = clk64() + (unsigned long long)(m_i == 123.456f);   // barrier RELEASED (the read depends on it)
-        const float mn = warp_max_redux(m_i);
+        const float mn = warp_max(m_i);
         const float f_i = (m_i == -CUDART_INF_F) ? 0.f : exp2f((m_i - mn) * LOG2E_F);
         const int dd = warp * 32 + lane;
         float a = 0.f, a_odd = 0.f;   // two accumulation chains (even / odd states)
@@ -951,7 +951,34 @@ struct FusedPlan {
     size_t smem;
     bool hash_in_kernel;
     FusedSmem lay;
+    int cluster_waves;  // waves of clusters the grid needs (cudaOccupancyMaxActiveClusters; 0 = unknown)
 };
+
+// Clusters of this plan's variant that the device keeps resident at once.  A cluster occupies SMs of ONE GPC, and the
+// H100's GPCs have unequal SM counts, so #SMs / C over-counts; the runtime knows the real number.
+template <int THREADS, bool KREG>
+static int fused_max_active_clusters(const FusedPlan &fp) {
+    const void *fn = (const void *)fused_decode_kernel<uint8_t, THREADS, false, KREG>;
+    if (func_attr_once(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, THREADS == 1024 ? 227 * 1024 - 1024 : 228 * 1024 / 2 - 2048) != MPIG_OK)
+        return 0;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(fp.gm.C);
+    cfg.blockDim = dim3(THREADS);
+    cfg.dynamicSmemBytes = fp.smem;
+    cudaLaunchAttribute attr;
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = fp.gm.C;
+    attr.val.clusterDim.y = 1;
+    attr.val.clusterDim.z = 1;
+    cfg.attrs = &attr;
+    cfg.numAttrs = 1;
+    int n = 0;
+    if (cudaOccupancyMaxActiveClusters(&n, fused_decode_kernel<uint8_t, THREADS, false, KREG>, &cfg) != cudaSuccess) {
+        cudaGetLastError();
+        return 0;
+    }
+    return n;
+}
 
 static FusedPlan fused_plan_compute(const mpig_ctx *ctx) {
     FusedPlan fp = {};
@@ -979,6 +1006,9 @@ static FusedPlan fused_plan_compute(const mpig_ctx *ctx) {
     // the cluster splits the tables; with one CTA per head (large batches) every CTA would stream all of hash_func from L2:
     // those shapes hash in the separate tensor-core kernel (simhash.cu) and hand the codes over
     fp.hash_in_kernel = fp.gm.C >= 2;
+    const int act = fp.threads == 1024 ? (ctx->fused_kreg ? fused_max_active_clusters<1024, true>(fp) : fused_max_active_clusters<1024, false>(fp))
+                                       : (ctx->fused_kreg ? fused_max_active_clusters<512, true>(fp) : fused_max_active_clusters<512, false>(fp));
+    fp.cluster_waves = act > 0 ? (ctx->H + act - 1) / act : 0;
     fp.ok = true;
     return fp;
 }
@@ -1005,6 +1035,13 @@ static const FusedPlan &fused_plan(const mpig_ctx *ctx) {
 }
 
 bool fused_applicable(const mpig_ctx *ctx) { return ctx->decode_impl == 1 && fused_plan(ctx).ok; }
+int fused_resident_clusters(int C, int threads) {
+    FusedPlan fp = {};
+    fp.gm.C = C;
+    fp.smem = threads == 1024 ? 227 * 1024 - 1024 : 228 * 1024 / 2 - 2048;   // the full carve-up the plan may use
+    return threads == 1024 ? fused_max_active_clusters<1024, false>(fp) : fused_max_active_clusters<512, false>(fp);
+}
+int fused_cluster_waves(const mpig_ctx *ctx) { return fused_plan(ctx).ok ? fused_plan(ctx).cluster_waves : 0; }
 
 template <int THREADS, bool DBG, bool KREG>
 static int launch_variant(const cudaLaunchConfig_t &cfg, const FusedParams &p) {

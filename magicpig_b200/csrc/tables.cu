@@ -391,7 +391,7 @@ ProbeGeom probe_geometry(const mpig_ctx *ctx) {
     gm.Sp = 1;
     while (gm.Sp < ctx->nseg) gm.Sp *= 2;
     gm.r = 1;
-    while (gm.Sp * gm.r * 2 <= 8 && ctx->H * gm.Sp * gm.r * 2 <= ctx->cta_per_sm * ctx->num_sms) gm.r *= 2;
+    while (gm.Sp * gm.r * 2 <= ctx->max_cluster && ctx->H * gm.Sp * gm.r * 2 <= ctx->cta_per_sm * ctx->num_sms) gm.r *= 2;
     gm.C = gm.Sp * gm.r;
     gm.Mc = ((ctx->seg_len + gm.r - 1) / gm.r + 31) & ~31;
     return gm;

@@ -45,7 +45,7 @@ class Context:
         self.lib = N.load()
         self.device = torch.device(device)
         if self.device.type != "cuda":
-            raise N.MagicPigError("magicpig_b200 runs on CUDA (sm_100a) only; there is no CPU path")
+            raise N.MagicPigError("magicpig_b200 runs on CUDA (sm_90a) only; there is no CPU path")
         self.K, self.L, self.num_layers = K, L, num_layers
         self.Hq, self.Hkv, self.d = num_attention_heads, num_key_value_heads, head_dim
         self.B, self.M = batch_size, max_length

@@ -8,7 +8,7 @@ Two checkers live here:
   * `oracle.port`  (this module): ctypes front-end of `mpig_oracle.c`, the plain-C restatement
     of the reference algorithm (each C function cites the reference file:line it follows).
   * `oracle.ref_loader`: the UNMODIFIED reference operators (`lsh.LSH`,
-    `sparse_attention_cpu.SparseAttentionServer`) compiled from /root/reference by
+    `sparse_attention_cpu.SparseAttentionServer`) compiled from a checkout of the reference by
     `oracle/build_ref.py` into `oracle/_ref/`.
 
 Parity status: pinned (see header of mpig_oracle.c and tests/test_oracle_cpu.py).
@@ -29,7 +29,7 @@ _lib = None
 
 
 def build(force: bool = False) -> str:
-    """gcc the C restatement into oracle/_build/ (git-ignored *.so, travels with gpurun)."""
+    """gcc the C restatement into oracle/_build/ (git-ignored build product)."""
     if force or (not os.path.exists(_SO)) or os.path.getmtime(_SO) < os.path.getmtime(_SRC):
         os.makedirs(_BUILD, exist_ok=True)
         cc = "/usr/bin/gcc" if os.path.exists("/usr/bin/gcc") else "gcc"

@@ -1,9 +1,9 @@
 """Build the UNMODIFIED reference CPU operators into oracle/_ref/  (TEST INFRASTRUCTURE ONLY).
 
 This compiles MagicPIG's own `library/lsh` and `library/sparse_attention` pybind modules
-straight from the sources where they lie under /root/reference (nothing is copied into
-this repository) and drops only the resulting shared objects under `oracle/_ref/`
-(git-ignored, NOT gpurun-ignored, so the binaries travel to the GPU box).
+straight from the sources where they lie in a checkout of the reference (`MAGICPIG_REFERENCE`;
+nothing is copied into this repository) and drops only the resulting shared objects under
+`oracle/_ref/` (git-ignored build products; a machine without the reference can use prebuilt ones).
 
 It mirrors the reference's own build lines:
   * library/lsh/setup.py:5-13                ->  oracle/_ref/lsh.so
@@ -15,7 +15,7 @@ It mirrors the reference's own build lines:
 Only `tests/`, `__graft_entry__.smoke()`, `__graft_entry__.build()` and `bench.py`'s CPU
 baseline / `--impl reference` legs may use the result.  The product path never does.
 
-Run:  python oracle/build_ref.py            (needs /root/reference; ~2-3 min)
+Run:  python oracle/build_ref.py            (needs the reference checkout; ~2-3 min)
 """
 from __future__ import annotations
 
@@ -82,7 +82,7 @@ def build(force: bool = False) -> bool:
     if have and not force:
         return True
     if not os.path.isdir(os.path.join(REF, "library", "lsh")):
-        # e.g. on the GPU box: no /root/reference -> only prebuilt files can be used
+        # no reference checkout here -> only prebuilt files can be used
         return have
     t0 = time.time()
     lsh_dir = os.path.join(REF, "library", "lsh")
@@ -104,4 +104,4 @@ def build(force: bool = False) -> bool:
 
 if __name__ == "__main__":
     ok = build(force="--force" in sys.argv)
-    print("oracle/_ref:", "ready" if ok else "unavailable (no /root/reference and no prebuilt files)")
+    print("oracle/_ref:", "ready" if ok else "unavailable (no reference checkout and no prebuilt files)")

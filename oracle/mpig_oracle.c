@@ -6,13 +6,13 @@
  * --impl reference legs may load it.  The product path never calls into oracle/.
  *
  * Parity status: PINNED.  tests/test_oracle_cpu.py checks every function here against
- *   (1) the unmodified reference operators compiled from /root/reference into oracle/_ref/
+ *   (1) the unmodified reference operators compiled from a reference checkout into oracle/_ref/
  *       (oracle/build_ref.py), when those binaries are present, and
  *   (2) the committed golden vectors under tests/golden/ that were produced by running
  *       those reference binaries (tests/golden/make_golden.py).
  *
  * Plain scalar C, single threaded, one function per reference function.  Each function
- * cites the reference file:line it restates (paths relative to /root/reference).
+ * cites the reference file:line it restates (paths relative to the reference repository).
  *
  * Build: gcc -O2 -shared -fPIC -o oracle/_build/libmpig_oracle.so oracle/mpig_oracle.c -lm
  */
@@ -273,7 +273,7 @@ void orc_attention_wrapper(const uint16_t *key, const uint16_t *value, const flo
  * local + generated tokens the reference hands to FlashInfer, models/attnserver.py:281-296),
  * returning the fp32 output and the base-2 LSE (FlashInfer convention), and the LSE-weighted
  * merge of two partial states (flashinfer.merge_state, models/attnserver.py:308; math restated
- * in SURVEY.md 8(a) a11).  FlashInfer is third-party and absent from /root/reference
+ * in SURVEY.md 8(a) a11).  FlashInfer is third-party and absent from the reference repository
  * (install.sh:4, unpinned wheel): "merge/window parity unpinned" -- these two follow the
  * published definition only.
  * ------------------------------------------------------------------------------------------ */

@@ -1,8 +1,8 @@
 """Load the UNMODIFIED reference operators from oracle/_ref/ (TEST INFRASTRUCTURE ONLY).
 
 `lsh.LSH` (library/lsh/lsh.cc:316-326) and `sparse_attention_cpu.SparseAttentionServer`
-(library/sparse_attention/sparse_attention.cc:1243-1263) are compiled from /root/reference
-by `oracle/build_ref.py`.  Two flavours of sparse_attention_cpu exist; the loader picks the
+(library/sparse_attention/sparse_attention.cc:1243-1263) are compiled from a checkout of the
+reference by `oracle/build_ref.py`.  Two flavours of sparse_attention_cpu exist; the loader picks the
 AVX512_BF16 one only when the running CPU has that extension (it would SIGILL otherwise).
 """
 from __future__ import annotations
@@ -53,7 +53,7 @@ def load():
     """Returns (lsh_module, sparse_attention_cpu_module, flavour).  Raises if unavailable."""
     if "mods" not in _cache:
         if not available():
-            raise RuntimeError("oracle/_ref not built (run `python oracle/build_ref.py` where /root/reference exists) "
+            raise RuntimeError("oracle/_ref not built (run `python oracle/build_ref.py` where the reference is checked out) "
                                "or CPU lacks AVX-512F")
         fl = flavour()
         _cache["mods"] = (_load("lsh", os.path.join(_REF, "lsh.so")),

@@ -39,7 +39,7 @@ for frac, tma in itertools.product((1.0,), (1, 0)):
         for l in range(nl):
             ctx.attention_wrapper(l, K, L, out, mve, q[l], qn[l], res[l], nz[l])
     # run ONE more launch on a layer whose data is cold in L2
-    nw = 148 * 12
+    nw = torch.cuda.get_device_properties(0).multi_processor_count * 12   # 12 warps per SM
     ctx.attention_wrapper(1, K, L, out, mve, q[1], qn[1], res[1], nz[1])
     ctx.attention_wrapper(2, K, L, out, mve, q[2], qn[2], res[2], nz[2])
     torch.cuda.synchronize()

@@ -1,4 +1,4 @@
-"""Throughput of the tcgen05 key-hash kernel at the BASELINE shape (8 KV heads x 98K keys, K=10, L=150) against the
+"""Throughput of the wgmma key-hash kernel at the BASELINE shape (8 KV heads x 98K keys, K=10, L=150) against the
 torch bf16 GEMM + sign-pack glue the reference uses (attnserver.py:159-168).   python scripts/keyhash_bench.py"""
 import os
 import sys
@@ -35,7 +35,7 @@ flop = 2.0 * Hkv * n * d * K * L
 for impl in (1, 0):
     ctx.set_option("keyhash_impl", impl)
     ms = timeit(lambda: ctx.hash_keys(keys, out=out))
-    print(f"mpig_hash_keys impl={impl} (tcgen05): {ms * 1e3:8.1f} us   {flop / ms / 1e9:7.1f} TFLOP/s   out {out.numel() * 2 / 1e6:.0f} MB -> {out.numel() * 2 / ms / 1e6:.0f} GB/s")
+    print(f"mpig_hash_keys impl={impl} (wgmma): {ms * 1e3:8.1f} us   {flop / ms / 1e9:7.1f} TFLOP/s   out {out.numel() * 2 / 1e6:.0f} MB -> {out.numel() * 2 / ms / 1e6:.0f} GB/s")
 ctx.set_option("keyhash_impl", 1)
 ctx.set_option("keyhash_stages", 3)
 ms = timeit(lambda: ctx.hash_keys(keys, out=out))
@@ -44,7 +44,7 @@ ctx.set_option("keyhash_stages", 2)
 for sk in (1, 2, 3, 4, 7):
     ctx.set_option("keyhash_skip", sk)
     ms = timeit(lambda: ctx.hash_keys(keys, out=out))
-    print(f"  skip={sk} (1 no stores, 2 no TMEM reads, 4 no MMAs): {ms * 1e3:8.1f} us")
+    print(f"  skip={sk} (1 no stores, 2 no sign pack, 4 no MMAs): {ms * 1e3:8.1f} us")
 ctx.set_option("keyhash_skip", 0)
 out.zero_()
 ctx.hash_keys(keys, out=out)

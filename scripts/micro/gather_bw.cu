@@ -4,7 +4,7 @@
 // 24.5K records, ~400 sampled records per CTA, ascending within the CTA) -- wait for all of them, and exit.  Buffers rotate so
 // that every launch reads cold lines.  Reported: launch time (CUDA events), in-kernel time from the first request to the last
 // arrival, and the fit  t(R) = t0 + bytes / BW  over R.
-//   nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o gather_bw gather_bw.cu && ./gather_bw
+//   nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o gather_bw gather_bw.cu && ./gather_bw
 #include <cuda_runtime.h>
 #include <algorithm>
 #include <cstdint>
@@ -65,7 +65,7 @@ __global__ void __launch_bounds__(1024, 1) gather_kernel(const uint8_t *__restri
 int main() {
     const int heads = 32, cph = 4, ctas = heads * cph, kvh = 8;
     const size_t rows_per_head = 98304, seg = rows_per_head / cph;
-    const size_t bytes = kvh * rows_per_head * REC;   // one layer's records (402 MB): > the 126 MB L2
+    const size_t bytes = kvh * rows_per_head * REC;   // one layer's records (402 MB): > the 50 MB L2
     const int NBUF = 6;
     std::vector<uint8_t *> bufs(NBUF);
     for (auto &b : bufs) { cudaMalloc(&b, bytes); cudaMemset(b, 1, bytes); }

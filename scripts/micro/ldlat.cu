@@ -22,7 +22,7 @@ __global__ void k(const int* __restrict__ buf, size_t stride_elems, int per_head
     if (lane == 0) out[warp] = t1 - t0;
 }
 int main() {
-    int warps = 148 * 12;
+    int warps = 132 * 12;   // 12 warps on each of an H100 SXM's 132 SMs
     size_t stride = 98304;
     int heads = 32, per_head = (warps + heads - 1) / heads;
     std::vector<int*> bufs;
@@ -35,7 +35,7 @@ int main() {
         for (int mode = 0; mode < 4; ++mode) {
             for (int rep = 0; rep < 2; ++rep) {
                 int* b = bufs[(mode * 9 + smem_kb) % bufs.size()];   // rep 0: cold buffer, rep 1: same lines again (L2 resident)
-                k<<<148, 384, smem_kb * 1024>>>(b, stride, per_head, out, mode);
+                k<<<132, 384, smem_kb * 1024>>>(b, stride, per_head, out, mode);
                 cudaDeviceSynchronize();
                 cudaMemcpy(h.data(), out, warps * 8, cudaMemcpyDeviceToHost);
                 std::sort(h.begin(), h.end());

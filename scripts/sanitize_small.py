@@ -5,7 +5,7 @@
 Sizes are tiny (the tools slow kernels down 10-100x) but cover: the stand-alone SimHash / probe (uint8 tags, several clusters
 shapes, two key segments) / gather-attention kernels, the fused single-launch decode (cluster of 8, cluster of 4 over two
 segments, one CTA per head with codes from the SimHash kernel, several selection passes), the three-launch decode, the dense
-kernel, the tcgen05 key hash and the table build.  Results are also checked against each other so a tool run doubles as a test.
+kernel, the tensor-core key hash and the table build.  Results are also checked against each other so a tool run doubles as a test.
 """
 import os
 import sys

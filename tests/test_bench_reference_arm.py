@@ -1,6 +1,7 @@
-"""`bench.py --impl reference` (the reference's CPU operators timed on host cores) needs no GPU, so its contract is
-checked here: one JSON line with the shared keys, `impl: reference`, a `cpu_baseline` describing the run and an `e2e`
-equal to the line's own value with no host<->device bytes; under torchrun only rank 0 works and prints."""
+"""`bench.py --impl reference` (the reference's CPU operators timed on host cores; the C restatement in oracle/ where they
+have not been built) needs no GPU, so its contract is checked here: one JSON line with the shared keys, `impl: reference`, a
+`cpu_baseline` describing the run and an `e2e` equal to the line's own value with no host<->device bytes; under torchrun
+only rank 0 works and prints."""
 import json
 import os
 import subprocess
@@ -9,7 +10,6 @@ import sys
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF_OK = os.path.exists(os.path.join(ROOT, "oracle", "_ref", "lsh.so")) or os.path.isdir("/root/reference")
 
 
 def _json_lines(text: str):
@@ -40,7 +40,6 @@ def _check(line):
     assert abs(best - cb["ms_per_layer"]) < 1e-9
 
 
-@pytest.mark.skipif(not REF_OK, reason="needs oracle/_ref (built from /root/reference by __graft_entry__.build())")
 @pytest.mark.timeout(600)
 def test_reference_arm_single():
     r = subprocess.run([sys.executable, os.path.join(ROOT, "bench.py"), "--impl", "reference", "--steps", "1", "--warmup", "1"],
@@ -52,7 +51,6 @@ def test_reference_arm_single():
     assert lines[0]["n_gpus"] == 1 and lines[0]["steps"] == 1 and lines[0]["warmup"] == 1
 
 
-@pytest.mark.skipif(not REF_OK, reason="needs oracle/_ref (built from /root/reference by __graft_entry__.build())")
 @pytest.mark.timeout(600)
 def test_reference_arm_under_torchrun_rank0_only():
     env = dict(os.environ, MASTER_ADDR="127.0.0.1")
@@ -71,16 +69,16 @@ def test_tracked_bench_lines_keep_the_contract():
     """The bench lines committed under profiles/ (what DESIGN.md quotes) carry every key of the bench.py contract and their
     derived numbers are consistent with each other."""
     BASE = json.load(open(os.path.join(ROOT, "BASELINE.json")))
-    for name, full in [("r2_bench_line.json", True), ("r2_bench_line_final_kernel.json", False), ("r2_bench_c3_b8.json", False),
-                       ("r2_bench_c4_prolong.json", False)]:
+    for name, full in [("h100_bench_line.json", True)]:
         path = os.path.join(ROOT, "profiles", name)
         if not os.path.exists(path):
             pytest.skip(f"{name} not tracked")
         d = _json_lines(open(path).read())[-1]
         for k in ("metric", "value", "unit", "n_gpus", "steps", "warmup", "ms_per_step", "higher_is_better", "scaling", "vs_baseline",
-                  "dtype", "data", "config", "clocks", "e2e", "gpu_launches", "roofline"):
+                  "dtype", "data", "config", "gpu", "clocks", "e2e", "gpu_launches", "roofline"):
             assert k in d, (name, k)
         assert d["unit"] == "tokens/s" and d["higher_is_better"] is True and d["n_gpus"] == 1 and d["warmup"] >= 3
+        assert d["gpu"]["name"] and d["gpu"]["power_limit_w"] > 0       # the card and power limit the numbers belong to
         assert d["gpu_launches"] > 0 and d["data"].startswith("synthetic")
         assert abs(d["value"] - 1e3 / d["ms_per_step"] * d["config"].get("global_batch", 1)) / d["value"] < 1e-6
         e2e = d["e2e"]
@@ -93,4 +91,4 @@ def test_tracked_bench_lines_keep_the_contract():
             assert BASE["metric"].startswith(d["metric"])   # BASELINE.json names the metric (+ the roofline it wants beside it)
             cb = d["cpu_baseline"]
             assert cb["kind"] == "reference" and cb["cores"] >= 1 and cb["sample"] and cb["value"] > 0
-            assert r["traffic"] is None or r["traffic"] >= 0.9 * r["bytes_per_launch"]
+            assert r.get("traffic") is None or r["traffic"] >= 0.9 * r["bytes_per_launch"]

@@ -1,4 +1,4 @@
-"""GPU parity suite (`-m gpu`, runs on the B200 box through the C ABI).
+"""GPU parity suite (`-m gpu`, runs on an H100 through the C ABI).
 
 Every test drives the CUDA library (ctypes -> libmagicpig_b200.so) and checks it against the oracle
 (oracle/mpig_oracle.c, pinned to the reference -- see tests/test_oracle_cpu.py) on the same seeded
@@ -671,7 +671,8 @@ def test_attnserver_dropin(cuda_lib, table_build, key_hash):
 
 # ------------------------------------------------------------------------------------------------
 # BASELINE full sizes: size-independent properties, one sparse layer each
-#   C2 = config[1] Llama-3.1-8B B=1 P=98000 K10 L150; C3 = B=8 P=32768; C4 = ProLong B=1 P=500000 K11 L300
+#   C2 = config[1] Llama-3.1-8B B=1 P=98000 K10 L150; C3 = B=8 P=32768; C4 = the ProLong shape K11 L300 at its full
+#   P=500000 (BASELINE's 32-layer C4 runs at P=200000 to fit 80 GB; one layer fits at 500K, the harder case for the tables)
 #   C5 = Llama-3.1-70B under KV-head TP=8: the per-rank shape Hq 8, Hkv 1, n = 97 932 (attnserver_dist.py:252-254)
 # ------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("name,B,P,K,L,Hq,Hkv", [("C2", 1, 98000, 10, 150, 32, 8), ("C3", 8, 32768, 10, 150, 32, 8),
@@ -684,6 +685,10 @@ def test_full_size_properties(cuda_lib, name, B, P, K, L, Hq, Hkv):
     G = Hq // Hkv
     H = B * Hq
     ctx = Context(K, L, 1, Hq, Hkv, d, B, M, device=DEV)
+    if name in ("C2", "C5rank"):
+        # every head's cluster resident at once: where the context needs no more key segments than that allows, the cluster
+        # size is chosen so that one launch is ONE wave of clusters
+        assert ctx.get_info("fused_cluster_waves") == 1
     ctx.set_option("save_mask", 1)
     g = torch.Generator(device=DEV).manual_seed(0)
     hf = torch.randn((d, K * L), generator=g, device=DEV).bfloat16()
@@ -698,7 +703,7 @@ def test_full_size_properties(cuda_lib, name, B, P, K, L, Hq, Hkv):
         key = key - key.mean(dim=1, keepdim=True)
         value = torch.randn((Hkv, n, d), generator=g, device=DEV).bfloat16()
         kn = key.norm(p=2, dim=-1).float()
-        kcodes = ctx.hash_keys(key)                                    # tcgen05 key-side SimHash at full size
+        kcodes = ctx.hash_keys(key)                                    # tensor-core key-side SimHash at full size
         if name == "C2":                                               # ... equal to the reference-style torch glue
             ref_codes = synth.hash_keys(key, hf, K, L)
             bad = torch.nonzero(ref_codes != kcodes)                   # (g, l, key) triples, a few dozen of 117 M
@@ -914,7 +919,7 @@ def test_runner_fused_matches_eager_and_graph(cuda_lib):
 
 
 # ------------------------------------------------------------------------------------------------
-# key-side SimHash on tcgen05 (table build, SURVEY 8(f)-1): mirrors attnserver.py:159-168
+# key-side SimHash on the tensor cores (table build, SURVEY 8(f)-1): mirrors attnserver.py:159-168
 # ------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("impl", [1, 0])
 @pytest.mark.parametrize("K,L,Hkv,n", [(10, 150, 2, 1000), (11, 300, 1, 777), (4, 50, 8, 128), (15, 16, 1, 4097), (7, 13, 3, 130),

@@ -2,8 +2,7 @@
 
   * oracle/mpig_oracle.c (the C restatement) against the committed golden vectors produced by the
     reference's own compiled operators (tests/golden/make_golden.py), and against those operators
-    live when oracle/_ref is present (it is in the build container; on the GPU box it travels as a
-    prebuilt binary);
+    live as well wherever oracle/_ref has been built;
   * the selection rule and the attention math against the reference tests' torch formulas
     (library/lsh/test.py:43, library/sparse_attention/test_sparse.py:68-84);
   * the C-ABI shared library loads and exports every symbol include/magicpig_b200.h declares.
@@ -18,6 +17,8 @@ import torch
 import oracle
 from oracle import ref_loader
 from magicpig_b200 import synth, _native
+from tests.golden.make_golden import (LIVE_PROBE_CASES, checksum, live_attention_inputs, live_probe_inputs, reference_attention,
+                                      reference_probe)
 
 GOLD = os.path.join(os.path.dirname(__file__), "golden")
 
@@ -118,7 +119,6 @@ def test_port_c1_matches_golden():
     hf = synth.make_hash_func(d, K, L, seed=0)
     q = synth.make_query(B, Hq, d, seed=1)
     key, value, kn, _ = synth.make_kv(B, Hkv, n, d, seed=2, dist="clustered", q_dirs=q.reshape(B, Hq, d)[:, :1].float())
-    from tests.golden.make_golden import checksum
     if checksum(hf, q, key, value, kn) != str(z["input_sha256"]):
         pytest.skip("torch RNG stream differs from the one that produced the fixture")
     kcodes = synth.hash_keys(key, hf, K, L)
@@ -198,26 +198,21 @@ def test_window_and_merge_restatement():
     assert torch.allclose(om, ou, atol=1e-5) and abs(float(lm[0] - lu[0])) < 1e-4
 
 
-@pytest.mark.skipif(not ref_loader.available(), reason="oracle/_ref not built / CPU lacks AVX-512")
-@pytest.mark.parametrize("K,L,seq,delta,group,bsz", [(4, 50, 1024, 128, 4, 1), (8, 100, 1024, 128, 8, 2), (8, 50, 4096, 1024, 4, 1)])
+@pytest.mark.parametrize("K,L,seq,delta,group,bsz", LIVE_PROBE_CASES)
 def test_port_probe_vs_live_reference(K, L, seq, delta, group, bsz):
-    """library/lsh/test.py's own case shape, checked three ways: reference binary, port, torch formula."""
-    lsh_m, _, _ = ref_loader.load()
-    g = torch.Generator().manual_seed(K * 1000 + L)
-    Hq = 32
-    Hkv = Hq // group
-    NB, M = 1 << K, seq + delta
-    codes = torch.randint(0, NB, (bsz, Hkv, L, seq), generator=g, dtype=torch.int16)
+    """library/lsh/test.py's own case shape, checked three ways: reference binary (its stored outputs, and the binary itself
+    when oracle/_ref is built here), port, torch formula."""
+    i = LIVE_PROBE_CASES.index((K, L, seq, delta, group, bsz))
+    codes, query, Hq, Hkv, M = live_probe_inputs(K, L, seq, delta, group, bsz)
+    z = np.load(os.path.join(GOLD, "live_reference.npz"))
+    if checksum(codes, query) != str(z[f"probe{i}_sha256"]):
+        pytest.skip("torch RNG stream differs from the one that produced the fixture")
+    results, nnz, mask = (torch.from_numpy(z[f"probe{i}_{k}"]) for k in ("results", "nnz", "mask"))
+    if ref_loader.available():
+        lsh_m, _, _ = ref_loader.load()
+        live = reference_probe(lsh_m, K, codes, query, Hq, Hkv, M)
+        assert all(torch.equal(a, b) for a, b in zip(live, (results, nnz, mask)))
     sc, si = codes.sort()
-    R = lsh_m.LSH()
-    R.alloc(K, L, 1, Hq, Hkv, bsz, M)
-    for b in range(bsz):
-        R.fill(0, b, sc[b].contiguous(), si[b].int().contiguous())
-    query = torch.randint(0, NB, (bsz * Hq, L), generator=g, dtype=torch.int32)
-    results = torch.zeros((bsz * Hq, M), dtype=torch.int32)
-    nnz = torch.zeros((bsz * Hq,), dtype=torch.int32)
-    R.batch_retrieve(0, query, results, nnz)
-    mask = R.get_mask().clone().view(torch.uint8).reshape(bsz * Hq, M)
     for b in range(bsz):
         T = oracle.Tables(Hkv, L, K, M)
         T.fill(sc[b].contiguous(), si[b].int().contiguous())
@@ -228,29 +223,22 @@ def test_port_probe_vs_live_reference(K, L, seq, delta, group, bsz):
         assert torch.equal((cnt > 1).sum(-1).int(), nz)
 
 
-@pytest.mark.skipif(not ref_loader.available(), reason="oracle/_ref not built / CPU lacks AVX-512")
 def test_port_attention_vs_live_reference():
-    _, sa_m, _ = ref_loader.load()
-    g = torch.Generator().manual_seed(77)
-    B, Hq, Hkv, d, K, L, n, M = 1, 8, 2, 128, 10, 150, 2048, 2048 + 128
-    key = torch.randn((B, Hkv, n, d), generator=g).bfloat16()
-    value = torch.randn((B, Hkv, n, d), generator=g).bfloat16()
-    kn = key.norm(p=2, dim=-1).float()
-    q = torch.randn((B * Hq, d), generator=g).bfloat16()
-    nnz = torch.randint(1, n, (B * Hq,), generator=g).int()
-    ind = torch.zeros((B * Hq, M), dtype=torch.int32)
-    for h in range(B * Hq):
-        ind[h, : nnz[h]] = torch.randperm(n, generator=g)[: nnz[h]].int()
-    S = sa_m.SparseAttentionServer()
-    S.alloc(1, Hq, Hkv, d, B, M)
-    S.fill(0, 0, key[0].contiguous(), value[0].contiguous(), kn[0].contiguous())
-    out_ref = torch.zeros((B * Hq, d), dtype=torch.bfloat16)
-    mve_ref = torch.zeros((2, B * Hq))
-    qn = q.float().norm(p=2, dim=-1)
-    S.attention_wrapper(0, K, L, out_ref, mve_ref, q, qn, ind, nnz)
+    dims, key, value, kn, q, ind, nnz = live_attention_inputs()
+    z = np.load(os.path.join(GOLD, "live_reference.npz"))
+    if checksum(key, value, kn, q, ind, nnz) != str(z["attn_sha256"]):
+        pytest.skip("torch RNG stream differs from the one that produced the fixture")
+    out_ref, mve_ref = bf16_from_u16(z["attn_out_bf16"]).reshape(q.shape), torch.from_numpy(z["attn_mve"])
+    if ref_loader.available():
+        _, sa_m, _ = ref_loader.load()
+        out_live, mve_live = reference_attention(sa_m, dims, key, value, kn, q, ind, nnz)
+        # the stored outputs may come from the other flavour (AVX512_BF16 or not) of the reference build
+        assert torch.allclose(out_live.float(), out_ref.float(), rtol=1e-2, atol=1e-2)
+        assert torch.allclose(mve_live[1], mve_ref[1], atol=2e-2)
+    B, Hq, Hkv, d, K, L, n, M = dims
     t = dict(B=B, Hkv=Hkv, n=n, d=d, M=M, key=key, value=value, key_norm=kn)
     k, v, knp = pad_store(t)
-    out, mve, _ = oracle.attention_wrapper(k, v, knp, K, L, q, qn, ind, nnz)
+    out, mve, _ = oracle.attention_wrapper(k, v, knp, K, L, q, q.float().norm(p=2, dim=-1), ind, nnz)
     assert torch.allclose(out.float(), out_ref.float(), rtol=1e-2, atol=1e-2)
     assert torch.allclose(mve[1], mve_ref[1], atol=2e-2)
 
