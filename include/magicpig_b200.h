@@ -115,12 +115,14 @@ size_t mpig_device_bytes(const mpig_ctx *ctx);
 int mpig_set_option(mpig_ctx *ctx, const char *key, int64_t value);
 /* Read-only facts: "last_decode_fused" (1 if the last mpig_decode ran the fused kernel), "fused_applicable",
  * "fused_cluster_waves" (waves of thread-block clusters one fused launch takes on this device; 1 = all resident at once,
- * 0 = fused decode not applicable), "window_capacity" (sink + local + generation_buffer rows). */
+ * 0 = fused decode not applicable), "window_capacity" (sink + local + generation_buffer rows), "table_segments" (key segments S
+ * of the tables, see mpig_lsh_table_ptrs). */
 int mpig_get_info(mpig_ctx *ctx, const char *key, int64_t *value);
 /* Capacity errors the DEVICE detected (the lengths saturate there): bit 0 = a sparse window is full (generation_buffer
  * exhausted: each further token overwrites the previous one's K/V), bit 1 = a dense cache reached max_length.  mpig_plan
  * itself returns MPIG_ESTATE for the same conditions as long as it has not been captured into a CUDA graph (replays advance
- * only the device-side lengths).  Synchronises `stream`.  The reference has no such check (flashinfer append past the page). */
+ * only the device-side lengths).  mpig_spill_window is the way out of a full sparse window.  Synchronises `stream`.  The
+ * reference has no such check (flashinfer append past the page). */
 int mpig_error_flags(mpig_ctx *ctx, int32_t *flags_out, void *stream);
 
 /* LSHSparseAttnServer.clear (attnserver.py:314-331) = LSH::clear (lsh.cc:293-306) +
@@ -181,8 +183,21 @@ int mpig_simhash(mpig_ctx *ctx, const void *query_bf16, int32_t *codes, float *q
  * window rows of a sparse layer, keys ALREADY centred: k, v bf16 (Hkv, w, d). */
 int mpig_window_fill(mpig_ctx *ctx, int layer, int request, const void *avg_k_bf16, const void *k_bf16,
                      const void *v_bf16, int w, void *stream);
-/* LSHSparseAttnServer.plan (attnserver.py:196-224): advance every request's window length by one. */
+/* LSHSparseAttnServer.plan (attnserver.py:196-224): advance every request's window length by one.  Refuses (MPIG_ESTATE) when a
+ * window is full; mpig_spill_window between tokens frees it. */
 int mpig_plan(mpig_ctx *ctx, void *stream);
+/* Move the oldest non-sink rows of every request's sparse window into the sampled store (no reference equivalent; the
+ * reference caps a generation at generation_buffer tokens).  For every request b and every sparse layer, window rows
+ * [sink, win_len[b] - keep) become offloaded keys n_old .. n_old + g_b - 1 (records, key norms, and their codes merged into the
+ * L hash tables), rows [win_len[b] - keep, win_len[b]) move down to [sink, sink + keep) and win_len[b] = sink + keep, with
+ * g_b = max(0, win_len[b] - sink - keep), sink = num_sink_tokens and n_old the count mpig_attn_fill recorded plus earlier
+ * spills (the tables must have been built over the same keys).  keep = num_local_tokens gives a layer the shape a prefill of
+ * P + g tokens would have, centred with the prefill's mean key.  spilled_out int32 [B] (host, may be NULL) receives g_b.
+ * Reads the device window lengths (synchronises `stream`), so it is correct after eager plan() calls and after replays of a
+ * captured step alike.  Not capturable.  A decode step captured before a spill stays valid after it.  Dense layers are
+ * untouched.  MPIG_EINVAL: keep < 0 or sink + keep >= window capacity; MPIG_ESTATE: n_old + g_b > max_length for some sparse
+ * layer, or no hash_func set.  On these errors nothing is modified. */
+int mpig_spill_window(mpig_ctx *ctx, int keep, int32_t *spilled_out, void *stream);
 /* Fused sparse-layer decode (attnserver.py:261-312): centre + append the new key/value to the
  * window, SimHash, probe, gather attention over window + sample with the LSE merge folded in -- one kernel launch.
  * query bf16 (B, Hq, d); key/value bf16 (B, Hkv, d); out bf16 (B, Hq*d).

@@ -136,6 +136,13 @@ class LSHSparseAttnServer:
         """attnserver.py:196-224."""
         self.ctx.plan()
 
+    def spill_window(self, keep: Optional[int] = None) -> torch.Tensor:
+        """Not in the reference.  Moves the oldest generated tokens of every sparse layer's window into the sampled store and
+        the hash tables, keeping the newest `keep` (default num_local_tokens) in the window, so that a generation can run past
+        generation_buffer tokens.  Call it between tokens, never inside a captured step (it synchronises); plan() does not
+        spill on its own.  Returns the spilled token count per request, int32 (B,) on the host."""
+        return self.ctx.spill_window(keep)
+
     def decode(self, query_states: torch.Tensor, key_states: torch.Tensor, value_states: torch.Tensor, layer_idx: int):
         """attnserver.py:228-312.  q (B,Hq,1,d), k/v (B,Hkv,1,d) -> (B, 1, Hq*d)."""
         q = query_states.to(torch.bfloat16).contiguous()

@@ -148,6 +148,9 @@ struct mpig_ctx {
     bool h_len_exact = true;
     void *host_stage_dev = nullptr;          // device-side address of the mapped pinned block host_stage
     uint32_t host_epoch = 0;                 // completion-flag value of the last mpig_decode_host (flags live at the end of host_stage)
+    // mpig_spill_window scratch, allocated by the first spill: per-request counts | spilled keys (Hkv, g, d) bf16 per request |
+    // their codes (Hkv, L, g) int16 per request, sized for every request spilling all its non-sink window rows
+    uint8_t *spill_buf = nullptr;
 };
 
 namespace mpig {
@@ -315,6 +318,11 @@ bool fused_applicable(const mpig_ctx *ctx);
 int fused_resident_clusters(int C, int threads);
 int fused_cluster_waves(const mpig_ctx *ctx);   // waves of clusters one fused launch takes (0 = not applicable / unknown)
 int launch_pack_nhd(mpig_ctx *ctx, const void *k, const void *v, uint8_t *rec, int Hkv, int n, int rows_cap, cudaStream_t s);
+// window spill, table side (tables.cu): merge the codes of the keys [n_old[b], n_old[b] + g[b]) of every request into the
+// tables of `layer`.  codes (Hkv, L, g[b]) int16 per request, request b's block starting at pre[b] * Hkv * L; g / pre / n_old
+// are device arrays [B].
+int launch_table_merge(mpig_ctx *ctx, int layer, const int16_t *codes, const int32_t *g, const int32_t *pre, const int32_t *n_old,
+                       cudaStream_t s);
 
 // ---- host helpers --------------------------------------------------------------------------
 int check_layer(mpig_ctx *ctx, int layer, bool need_sparse, const char *who);

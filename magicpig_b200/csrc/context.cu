@@ -240,6 +240,7 @@ void mpig_destroy(mpig_ctx *ctx) {
     cudaFree(ctx->fused_dbg);
     free(ctx->fused_plan_cache);
     cudaFree(ctx->dev_stage);
+    cudaFree(ctx->spill_buf);
     if (ctx->host_stage) cudaFreeHost(ctx->host_stage);
     for (auto e : ctx->timing_events) cudaEventDestroy(e);
     }
@@ -389,6 +390,7 @@ int mpig_get_info(mpig_ctx *ctx, const char *key, int64_t *value) {
     else if (k == "fused_applicable") *value = fused_applicable(ctx) ? 1 : 0;
     else if (k == "fused_cluster_waves") *value = fused_cluster_waves(ctx);
     else if (k == "window_capacity") *value = ctx->Wcap;
+    else if (k == "table_segments") *value = ctx->nseg;
     else {
         set_error("mpig_get_info: unknown key '%s'", key);
         return MPIG_EINVAL;

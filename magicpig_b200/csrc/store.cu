@@ -4,7 +4,8 @@
 //   SparseAttentionServer::fill          :601-627   -> pack_records_kernel (K|V interleaved 512-byte records + fp32 norms)
 //   get_key_cache / get_value_cache / get_key_norm :1213-1234 -> unpack_records_kernel
 //   attention_wrapper                    :629-745   -> mpig_attention_wrapper (launches attend_mma_kernel, attend_mma.cu)
-// and the dense layers' prefill copy (attnserver.py:116-120) -> pack_records_nhd_kernel.
+// and the dense layers' prefill copy (attnserver.py:116-120) -> pack_records_nhd_kernel; mpig_spill_window (no reference
+// equivalent: generated window rows -> store + tables) -> spill_move_kernel, mpig_hash_keys, table_merge_kernel (tables.cu).
 #include "attend_common.cuh"
 
 namespace mpig {
@@ -52,6 +53,64 @@ __global__ void pack_records_nhd_kernel(const uint4 *__restrict__ k, const uint4
         const int j = (int)(row / Hkv), g = (int)(row % Hkv);
         const uint4 val = (chunk < 16) ? k[row * 16 + chunk] : v[row * 16 + (chunk - 16)];
         rec[((size_t)g * rows_cap + j) * 32 + chunk] = val;
+    }
+}
+
+// Window spill, store side (mpig_spill_window): one CTA per (kv-head, request) of one sparse layer, 8 warps.  With g = spill_g[b]:
+//   window rows [sink, sink + g) -> records n_old .. n_old + g - 1 of the store (bitwise), their key norms
+//   kn = bf16(||k||_2) widened to fp32 (fp32 sum of squares, one rounding: what fill() stores), and their key halves -> stage
+//   (Hkv, g, d) bf16 at row spill_pre[b] * Hkv for the key hash;
+//   window rows [sink + g, sink + g + keep) -> [sink, sink + keep).
+// The kept rows move down in place, so they are copied in chunks of ascending rows, each chunk read completely before any of
+// it is written (a row is only ever written after every row it lands on has been read).  One CTA owns the whole window of its
+// (request, kv-head): no ordering between CTAs is involved.
+__global__ void __launch_bounds__(256) spill_move_kernel(uint4 *win, uint4 *__restrict__ rec, float *__restrict__ kn_store,
+                                                         uint4 *__restrict__ stage, const int32_t *__restrict__ spill_g,
+                                                         const int32_t *__restrict__ spill_pre, const int32_t *__restrict__ n_old_b,
+                                                         int Hkv, int M, int Wcap, int sink, int keep) {
+    constexpr int T = 256, UN = 4;
+    const int gi = blockIdx.x, b = blockIdx.y, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int g = spill_g[b];
+    if (g == 0) return;
+    const size_t bg = (size_t)b * Hkv + gi;
+    uint4 *w = win + bg * Wcap * 32;
+    uint4 *r = rec + (bg * M + n_old_b[b]) * 32;
+    float *kns = kn_store + bg * M + n_old_b[b];
+    uint4 *st = stage + ((size_t)spill_pre[b] * Hkv + (size_t)gi * g) * 16;
+    for (int j = warp; j < g; j += T / 32) {
+        const uint4 x = w[(size_t)(sink + j) * 32 + lane];
+        r[(size_t)j * 32 + lane] = x;
+        float ss = 0.f;
+        if (lane < 16) {   // lanes 0..15 hold the key half of the record
+            st[(size_t)j * 16 + lane] = x;
+            const uint32_t p[4] = {x.x, x.y, x.z, x.w};
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const float a = bf16lo(p[i]), c = bf16hi(p[i]);
+                ss = fmaf(a, a, ss);
+                ss = fmaf(c, c, ss);
+            }
+        }
+        ss = warp_sum(ss);
+        if (lane == 0) kns[j] = __uint_as_float((uint32_t)f32_to_bf16_rne(sqrtf(ss)) << 16);
+    }
+    __syncthreads();
+    const int total = keep * 32;   // 16-byte chunks of the kept rows
+    uint4 *src = w + (size_t)(sink + g) * 32, *dst = w + (size_t)sink * 32;
+    for (int c0 = 0; c0 < total; c0 += T * UN) {
+        uint4 v[UN];
+#pragma unroll
+        for (int u = 0; u < UN; ++u) {
+            const int i = c0 + u * T + tid;
+            if (i < total) v[u] = src[i];
+        }
+        __syncthreads();
+#pragma unroll
+        for (int u = 0; u < UN; ++u) {
+            const int i = c0 + u * T + tid;
+            if (i < total) dst[i] = v[u];
+        }
+        __syncthreads();
     }
 }
 
@@ -138,6 +197,90 @@ int mpig_attn_read_cache(mpig_ctx *ctx, int layer, void *k_bf16, void *v_bf16, f
         MPIG_LAUNCH_CHECK(ctx);
     }
     if (kn) MPIG_CUDA(cudaMemcpyAsync(kn, ls.kn, rows * sizeof(float), cudaMemcpyDeviceToDevice, as_stream(stream)));
+    return MPIG_OK;
+}
+
+int mpig_spill_window(mpig_ctx *ctx, int keep, int32_t *spilled_out, void *stream) {
+    mpig::DeviceGuard _dg(ctx);  // run on the context's device whatever the caller's current device is
+    MPIG_REQUIRE(ctx, MPIG_EINVAL, "mpig_spill_window: null context");
+    const int B = ctx->cfg.batch_size, sink = ctx->cfg.num_sink_tokens, M = ctx->cfg.max_length;
+    const int Hkv = ctx->cfg.num_key_value_heads, L = ctx->cfg.L, d = ctx->cfg.head_dim, nl = ctx->cfg.num_layers;
+    MPIG_REQUIRE(keep >= 0 && sink + keep < ctx->Wcap, MPIG_EINVAL,
+                 "mpig_spill_window: keep=%d: sink (%d) + keep must leave a free row in the window (capacity %d)", keep, sink, ctx->Wcap);
+    MPIG_REQUIRE(ctx->hash_func_set, MPIG_ESTATE, "mpig_spill_window before mpig_set_hash_func: the spilled keys cannot be hashed");
+    cudaStream_t s = as_stream(stream);
+    // the device lengths are the truth (replays of a captured plan() advance only them)
+    std::vector<int32_t> wl(B);
+    MPIG_CUDA(cudaMemcpyAsync(wl.data(), ctx->win_len, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    MPIG_CUDA(cudaStreamSynchronize(s));
+    // meta = g[B] | pre[B] (exclusive prefix of g) | n_old[num_layers][B]
+    std::vector<int32_t> meta((size_t)(2 + nl) * B, 0);
+    int tot = 0;
+    for (int b = 0; b < B; ++b) {
+        const int g = std::max(0, wl[b] - sink - keep);
+        meta[b] = g;
+        meta[B + b] = tot;
+        tot += g;
+    }
+    for (int l = 0; l < nl; ++l) {
+        if (!ctx->layers[l].sparse) continue;
+        for (int b = 0; b < B; ++b) {
+            MPIG_REQUIRE(ctx->n_off[l][b] + meta[b] <= M, MPIG_ESTATE,
+                         "mpig_spill_window: layer %d request %d: %d offloaded + %d spilled keys exceed max_length=%d", l, b,
+                         ctx->n_off[l][b], meta[b], M);
+            meta[(size_t)(2 + l) * B + b] = ctx->n_off[l][b];
+        }
+    }
+    if (tot > 0) {
+        // scratch for the worst case (every request spills all its non-sink rows), allocated once
+        const size_t meta_bytes = (((size_t)(2 + nl) * B * sizeof(int32_t)) + 255) & ~(size_t)255;
+        const size_t rows_cap = (size_t)B * std::max(ctx->Wcap - sink, 1);
+        const size_t key_bytes = rows_cap * Hkv * d * sizeof(__nv_bfloat16);
+        if (!ctx->spill_buf) {
+            const size_t bytes = meta_bytes + key_bytes + rows_cap * Hkv * L * sizeof(int16_t);
+            cudaError_t e = cudaMalloc(&ctx->spill_buf, bytes);
+            if (e != cudaSuccess) {
+                ctx->spill_buf = nullptr;
+                (void)cudaGetLastError();
+                set_error("mpig_spill_window: cudaMalloc(%zu bytes) failed: %s", bytes, cudaGetErrorString(e));
+                return MPIG_ENOMEM;
+            }
+            ctx->bytes += bytes;
+        }
+        int32_t *d_meta = reinterpret_cast<int32_t *>(ctx->spill_buf);
+        __nv_bfloat16 *keys = reinterpret_cast<__nv_bfloat16 *>(ctx->spill_buf + meta_bytes);
+        int16_t *codes = reinterpret_cast<int16_t *>(ctx->spill_buf + meta_bytes + key_bytes);
+        MPIG_CUDA(cudaMemcpyAsync(d_meta, meta.data(), meta.size() * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+        for (int l = 0; l < nl; ++l) {
+            LayerStore &ls = ctx->layers[l];
+            if (!ls.sparse) continue;
+            const int32_t *n_old = d_meta + (size_t)(2 + l) * B;
+            spill_move_kernel<<<dim3(Hkv, B), 256, 0, s>>>(reinterpret_cast<uint4 *>(ls.win), reinterpret_cast<uint4 *>(ls.kv), ls.kn,
+                                                          reinterpret_cast<uint4 *>(keys), d_meta, d_meta + B, n_old, Hkv, M, ctx->Wcap,
+                                                          sink, keep);
+            MPIG_LAUNCH_CHECK(ctx);
+            for (int b = 0; b < B; ++b) {
+                if (meta[b] == 0) continue;
+                const int rc = mpig_hash_keys(ctx, keys + (size_t)meta[B + b] * Hkv * d, meta[b], codes + (size_t)meta[B + b] * Hkv * L,
+                                              stream);
+                if (rc) return rc;
+            }
+            const int rc = launch_table_merge(ctx, l, codes, d_meta, d_meta + B, n_old, s);
+            if (rc) return rc;
+        }
+        for (int b = 0; b < B; ++b)
+            if (meta[b] > 0) wl[b] = sink + keep;
+        MPIG_CUDA(cudaMemcpyAsync(ctx->win_len, wl.data(), B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+        // the pageable host buffers above must outlive the copies
+        MPIG_CUDA(cudaStreamSynchronize(s));
+        for (int l = 0; l < nl; ++l)
+            if (ctx->layers[l].sparse)
+                for (int b = 0; b < B; ++b) ctx->n_off[l][b] += meta[b];
+        if (ctx->h_len_exact)
+            for (int b = 0; b < B; ++b) ctx->h_win_len[b] = wl[b];
+    }
+    if (spilled_out)
+        for (int b = 0; b < B; ++b) spilled_out[b] = meta[b];
     return MPIG_OK;
 }
 

@@ -5,6 +5,7 @@
 //   sort()+LSH::fill     attnserver.py:186-193 -> build_segments_kernel<false> (counting sort on device)
 //   LSH::batch_retrieve  :210-241, LSH::retrieve :243-288 -> probe_kernel
 //   LSH::get_mask        :308-314  -> expand_mask_kernel
+// and, with no reference equivalent, the table side of a window spill (mpig_spill_window, store.cu) -> table_merge_kernel
 //
 // Table format (per request b, kv-head g, table l; row = (b*Hkv+g)*L + l): segmented compact CSR.
 //   Keys are cut into S = ceil(M / 65536) segments of EQUAL length seg_len = ceil(M / S) rounded up to 64 (<= 65536; equal so
@@ -116,6 +117,111 @@ __global__ void __launch_bounds__(1024) build_segments_kernel(const int16_t *__r
     } else {
         for_each_pair([&](int cc, int key) { it[atomicAdd(&hist[cc], 1)] = (uint16_t)(key - seg_lo); });
     }
+}
+
+// ---------------------------------------------------------------------------------------------
+// Table merge of a window spill (mpig_spill_window): add the keys [n_old, n_old + g) of a request, whose codes are given, to
+// its tables in place.  One CTA per (table, kv-head, request x key segment); segments the new keys do not touch return at once.
+// With ex[c] = exclusive prefix of the histogram of the new codes over buckets and ro[c] = old offset relative to the segment:
+//   new offset of bucket c           = ro[c] + ex[c]
+//   old item at relative position p  -> p + ex[bucket(p)]          (old items of a bucket first ...)
+//   new key of code c                -> ro[c + 1] + ex[c] + rank   (... then the new ones)
+// The shift ex[bucket(p)] never decreases with p, so the old items are moved from the top of the segment down in chunks, each
+// chunk read completely before any of it is written: a write lands only on positions already read.  No staging copy of the
+// segment is needed, so every K works in place (the old offsets are kept in shared memory when they fit beside the
+// histogram, K <= 14, and read from HBM otherwise).  A segment whose offsets are all equal has no old items, which covers a
+// segment beyond the old keys and tables that were never built (offsets still zero).  grid (L, Hkv, B * S), 512 threads;
+// dynamic smem = (NB + 1 + 40 [+ NB + 1 when staged]) ints.
+// ---------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(512) table_merge_kernel(const int16_t *__restrict__ codes, int32_t *offsets, uint16_t *items,
+                                                          const int32_t *__restrict__ spill_g, const int32_t *__restrict__ spill_pre,
+                                                          const int32_t *__restrict__ n_old_b, int Hkv, int L, int NB, int M, int S,
+                                                          int seg_len, int staged) {
+    extern __shared__ int smem_i[];
+    constexpr int T = 512, UN = 4;
+    int *ex = smem_i;                // NB + 1: histogram of the new codes -> exclusive prefix -> placement cursors
+    int *wsum = smem_i + NB + 1;     // 40
+    int *oo_s = wsum + 40;           // NB + 1 old offsets (staged)
+    const int l = blockIdx.x, gi = blockIdx.y, b = blockIdx.z / S, seg = blockIdx.z % S, tid = threadIdx.x;
+    const int g = spill_g[b], n_old = n_old_b[b];
+    const int seg_lo = seg * seg_len, seg_hi = min(seg_lo + seg_len, M);
+    const int k0 = max(n_old, seg_lo), k1 = min(n_old + g, seg_hi);   // new keys of this segment
+    const size_t row = ((size_t)b * Hkv + gi) * L + l;
+    int32_t *off = offsets + (row * S + seg) * (size_t)(NB + 1);
+    if (k0 >= k1) {
+        // a segment beyond all keys gets the offsets a build writes there (every bucket empty at seg_lo), so that tables that
+        // were never built end up identical to a rebuild too
+        if (g > 0 && seg_lo >= n_old + g)
+            for (int c = tid; c <= NB; c += T) off[c] = seg_lo;
+        return;
+    }
+    uint16_t *it = items + row * (size_t)M + seg_lo;
+    const int16_t *cn = codes + (size_t)spill_pre[b] * Hkv * L + ((size_t)gi * L + l) * g - n_old;   // cn[key]
+    const int base0 = off[0];
+    const int32_t *oo = off;
+    if (staged) {
+        for (int c = tid; c <= NB; c += T) oo_s[c] = off[c];
+        oo = oo_s;
+    }
+    for (int c = tid; c <= NB; c += T) ex[c] = 0;
+    __syncthreads();
+    for (int k = k0 + tid; k < k1; k += T) {
+        const int c = cn[k];
+        if (c >= 0 && c < NB) atomicAdd(&ex[c], 1);
+    }
+    __syncthreads();
+    {   // exclusive scan of ex[0..NB) in place; ex[NB] = number of new keys
+        const int per = (NB + T - 1) / T;
+        const int c0 = min(tid * per, NB), c1 = min(c0 + per, NB);
+        int local = 0;
+        for (int c = c0; c < c1; ++c) local += ex[c];
+        int total;
+        int run = block_exclusive_scan(local, wsum, &total);
+        for (int c = c0; c < c1; ++c) {
+            const int h = ex[c];
+            ex[c] = run;
+            run += h;
+        }
+        if (tid == 0) ex[NB] = total;
+    }
+    __syncthreads();
+    // old items, top chunk first
+    const int old_cnt = oo[NB] - base0;
+    for (int top = old_cnt; top > 0; top -= T * UN) {
+        const int lo = max(0, top - T * UN);
+        uint16_t v[UN];
+        int dst[UN];
+#pragma unroll
+        for (int u = 0; u < UN; ++u) {
+            const int p = lo + u * T + tid;
+            dst[u] = -1;
+            if (p < top) {
+                int a = 0, z = NB;   // last bucket whose start is <= p: the bucket holding p
+                while (z - a > 1) {
+                    const int mid = (a + z) >> 1;
+                    if (oo[mid] - base0 <= p) a = mid; else z = mid;
+                }
+                const int sh = ex[a];
+                if (sh) {
+                    v[u] = it[p];
+                    dst[u] = p + sh;
+                }
+            }
+        }
+        __syncthreads();
+#pragma unroll
+        for (int u = 0; u < UN; ++u)
+            if (dst[u] >= 0) it[dst[u]] = v[u];
+        __syncthreads();
+    }
+    // new keys behind the old items of their bucket; ex[c] ends as the inclusive prefix
+    for (int k = k0 + tid; k < k1; k += T) {
+        const int c = cn[k];
+        if (c >= 0 && c < NB) it[oo[c + 1] - base0 + atomicAdd(&ex[c], 1)] = (uint16_t)(k - seg_lo);
+    }
+    __syncthreads();
+    // every thread reads and rewrites only its own entries of `off` (base0 was read before the first barrier)
+    for (int c = tid; c <= NB; c += T) off[c] = seg_lo + (oo[c] - base0) + (c ? ex[c - 1] : 0);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -438,6 +544,21 @@ static int launch_build(mpig_ctx *ctx, int layer, int request, const int16_t *co
         build_segments_kernel<true><<<dim3(L, Hkv, S), 1024, smem, s>>>(codes, idx, off, it, n, ctx->NB, M, L, S, staged, ctx->seg_len);
     else
         build_segments_kernel<false><<<dim3(L, Hkv, S), 1024, smem, s>>>(codes, nullptr, off, it, n, ctx->NB, M, L, S, staged, ctx->seg_len);
+    MPIG_LAUNCH_CHECK(ctx);
+    return MPIG_OK;
+}
+
+int mpig::launch_table_merge(mpig_ctx *ctx, int layer, const int16_t *codes, const int32_t *g, const int32_t *pre,
+                             const int32_t *n_old, cudaStream_t s) {
+    const LayerStore &ls = ctx->layers[layer];
+    const int Hkv = ctx->cfg.num_key_value_heads, L = ctx->cfg.L, S = ctx->nseg, NB = ctx->NB;
+    const size_t base = (size_t)(NB + 1 + 40) * sizeof(int);
+    const int staged = base + (size_t)(NB + 1) * sizeof(int) <= 200 * 1024;   // K <= 14
+    const size_t smem = base + (staged ? (size_t)(NB + 1) * sizeof(int) : 0);
+    MPIG_FUNC_ATTR(table_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    table_merge_kernel<<<dim3(L, Hkv, ctx->cfg.batch_size * S), 512, smem, s>>>(
+        codes, ls.offsets, reinterpret_cast<uint16_t *>(ls.items), g, pre, n_old, Hkv, L, NB, ctx->cfg.max_length, S, ctx->seg_len,
+        staged);
     MPIG_LAUNCH_CHECK(ctx);
     return MPIG_OK;
 }

@@ -52,6 +52,7 @@ class Context:
         self.H = self.B * self.Hq
         self.G = self.Hq // max(self.Hkv, 1)
         self.NB = 1 << K
+        self.num_sink_tokens, self.num_local_tokens = num_sink_tokens, num_local_tokens
         self.Wcap = num_sink_tokens + num_local_tokens + generation_buffer
         self.dense_layers = sorted(set(int(x) for x in dense_layers if 0 <= int(x) < num_layers))
         cfg = N.MpigConfig()
@@ -237,6 +238,15 @@ class Context:
 
     def plan(self):
         N.check(self.lib.mpig_plan(self._h, _stream()), "mpig_plan")
+
+    def spill_window(self, keep: Optional[int] = None) -> torch.Tensor:
+        """Move the oldest non-sink window rows of every request and sparse layer into the sampled store and the hash tables,
+        keeping the newest `keep` (default num_local_tokens) in the window.  Returns the spilled row count per request, int32 (B,)
+        on the host.  Synchronises; not capturable, but a decode step captured before the spill stays valid after it."""
+        keep = self.num_local_tokens if keep is None else int(keep)
+        out = (ctypes.c_int32 * self.B)()
+        N.check(self.lib.mpig_spill_window(self._h, keep, out, _stream()), "mpig_spill_window")
+        return torch.tensor(list(out), dtype=torch.int32)
 
     def decode(self, layer: int, query: torch.Tensor, key: torch.Tensor, value: torch.Tensor,
                out: Optional[torch.Tensor] = None) -> torch.Tensor:

@@ -150,8 +150,53 @@ def host_and_peer_case():
     print("host buffers + peer exchange ok")
 
 
+def spill_case():
+    """Window spill (store move + norms, key hash of the spilled keys, table merge across a segment boundary) followed by a decode;
+    the tables must equal a device rebuild over all stored keys."""
+    B, Hq, Hkv, n, K, L, M = 1, 4, 2, 1000, 6, 16, 4096   # 4 segments of 1024 keys: the spill crosses 1024
+    g = torch.Generator(device=dev).manual_seed(12)
+    hf = torch.randn((d, K * L), generator=g, device=dev).bfloat16()
+    ctxs = []
+    for _ in range(2):
+        ctx = Context(K, L, 1, Hq, Hkv, d, B, M, generation_buffer=40, device=dev)
+        ctx.set_hash_func(hf)
+        ctxs.append(ctx)
+    ctx, other = ctxs
+    key = torch.randn((Hkv, n, d), generator=g, device=dev).bfloat16()
+    ctx.attn_fill(0, 0, key, torch.randn((Hkv, n, d), generator=g, device=dev).bfloat16(), key.norm(p=2, dim=-1).float())
+    ctx.lsh_build(0, 0, ctx.hash_keys(key))
+    ctx.window_fill(0, 0, torch.zeros((Hkv, d), dtype=torch.bfloat16, device=dev), torch.randn((Hkv, 68, d), generator=g, device=dev).bfloat16(),
+                    torch.randn((Hkv, 68, d), generator=g, device=dev).bfloat16())
+    q = torch.randn((B * Hq, d), generator=g, device=dev).bfloat16()
+    for _ in range(40):
+        ctx.plan()
+        ctx.decode(0, q, torch.randn((B * Hkv, d), generator=g, device=dev).bfloat16(), torch.randn((B * Hkv, d), generator=g, device=dev).bfloat16())
+    assert ctx.spill_window().tolist() == [40]
+    ctx.plan()
+    ctx.decode(0, q, torch.randn((B * Hkv, d), generator=g, device=dev).bfloat16(), torch.randn((B * Hkv, d), generator=g, device=dev).bfloat16())
+    k_st, _, _ = ctx.read_cache(0, True, False, False)
+    other.lsh_build(0, 0, ctx.hash_keys(k_st[0, :, : n + 40].contiguous()))
+    torch.cuda.synchronize()
+    from ctypes import byref, c_void_p
+
+    class _View:   # a device buffer the library owns, seen by torch without a copy
+        def __init__(self, ptr, count):
+            self.__cuda_array_interface__ = {"shape": (count,), "typestr": "<i4", "data": (ptr, False), "version": 2}
+
+    count = B * Hkv * L * ctx.get_info("table_segments") * ((1 << K) + 1)
+    offs = []
+    for c in (ctx, other):
+        p = c_void_p()
+        c.lib.mpig_lsh_table_ptrs(c._h, 0, byref(p), None)
+        offs.append(torch.as_tensor(_View(p.value, count), device=dev))
+    assert torch.equal(offs[0], offs[1]), "tables after the spill differ from a rebuild"
+    print("spill ok")
+
+
 if __name__ == "__main__":
-    which = sys.argv[1:] or ["stages", "dense", "decode", "hostpeer"]
+    which = sys.argv[1:] or ["stages", "dense", "decode", "hostpeer", "spill"]
+    if "spill" in which:
+        spill_case()
     if "hostpeer" in which:
         host_and_peer_case()
     if "stages" in which:
