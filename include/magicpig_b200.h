@@ -116,10 +116,12 @@ int mpig_set_option(mpig_ctx *ctx, const char *key, int64_t value);
 /* Read-only facts: "last_decode_fused" (1 if the last mpig_decode ran the fused kernel), "fused_applicable",
  * "fused_cluster_waves" (waves of thread-block clusters one fused launch takes on this device; 1 = all resident at once,
  * 0 = fused decode not applicable), "window_capacity" (sink + local + generation_buffer rows), "table_segments" (key segments S
- * of the tables, see mpig_lsh_table_ptrs). */
+ * of the tables, see mpig_lsh_table_ptrs), "query_tokens_max" (t_max of mpig_reserve_query_tokens, 1 without), "tokens_cluster_waves"
+ * (waves of clusters the last mpig_decode_tokens launch with T > 1 took). */
 int mpig_get_info(mpig_ctx *ctx, const char *key, int64_t *value);
 /* Capacity errors the DEVICE detected (the lengths saturate there): bit 0 = a sparse window is full (generation_buffer
- * exhausted: each further token overwrites the previous one's K/V), bit 1 = a dense cache reached max_length.  mpig_plan
+ * exhausted: each further token overwrites the previous one's K/V), bit 1 = a dense cache reached max_length, bit 2 = mpig_rewind
+ * met a drop outside [0, T] (that request was left untouched).  mpig_plan
  * itself returns MPIG_ESTATE for the same conditions as long as it has not been captured into a CUDA graph (replays advance
  * only the device-side lengths).  mpig_spill_window is the way out of a full sparse window.  Synchronises `stream`.  The
  * reference has no such check (flashinfer append past the page). */
@@ -231,6 +233,45 @@ int mpig_last_out_f32(mpig_ctx *ctx, float *out_f32, void *stream);
  * copied to HOST memory. */
 int mpig_debug_read(mpig_ctx *ctx, unsigned long long *host_out, int nwarps);
 int mpig_fused_debug_read(mpig_ctx *ctx, unsigned long long *host_out, int nctas);
+
+/* ---- verification steps of T tokens (speculative decoding; no reference equivalent) ------------------------------------------
+ * A step checks T candidate tokens (1 <= T <= 8) of every request in one pass over the weights:
+ *   mpig_plan_tokens(T) -> per layer mpig_decode_tokens / mpig_dense_decode_tokens(T) -> mpig_rewind(drop).
+ * The layer appends the T new K/V rows of request b at positions base_b .. base_b + T - 1 (base_b = length before the plan) and
+ * query token t attends causally: window / dense rows [0, base_b + t] and, on sparse layers, its own LSH sample (own codes, probe
+ * and importance weights).  The result equals T single-token steps on the same inputs: identical codes, nnz and index sets, fp32
+ * outputs equal up to summation order.  mpig_rewind then drops the last drop[b] of the T tokens of request b.  The tables and the
+ * sampled store are never touched; mpig_spill_window keeps working because it reads the device lengths.
+ *
+ * Allocates the per-step scratch for up to t_max <= 8 tokens: query codes, norms, nnz, LSE pairs, the fp32 output copy and the
+ * save_mask index lists / bitmaps grow from B*Hq to B*t_max*Hq rows.  Not capturable (allocates, synchronises the device).  The
+ * scratch moves to new addresses, so the call is refused (MPIG_ESTATE) once a plan has been captured into a CUDA graph: reserve
+ * before capturing.  Without it only T = 1 is accepted. */
+int mpig_reserve_query_tokens(mpig_ctx *ctx, int t_max);
+/* mpig_plan for a step of T tokens: every window and dense length advances by T.  T = 1 is exactly mpig_plan.  The host-mirror
+ * checks of mpig_plan apply to +T and refuse (MPIG_ESTATE) before anything is modified; the device saturates and raises the same
+ * mpig_error_flags bits.  Records T as the pending step size (host state, also when captured); MPIG_EINVAL for T outside
+ * [1, reserved]. */
+int mpig_plan_tokens(mpig_ctx *ctx, int T, void *stream);
+/* Sparse layer, T tokens: query bf16 (B, T, Hq, d), key / value bf16 (B, T, Hkv, d), out bf16 (B, T, Hq*d).  T must equal the
+ * pending T (MPIG_ESTATE).  T = 1 is mpig_decode (bitwise).  T > 1: one append launch for the T centred rows, then the T-token
+ * instantiation of the fused kernel under PDL (B*T*Hq clusters, several waves where one does not hold them; shapes with one CTA
+ * per head hash the B*T*Hq rows in the stand-alone SimHash kernel first).  MPIG_EUNSUPPORTED with decode_impl = 0 or a shape the
+ * fused kernel does not take.  After a T > 1 call, mpig_last_probe / mpig_last_codes / mpig_last_out_f32 return B*T*Hq rows in
+ * (b, t, h) order (size the buffers accordingly); after any single-token decode they return B*Hq rows as before. */
+int mpig_decode_tokens(mpig_ctx *ctx, int layer, int T, const void *query_bf16, const void *key_bf16, const void *value_bf16,
+                       void *out_bf16, void *stream);
+/* Dense layer, same shapes: one append launch for the T rows, then one launch per (request, kv-group) in which the T*G query rows
+ * share every fetched K|V record (dense KV bytes per step do not grow with T).  MPIG_EUNSUPPORTED for T*G > 32 or dense_impl = 0. */
+int mpig_dense_decode_tokens(mpig_ctx *ctx, int layer, int T, const void *query_bf16, const void *key_bf16, const void *value_bf16,
+                             void *out_bf16, void *stream);
+/* Drop the last drop[b] tokens of the pending step of request b (drop: DEVICE int32 (B,), 0 <= drop[b] <= T): both lengths shrink by
+ * drop[b]; stale rows past the length are overwritten by the next plan.  Capturable (acceptance can be decided on the GPU).  A
+ * request whose drop is outside [0, T] is left untouched and raises mpig_error_flags bit 2.  At most one rewind per plan
+ * (MPIG_ESTATE).  Outside a capture the call synchronises `stream` and checks the drops first: if one is outside [0, T] it raises
+ * bit 2, changes no length and returns MPIG_EINVAL (the rewind may then be repeated with valid drops); otherwise it rewinds and
+ * refreshes the host mirror of the lengths from the device.  mpig_clear forgets the pending step. */
+int mpig_rewind(mpig_ctx *ctx, const int32_t *drop, void *stream);
 
 /* ---- dense layers (attnserver.py:116-120, 235-259), only with cfg.alloc_dense_kv -------------- */
 /* k, v bf16 (P, Hkv, d) -- the prefill cache in NHD layout as models/llama.py:282 passes it. */

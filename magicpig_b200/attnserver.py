@@ -40,7 +40,8 @@ class LSHSparseAttnServer:
                  table_build: str = "device",
                  key_hash: str = "tcgen05",
                  num_key_value_heads: Optional[int] = None,
-                 num_attention_heads: Optional[int] = None) -> None:
+                 num_attention_heads: Optional[int] = None,
+                 max_query_tokens: int = 1) -> None:
         """Keywords up to `dtype` are the reference's (attnserver.py:9-20).  Extras:
         hash_func   inject the (d, K*L) bf16 projection (the reference draws it unseeded, :55);
         table_build "device" = counting sort on the GPU (mpig_lsh_build); "sorted" = the reference's
@@ -48,7 +49,9 @@ class LSHSparseAttnServer:
         key_hash    "tcgen05" (the name of the first target's tensor cores, kept for compatibility) = key-side SimHash GEMM +
                     sign pack in one tensor-core kernel (mpig_hash_keys, wgmma on sm_90a);
                     "torch" = the reference's chunked `matmul(...).gt(0)` + pack glue (attnserver.py:159-168);
-        num_*_heads per-rank head counts under KV-head tensor parallelism (attnserver_dist.py:252-254).
+        num_*_heads per-rank head counts under KV-head tensor parallelism (attnserver_dist.py:252-254);
+        max_query_tokens  largest number of draft tokens a verification step may check (plan(num_tokens), decode of q_len > 1,
+                    rewind); 1 = single-token decoding only.
         """
         self.K, self.L = K, L
         self.config = config
@@ -74,7 +77,8 @@ class LSHSparseAttnServer:
 
         self.ctx = Context(K, L, self.num_layers, self.num_attention_heads, self.num_key_value_heads, self.head_dim,
                            batch_size, max_length, num_sink_tokens, num_local_tokens, generation_buffer,
-                           dense_layers=self.dense_layers, alloc_dense_kv=True, device=self.device)
+                           dense_layers=self.dense_layers, alloc_dense_kv=True, device=self.device,
+                           max_query_tokens=max_query_tokens)
         if hash_func is None:
             hash_func = torch.randn((self.head_dim, K * L), device=self.device, dtype=torch.bfloat16)  # attnserver.py:55
         self.hash_func = hash_func.to(device=self.device, dtype=torch.bfloat16).contiguous()
@@ -83,7 +87,8 @@ class LSHSparseAttnServer:
                                   dtype=torch.bfloat16) for _ in range(self.num_layers)]
         # key codes of the layer whose table is being built (one layer in flight, as the reference)
         self.hash_code_buffer = torch.zeros((self.num_key_value_heads, L, max_length), dtype=torch.int16, device=self.device)
-        self._out = {}   # layer -> decode output buffer (allocated on first use)
+        self._out = {}   # layer (one token) or (layer, T) (T-token steps) -> decode output buffer (allocated on first use)
+        self._drop = None   # staging of host-side rewind counts
 
     # ------------------------------------------------------------------------------------------
     def alloc_buffer(self, seq_len: int):
@@ -132,9 +137,24 @@ class LSHSparseAttnServer:
         else:
             self.ctx.lsh_build(layer_idx, request_id, codes.contiguous())
 
-    def plan(self):
-        """attnserver.py:196-224."""
-        self.ctx.plan()
+    def plan(self, num_tokens: int = 1):
+        """attnserver.py:196-224.  num_tokens > 1: a verification step of that many tokens per request (the decode calls of the
+        step then take q_len = num_tokens); rewind() afterwards drops the rejected ones."""
+        self.ctx.plan(num_tokens)
+
+    def rewind(self, num_rejected):
+        """Not in the reference.  Drops the last `num_rejected` tokens of the pending verification step: an int (every request),
+        a sequence of B ints, or a device int32 (B,) tensor (capturable: acceptance can be decided on the GPU)."""
+        if isinstance(num_rejected, torch.Tensor) and num_rejected.is_cuda:
+            drop = num_rejected.to(torch.int32).contiguous()
+        else:
+            if isinstance(num_rejected, int):
+                num_rejected = [num_rejected] * self.batch_size
+            if self._drop is None:
+                self._drop = torch.zeros(self.batch_size, dtype=torch.int32, device=self.device)
+            self._drop.copy_(torch.as_tensor(list(num_rejected), dtype=torch.int32))
+            drop = self._drop
+        self.ctx.rewind(drop)
 
     def spill_window(self, keep: Optional[int] = None) -> torch.Tensor:
         """Not in the reference.  Moves the oldest generated tokens of every sparse layer's window into the sampled store and
@@ -144,7 +164,11 @@ class LSHSparseAttnServer:
         return self.ctx.spill_window(keep)
 
     def decode(self, query_states: torch.Tensor, key_states: torch.Tensor, value_states: torch.Tensor, layer_idx: int):
-        """attnserver.py:228-312.  q (B,Hq,1,d), k/v (B,Hkv,1,d) -> (B, 1, Hq*d)."""
+        """attnserver.py:228-312.  q (B,Hq,1,d), k/v (B,Hkv,1,d) -> (B, 1, Hq*d).  In a verification step of T tokens (plan(T)):
+        q (B,Hq,T,d), k/v (B,Hkv,T,d) -> (B, T, Hq*d), token t attending causally to the tokens before it."""
+        T = query_states.shape[2]
+        if T > 1:
+            return self._decode_tokens(query_states, key_states, value_states, layer_idx, T)
         q = query_states.to(torch.bfloat16).contiguous()
         k = key_states.to(torch.bfloat16).contiguous()
         v = value_states.to(torch.bfloat16).contiguous()
@@ -159,6 +183,21 @@ class LSHSparseAttnServer:
         else:
             self.ctx.decode(layer_idx, q, k, v, out)
         return out.reshape(self.batch_size, 1, self.num_attention_heads * self.head_dim).to(query_states.dtype)
+
+    def _decode_tokens(self, query_states, key_states, value_states, layer_idx: int, T: int):
+        # (B, H, T, d) -> the (B, T, H, d) layout of the T-token entry points
+        q = query_states.to(torch.bfloat16).transpose(1, 2).contiguous()
+        k = key_states.to(torch.bfloat16).transpose(1, 2).contiguous()
+        v = value_states.to(torch.bfloat16).transpose(1, 2).contiguous()
+        out = self._out.get((layer_idx, T))
+        if out is None:
+            out = self._out[(layer_idx, T)] = torch.empty((self.batch_size, T, self.num_attention_heads * self.head_dim),
+                                                          dtype=torch.bfloat16, device=self.device)
+        if layer_idx in self.dense_layers:
+            self.ctx.dense_decode_tokens(layer_idx, T, q, k, v, out)
+        else:
+            self.ctx.decode_tokens(layer_idx, T, q, k, v, out)
+        return out.to(query_states.dtype)
 
     def clear(self):
         """attnserver.py:314-331."""

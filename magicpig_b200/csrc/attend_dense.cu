@@ -63,6 +63,58 @@ __device__ __forceinline__ void finalize_dense_head(const DenseParams &p, int h,
     *reinterpret_cast<uint2 *>(reinterpret_cast<uint8_t *>(out) + ((size_t)h * D + 4 * lane) * 2) = make_uint2(lo, hi);
 }
 
+// Partition of the groups' rows over the nw warps of the grid (one warp runs it): s_prefix[bg] = first row of group bg in the
+// concatenation of all groups' rows, s_wpre[bg] = its first work item; a group of t rows gets max(1, t / Rp) items of >= TILE
+// rows, so the items number at most nw whenever nw > BG (a warp then takes at most one item).
+__device__ __forceinline__ void dense_partition(const DenseParams &p, int *s_prefix, int *s_wpre, int nw, int lane) {
+    int run = 0;
+    for (int g0 = 0; g0 < p.BG; g0 += 32) {
+        const int bg = g0 + lane;
+        const int t = (bg < p.BG) ? min(max(p.len[bg / p.Hkv], 0), p.M) : 0;
+        int inc = t;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            int v = __shfl_up_sync(0xffffffffu, inc, o);
+            if (lane >= o) inc += v;
+        }
+        if (bg < p.BG) s_prefix[bg] = run + inc - t;
+        run += __shfl_sync(0xffffffffu, inc, 31);
+    }
+    const int total = run;
+    if (lane == 0) s_prefix[p.BG] = total;
+    const int Rp = (nw > p.BG) ? max(TILE, (total + (nw - p.BG) - 1) / (nw - p.BG)) : 0x3fffffff;
+    __syncwarp();
+    run = 0;
+    for (int g0 = 0; g0 < p.BG; g0 += 32) {
+        const int bg = g0 + lane;
+        int w = 0;
+        if (bg < p.BG) {
+            const int t = s_prefix[bg + 1] - s_prefix[bg];
+            w = (t > 0) ? max(1, t / Rp) : 0;
+        }
+        int inc = w;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            int v = __shfl_up_sync(0xffffffffu, inc, o);
+            if (lane >= o) inc += v;
+        }
+        if (bg < p.BG) s_wpre[bg] = run + inc - w;
+        run += __shfl_sync(0xffffffffu, inc, 31);
+    }
+    if (lane == 0) s_wpre[p.BG] = run;
+}
+
+// the group work item `item` belongs to (s_wpre ascending)
+__device__ __forceinline__ int dense_item_group(const int *s_wpre, int BG, int item) {
+    int a = 0, b = BG;
+    while (b - a > 1) {
+        const int mid = (a + b) >> 1;
+        if (s_wpre[mid] <= item) a = mid; else b = mid;
+    }
+    while (s_wpre[a + 1] <= item) ++a;
+    return a;
+}
+
 // smem: ring [warps][32][528] (reused as merge scratch once a warp's rows are done) | bars [warps] u64 | s_cnt [warps]
 //       | s_prefix [BG+1] | s_wpre [BG+1]
 __global__ void __launch_bounds__(384) attend_dense_kernel(const DenseParams p) {
@@ -88,43 +140,7 @@ __global__ void __launch_bounds__(384) attend_dense_kernel(const DenseParams p) 
     pdl_wait();
 
     const int nw = gridDim.x * warps;
-    if (warp == 0) {
-        int run = 0;
-        for (int g0 = 0; g0 < p.BG; g0 += 32) {
-            const int bg = g0 + lane;
-            const int t = (bg < p.BG) ? min(max(p.len[bg / p.Hkv], 0), p.M) : 0;
-            int inc = t;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                int v = __shfl_up_sync(0xffffffffu, inc, o);
-                if (lane >= o) inc += v;
-            }
-            if (bg < p.BG) s_prefix[bg] = run + inc - t;
-            run += __shfl_sync(0xffffffffu, inc, 31);
-        }
-        const int total = run;
-        if (lane == 0) s_prefix[p.BG] = total;
-        const int Rp = (nw > p.BG) ? max(TILE, (total + (nw - p.BG) - 1) / (nw - p.BG)) : 0x3fffffff;
-        __syncwarp();
-        run = 0;
-        for (int g0 = 0; g0 < p.BG; g0 += 32) {
-            const int bg = g0 + lane;
-            int w = 0;
-            if (bg < p.BG) {
-                const int t = s_prefix[bg + 1] - s_prefix[bg];
-                w = (t > 0) ? max(1, t / Rp) : 0;
-            }
-            int inc = w;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                int v = __shfl_up_sync(0xffffffffu, inc, o);
-                if (lane >= o) inc += v;
-            }
-            if (bg < p.BG) s_wpre[bg] = run + inc - w;
-            run += __shfl_sync(0xffffffffu, inc, 31);
-        }
-        if (lane == 0) s_wpre[p.BG] = run;
-    }
+    if (warp == 0) dense_partition(p, s_prefix, s_wpre, nw, lane);
     __syncthreads();
     pdl_launch_dependents();
 
@@ -150,16 +166,7 @@ __global__ void __launch_bounds__(384) attend_dense_kernel(const DenseParams p) 
     uint32_t phase = 0;
 
     for (int item = u; item < n_items; item += nw) {
-        int bg;
-        {
-            int a = 0, b = p.BG;
-            while (b - a > 1) {
-                const int mid = (a + b) >> 1;
-                if (s_wpre[mid] <= item) a = mid; else b = mid;
-            }
-            bg = a;
-            while (s_wpre[bg + 1] <= item) ++bg;
-        }
+        const int bg = dense_item_group(s_wpre, p.BG, item);
         const int T = s_prefix[bg + 1] - s_prefix[bg];
         const int w_g = s_wpre[bg + 1] - s_wpre[bg];
         const int part = item - s_wpre[bg];
@@ -340,8 +347,361 @@ __global__ void __launch_bounds__(384) attend_dense_kernel(const DenseParams p) 
     }
 }
 
+// ---- verification step of T tokens ------------------------------------------------------------------------------------------
+// The same per-(request, kv-head) organisation for the T*G <= 32 query rows of a group: row r = t*G + j is q-head j of the group
+// for token t, the rows sit on the M axis of NMT m16 tiles, and every K|V record is fetched ONCE for all of them (dense KV bytes per
+// step do not grow with T).  Token t sees rows [0, len - (T-1-t)) (causal over the T rows the step appended).
+//   PACK (T*G <= 8): one m-tile whose rows 8..15 are free carry the lo halves of the bf16 hi/lo split of P, as above;
+//   otherwise the lo halves are a second pass of MMAs over each m-tile into the same accumulators.
+// States of the T*G rows fill a warp's whole ring (32 x 132 floats at T*G = 32): the CTA-level merge reads the other warps' rings in
+// place.  That is safe because a warp whose group is split (w_g > 1) never takes a second item (see the partition: then the items
+// number at most the warps).
+template <int NMT, bool PACK>
+__global__ void __launch_bounds__(256) attend_dense_tokens_kernel(const DenseParams p, int T) {
+    extern __shared__ __align__(128) uint8_t smem[];
+    const int warps = blockDim.x >> 5, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    uint8_t *slots = smem + (size_t)warp * TILE * DSLOT;
+    uint8_t *sp = smem + (size_t)warps * TILE * DSLOT;
+    uint64_t *bar = reinterpret_cast<uint64_t *>(sp) + warp;
+    sp += (size_t)warps * sizeof(uint64_t);
+    int *s_cnt = reinterpret_cast<int *>(sp);
+    sp += (size_t)warps * sizeof(int);
+    int *s_prefix = reinterpret_cast<int *>(sp);
+    int *s_wpre = s_prefix + p.BG + 1;
+    float *s_own = reinterpret_cast<float *>(slots);
+    auto s_part_of = [&](int w) { return reinterpret_cast<float *>(smem + (size_t)w * TILE * DSLOT); };
+    const int G = p.G, TG = T * G;
+
+    if (lane == 0) {
+        mbar_init(bar, 1);
+        fence_proxy_async();
+    }
+    if (threadIdx.x < warps) s_cnt[threadIdx.x] = 0;
+    pdl_wait();
+
+    const int nw = gridDim.x * warps;
+    if (warp == 0) dense_partition(p, s_prefix, s_wpre, nw, lane);   // the partition of attend_dense_kernel
+    __syncthreads();
+    pdl_launch_dependents();
+
+    const int u = blockIdx.x * warps + warp;
+    const int n_items = s_wpre[p.BG];
+    const int cta_w0 = blockIdx.x * warps;
+    // output row of query row r of group bg: (B, T, Hq) order
+    auto out_row = [&](int bg, int r) { return ((bg / p.Hkv) * T + r / G) * p.Hq + (bg % p.Hkv) * G + r % G; };
+
+    for (int bg = u; bg < p.BG; bg += nw) {
+        if (s_prefix[bg + 1] == s_prefix[bg]) {
+            const float z4[4] = {0.f, 0.f, 0.f, 0.f};
+            for (int r = 0; r < TG; ++r) finalize_dense_head(p, out_row(bg, r), 0.f, z4, lane);
+        }
+    }
+
+    const float scale_log2 = rsqrtf((float)D) * LOG2E_F;
+    const int grp = lane >> 2, tig = lane & 3;
+    const uint32_t slots_s = smem_u32(slots);
+    const uint32_t k_lane_off = (uint32_t)(((lane & 7) + (lane >> 4) * 8) * DSLOT + ((lane >> 3) & 1) * 16);
+    const uint32_t v_lane_off = (uint32_t)(((lane & 7) + ((lane >> 3) & 1) * 8) * DSLOT + D * 2 + (lane >> 4) * 16);
+    constexpr int NI = PACK ? 1 : 2;   // query rows a lane holds per m-tile: grp (and grp + 8)
+    constexpr bool QREG = (NMT == 1);  // one m-tile: the q fragments stay in registers; two: re-read per tile (L1)
+    uint32_t phase = 0;
+
+    for (int item = u; item < n_items; item += nw) {
+        const int bg = dense_item_group(s_wpre, p.BG, item);
+        const int len = s_prefix[bg + 1] - s_prefix[bg];
+        const int w_g = s_wpre[bg + 1] - s_wpre[bg];
+        const int part = item - s_wpre[bg];
+        const int c_g = (len + w_g - 1) / w_g;
+        const int r_lo = part * c_g, r_hi = min(r_lo + c_g, len);
+        const uint8_t *rows = p.kv + (size_t)bg * p.M * REC;
+
+        // this lane's query rows: r = mt*16 + i*8 + grp; rows past T*G are zero and unmasked
+        const uint32_t *qrow[NMT][2];
+        int lim[NMT][2];
+#pragma unroll
+        for (int mt = 0; mt < NMT; ++mt)
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                const int r = mt * 16 + i * 8 + grp;
+                const bool ok = r < TG && !(PACK && i == 1);
+                qrow[mt][i] = ok ? reinterpret_cast<const uint32_t *>(p.q + (size_t)out_row(bg, r) * D) : nullptr;
+                lim[mt][i] = ok ? len - (T - 1 - r / G) : len;
+            }
+        auto q_frag = [&](int mt, int ks, uint32_t (&a)[4]) {
+            a[0] = qrow[mt][0] ? __ldg(qrow[mt][0] + ks * 8 + tig) : 0u;
+            a[1] = qrow[mt][1] ? __ldg(qrow[mt][1] + ks * 8 + tig) : 0u;
+            a[2] = qrow[mt][0] ? __ldg(qrow[mt][0] + ks * 8 + 4 + tig) : 0u;
+            a[3] = qrow[mt][1] ? __ldg(qrow[mt][1] + ks * 8 + 4 + tig) : 0u;
+        };
+        uint32_t qa[QREG ? 8 : 1][4];
+        if (QREG) {
+#pragma unroll
+            for (int ks = 0; ks < 8; ++ks) q_frag(0, ks, qa[QREG ? ks : 0]);
+        }
+        __syncwarp();
+        fence_proxy_async();
+        float m_run[NMT][2], l_run[NMT][2];
+        float acc[NMT][16][4];
+#pragma unroll
+        for (int mt = 0; mt < NMT; ++mt) {
+            m_run[mt][0] = m_run[mt][1] = -CUDART_INF_F;
+            l_run[mt][0] = l_run[mt][1] = 0.f;
+#pragma unroll
+            for (int i = 0; i < 16; ++i) acc[mt][i][0] = acc[mt][i][1] = acc[mt][i][2] = acc[mt][i][3] = 0.f;
+        }
+
+        for (int cr = r_lo; cr < r_hi; cr += TILE) {
+            const int nrows = min(TILE, r_hi - cr);
+            if (lane == 0) mbar_arrive_expect_tx(bar, (uint32_t)nrows * REC);
+            __syncwarp();
+            if (lane < nrows) {
+                bulk_g2s(slots + (size_t)lane * DSLOT, rows + (size_t)(cr + lane) * REC, REC, bar);
+            } else {
+                uint4 *vz = reinterpret_cast<uint4 *>(slots + (size_t)lane * DSLOT);
+#pragma unroll
+                for (int i = 0; i < 32; ++i) vz[i] = make_uint4(0, 0, 0, 0);
+            }
+            __syncwarp();
+            mbar_wait(bar, phase);
+            phase ^= 1;
+
+            // ---- S^T = Q . K_tile^T per m-tile ----------------------------------------------------------------------
+            float s[NMT][4][4];
+#pragma unroll
+            for (int mt = 0; mt < NMT; ++mt)
+#pragma unroll
+                for (int nt = 0; nt < 4; ++nt) s[mt][nt][0] = s[mt][nt][1] = s[mt][nt][2] = s[mt][nt][3] = 0.f;
+#pragma unroll
+            for (int ks = 0; ks < 8; ++ks) {
+                uint32_t a[NMT][4];
+#pragma unroll
+                for (int mt = 0; mt < NMT; ++mt) {
+                    if (QREG) {
+                        a[mt][0] = qa[QREG ? ks : 0][0]; a[mt][1] = qa[QREG ? ks : 0][1];
+                        a[mt][2] = qa[QREG ? ks : 0][2]; a[mt][3] = qa[QREG ? ks : 0][3];
+                    } else {
+                        q_frag(mt, ks, a[mt]);
+                    }
+                }
+#pragma unroll
+                for (int j = 0; j < 2; ++j) {
+                    uint32_t b[4];
+                    ldsm4(b, slots_s + (uint32_t)(j * 16 * DSLOT + ks * 32) + k_lane_off);
+#pragma unroll
+                    for (int mt = 0; mt < NMT; ++mt) {
+                        mma16816(s[mt][2 * j], a[mt], b[0], b[1]);
+                        mma16816(s[mt][2 * j + 1], a[mt], b[2], b[3]);
+                    }
+                }
+            }
+            // ---- online softmax per query row (lane holds keys nt*8 + tig*2 + {0,1} of rows grp and grp+8) --------
+            float corr[NMT][2];
+#pragma unroll
+            for (int mt = 0; mt < NMT; ++mt)
+#pragma unroll
+                for (int i = 0; i < NI; ++i) {
+                    float mloc = -CUDART_INF_F;
+#pragma unroll
+                    for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const int r = nt * 8 + tig * 2 + e;
+                            float &x = s[mt][nt][2 * i + e];
+                            x = (r < nrows && cr + r < lim[mt][i]) ? x * scale_log2 : -CUDART_INF_F;
+                            mloc = fmaxf(mloc, x);
+                        }
+                    mloc = fmaxf(mloc, __shfl_xor_sync(0xffffffffu, mloc, 1));
+                    mloc = fmaxf(mloc, __shfl_xor_sync(0xffffffffu, mloc, 2));
+                    const float m_new = fmaxf(m_run[mt][i], mloc);
+                    const float m_use = (m_new == -CUDART_INF_F) ? 0.f : m_new;   // a row with no visible key yet: all p = 0
+                    corr[mt][i] = (m_run[mt][i] == -CUDART_INF_F) ? 0.f : exp2f(m_run[mt][i] - m_new);
+                    float lsum = 0.f;
+#pragma unroll
+                    for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            float &x = s[mt][nt][2 * i + e];
+                            x = exp2f(x - m_use);
+                            lsum += x;
+                        }
+                    lsum += __shfl_xor_sync(0xffffffffu, lsum, 1);
+                    lsum += __shfl_xor_sync(0xffffffffu, lsum, 2);
+                    l_run[mt][i] = l_run[mt][i] * corr[mt][i] + lsum;
+                    m_run[mt][i] = m_new;
+                }
+            if (cr > r_lo) {
+#pragma unroll
+                for (int mt = 0; mt < NMT; ++mt)
+#pragma unroll
+                    for (int i = 0; i < 16; ++i) {
+                        acc[mt][i][0] *= corr[mt][0]; acc[mt][i][1] *= corr[mt][0];
+                        acc[mt][i][2] *= corr[mt][NI - 1]; acc[mt][i][3] *= corr[mt][NI - 1];
+                    }
+            }
+            // ---- O += P . V (P as bf16 hi + lo) --------------------------------------------------------------------
+            // (one m-tile at a time: its fragments only are live; the V fragments are re-read from shared memory per m-tile)
+#pragma unroll
+            for (int ks = 0; ks < 2; ++ks)
+#pragma unroll
+                for (int mt = 0; mt < NMT; ++mt) {
+                    uint32_t ahi[4], alo[4];
+#pragma unroll
+                    for (int half = 0; half < 2; ++half)
+#pragma unroll
+                        for (int i = 0; i < 2; ++i) {
+                            // PACK: a[2*half] = hi of row grp, a[2*half+1] = lo of row grp (in row grp + 8)
+                            const int src = PACK ? 0 : i;
+                            const float p0 = s[mt][2 * ks + half][2 * src], p1 = s[mt][2 * ks + half][2 * src + 1];
+                            const uint32_t h0 = f32_to_bf16_rne(p0), h1 = f32_to_bf16_rne(p1);
+                            const uint32_t l0 = f32_to_bf16_rne(p0 - bf16_bits_to_f32(h0)), l1 = f32_to_bf16_rne(p1 - bf16_bits_to_f32(h1));
+                            if (PACK) {
+                                if (i == 0) ahi[2 * half] = h0 | (h1 << 16);
+                                else ahi[2 * half + 1] = l0 | (l1 << 16);
+                            } else {
+                                ahi[2 * half + i] = h0 | (h1 << 16);
+                                alo[2 * half + i] = l0 | (l1 << 16);
+                            }
+                        }
+#pragma unroll
+                    for (int n2 = 0; n2 < 8; ++n2) {
+                        uint32_t b[4];
+                        ldsm4t(b, slots_s + (uint32_t)(ks * 16 * DSLOT + n2 * 32) + v_lane_off);
+                        mma16816(acc[mt][2 * n2], ahi, b[0], b[1]);
+                        mma16816(acc[mt][2 * n2 + 1], ahi, b[2], b[3]);
+                        if (!PACK) {
+                            mma16816(acc[mt][2 * n2], alo, b[0], b[1]);
+                            mma16816(acc[mt][2 * n2 + 1], alo, b[2], b[3]);
+                        }
+                    }
+                }
+            __syncwarp();
+            fence_proxy_async();
+        }
+
+        // ---- part done: states of the T*G rows -> [T*G][132] floats in the warp's idle ring -------------------------
+        __syncwarp();
+#pragma unroll
+        for (int mt = 0; mt < NMT; ++mt)
+#pragma unroll
+            for (int i = 0; i < NI; ++i) {
+                const int r = mt * 16 + i * 8 + grp;
+                if (r < TG) {
+                    float *st = s_own + (size_t)r * PART_FLOATS;
+                    if (tig == 0) {
+                        st[0] = m_run[mt][i] * 0.6931471805599453f;
+                        st[1] = l_run[mt][i];
+                    }
+#pragma unroll
+                    for (int nt = 0; nt < 16; ++nt) {
+                        const float2 v = PACK ? make_float2(acc[mt][nt][0] + acc[mt][nt][2], acc[mt][nt][1] + acc[mt][nt][3])
+                                              : make_float2(acc[mt][nt][2 * i], acc[mt][nt][2 * i + 1]);
+                        *reinterpret_cast<float2 *>(st + 4 + nt * 8 + tig * 2) = v;
+                    }
+                }
+            }
+        __syncwarp();
+
+        const int i0 = s_wpre[bg], i1 = i0 + w_g - 1;
+        const int wa = max(i0, cta_w0), wb = min(i1, cta_w0 + warps - 1);
+        bool carry = true;
+        if (w_g > 1 && wb > wa) {
+            // level 1: the states stay in each warp's ring; the last arriver of this CTA combines them
+            int ticket = 0;
+            if (lane == 0) ticket = atom_add_acq_rel_cta_shared_d(&s_cnt[wa - cta_w0], 1);
+            ticket = __shfl_sync(0xffffffffu, ticket, 0);
+            carry = (ticket == wb - wa);
+        }
+        if (!carry) continue;
+        const int cta_first = i0 / warps, cta_last = i1 / warps;
+        const bool need_l1 = (w_g > 1 && wb > wa);
+        const bool need_l2 = (w_g > 1 && cta_first != cta_last);
+        int ticket2 = 0;
+        float *gslot = p.partials + ((size_t)blockIdx.x * 2 + ((i0 >= cta_w0) ? 1 : 0)) * (size_t)TG * PART_FLOATS;
+        for (int r = 0; r < TG; ++r) {
+            float M_, L_, A[4];
+            if (need_l1) {
+                merge_states<false>([&](int i) { return (const float *)(s_part_of(wa - cta_w0 + i) + (size_t)r * PART_FLOATS); },
+                                    wb - wa + 1, lane, M_, L_, A);
+            } else {
+                const float *st = s_own + (size_t)r * PART_FLOATS;
+                M_ = st[0];
+                L_ = st[1];
+                const float4 o4 = *reinterpret_cast<const float4 *>(st + 4 + 4 * lane);
+                A[0] = o4.x; A[1] = o4.y; A[2] = o4.z; A[3] = o4.w;
+            }
+            if (!need_l2) finalize_dense_head(p, out_row(bg, r), L_, A, lane);
+            else store_state(gslot + (size_t)r * PART_FLOATS, M_, L_, A, lane);
+        }
+        if (!need_l2) continue;
+        __syncwarp();
+        if (lane == 0) ticket2 = atom_add_acq_rel_gpu_d(p.counters + bg, 1);
+        ticket2 = __shfl_sync(0xffffffffu, ticket2, 0);
+        if (ticket2 == cta_last - cta_first) {
+            for (int r = 0; r < TG; ++r) {
+                float M_, L_, A[4];
+                merge_states<true>(
+                    [&](int i) {
+                        const int c2 = cta_first + i;
+                        return (const float *)(p.partials + ((size_t)c2 * 2 + ((i0 >= c2 * warps) ? 1 : 0)) * (size_t)TG * PART_FLOATS +
+                                               (size_t)r * PART_FLOATS);
+                    },
+                    cta_last - cta_first + 1, lane, M_, L_, A);
+                finalize_dense_head(p, out_row(bg, r), L_, A, lane);
+            }
+            if (lane == 0) p.counters[bg] = 0;
+        }
+    }
+}
+
+int launch_attend_dense_tokens(mpig_ctx *ctx, const uint8_t *kv, const int32_t *len, int T, const void *q, void *out, cudaStream_t s,
+                               bool pdl) {
+    const int TG = T * ctx->G;
+    MPIG_REQUIRE(TG >= 1 && TG <= 32, MPIG_EUNSUPPORTED, "dense attention: T*G = %d query rows per group (at most 32)", TG);
+    DenseParams p = {};
+    p.kv = kv;
+    p.len = len;
+    p.q = (const __nv_bfloat16 *)q;
+    p.out = (__nv_bfloat16 *)out;
+    p.out_f32 = ctx->want_out_f32 ? ctx->out_f32 : nullptr;
+    p.partials = ctx->partials;
+    p.counters = ctx->counters;
+    p.BG = ctx->BG;
+    p.G = ctx->G;
+    p.Hkv = ctx->cfg.num_key_value_heads;
+    p.Hq = ctx->cfg.num_attention_heads;
+    p.M = ctx->cfg.max_length;
+    const int warps = 8;
+    const size_t smem = (size_t)warps * TILE * DSLOT + (size_t)warps * 8 + (size_t)warps * 4 + 2 * (size_t)(p.BG + 1) * sizeof(int) + 16;
+    MPIG_REQUIRE(smem <= 227 * 1024, MPIG_EINVAL, "dense attention: %zu B shared memory", smem);
+    MPIG_REQUIRE((size_t)ctx->num_sms * 2 * TG <= (size_t)ctx->max_partial_warps * 2, MPIG_EINVAL, "dense attention: partial scratch too small");
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(ctx->num_sms);
+    cfg.blockDim = dim3(warps * 32);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = s;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = pdl ? 1 : 0;
+    if (TG <= 8) {
+        MPIG_FUNC_ATTR((attend_dense_tokens_kernel<1, true>), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+        MPIG_CUDA(cudaLaunchKernelEx(&cfg, attend_dense_tokens_kernel<1, true>, p, T));
+    } else if (TG <= 16) {
+        MPIG_FUNC_ATTR((attend_dense_tokens_kernel<1, false>), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+        MPIG_CUDA(cudaLaunchKernelEx(&cfg, attend_dense_tokens_kernel<1, false>, p, T));
+    } else {
+        MPIG_FUNC_ATTR((attend_dense_tokens_kernel<2, false>), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+        MPIG_CUDA(cudaLaunchKernelEx(&cfg, attend_dense_tokens_kernel<2, false>, p, T));
+    }
+    MPIG_LAUNCH_CHECK(ctx);
+    ctx->last_tokens = T;
+    return MPIG_OK;
+}
+
 int launch_attend_dense(mpig_ctx *ctx, const uint8_t *kv, const int32_t *len, const void *q, void *out, cudaStream_t s, bool pdl) {
     MPIG_REQUIRE(ctx->G >= 1 && ctx->G <= GMAX, MPIG_EUNSUPPORTED, "dense attention: group size %d > %d", ctx->G, GMAX);
+    ctx->last_tokens = 1;
     DenseParams p = {};
     p.kv = kv;
     p.len = len;

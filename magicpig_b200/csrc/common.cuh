@@ -135,8 +135,8 @@ struct mpig_ctx {
     int fused_debug = 0;                     // record per-CTA phase clocks of the fused kernel into fused_dbg
     unsigned long long *fused_dbg = nullptr; // [max CTAs][16]
     int fused_issue_win = 8;                 // warps of a fused-kernel CTA that issue row requests at the same time (fused.cu, P5); 0 = all
-    void *fused_plan_cache = nullptr;        // fused.cu: the launch plan (geometry, shared-memory carve-up), computed once
-    long long fused_plan_key = 0;            //   ... and the option values it was computed for
+    void *fused_plan_cache = nullptr;        // fused.cu: the launch plans (geometry, shared-memory carve-up) for T = 1..8 tokens
+    long long fused_plan_key[9] = {0};       //   ... and the option values each was computed for
     int last_decode_fused = 0;               // which variant the last mpig_decode ran (mpig_get_info)
     // fp32 copy of the attention output before the ABI's bf16 rounding (option "out_f32"; parity tests apply the 1e-3 bar here)
     int want_out_f32 = 0;
@@ -151,6 +151,14 @@ struct mpig_ctx {
     // mpig_spill_window scratch, allocated by the first spill: per-request counts | spilled keys (Hkv, g, d) bf16 per request |
     // their codes (Hkv, L, g) int16 per request, sized for every request spilling all its non-sink window rows
     uint8_t *spill_buf = nullptr;
+    // multi-token verification steps (mpig_reserve_query_tokens / mpig_plan_tokens / mpig_decode_tokens / mpig_rewind).  After the
+    // reservation the per-step scratch above (codes, qnorm, results, nnz, bitmaps, mve, out_f32) holds B*tok_max*Hq rows.
+    int tok_max = 1;                         // largest T a step may verify (1 until mpig_reserve_query_tokens)
+    int pending_T = 0;                       // T of the last plan (0 = no plan yet); decode_tokens must match it
+    bool rewound = true;                     // the last plan has been rewound already (at most one rewind per plan)
+    int last_tokens = 1;                     // rows of the readers (mpig_last_probe / _codes / _out_f32) = B * last_tokens * Hq
+    bool plan_captured = false;              // a plan has been captured into a CUDA graph (the scratch addresses are baked in)
+    int last_tokens_waves = 0;               // cluster waves of the last mpig_decode_tokens launch
 };
 
 namespace mpig {
@@ -304,9 +312,18 @@ struct AttendParams {
     int skip;                 // measurement aid (option "attend_skip"): 1 = no row fetch, 2 = no tile math, 4 = no merges
 };
 
+// rows = query rows to hash (0 = B*Hq)
 int launch_simhash(mpig_ctx *ctx, const void *query_bf16, int32_t *codes, float *qnorm, const AppendParams *ap,
-                   cudaStream_t s, bool pdl);
+                   cudaStream_t s, bool pdl, int rows = 0);
 int launch_append(mpig_ctx *ctx, const AppendParams &ap, cudaStream_t s);
+// the T new rows of every (request, kv-head): k/v (B, T, Hkv, d) -> rows len[b] - T + t (centred when ap.avg_k != null)
+int launch_append_tokens(mpig_ctx *ctx, const AppendParams &ap, int T, cudaStream_t s);
+// T-token sparse decode (fused.cu): append of the T window rows, then the T-token fused kernel; q (B, T, Hq, d), k / v
+// (B, T, Hkv, d), out (B, T, Hq*d).  Refuses (nothing launched) when the fused decode does not apply.
+int launch_fused_tokens(mpig_ctx *ctx, int layer, int T, const void *q, const void *k, const void *v, void *out, cudaStream_t s);
+// T-token dense decode (attend_dense.cu): q (B, T, Hq, d), rows already appended, causal over the last T rows
+int launch_attend_dense_tokens(mpig_ctx *ctx, const uint8_t *kv, const int32_t *len, int T, const void *q, void *out, cudaStream_t s,
+                               bool pdl);
 int launch_probe(mpig_ctx *ctx, int layer, const int32_t *query, int32_t *results, int32_t *nnz, cudaStream_t s, bool pdl);
 int launch_attend_mma(mpig_ctx *ctx, const AttendParams &p, cudaStream_t s, bool pdl);
 int launch_attend_dense(mpig_ctx *ctx, const uint8_t *kv, const int32_t *len, const void *q, void *out, cudaStream_t s, bool pdl);

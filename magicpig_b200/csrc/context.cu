@@ -266,14 +266,18 @@ int mpig_clear(mpig_ctx *ctx, void *stream) {
     }
     MPIG_CUDA(cudaMemsetAsync(ctx->win_len, 0, ctx->cfg.batch_size * sizeof(int32_t), s));
     MPIG_CUDA(cudaMemsetAsync(ctx->dense_len, 0, ctx->cfg.batch_size * sizeof(int32_t), s));
-    MPIG_CUDA(cudaMemsetAsync(ctx->nnz, 0, ctx->H * sizeof(int32_t), s));
+    const size_t rows = (size_t)ctx->H * ctx->tok_max;   // the per-step scratch holds B*t_max*Hq rows after a reservation
+    MPIG_CUDA(cudaMemsetAsync(ctx->nnz, 0, rows * sizeof(int32_t), s));
     MPIG_CUDA(cudaMemsetAsync(ctx->counters, 0, ctx->H * sizeof(int32_t), s));
     // lsh.cc:305 zeroes the mask: get_mask after clear must not return the previous probe's counters
-    MPIG_CUDA(cudaMemsetAsync(ctx->bitmaps, 0, (size_t)ctx->H * 2 * ctx->bitmap_words * sizeof(uint32_t), s));
+    MPIG_CUDA(cudaMemsetAsync(ctx->bitmaps, 0, rows * 2 * ctx->bitmap_words * sizeof(uint32_t), s));
     MPIG_CUDA(cudaMemsetAsync(ctx->err_flag, 0, 4 * sizeof(int32_t), s));
     for (auto &n : ctx->h_win_len) n = 0;
     for (auto &n : ctx->h_dense_len) n = 0;
     ctx->h_len_exact = true;
+    ctx->last_tokens = 1;
+    ctx->pending_T = 0;     // no plan to decode or rewind since the clear
+    ctx->rewound = true;
     return MPIG_OK;
 }
 
@@ -315,8 +319,9 @@ int mpig_set_option(mpig_ctx *ctx, const char *key, int64_t value) {
     else if (k == "out_f32") {
         ctx->want_out_f32 = (int)value;
         if (value && !ctx->out_f32) {
-            MPIG_CUDA(cudaMalloc(&ctx->out_f32, (size_t)ctx->H * ctx->cfg.head_dim * sizeof(float)));
-            MPIG_CUDA(cudaMemset(ctx->out_f32, 0, (size_t)ctx->H * ctx->cfg.head_dim * sizeof(float)));
+            const size_t bytes = (size_t)ctx->H * ctx->tok_max * ctx->cfg.head_dim * sizeof(float);
+            MPIG_CUDA(cudaMalloc(&ctx->out_f32, bytes));
+            MPIG_CUDA(cudaMemset(ctx->out_f32, 0, bytes));
         }
     }
     else if (k == "attend_tma") ctx->attend.tma = (int)value;
@@ -351,8 +356,46 @@ int mpig_last_codes(mpig_ctx *ctx, int32_t *codes_out, void *stream) {
     MPIG_REQUIRE(ctx && codes_out, MPIG_EINVAL, "mpig_last_codes: null argument");
     MPIG_REQUIRE(!ctx->last_decode_fused || ctx->save_mask, MPIG_ESTATE,
                  "mpig_last_codes: the fused decode keeps the query codes in shared memory; set option save_mask before the decode");
-    MPIG_CUDA(cudaMemcpyAsync(codes_out, ctx->codes, (size_t)ctx->H * ctx->cfg.L * sizeof(int32_t), cudaMemcpyDeviceToDevice,
-                              as_stream(stream)));
+    MPIG_CUDA(cudaMemcpyAsync(codes_out, ctx->codes, (size_t)ctx->H * ctx->last_tokens * ctx->cfg.L * sizeof(int32_t),
+                              cudaMemcpyDeviceToDevice, as_stream(stream)));
+    return MPIG_OK;
+}
+
+int mpig_reserve_query_tokens(mpig_ctx *ctx, int t_max) {
+    mpig::DeviceGuard _dg(ctx);
+    MPIG_REQUIRE(ctx, MPIG_EINVAL, "mpig_reserve_query_tokens: null context");
+    MPIG_REQUIRE(t_max >= 1 && t_max <= 8, MPIG_EINVAL, "mpig_reserve_query_tokens: t_max=%d outside [1, 8]", t_max);
+    if (t_max <= ctx->tok_max) return MPIG_OK;
+    // the scratch moves to new addresses: a step captured before would replay on freed memory
+    MPIG_REQUIRE(!ctx->plan_captured, MPIG_ESTATE,
+                 "mpig_reserve_query_tokens: a step has been captured into a CUDA graph; reserve before capturing");
+    // the per-step scratch grows from B*Hq to B*t_max*Hq rows; the first B*Hq rows keep their meaning for single-token calls.
+    // Everything is allocated first, so a failed allocation leaves the context as it was.
+    const size_t H = (size_t)ctx->H * t_max, L = ctx->cfg.L, M = ctx->cfg.max_length, d = ctx->cfg.head_dim;
+    const size_t sz[7] = {H * L * sizeof(int32_t), H * sizeof(float), H * M * sizeof(int32_t), H * sizeof(int32_t),
+                          H * 2 * (size_t)ctx->bitmap_words * sizeof(uint32_t), 2 * H * sizeof(float), H * d * sizeof(float)};
+    const int n = ctx->out_f32 ? 7 : 6;
+    void *nb[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+    MPIG_CUDA(cudaDeviceSynchronize());   // scratch of a decode still in flight is about to be freed
+    for (int i = 0; i < n; ++i) {
+        cudaError_t e = cudaMalloc(&nb[i], sz[i]);
+        if (e == cudaSuccess) e = cudaMemset(nb[i], 0, sz[i]);
+        if (e != cudaSuccess) {
+            for (int j = 0; j <= i; ++j) cudaFree(nb[j]);
+            (void)cudaGetLastError();
+            set_error("mpig_reserve_query_tokens: cudaMalloc(%zu bytes) failed: %s", sz[i], cudaGetErrorString(e));
+            return MPIG_ENOMEM;
+        }
+    }
+    void **old[7] = {(void **)&ctx->codes, (void **)&ctx->qnorm, (void **)&ctx->results, (void **)&ctx->nnz, (void **)&ctx->bitmaps,
+                     (void **)&ctx->mve, (void **)&ctx->out_f32};
+    const size_t old_rows = (size_t)ctx->H * ctx->tok_max;
+    for (int i = 0; i < n; ++i) {
+        cudaFree(*old[i]);
+        *old[i] = nb[i];
+        if (i < 6) ctx->bytes += sz[i] - sz[i] / H * old_rows;   // (out_f32, an option's buffer, is not counted)
+    }
+    ctx->tok_max = t_max;
     return MPIG_OK;
 }
 
@@ -378,8 +421,8 @@ int mpig_last_out_f32(mpig_ctx *ctx, float *out_f32, void *stream) {
     mpig::DeviceGuard _dg(ctx);
     MPIG_REQUIRE(ctx && out_f32, MPIG_EINVAL, "mpig_last_out_f32: null argument");
     MPIG_REQUIRE(ctx->want_out_f32 && ctx->out_f32, MPIG_ESTATE, "mpig_last_out_f32: enable mpig_set_option(ctx, \"out_f32\", 1) before the decode");
-    MPIG_CUDA(cudaMemcpyAsync(out_f32, ctx->out_f32, (size_t)ctx->H * ctx->cfg.head_dim * sizeof(float), cudaMemcpyDeviceToDevice,
-                              as_stream(stream)));
+    MPIG_CUDA(cudaMemcpyAsync(out_f32, ctx->out_f32, (size_t)ctx->H * ctx->last_tokens * ctx->cfg.head_dim * sizeof(float),
+                              cudaMemcpyDeviceToDevice, as_stream(stream)));
     return MPIG_OK;
 }
 
@@ -391,6 +434,8 @@ int mpig_get_info(mpig_ctx *ctx, const char *key, int64_t *value) {
     else if (k == "fused_cluster_waves") *value = fused_cluster_waves(ctx);
     else if (k == "window_capacity") *value = ctx->Wcap;
     else if (k == "table_segments") *value = ctx->nseg;
+    else if (k == "query_tokens_max") *value = ctx->tok_max;
+    else if (k == "tokens_cluster_waves") *value = ctx->last_tokens_waves;
     else {
         set_error("mpig_get_info: unknown key '%s'", key);
         return MPIG_EINVAL;
@@ -401,9 +446,10 @@ int mpig_get_info(mpig_ctx *ctx, const char *key, int64_t *value) {
 int mpig_last_probe(mpig_ctx *ctx, int32_t *nnz_out, int32_t *results_out, void *stream) {
     mpig::DeviceGuard _dg(ctx);  // run on the context's device whatever the caller's current device is
     MPIG_REQUIRE(ctx && nnz_out, MPIG_EINVAL, "mpig_last_probe: null argument");
-    MPIG_CUDA(cudaMemcpyAsync(nnz_out, ctx->nnz, (size_t)ctx->H * sizeof(int32_t), cudaMemcpyDeviceToDevice, as_stream(stream)));
+    const size_t rows = (size_t)ctx->H * ctx->last_tokens;
+    MPIG_CUDA(cudaMemcpyAsync(nnz_out, ctx->nnz, rows * sizeof(int32_t), cudaMemcpyDeviceToDevice, as_stream(stream)));
     if (results_out)
-        MPIG_CUDA(cudaMemcpyAsync(results_out, ctx->results, (size_t)ctx->H * ctx->cfg.max_length * sizeof(int32_t),
+        MPIG_CUDA(cudaMemcpyAsync(results_out, ctx->results, rows * ctx->cfg.max_length * sizeof(int32_t),
                                   cudaMemcpyDeviceToDevice, as_stream(stream)));
     return MPIG_OK;
 }

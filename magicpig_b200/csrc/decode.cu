@@ -15,6 +15,7 @@ static int decode_sparse(mpig_ctx *ctx, int layer, const void *q, const void *k,
                          cudaEvent_t *ev = nullptr) {
     if (!ev && fused_applicable(ctx)) return launch_fused(ctx, layer, q, k, v, out, s, true);
     ctx->last_decode_fused = 0;
+    ctx->last_tokens = 1;
     const LayerStore &ls = ctx->layers[layer];
     AppendParams ap = {};
     ap.k_new = (const __nv_bfloat16 *)k;
@@ -221,7 +222,54 @@ int mpig_dense_decode(mpig_ctx *ctx, int layer, const void *query_bf16, const vo
     p.K = ctx->cfg.K;
     p.L = ctx->cfg.L;
     p.out_f32 = ctx->want_out_f32 ? ctx->out_f32 : nullptr;
+    ctx->last_tokens = 1;
     return launch_attend_mma(ctx, p, s, false);
+}
+
+// shared checks of the two T-token entry points
+static int tokens_checks(mpig_ctx *ctx, int layer, int T, const void *q, const void *k, const void *v, const void *out, bool sparse,
+                         const char *who) {
+    int rc = check_layer(ctx, layer, sparse, who);
+    if (rc) return rc;
+    MPIG_REQUIRE(q && k && v && out, MPIG_EINVAL, "%s: null argument", who);
+    MPIG_REQUIRE(T >= 1 && T <= ctx->tok_max, MPIG_EINVAL, "%s: T=%d outside [1, %d] (mpig_reserve_query_tokens sets the upper bound)",
+                 who, T, ctx->tok_max);
+    MPIG_REQUIRE(T == ctx->pending_T, MPIG_ESTATE, "%s: T=%d but the last plan was for %d token(s)", who, T, ctx->pending_T);
+    return MPIG_OK;
+}
+
+int mpig_decode_tokens(mpig_ctx *ctx, int layer, int T, const void *query_bf16, const void *key_bf16, const void *value_bf16,
+                       void *out_bf16, void *stream) {
+    mpig::DeviceGuard _dg(ctx);
+    int rc = tokens_checks(ctx, layer, T, query_bf16, key_bf16, value_bf16, out_bf16, true, "mpig_decode_tokens");
+    if (rc) return rc;
+    if (T == 1) return mpig_decode(ctx, layer, query_bf16, key_bf16, value_bf16, out_bf16, stream);
+    return launch_fused_tokens(ctx, layer, T, query_bf16, key_bf16, value_bf16, out_bf16, as_stream(stream));
+}
+
+int mpig_dense_decode_tokens(mpig_ctx *ctx, int layer, int T, const void *query_bf16, const void *key_bf16, const void *value_bf16,
+                             void *out_bf16, void *stream) {
+    mpig::DeviceGuard _dg(ctx);
+    int rc = tokens_checks(ctx, layer, T, query_bf16, key_bf16, value_bf16, out_bf16, false, "mpig_dense_decode_tokens");
+    if (rc) return rc;
+    const LayerStore &ls = ctx->layers[layer];
+    MPIG_REQUIRE(ls.dense && ls.dense_kv, MPIG_ESTATE, "mpig_dense_decode_tokens: layer %d has no dense KV", layer);
+    if (T == 1) return mpig_dense_decode(ctx, layer, query_bf16, key_bf16, value_bf16, out_bf16, stream);
+    MPIG_REQUIRE(ctx->dense_impl == 1, MPIG_EUNSUPPORTED, "mpig_dense_decode_tokens: T=%d needs the GQA-shared dense kernel (dense_impl = 1)", T);
+    MPIG_REQUIRE(T * ctx->G <= 32, MPIG_EUNSUPPORTED, "mpig_dense_decode_tokens: T*G = %d query rows per kv-group (at most 32)", T * ctx->G);
+    cudaStream_t s = as_stream(stream);
+    AppendParams ap = {};
+    ap.k_new = (const __nv_bfloat16 *)key_bf16;
+    ap.v_new = (const __nv_bfloat16 *)value_bf16;
+    ap.avg_k = nullptr;
+    ap.rows = ls.dense_kv;
+    ap.len = ctx->dense_len;
+    ap.BG = ctx->BG;
+    ap.Hkv = ctx->cfg.num_key_value_heads;
+    ap.cap = ctx->cfg.max_length;
+    rc = launch_append_tokens(ctx, ap, T, s);
+    if (rc) return rc;
+    return launch_attend_dense_tokens(ctx, ls.dense_kv, ctx->dense_len, T, query_bf16, out_bf16, s, true);
 }
 
 }  // extern "C"

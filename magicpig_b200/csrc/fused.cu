@@ -121,6 +121,7 @@ struct FusedParams {
     int peer_rank, peer_world;
     int H, G, Hq, M, Wcap, K, L, NB, S, r, Mc, words, ncw, selcap, C, seg_len;
     FusedSmem lay;                 // shared-memory carve-up, computed once on the host
+    int ntok;                      // TOK instantiation: query tokens T per request (H = B*T*Hq virtual heads)
 };
 
 __device__ __forceinline__ unsigned long long clk64() {
@@ -155,7 +156,11 @@ __device__ __forceinline__ int block_exclusive_scan_redux(int v, int *wtot, int 
 // k-permutation shared with the q operand, like the hash phase) and only the V half is staged in shared memory by the TMA
 // engine: 256 B instead of 528 B of shared memory per row in flight, so ALL of a CTA's rows (~400 at C2) are in flight at once
 // instead of ~300 in two rounds.  KREG = false: whole 512-byte records through TMA + ldmatrix (the stand-alone kernel's way).
-template <typename TagT, int THREADS, bool DBG, bool KREG>
+// TOK = true: a verification step of T = gp.ntok tokens per request.  Cluster v serves VIRTUAL head v = (b*T + t)*Hq + h: q, out
+// and every per-head output are indexed by v (the (B, T, Hq, d) layout), the tables / records / window of group b*Hkv + h/G are
+// read, and the window ends T-1-t rows before win_len[b] (causal).  The T new rows were appended by append_tokens_kernel, so
+// k_new is null: no in-kernel row build.
+template <typename TagT, int THREADS, bool DBG, bool KREG, bool TOK = false>
 __global__ void __launch_bounds__(THREADS, (THREADS == 1024) ? 1 : 2) fused_decode_kernel(const __grid_constant__ FusedParams gp) {
     extern __shared__ __align__(128) uint8_t smem_raw[];
     __shared__ FusedParams p_s;   // parameters staged once (constant-bank misses were microseconds on the critical path)
@@ -170,8 +175,15 @@ __global__ void __launch_bounds__(THREADS, (THREADS == 1024) ? 1 : 2) fused_deco
         const unsigned C_ = cluster_nctarank(), c_ = cluster_ctarank();
         const int h_ = blockIdx.x / C_;
         s_geo[0] = h_;
-        s_geo[1] = h_ / gp.G;
-        s_geo[2] = h_ / gp.Hq;
+        if (TOK) {
+            const int hq = h_ % gp.Hq, bt = h_ / gp.Hq, b = bt / gp.ntok;
+            s_geo[1] = b * (gp.Hq / gp.G) + hq / gp.G;
+            s_geo[2] = b;
+            s_geo[5] = gp.ntok - 1 - (bt - b * gp.ntok);   // rows of later tokens at the end of the window
+        } else {
+            s_geo[1] = h_ / gp.G;
+            s_geo[2] = h_ / gp.Hq;
+        }
         s_geo[3] = (int)c_ / gp.r;
         s_geo[4] = ((int)c_ % gp.r) * gp.Mc;
     }
@@ -265,7 +277,7 @@ __global__ void __launch_bounds__(THREADS, (THREADS == 1024) ? 1 : 2) fused_deco
         reinterpret_cast<uint2 *>(s_nq32)[lane] = o;
         if (lane == 0) s_misc[0] = nrm32;
     } else if (warp == 1) {
-        const int wl = p.win ? min(max(__ldg(p.win_len + bq), 0), p.Wcap) : 0;
+        const int wl = p.win ? min(max(__ldg(p.win_len + bq) - (TOK ? s_geo[5] : 0), 0), p.Wcap) : 0;
         if (lane == 0) s_misc[1] = __int_as_float(wl);
         if (c == 0 && (h % p.G) == 0 && wl > 0 && p.k_new) {
             // centred key (bf16 arithmetic as torch: fp32 subtract, RNE) | value -> window row wl-1 (attnserver.py:275-290)
@@ -956,9 +968,9 @@ struct FusedPlan {
 
 // Clusters of this plan's variant that the device keeps resident at once.  A cluster occupies SMs of ONE GPC, and the
 // H100's GPCs have unequal SM counts, so #SMs / C over-counts; the runtime knows the real number.
-template <int THREADS, bool KREG>
+template <int THREADS, bool KREG, bool TOK = false>
 static int fused_max_active_clusters(const FusedPlan &fp) {
-    const void *fn = (const void *)fused_decode_kernel<uint8_t, THREADS, false, KREG>;
+    const void *fn = (const void *)fused_decode_kernel<uint8_t, THREADS, false, KREG, TOK>;
     if (func_attr_once(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, THREADS == 1024 ? 227 * 1024 - 1024 : 228 * 1024 / 2 - 2048) != MPIG_OK)
         return 0;
     cudaLaunchConfig_t cfg = {};
@@ -973,24 +985,27 @@ static int fused_max_active_clusters(const FusedPlan &fp) {
     cfg.attrs = &attr;
     cfg.numAttrs = 1;
     int n = 0;
-    if (cudaOccupancyMaxActiveClusters(&n, fused_decode_kernel<uint8_t, THREADS, false, KREG>, &cfg) != cudaSuccess) {
+    if (cudaOccupancyMaxActiveClusters(&n, fused_decode_kernel<uint8_t, THREADS, false, KREG, TOK>, &cfg) != cudaSuccess) {
         cudaGetLastError();
         return 0;
     }
     return n;
 }
 
-static FusedPlan fused_plan_compute(const mpig_ctx *ctx) {
+// T > 1: the plan of the T-token instantiation for B*T*Hq virtual heads.  The segment geometry (and with it the cluster size C)
+// was fixed at creation for B*Hq heads, so here B*T*Hq clusters may need several waves; they are independent of each other.
+static FusedPlan fused_plan_compute(const mpig_ctx *ctx, int T = 1) {
     FusedPlan fp = {};
     fp.gm = probe_geometry(ctx);
     const int L = ctx->cfg.L, K = ctx->cfg.K;
+    const int HT = ctx->H * T;
     if (L > 4 * 253) return fp;                              // one-byte tags: at most four passes of 253 tables
     if ((long long)L * ctx->cfg.max_length >= (1ll << 31)) return fp;   // chunk records hold 32-bit item offsets
     if (fp.gm.Sp > 8) return fp;
     // one wave of 1024-thread CTAs (one per SM), or 512-thread CTAs, two per SM: one wave up to 2 x #SMs CTAs, several waves
     // beyond that (large batches: one CTA per head, the CTAs are independent of each other)
-    if (ctx->H * fp.gm.C > 2 * ctx->num_sms && fp.gm.C > 1) return fp;
-    fp.threads = (ctx->H * fp.gm.C > ctx->num_sms) ? 512 : 1024;
+    if (T == 1 && ctx->H * fp.gm.C > 2 * ctx->num_sms && fp.gm.C > 1) return fp;
+    fp.threads = (HT * fp.gm.C > ctx->num_sms) ? 512 : 1024;
     // per CTA: dynamic + static (parameter block) + 1 KB the system reserves, out of 228 KB per SM
     const size_t cap = (fp.threads == 1024) ? (227 * 1024 - 1024) : (size_t)(228 * 1024 / 2 - 2048);
     const int stride = ctx->fused_kreg ? VSLOT : SLOT;
@@ -1006,30 +1021,36 @@ static FusedPlan fused_plan_compute(const mpig_ctx *ctx) {
     // the cluster splits the tables; with one CTA per head (large batches) every CTA would stream all of hash_func from L2:
     // those shapes hash in the separate tensor-core kernel (simhash.cu) and hand the codes over
     fp.hash_in_kernel = fp.gm.C >= 2;
-    const int act = fp.threads == 1024 ? (ctx->fused_kreg ? fused_max_active_clusters<1024, true>(fp) : fused_max_active_clusters<1024, false>(fp))
-                                       : (ctx->fused_kreg ? fused_max_active_clusters<512, true>(fp) : fused_max_active_clusters<512, false>(fp));
-    fp.cluster_waves = act > 0 ? (ctx->H + act - 1) / act : 0;
+    int act;
+    if (T == 1)
+        act = fp.threads == 1024 ? (ctx->fused_kreg ? fused_max_active_clusters<1024, true>(fp) : fused_max_active_clusters<1024, false>(fp))
+                                 : (ctx->fused_kreg ? fused_max_active_clusters<512, true>(fp) : fused_max_active_clusters<512, false>(fp));
+    else
+        act = fp.threads == 1024 ? (ctx->fused_kreg ? fused_max_active_clusters<1024, true, true>(fp) : fused_max_active_clusters<1024, false, true>(fp))
+                                 : (ctx->fused_kreg ? fused_max_active_clusters<512, true, true>(fp) : fused_max_active_clusters<512, false, true>(fp));
+    fp.cluster_waves = act > 0 ? (HT + act - 1) / act : 0;
     fp.ok = true;
     return fp;
 }
 
-// The plan depends on the (immutable) configuration and two options: computed once, kept in the context.
-static const FusedPlan &fused_plan(const mpig_ctx *ctx) {
+// The plan depends on the (immutable) configuration, two options and the step size T: computed once per T (1..8), kept in the
+// context.
+static const FusedPlan &fused_plan(const mpig_ctx *ctx, int T = 1) {
     mpig_ctx *c = const_cast<mpig_ctx *>(ctx);
     const long long key = ((long long)ctx->fused_selcap << 8) | (ctx->fused_kreg ? 3 : 2);
     if (!c->fused_plan_cache) {
-        c->fused_plan_cache = calloc(1, sizeof(FusedPlan));
-        c->fused_plan_key = 0;
+        c->fused_plan_cache = calloc(9, sizeof(FusedPlan));
+        for (auto &k : c->fused_plan_key) k = 0;
     }
     if (!c->fused_plan_cache) {   // out of host memory: compute every time
         static thread_local FusedPlan tmp;
-        tmp = fused_plan_compute(ctx);
+        tmp = fused_plan_compute(ctx, T);
         return tmp;
     }
-    FusedPlan *fp = static_cast<FusedPlan *>(c->fused_plan_cache);
-    if (c->fused_plan_key != key) {
-        *fp = fused_plan_compute(ctx);
-        c->fused_plan_key = key;
+    FusedPlan *fp = static_cast<FusedPlan *>(c->fused_plan_cache) + T;
+    if (c->fused_plan_key[T] != key) {
+        *fp = fused_plan_compute(ctx, T);
+        c->fused_plan_key[T] = key;
     }
     return *fp;
 }
@@ -1143,6 +1164,104 @@ int launch_fused(mpig_ctx *ctx, int layer, const void *q, const void *k, const v
     if (rc) return rc;
     MPIG_LAUNCH_CHECK(ctx);
     ctx->last_decode_fused = 1;
+    ctx->last_tokens = 1;
+    return MPIG_OK;
+}
+
+template <int THREADS, bool KREG>
+static int launch_tokens_variant(const cudaLaunchConfig_t &cfg, const FusedParams &p) {
+    MPIG_FUNC_ATTR((fused_decode_kernel<uint8_t, THREADS, false, KREG, true>), cudaFuncAttributeMaxDynamicSharedMemorySize,
+                   THREADS == 1024 ? 227 * 1024 - 1024 : 228 * 1024 / 2 - 2048);
+    MPIG_CUDA(cudaLaunchKernelEx(&cfg, fused_decode_kernel<uint8_t, THREADS, false, KREG, true>, p));
+    return MPIG_OK;
+}
+
+int launch_fused_tokens(mpig_ctx *ctx, int layer, int T, const void *q, const void *k, const void *v, void *out, cudaStream_t s) {
+    MPIG_REQUIRE(ctx->decode_impl == 1, MPIG_EUNSUPPORTED, "mpig_decode_tokens: T=%d needs the fused decode (decode_impl = 1)", T);
+    const FusedPlan &fp = fused_plan(ctx, T);
+    MPIG_REQUIRE(fp.ok, MPIG_EUNSUPPORTED, "mpig_decode_tokens: shape not supported by the fused decode (L=%d, H=%d, T=%d, segments=%d)",
+                 ctx->cfg.L, ctx->H, T, ctx->nseg);
+    MPIG_REQUIRE(ctx->hash_func_set, MPIG_ESTATE, "SimHash before mpig_set_hash_func: the projection has not been set");
+    const LayerStore &ls = ctx->layers[layer];
+    const int HT = ctx->H * T;
+    ctx->last_probe_layer = layer;
+    int rc = MPIG_OK;
+    if (ctx->Wcap > 0) {   // the T new rows (centred keys) go to the window first: the attention reads them from HBM
+        AppendParams ap = {};
+        ap.k_new = (const __nv_bfloat16 *)k;
+        ap.v_new = (const __nv_bfloat16 *)v;
+        ap.avg_k = ls.avg_k;
+        ap.rows = ls.win;
+        ap.len = ctx->win_len;
+        ap.BG = ctx->BG;
+        ap.Hkv = ctx->cfg.num_key_value_heads;
+        ap.cap = ctx->Wcap;
+        rc = launch_append_tokens(ctx, ap, T, s);
+        if (rc) return rc;
+    }
+    if (!fp.hash_in_kernel) {
+        // one CTA per virtual head: the B*T*Hq query rows are hashed by the stand-alone tensor-core kernel
+        rc = launch_simhash(ctx, q, ctx->codes, ctx->qnorm, nullptr, s, true, HT);
+        if (rc) return rc;
+    }
+    FusedParams p = {};
+    p.q = (const __nv_bfloat16 *)q;
+    p.avg_k = ls.avg_k;
+    p.hf_t = ctx->hash_func_t;
+    p.codes_in = fp.hash_in_kernel ? nullptr : ctx->codes;
+    p.offsets = ls.offsets;
+    p.items = reinterpret_cast<const uint16_t *>(ls.items);
+    p.kv = ls.kv;
+    p.kn = ls.kn;
+    p.win = ctx->Wcap > 0 ? ls.win : nullptr;
+    p.win_len = ctx->win_len;
+    p.out = (__nv_bfloat16 *)out;
+    p.out_f32 = ctx->want_out_f32 ? ctx->out_f32 : nullptr;
+    p.mve = ctx->mve;
+    p.nnz_out = ctx->nnz;
+    p.results_out = ctx->save_mask ? ctx->results : nullptr;
+    p.bitmaps_out = ctx->save_mask ? ctx->bitmaps : nullptr;
+    p.codes_out = (ctx->save_mask && fp.hash_in_kernel) ? ctx->codes : nullptr;
+    p.issue_win = ctx->fused_issue_win;
+    p.H = HT;
+    p.G = ctx->G;
+    p.Hq = ctx->cfg.num_attention_heads;
+    p.M = ctx->cfg.max_length;
+    p.Wcap = ctx->Wcap;
+    p.K = ctx->cfg.K;
+    p.L = ctx->cfg.L;
+    p.NB = ctx->NB;
+    p.S = ctx->nseg;
+    p.r = fp.gm.r;
+    p.Mc = fp.gm.Mc;
+    p.words = ctx->bitmap_words;
+    p.ncw = fp.ncw;
+    p.selcap = ctx->fused_selcap;
+    p.C = fp.gm.C;
+    p.seg_len = ctx->seg_len;
+    p.lay = fp.lay;
+    p.ntok = T;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(HT * fp.gm.C);
+    cfg.blockDim = dim3(fp.threads);
+    cfg.dynamicSmemBytes = fp.smem;
+    cfg.stream = s;
+    cudaLaunchAttribute attr[2];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = fp.gm.C;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[1].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 2;   // under PDL behind the append (or the SimHash kernel)
+    if (fp.threads == 1024) rc = ctx->fused_kreg ? launch_tokens_variant<1024, true>(cfg, p) : launch_tokens_variant<1024, false>(cfg, p);
+    else rc = ctx->fused_kreg ? launch_tokens_variant<512, true>(cfg, p) : launch_tokens_variant<512, false>(cfg, p);
+    if (rc) return rc;
+    MPIG_LAUNCH_CHECK(ctx);
+    ctx->last_decode_fused = 1;
+    ctx->last_tokens = T;
+    ctx->last_tokens_waves = fp.cluster_waves;
     return MPIG_OK;
 }
 

@@ -164,14 +164,55 @@ __global__ void __launch_bounds__(SH_THREADS) simhash_kernel(const __nv_bfloat16
 
 __global__ void append_kernel(AppendParams ap) { append_rows(ap); }
 
-// Lengths saturate at the capacity (the append then overwrites the last row); saturation of a store that is in use raises the
-// context's device error flag (bit 0: sparse window = generation_buffer exhausted, bit 1: dense cache = max_length exhausted),
-// readable with mpig_error_flags -- the host-side check in mpig_plan cannot see replays of a captured graph.
-__global__ void plan_kernel(int32_t *win_len, int32_t *dense_len, int32_t *err_flag, int B, int wcap, int dcap, int has_window,
-                            int has_dense) {
+// T new rows per (request, kv-head) of a verification step: one warp per (b, t, kv-head), the same bf16 arithmetic as
+// append_rows.  k_new / v_new are (B, T, Hkv, D); row t of request b goes to position len[b] - T + t (len already advanced by
+// mpig_plan_tokens).  The attention launch that reads the rows follows under programmatic dependent launch.
+__global__ void append_tokens_kernel(AppendParams a, int T) {
+    pdl_launch_dependents();
+    const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (warp >= a.BG * T) return;
+    const int kh = warp % a.Hkv, bt = warp / a.Hkv, b = bt / T, t = bt % T;
+    const int bg = b * a.Hkv + kh;
+    const int pos = a.len[b] - T + t;
+    if (pos < 0 || pos >= a.cap) return;
+    uint8_t *rec = a.rows + ((size_t)bg * a.cap + pos) * (4 * SH_D);
+    const size_t src = (size_t)warp * SH_D + 4 * lane;   // warp = (b*T + t)*Hkv + kh: the row of the (B, T, Hkv, D) input
+    const uint2 kk = *reinterpret_cast<const uint2 *>(a.k_new + src);
+    uint2 ko = kk;
+    if (a.avg_k) {
+        const uint2 av = *reinterpret_cast<const uint2 *>(a.avg_k + (size_t)bg * SH_D + 4 * lane);
+        ko.x = (uint32_t)f32_to_bf16_rne(bf16lo(kk.x) - bf16lo(av.x)) | ((uint32_t)f32_to_bf16_rne(bf16hi(kk.x) - bf16hi(av.x)) << 16);
+        ko.y = (uint32_t)f32_to_bf16_rne(bf16lo(kk.y) - bf16lo(av.y)) | ((uint32_t)f32_to_bf16_rne(bf16hi(kk.y) - bf16hi(av.y)) << 16);
+    }
+    *reinterpret_cast<uint2 *>(rec + 8 * lane) = ko;
+    *reinterpret_cast<uint2 *>(rec + 2 * SH_D + 8 * lane) = *reinterpret_cast<const uint2 *>(a.v_new + src);
+}
+
+// mpig_rewind: both lengths of request b shrink by drop[b] in [0, T]; any other drop leaves the request untouched and raises bit 2
+// of the context's error flags.  apply = 0: only the flag (an eager call that refuses changes no length).
+__global__ void rewind_kernel(const int32_t *drop, int32_t *win_len, int32_t *dense_len, int32_t *err_flag, int B, int T, int apply) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b < B) {
-        int w = win_len[b] + 1, dl = dense_len[b] + 1;
+        const int d = drop[b];
+        if (d < 0 || d > T) {
+            atomicOr(err_flag, 4);
+            return;
+        }
+        if (!apply) return;
+        win_len[b] = max(win_len[b] - d, 0);
+        dense_len[b] = max(dense_len[b] - d, 0);
+    }
+}
+
+// Lengths advance by T (1 for mpig_plan) and saturate at the capacity (the append then overwrites the last row); saturation of a
+// store that is in use raises the context's device error flag (bit 0: sparse window = generation_buffer exhausted, bit 1: dense
+// cache = max_length exhausted), readable with mpig_error_flags -- the host-side check in mpig_plan cannot see replays of a
+// captured graph.
+__global__ void plan_kernel(int32_t *win_len, int32_t *dense_len, int32_t *err_flag, int B, int T, int wcap, int dcap,
+                            int has_window, int has_dense) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b < B) {
+        int w = win_len[b] + T, dl = dense_len[b] + T;
         if (w > wcap) {
             w = wcap;
             if (has_window) atomicOr(err_flag, 1);
@@ -202,9 +243,10 @@ __global__ void window_fill_kernel(const uint4 *__restrict__ k, const uint4 *__r
 }
 
 int launch_simhash(mpig_ctx *ctx, const void *query_bf16, int32_t *codes, float *qnorm, const AppendParams *ap,
-                   cudaStream_t s, bool pdl) {
+                   cudaStream_t s, bool pdl, int rows) {
     MPIG_REQUIRE(ctx->hash_func_set, MPIG_ESTATE, "SimHash before mpig_set_hash_func: the projection has not been set");
     const int K = ctx->cfg.K, L = ctx->cfg.L;
+    const int H = rows > 0 ? rows : ctx->H;
     const int n_hash = (L + SH_TABLES - 1) / SH_TABLES;
     AppendParams a = {};
     if (ap) a = *ap;
@@ -213,7 +255,7 @@ int launch_simhash(mpig_ctx *ctx, const void *query_bf16, int32_t *codes, float 
                         (size_t)SH_MBLOCK * SH_TABLES * K + 16;
     MPIG_FUNC_ATTR(simhash_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid, (ctx->H + SH_MBLOCK - 1) / SH_MBLOCK);
+    cfg.gridDim = dim3(grid, (H + SH_MBLOCK - 1) / SH_MBLOCK);
     cfg.blockDim = dim3(SH_THREADS);
     cfg.dynamicSmemBytes = smem;
     cfg.stream = s;
@@ -223,7 +265,7 @@ int launch_simhash(mpig_ctx *ctx, const void *query_bf16, int32_t *codes, float 
     cfg.attrs = attr;
     cfg.numAttrs = pdl ? 1 : 0;
     MPIG_CUDA(cudaLaunchKernelEx(&cfg, simhash_kernel, (const __nv_bfloat16 *)query_bf16,
-                                 (const __nv_bfloat16 *)ctx->hash_func_t, codes, qnorm, ctx->H, K, L, n_hash, a));
+                                 (const __nv_bfloat16 *)ctx->hash_func_t, codes, qnorm, H, K, L, n_hash, a));
     MPIG_LAUNCH_CHECK(ctx);
     return MPIG_OK;
 }
@@ -231,6 +273,25 @@ int launch_simhash(mpig_ctx *ctx, const void *query_bf16, int32_t *codes, float 
 int launch_append(mpig_ctx *ctx, const AppendParams &ap, cudaStream_t s) {
     append_kernel<<<1, 256, 0, s>>>(ap);
     MPIG_LAUNCH_CHECK(ctx);
+    return MPIG_OK;
+}
+
+int launch_append_tokens(mpig_ctx *ctx, const AppendParams &ap, int T, cudaStream_t s) {
+    const int warps = ap.BG * T;
+    append_tokens_kernel<<<(warps + 7) / 8, 256, 0, s>>>(ap, T);
+    MPIG_LAUNCH_CHECK(ctx);
+    return MPIG_OK;
+}
+
+// the host-mirror checks of mpig_plan for a step of T tokens (nothing is modified when one fails)
+static int plan_checks(mpig_ctx *ctx, int T, bool has_window, bool has_dense, const char *who) {
+    for (int b = 0; b < ctx->cfg.batch_size; ++b) {
+        MPIG_REQUIRE(!has_window || ctx->h_win_len[b] + T <= ctx->Wcap, MPIG_ESTATE,
+                     "%s: request %d: the sparse window is full (%d rows = sink + local + generation_buffer); "
+                     "raise generation_buffer or clear()", who, b, ctx->Wcap);
+        MPIG_REQUIRE(!has_dense || ctx->h_dense_len[b] == 0 || ctx->h_dense_len[b] + T <= ctx->cfg.max_length, MPIG_ESTATE,
+                     "%s: request %d: the dense KV cache is full (max_length = %d)", who, b, ctx->cfg.max_length);
+    }
     return MPIG_OK;
 }
 
@@ -246,35 +307,88 @@ int mpig_simhash(mpig_ctx *ctx, const void *query_bf16, int32_t *codes, float *q
     return launch_simhash(ctx, query_bf16, codes, query_norm, nullptr, as_stream(stream), false);
 }
 
-int mpig_plan(mpig_ctx *ctx, void *stream) {
-    mpig::DeviceGuard _dg(ctx);  // run on the context's device whatever the caller's current device is
-    MPIG_REQUIRE(ctx, MPIG_EINVAL, "mpig_plan: null context");
+// mpig_plan / mpig_plan_tokens: the host-mirror checks (exact until a plan is captured into a CUDA graph: replays advance only
+// the device side), then every length advances by T on the device
+static int plan_step(mpig_ctx *ctx, int T, cudaStream_t s, const char *who) {
     const int B = ctx->cfg.batch_size;
     int has_window = 0, has_dense = 0;
     for (const auto &ls : ctx->layers) {
         has_window |= (ls.sparse && ctx->Wcap > 0);
         has_dense |= (ls.dense && ls.dense_kv != nullptr);
     }
-    // host mirror of the lengths: exact until a plan() is captured into a CUDA graph (replays advance only the device side)
     cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-    MPIG_CUDA(cudaStreamIsCapturing(as_stream(stream), &cap));
-    if (cap != cudaStreamCaptureStatusNone) ctx->h_len_exact = false;
+    MPIG_CUDA(cudaStreamIsCapturing(s, &cap));
+    if (cap != cudaStreamCaptureStatusNone) {
+        ctx->h_len_exact = false;
+        ctx->plan_captured = true;
+    }
     if (ctx->h_len_exact) {
+        const int rc = plan_checks(ctx, T, has_window, has_dense, who);
+        if (rc) return rc;
         for (int b = 0; b < B; ++b) {
-            MPIG_REQUIRE(!has_window || ctx->h_win_len[b] + 1 <= ctx->Wcap, MPIG_ESTATE,
-                         "mpig_plan: request %d: the sparse window is full (%d rows = sink + local + generation_buffer); "
-                         "raise generation_buffer or clear()", b, ctx->Wcap);
-            MPIG_REQUIRE(!has_dense || ctx->h_dense_len[b] == 0 || ctx->h_dense_len[b] + 1 <= ctx->cfg.max_length, MPIG_ESTATE,
-                         "mpig_plan: request %d: the dense KV cache is full (max_length = %d)", b, ctx->cfg.max_length);
-        }
-        for (int b = 0; b < B; ++b) {
-            ctx->h_win_len[b] = std::min(ctx->h_win_len[b] + 1, ctx->Wcap);
-            ctx->h_dense_len[b] = std::min(ctx->h_dense_len[b] + 1, ctx->cfg.max_length);
+            ctx->h_win_len[b] = std::min(ctx->h_win_len[b] + T, ctx->Wcap);
+            ctx->h_dense_len[b] = std::min(ctx->h_dense_len[b] + T, ctx->cfg.max_length);
         }
     }
-    plan_kernel<<<(B + 127) / 128, 128, 0, as_stream(stream)>>>(ctx->win_len, ctx->dense_len, ctx->err_flag, B, ctx->Wcap,
-                                                                ctx->cfg.max_length, has_window, has_dense);
+    plan_kernel<<<(B + 127) / 128, 128, 0, s>>>(ctx->win_len, ctx->dense_len, ctx->err_flag, B, T, ctx->Wcap, ctx->cfg.max_length,
+                                               has_window, has_dense);
     MPIG_LAUNCH_CHECK(ctx);
+    ctx->pending_T = T;
+    ctx->rewound = false;
+    return MPIG_OK;
+}
+
+int mpig_plan(mpig_ctx *ctx, void *stream) {
+    mpig::DeviceGuard _dg(ctx);  // run on the context's device whatever the caller's current device is
+    MPIG_REQUIRE(ctx, MPIG_EINVAL, "mpig_plan: null context");
+    return plan_step(ctx, 1, as_stream(stream), "mpig_plan");
+}
+
+int mpig_plan_tokens(mpig_ctx *ctx, int T, void *stream) {
+    mpig::DeviceGuard _dg(ctx);
+    MPIG_REQUIRE(ctx, MPIG_EINVAL, "mpig_plan_tokens: null context");
+    MPIG_REQUIRE(T >= 1 && T <= ctx->tok_max, MPIG_EINVAL,
+                 "mpig_plan_tokens: T=%d outside [1, %d] (mpig_reserve_query_tokens sets the upper bound)", T, ctx->tok_max);
+    return plan_step(ctx, T, as_stream(stream), "mpig_plan_tokens");
+}
+
+int mpig_rewind(mpig_ctx *ctx, const int32_t *drop, void *stream) {
+    mpig::DeviceGuard _dg(ctx);
+    MPIG_REQUIRE(ctx && drop, MPIG_EINVAL, "mpig_rewind: null argument");
+    MPIG_REQUIRE(ctx->pending_T > 0 && !ctx->rewound, MPIG_ESTATE, "mpig_rewind: at most one rewind per plan (no plan since the last rewind)");
+    const int B = ctx->cfg.batch_size;
+    cudaStream_t s = as_stream(stream);
+    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+    MPIG_CUDA(cudaStreamIsCapturing(s, &cap));
+    const bool eager = (cap == cudaStreamCaptureStatusNone);
+    const int T = ctx->pending_T;
+    if (!eager) {
+        rewind_kernel<<<(B + 127) / 128, 128, 0, s>>>(drop, ctx->win_len, ctx->dense_len, ctx->err_flag, B, T, 1);
+        MPIG_LAUNCH_CHECK(ctx);
+        ctx->rewound = true;
+        ctx->h_len_exact = false;
+        return MPIG_OK;
+    }
+    // eager: the drops are checked first, so a refused call changes no length (only error flag bit 2 is raised) and may be
+    // repeated with valid drops
+    std::vector<int32_t> dh(B);
+    MPIG_CUDA(cudaMemcpyAsync(dh.data(), drop, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    MPIG_CUDA(cudaStreamSynchronize(s));
+    bool bad = false;
+    for (int b = 0; b < B; ++b) bad |= (dh[b] < 0 || dh[b] > T);
+    rewind_kernel<<<(B + 127) / 128, 128, 0, s>>>(drop, ctx->win_len, ctx->dense_len, ctx->err_flag, B, T, bad ? 0 : 1);
+    MPIG_LAUNCH_CHECK(ctx);
+    MPIG_REQUIRE(!bad, MPIG_EINVAL, "mpig_rewind: a drop outside [0, %d]; nothing was changed (error flag bit 2)", T);
+    ctx->rewound = true;
+    // the device lengths are the truth: the host mirror follows them, so the eager checks of mpig_plan stay exact
+    std::vector<int32_t> wl(B), dl(B);
+    MPIG_CUDA(cudaMemcpyAsync(wl.data(), ctx->win_len, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    MPIG_CUDA(cudaMemcpyAsync(dl.data(), ctx->dense_len, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    MPIG_CUDA(cudaStreamSynchronize(s));
+    for (int b = 0; b < B; ++b) {
+        ctx->h_win_len[b] = wl[b];
+        ctx->h_dense_len[b] = dl[b];
+    }
     return MPIG_OK;
 }
 

@@ -171,6 +171,7 @@ int mpig_attention_wrapper(mpig_ctx *ctx, int layer, int K, int L, void *output_
     p.qnorm = query_norm;
     p.out = (__nv_bfloat16 *)output_bf16;
     p.out_f32 = ctx->want_out_f32 ? ctx->out_f32 : nullptr;
+    ctx->last_tokens = 1;
     p.mve = max_value_expsum;
     p.partials = ctx->partials;
     p.counters = ctx->counters;

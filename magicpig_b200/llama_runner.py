@@ -57,13 +57,14 @@ class LlamaDecodeRunner:
     def __init__(self, shape: LlamaShape, K: int, L: int, batch_size: int, max_length: int, device: str = "cuda:0",
                  seed: int = 0, generation_buffer: int = 256, dense_layers=(0, 16, 32, 48, 64), num_layers: int | None = None,
                  tp_rank: int = 0, tp_world: int = 1, tp_group=None, fused: bool = True, tp_mode: str = "ag",
-                 tp_transport: str = "nccl"):
+                 tp_transport: str = "nccl", max_query_tokens: int = 1):
         """tp_mode (only with tp_world > 1; see magicpig_b200/tp.py):
              "ag"        attention sharded by KV head, one all-gather of head outputs per layer, wo / MLP replicated (north-star)
              "megatron"  + wo row-split, gate/up column-split, down row-split, two all-reduces per layer (llama_dist.py:49-70)
            tp_transport: "nccl" (torch.distributed collectives, captured in the CUDA graph) or "peer" (stores into the peers'
            buffers over NVLink: from the attention epilogue for "ag", one-shot all-reduce kernels for "megatron";
-           magicpig_b200/peer.py)."""
+           magicpig_b200/peer.py).
+           max_query_tokens: largest T of step_tokens(T) (verification steps of speculative decoding; 1 = step() only)."""
         assert tp_mode in ("ag", "megatron") and tp_transport in ("nccl", "peer")
         self.tp_mode, self.tp_transport = tp_mode, tp_transport
         self.shape = shape
@@ -100,7 +101,7 @@ class LlamaDecodeRunner:
         self.server = LSHSparseAttnServer(cfg, K=K, L=L, batch_size=batch_size, max_length=max_length,
                                           generation_buffer=generation_buffer, dense_layers=dense_layers, device=device,
                                           hash_func=hash_func, num_key_value_heads=self.Hkv_loc,
-                                          num_attention_heads=self.Hq_loc)
+                                          num_attention_heads=self.Hq_loc, max_query_tokens=max_query_tokens)
 
         def w(*shape_):
             return (torch.randn(shape_, generator=g, device=self.device, dtype=torch.float32) * 0.02).to(torch.bfloat16)
@@ -140,6 +141,11 @@ class LlamaDecodeRunner:
         self.ids = torch.zeros((batch_size, 1), dtype=torch.long, device=self.device)
         self.pos = torch.zeros((batch_size,), dtype=torch.long, device=self.device)
         self.logits = torch.zeros((batch_size, shape.vocab_size), dtype=torch.float32, device=self.device)
+        # step_tokens: the T candidate tokens of each request and the logits after each of them
+        self.max_query_tokens = max_query_tokens
+        if max_query_tokens > 1:
+            self.ids_tok = torch.zeros((batch_size, max_query_tokens), dtype=torch.long, device=self.device)
+            self.logits_tok = torch.zeros((batch_size, max_query_tokens, shape.vocab_size), dtype=torch.float32, device=self.device)
         self._gather_buf = None
         self.peer = None
         if tp_world > 1:
@@ -315,6 +321,45 @@ class LlamaDecodeRunner:
         x = F.rms_norm(h[:, -1], (sh.hidden_size,), self.norm, sh.rms_norm_eps)
         self.logits.copy_(F.linear(x, self.lm_head).float())
         return self.logits
+
+    def step_tokens(self, T: int, drop: torch.Tensor | None = None):
+        """A verification step of T tokens for the whole batch (speculative decoding): reads the candidates self.ids_tok[:, :T],
+        writes self.logits_tok[:, :T] (B, T, vocab), the logits after each candidate, and advances self.pos by T.  Eager-path math
+        (library GEMMs over the B*T rows) with per-token RoPE positions pos+1 .. pos+T; the attention server checks the T
+        tokens in one pass per layer (plan(T), decode of (B, H, T, d)).  With `drop` (device int32 (B,): rejected tokens per
+        request) the step ends with server.rewind(drop) and self.pos falls back by drop.  Graph-capturable; step() is separate."""
+        assert self.tp_world == 1, "verification steps are built for a single GPU"
+        assert 1 <= T <= self.max_query_tokens, f"T={T} outside [1, max_query_tokens={self.max_query_tokens}]"
+        sh, srv = self.shape, self.server
+        B, d, Hq, Hkv, hs, it = self.B, self.d, self.Hq_loc, self.Hkv_loc, sh.hidden_size, self.it_loc
+        srv.plan(T)
+        pos = self.pos[:, None] + torch.arange(1, T + 1, device=self.device)   # (B, T)
+        self.pos.add_(T)
+        h = F.embedding(self.ids_tok[:, :T], self.embed)   # (B, T, hs)
+        for li, lw in enumerate(self.layers):
+            x = F.rms_norm(h, (hs,), lw["ln1"], sh.rms_norm_eps)
+            qkv = F.linear(x, lw["wqkv"])   # (B, T, (Hq+2Hkv)d)
+            q = self._rope_at(qkv[..., : Hq * d].reshape(B, T, Hq, d).transpose(1, 2), pos)
+            k = self._rope_at(qkv[..., Hq * d:(Hq + Hkv) * d].reshape(B, T, Hkv, d).transpose(1, 2), pos)
+            v = qkv[..., (Hq + Hkv) * d:].reshape(B, T, Hkv, d).transpose(1, 2)
+            a = srv.decode(q, k, v, li)   # (B, T, Hq*d), token t attending causally   <- the hot path
+            h = h + F.linear(a, lw["wo"])
+            x = F.rms_norm(h, (hs,), lw["ln2"], sh.rms_norm_eps)
+            gu = F.linear(x, lw["w_gate_up"])
+            h = h + F.linear(F.silu(gu[..., :it]) * gu[..., it:], lw["w_down"])
+        x = F.rms_norm(h, (hs,), self.norm, sh.rms_norm_eps)
+        self.logits_tok[:, :T].copy_(F.linear(x, self.lm_head).float())
+        if drop is not None:
+            srv.rewind(drop)
+            self.pos.sub_(drop.long())
+        return self.logits_tok[:, :T]
+
+    def _rope_at(self, x: torch.Tensor, pos: torch.Tensor) -> torch.Tensor:
+        # x (B, H, T, d), pos (B, T): token t of request b rotated by its own position
+        cos = self.cos[pos][:, None]
+        sin = self.sin[pos][:, None]
+        x1, x2 = x[..., : self.d // 2], x[..., self.d // 2:]
+        return x * cos + torch.cat([-x2, x1], dim=-1) * sin
 
     def capture(self, warm: int = 3):
         """Capture step() into a CUDA graph (launch-bound otherwise: ~600 small kernels per token)."""

@@ -41,7 +41,7 @@ class Context:
     def __init__(self, K: int, L: int, num_layers: int, num_attention_heads: int, num_key_value_heads: int,
                  head_dim: int, batch_size: int, max_length: int, num_sink_tokens: int = 4, num_local_tokens: int = 64,
                  generation_buffer: int = 256, dense_layers: Sequence[int] = (), alloc_dense_kv: bool = False,
-                 device: str | torch.device = "cuda:0"):
+                 device: str | torch.device = "cuda:0", max_query_tokens: int = 1):
         self.lib = N.load()
         self.device = torch.device(device)
         if self.device.type != "cuda":
@@ -73,6 +73,10 @@ class Context:
         with torch.cuda.device(self.device):
             N.check(self.lib.mpig_create(ctypes.byref(cfg), ctypes.byref(h)), "mpig_create")
         self._h = h
+        self.max_query_tokens = 1
+        self.last_tokens = 1   # T of the last decode: the readers return B*T*Hq rows
+        if max_query_tokens > 1:
+            self.reserve_query_tokens(max_query_tokens)
 
     # -- lifetime ---------------------------------------------------------------------------
     def close(self):
@@ -99,6 +103,7 @@ class Context:
 
     def clear(self):
         N.check(self.lib.mpig_clear(self._h, _stream()), "mpig_clear")
+        self.last_tokens = 1
 
     def get_info(self, key: str) -> int:
         v = ctypes.c_int64(0)
@@ -112,14 +117,15 @@ class Context:
         return int(f.value)
 
     def last_out_f32(self) -> torch.Tensor:
-        """fp32 (B*Hq, d) output of the last decode before the ABI's bf16 rounding (set_option("out_f32", 1) first)."""
-        out = torch.empty((self.H, self.d), dtype=torch.float32, device=self.device)
+        """fp32 (B*T*Hq, d) output of the last decode (T = 1 for single-token decodes) before the ABI's bf16 rounding
+        (set_option("out_f32", 1) first)."""
+        out = torch.empty((self.H * self.last_tokens, self.d), dtype=torch.float32, device=self.device)
         N.check(self.lib.mpig_last_out_f32(self._h, _ptr(out), _stream()), "mpig_last_out_f32")
         return out
 
     def last_codes(self) -> torch.Tensor:
-        """int32 (B*Hq, L) query codes the last decode probed with (fused decode: set_option("save_mask", 1) first)."""
-        codes = torch.empty((self.H, self.L), dtype=torch.int32, device=self.device)
+        """int32 (B*T*Hq, L) query codes the last decode probed with (fused decode: set_option("save_mask", 1) first)."""
+        codes = torch.empty((self.H * self.last_tokens, self.L), dtype=torch.int32, device=self.device)
         N.check(self.lib.mpig_last_codes(self._h, _ptr(codes), _stream()), "mpig_last_codes")
         return codes
 
@@ -211,6 +217,7 @@ class Context:
         self._chk(nnz, torch.int32, (self.H,), "nnz")
         N.check(self.lib.mpig_attention_wrapper(self._h, layer, K, L, _ptr(output), _ptr(max_value_expsum), _ptr(query),
                                                 _ptr(query_norm), _ptr(ind), _ptr(nnz), _stream()), "mpig_attention_wrapper")
+        self.last_tokens = 1
 
     def read_cache(self, layer: int, want_k=True, want_v=True, want_kn=True):
         k = torch.empty((self.B, self.Hkv, self.M, self.d), dtype=torch.bfloat16, device=self.device) if want_k else None
@@ -236,8 +243,57 @@ class Context:
         N.check(self.lib.mpig_window_fill(self._h, layer, request, _ptr(avg_k), _ptr(k), _ptr(v), w, _stream()),
                 "mpig_window_fill")
 
-    def plan(self):
-        N.check(self.lib.mpig_plan(self._h, _stream()), "mpig_plan")
+    def plan(self, tokens: int = 1):
+        """Advance every request's lengths by `tokens` (a verification step of that many tokens; reserve them first)."""
+        if tokens == 1:
+            N.check(self.lib.mpig_plan(self._h, _stream()), "mpig_plan")
+        else:
+            N.check(self.lib.mpig_plan_tokens(self._h, int(tokens), _stream()), "mpig_plan_tokens")
+
+    def reserve_query_tokens(self, t_max: int):
+        """Allocate the per-step scratch for verification steps of up to t_max <= 8 tokens.  Not capturable, and refused once a
+        step has been captured into a CUDA graph (the scratch moves): reserve before capturing."""
+        N.check(self.lib.mpig_reserve_query_tokens(self._h, int(t_max)), "mpig_reserve_query_tokens")
+        self.max_query_tokens = max(self.max_query_tokens, int(t_max))
+
+    def rewind(self, drop: torch.Tensor):
+        """Drop the last drop[b] tokens of the pending step of request b; drop: int32 (B,) on the device.  Capturable; eager
+        calls synchronise and raise on a drop outside [0, T] without changing anything (the call may be repeated)."""
+        self._chk(drop, torch.int32, (self.B,), "drop")
+        N.check(self.lib.mpig_rewind(self._h, _ptr(drop), _stream()), "mpig_rewind")
+
+    def _tokens_args(self, T: int, query, key, value, out):
+        q = query.reshape(self.B * T * self.Hq, self.d)
+        k = key.reshape(self.B * T * self.Hkv, self.d)
+        v = value.reshape(self.B * T * self.Hkv, self.d)
+        self._chk(q, torch.bfloat16, None, "query")
+        self._chk(k, torch.bfloat16, None, "key")
+        self._chk(v, torch.bfloat16, None, "value")
+        if out is None:
+            out = torch.empty((self.B, T, self.Hq * self.d), dtype=torch.bfloat16, device=self.device)
+        else:
+            self._chk(out, torch.bfloat16, None, "out")
+            if out.numel() != self.B * T * self.Hq * self.d:
+                raise N.MagicPigError(f"out: expected {self.B * T * self.Hq * self.d} elements, got {out.numel()}")
+        return q, k, v, out
+
+    def decode_tokens(self, layer: int, T: int, query: torch.Tensor, key: torch.Tensor, value: torch.Tensor,
+                      out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Sparse layer, verification step of T tokens: query (B,T,Hq,d), key/value (B,T,Hkv,d) bf16 -> out (B, T, Hq*d)."""
+        q, k, v, out = self._tokens_args(T, query, key, value, out)
+        N.check(self.lib.mpig_decode_tokens(self._h, layer, int(T), _ptr(q), _ptr(k), _ptr(v), _ptr(out), _stream()),
+                "mpig_decode_tokens")
+        self.last_tokens = int(T)
+        return out
+
+    def dense_decode_tokens(self, layer: int, T: int, query: torch.Tensor, key: torch.Tensor, value: torch.Tensor,
+                            out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Dense layer, same shapes as decode_tokens."""
+        q, k, v, out = self._tokens_args(T, query, key, value, out)
+        N.check(self.lib.mpig_dense_decode_tokens(self._h, layer, int(T), _ptr(q), _ptr(k), _ptr(v), _ptr(out), _stream()),
+                "mpig_dense_decode_tokens")
+        self.last_tokens = int(T)
+        return out
 
     def spill_window(self, keep: Optional[int] = None) -> torch.Tensor:
         """Move the oldest non-sink window rows of every request and sparse layer into the sampled store and the hash tables,
@@ -262,6 +318,7 @@ class Context:
         else:
             self._chk(out, torch.bfloat16, None, "out")
         N.check(self.lib.mpig_decode(self._h, layer, _ptr(q), _ptr(k), _ptr(v), _ptr(out), _stream()), "mpig_decode")
+        self.last_tokens = 1
         return out
 
     def decode_timed(self, layer: int, query: torch.Tensor, key: torch.Tensor, value: torch.Tensor, out: torch.Tensor):
@@ -273,6 +330,7 @@ class Context:
         for t, nm in ((q, "query"), (k, "key"), (v, "value"), (out, "out")):
             self._chk(t, torch.bfloat16, None, nm)
         N.check(self.lib.mpig_decode_timed(self._h, layer, _ptr(q), _ptr(k), _ptr(v), _ptr(out), _stream()), "mpig_decode_timed")
+        self.last_tokens = 1
 
     def timing_collect(self, max_calls: int = 4096):
         """[(simhash_ms, probe_ms, attend_ms), ...] for every decode_timed() since the last collect (synchronises)."""
@@ -294,12 +352,14 @@ class Context:
         rc = self.lib.mpig_decode_host(self._h, layer, query.data_ptr(), key.data_ptr(), value.data_ptr(), out.data_ptr(), _stream())
         if rc:
             N.check(rc, "mpig_decode_host")
+        self.last_tokens = 1
         return out
 
     def last_probe(self, want_results: bool = False):
-        """nnz (B*Hq,) int32 [and results (B*Hq, M)] of the most recent decode's probe."""
-        nnz = torch.empty((self.H,), dtype=torch.int32, device=self.device)
-        res = torch.empty((self.H, self.M), dtype=torch.int32, device=self.device) if want_results else None
+        """nnz (B*T*Hq,) int32 [and results (B*T*Hq, M)] of the most recent decode's probe (T = 1 for single-token decodes)."""
+        rows = self.H * self.last_tokens
+        nnz = torch.empty((rows,), dtype=torch.int32, device=self.device)
+        res = torch.empty((rows, self.M), dtype=torch.int32, device=self.device) if want_results else None
         N.check(self.lib.mpig_last_probe(self._h, _ptr(nnz), _ptr(res), _stream()), "mpig_last_probe")
         return nnz, res
 
@@ -323,6 +383,7 @@ class Context:
             out = torch.empty((self.B, self.Hq * self.d), dtype=torch.bfloat16, device=self.device)
         N.check(self.lib.mpig_dense_decode(self._h, layer, _ptr(q), _ptr(k), _ptr(v), _ptr(out), _stream()),
                 "mpig_dense_decode")
+        self.last_tokens = 1
         return out
 
 

@@ -5,7 +5,7 @@
 Sizes are tiny (the tools slow kernels down 10-100x) but cover: the stand-alone SimHash / probe (uint8 tags, several clusters
 shapes, two key segments) / gather-attention kernels, the fused single-launch decode (cluster of 8, cluster of 4 over two
 segments, one CTA per head with codes from the SimHash kernel, several selection passes), the three-launch decode, the dense
-kernel, the tensor-core key hash and the table build.  Results are also checked against each other so a tool run doubles as a test.
+kernel, the tensor-core key hash, the table build, the window spill and verification steps of T tokens.  Results are also checked against each other so a tool run doubles as a test.
 """
 import os
 import sys
@@ -193,8 +193,56 @@ def spill_case():
     print("spill ok")
 
 
+def tokens_case(B, Hq, Hkv, n, K, L, T):
+    """A verification step of T tokens (row append, the T-token fused kernel / SimHash kernel over B*T*Hq rows, the T-token dense
+    kernel, rewind) against T single-token steps of a twin context."""
+    M = n + 160
+    g = torch.Generator(device=dev).manual_seed(20 + T)
+    hf = torch.randn((d, K * L), generator=g, device=dev).bfloat16()
+    ctxs = []
+    for tmax in (T, 1):
+        ctx = Context(K, L, 2, Hq, Hkv, d, B, M, generation_buffer=16, dense_layers=[0], alloc_dense_kv=True, device=dev,
+                      max_query_tokens=tmax)
+        ctx.set_option("out_f32", 1)
+        ctx.set_hash_func(hf)
+        ctxs.append(ctx)
+    g2 = torch.Generator(device=dev).manual_seed(21)
+    for b in range(B):
+        key = torch.randn((Hkv, n, d), generator=g2, device=dev).bfloat16()
+        val = torch.randn((Hkv, n, d), generator=g2, device=dev).bfloat16()
+        wk, wv = (torch.randn((Hkv, 68, d), generator=g2, device=dev).bfloat16() for _ in range(2))
+        dk, dv = (torch.randn((300, Hkv, d), generator=g2, device=dev).bfloat16() for _ in range(2))
+        for ctx in ctxs:
+            ctx.attn_fill(1, b, key, val, key.norm(p=2, dim=-1).float())
+            ctx.lsh_build(1, b, ctx.hash_keys(key))
+            ctx.window_fill(1, b, torch.zeros((Hkv, d), dtype=torch.bfloat16, device=dev), wk, wv)
+            ctx.dense_fill(0, b, dk, dv, 300)
+    q = torch.randn((B, T, Hq, d), generator=g, device=dev).bfloat16()
+    k, v = (torch.randn((B, T, Hkv, d), generator=g, device=dev).bfloat16() for _ in range(2))
+    tok, seq = ctxs
+    tok.plan(T)
+    tok.decode_tokens(1, T, q, k, v)
+    o_s = tok.last_out_f32().reshape(B, T, Hq, d)
+    tok.dense_decode_tokens(0, T, q, k, v)
+    o_d = tok.last_out_f32().reshape(B, T, Hq, d)
+    tok.rewind(torch.full((B,), 1, dtype=torch.int32, device=dev))
+    for t in range(T):
+        seq.plan()
+        seq.decode(1, q[:, t].contiguous(), k[:, t].contiguous(), v[:, t].contiguous())
+        r_s = seq.last_out_f32().reshape(B, Hq, d)
+        seq.dense_decode(0, q[:, t].contiguous(), k[:, t].contiguous(), v[:, t].contiguous())
+        r_d = seq.last_out_f32().reshape(B, Hq, d)
+        for a, r in ((o_s[:, t], r_s), (o_d[:, t], r_d)):
+            assert float((a - r).abs().max()) <= 1e-5 * float(r.abs().max()), f"token {t} differs from the single-token step"
+    torch.cuda.synchronize()
+    print(f"tokens B={B} Hq={Hq} Hkv={Hkv} n={n} T={T}: waves {tok.get_info('tokens_cluster_waves')} ok")
+
+
 if __name__ == "__main__":
-    which = sys.argv[1:] or ["stages", "dense", "decode", "hostpeer", "spill"]
+    which = sys.argv[1:] or ["stages", "dense", "decode", "hostpeer", "spill", "tokens"]
+    if "tokens" in which:
+        tokens_case(2, 4, 1, 800, 6, 24, 3)              # clusters of 8 per virtual head, dense T*G = 12
+        tokens_case(4, 32, 8, 400, 6, 24, 2)             # one CTA per virtual head (codes from the SimHash kernel), dense T*G = 8
     if "spill" in which:
         spill_case()
     if "hostpeer" in which:
