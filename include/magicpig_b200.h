@@ -121,7 +121,8 @@ int mpig_set_option(mpig_ctx *ctx, const char *key, int64_t value);
 int mpig_get_info(mpig_ctx *ctx, const char *key, int64_t *value);
 /* Capacity errors the DEVICE detected (the lengths saturate there): bit 0 = a sparse window is full (generation_buffer
  * exhausted: each further token overwrites the previous one's K/V), bit 1 = a dense cache reached max_length, bit 2 = mpig_rewind
- * met a drop outside [0, T] (that request was left untouched).  mpig_plan
+ * met a drop outside [0, T] (that request was left untouched), bit 3 = mpig_plan_tree met a malformed tree (that request ran as a
+ * chain) or mpig_accept met a path that is not a root path of the step (that request was left untouched).  mpig_plan
  * itself returns MPIG_ESTATE for the same conditions as long as it has not been captured into a CUDA graph (replays advance
  * only the device-side lengths).  mpig_spill_window is the way out of a full sparse window.  Synchronises `stream`.  The
  * reference has no such check (flashinfer append past the page). */
@@ -270,8 +271,35 @@ int mpig_dense_decode_tokens(mpig_ctx *ctx, int layer, int T, const void *query_
  * request whose drop is outside [0, T] is left untouched and raises mpig_error_flags bit 2.  At most one rewind per plan
  * (MPIG_ESTATE).  Outside a capture the call synchronises `stream` and checks the drops first: if one is outside [0, T] it raises
  * bit 2, changes no length and returns MPIG_EINVAL (the rewind may then be repeated with valid drops); otherwise it rewinds and
- * refreshes the host mirror of the lengths from the device.  mpig_clear forgets the pending step. */
+ * refreshes the host mirror of the lengths from the device.  mpig_clear forgets the pending step.  Refused (MPIG_ESTATE) after
+ * mpig_plan_tree: dropping a suffix of a tree is meaningless. */
 int mpig_rewind(mpig_ctx *ctx, const int32_t *drop, void *stream);
+
+/* ---- token trees (speculative decoding with several candidates per position; no reference equivalent) ---------------------------
+ *   mpig_plan_tree(T, parents) -> per layer mpig_decode_tokens / mpig_dense_decode_tokens(T) -> mpig_accept(nodes, count).
+ * A step of T nodes (1 <= T <= the reserved t_max) takes per request b a parent array parents[b][0..T): parents[b][0] = -1 and
+ * 0 <= parents[b][t] < t (topological order, node 0 is the root).  The T new rows are appended at base_b .. base_b + T - 1 in node
+ * order, as for a chain.  Node t attends to the context rows [0, base_b), the rows of its ancestors, its own row and, on sparse
+ * layers, its own LSH sample; rows of the other nodes of the step are invisible.  Per node, the result equals a chain step over the
+ * node's root path: identical codes, nnz and index lists, fp32 outputs equal up to summation order.  A chain (parents[t] = t - 1) is
+ * exactly mpig_plan_tokens.  RoPE positions are the caller's: node t sits at position base + depth(t).
+ *
+ * mpig_plan_tree does the work of mpig_plan_tokens(T) (same host-mirror checks, same device saturation bits), and its plan kernel
+ * checks every request's tree and records the per-node ancestor masks and a copy of the parents in context scratch allocated at
+ * create time (nothing moves after a capture; parents may be reused right after the call).  parents: DEVICE int32 (B, T).
+ * Capturable: under capture a malformed tree makes that request a chain and raises mpig_error_flags bit 3.  Eager calls read the
+ * parents back first: on a malformed tree they raise bit 3, change nothing and return MPIG_EINVAL.  MPIG_EINVAL for T outside
+ * [1, reserved]. */
+int mpig_plan_tree(mpig_ctx *ctx, int T, const int32_t *parents, void *stream);
+/* Commit the root path nodes[b][0..count[b]) of the pending step of request b (nodes: DEVICE int32 (B, T), count: DEVICE int32 (B)).
+ * A path is valid when 0 <= count[b] <= T, nodes[b][0] = 0 and parents[nodes[b][i]] = nodes[b][i-1].  Row base + nodes[b][i] moves
+ * to base + i in every sparse layer's window (all kv-heads) and every dense layer's KV, in one launch, and both lengths become
+ * base + count[b].  Works after mpig_plan_tokens / mpig_plan too (a chain prefix of count nodes equals mpig_rewind(T - count)).
+ * Capturable (acceptance can be decided on the GPU): a bad path leaves that request untouched and raises bit 3.  Outside a capture
+ * the call synchronises `stream` and checks the paths first: on a bad one it raises bit 3, changes nothing and returns MPIG_EINVAL
+ * (the accept may then be repeated).  At most one rewind or accept per plan (MPIG_ESTATE).  Row accesses stay inside the window and
+ * dense capacities even after a plan that saturated.  mpig_clear forgets the pending step. */
+int mpig_accept(mpig_ctx *ctx, const int32_t *nodes, const int32_t *count, void *stream);
 
 /* ---- dense layers (attnserver.py:116-120, 235-259), only with cfg.alloc_dense_kv -------------- */
 /* k, v bf16 (P, Hkv, d) -- the prefill cache in NHD layout as models/llama.py:282 passes it. */

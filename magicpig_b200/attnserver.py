@@ -89,6 +89,7 @@ class LSHSparseAttnServer:
         self.hash_code_buffer = torch.zeros((self.num_key_value_heads, L, max_length), dtype=torch.int16, device=self.device)
         self._out = {}   # layer (one token) or (layer, T) (T-token steps) -> decode output buffer (allocated on first use)
         self._drop = None   # staging of host-side rewind counts
+        self._tree_stage = {}   # staging of host-side tree parents / accepted paths, per (name, T)
 
     # ------------------------------------------------------------------------------------------
     def alloc_buffer(self, seq_len: int):
@@ -137,10 +138,48 @@ class LSHSparseAttnServer:
         else:
             self.ctx.lsh_build(layer_idx, request_id, codes.contiguous())
 
-    def plan(self, num_tokens: int = 1):
+    def plan(self, num_tokens: int = 1, parents=None):
         """attnserver.py:196-224.  num_tokens > 1: a verification step of that many tokens per request (the decode calls of the
-        step then take q_len = num_tokens); rewind() afterwards drops the rejected ones."""
-        self.ctx.plan(num_tokens)
+        step then take q_len = num_tokens); rewind() afterwards drops the rejected ones.  With `parents` the step is a token tree
+        of num_tokens nodes: parents[b][t] is node t's parent (parents[b][0] = -1, 0 <= parents[b][t] < t), a (T,) list applies to
+        every request, a device int32 (B, T) tensor goes through without a copy (capturable).  Node t attends to the context, its
+        ancestors and itself; accept() afterwards commits one root path per request."""
+        if parents is None:
+            self.ctx.plan(num_tokens)
+            return
+        T = int(num_tokens)
+        self.ctx.plan(T, parents=self._stage_int32("parents", parents, (self.batch_size, T)))
+
+    def accept(self, nodes, num_accepted):
+        """Not in the reference.  Commits the root path nodes[b][0 .. num_accepted[b]) of the pending step (tree or chain): the
+        path's K/V rows become the step's first rows in every layer and the lengths grow by num_accepted[b] only.  nodes: (T,) list
+        (every request), (B, <= T) sequences or a device int32 (B, T) tensor; num_accepted: an int, B ints or a device int32 (B,)
+        tensor.  Device tensors go through without a copy (capturable: acceptance can be decided on the GPU)."""
+        T = self.ctx.pending_tokens
+        if isinstance(num_accepted, int):
+            num_accepted = [num_accepted] * self.batch_size
+        self.ctx.accept(self._stage_int32("nodes", nodes, (self.batch_size, T)),
+                        self._stage_int32("count", num_accepted, (self.batch_size,)))
+
+    def _stage_int32(self, name: str, x, shape) -> torch.Tensor:
+        """A device int32 tensor of `shape` for x: device tensors as they are, host sequences copied into a staging buffer
+        (a per-request sequence shorter than the row is padded with zeros; one row broadcasts to every request)."""
+        if isinstance(x, torch.Tensor) and x.is_cuda:
+            return x.to(torch.int32).reshape(shape).contiguous()
+        rows = [list(r) for r in x] if len(shape) == 2 and len(x) and not isinstance(x[0], int) else None
+        host = torch.zeros(shape, dtype=torch.int32)
+        if len(shape) == 1:
+            host[:] = torch.as_tensor(list(x), dtype=torch.int32)
+        elif rows is None:
+            host[:, :len(x)] = torch.as_tensor(list(x), dtype=torch.int32)
+        else:
+            for b, r in enumerate(rows):
+                host[b, :len(r)] = torch.as_tensor(r, dtype=torch.int32)
+        buf = self._tree_stage.get((name, shape))
+        if buf is None:
+            buf = self._tree_stage[(name, shape)] = torch.zeros(shape, dtype=torch.int32, device=self.device)
+        buf.copy_(host)
+        return buf
 
     def rewind(self, num_rejected):
         """Not in the reference.  Drops the last `num_rejected` tokens of the pending verification step: an int (every request),

@@ -350,14 +350,15 @@ __global__ void __launch_bounds__(384) attend_dense_kernel(const DenseParams p) 
 // ---- verification step of T tokens ------------------------------------------------------------------------------------------
 // The same per-(request, kv-head) organisation for the T*G <= 32 query rows of a group: row r = t*G + j is q-head j of the group
 // for token t, the rows sit on the M axis of NMT m16 tiles, and every K|V record is fetched ONCE for all of them (dense KV bytes per
-// step do not grow with T).  Token t sees rows [0, len - (T-1-t)) (causal over the T rows the step appended).
+// step do not grow with T).  Token t sees the rows [0, len - T) before the step and those of the step's rows len - T + j whose bit j
+// is set in its ancestor mask anc[b*T + t] (plan_kernel; a chain sets bits 0..t, i.e. rows [0, len - (T-1-t)): causal).
 //   PACK (T*G <= 8): one m-tile whose rows 8..15 are free carry the lo halves of the bf16 hi/lo split of P, as above;
 //   otherwise the lo halves are a second pass of MMAs over each m-tile into the same accumulators.
 // States of the T*G rows fill a warp's whole ring (32 x 132 floats at T*G = 32): the CTA-level merge reads the other warps' rings in
 // place.  That is safe because a warp whose group is split (w_g > 1) never takes a second item (see the partition: then the items
 // number at most the warps).
 template <int NMT, bool PACK>
-__global__ void __launch_bounds__(256) attend_dense_tokens_kernel(const DenseParams p, int T) {
+__global__ void __launch_bounds__(256) attend_dense_tokens_kernel(const DenseParams p, int T, const int32_t *anc) {
     extern __shared__ __align__(128) uint8_t smem[];
     const int warps = blockDim.x >> 5, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     uint8_t *slots = smem + (size_t)warp * TILE * DSLOT;
@@ -415,9 +416,11 @@ __global__ void __launch_bounds__(256) attend_dense_tokens_kernel(const DensePar
         const int r_lo = part * c_g, r_hi = min(r_lo + c_g, len);
         const uint8_t *rows = p.kv + (size_t)bg * p.M * REC;
 
-        // this lane's query rows: r = mt*16 + i*8 + grp; rows past T*G are zero and unmasked
+        // this lane's query rows: r = mt*16 + i*8 + grp; rows past T*G are zero and unmasked.  Key row k is visible to query row r
+        // when k < lim or bit k - lim of vis is set (lim = the first row of the step, vis = the token's ancestor mask)
         const uint32_t *qrow[NMT][2];
         int lim[NMT][2];
+        uint32_t vis[NMT][2];
 #pragma unroll
         for (int mt = 0; mt < NMT; ++mt)
 #pragma unroll
@@ -425,7 +428,8 @@ __global__ void __launch_bounds__(256) attend_dense_tokens_kernel(const DensePar
                 const int r = mt * 16 + i * 8 + grp;
                 const bool ok = r < TG && !(PACK && i == 1);
                 qrow[mt][i] = ok ? reinterpret_cast<const uint32_t *>(p.q + (size_t)out_row(bg, r) * D) : nullptr;
-                lim[mt][i] = ok ? len - (T - 1 - r / G) : len;
+                lim[mt][i] = ok ? len - T : len;
+                vis[mt][i] = ok ? (uint32_t)__ldg(anc + (bg / p.Hkv) * T + r / G) : 0u;
             }
         auto q_frag = [&](int mt, int ks, uint32_t (&a)[4]) {
             a[0] = qrow[mt][0] ? __ldg(qrow[mt][0] + ks * 8 + tig) : 0u;
@@ -507,7 +511,9 @@ __global__ void __launch_bounds__(256) attend_dense_tokens_kernel(const DensePar
                         for (int e = 0; e < 2; ++e) {
                             const int r = nt * 8 + tig * 2 + e;
                             float &x = s[mt][nt][2 * i + e];
-                            x = (r < nrows && cr + r < lim[mt][i]) ? x * scale_log2 : -CUDART_INF_F;
+                            const int o = cr + r - lim[mt][i];
+                            const bool seen = o < 0 || ((unsigned)o < (unsigned)TREE_MAX && ((vis[mt][i] >> o) & 1u));
+                            x = (r < nrows && seen) ? x * scale_log2 : -CUDART_INF_F;
                             mloc = fmaxf(mloc, x);
                         }
                     mloc = fmaxf(mloc, __shfl_xor_sync(0xffffffffu, mloc, 1));
@@ -686,13 +692,13 @@ int launch_attend_dense_tokens(mpig_ctx *ctx, const uint8_t *kv, const int32_t *
     cfg.numAttrs = pdl ? 1 : 0;
     if (TG <= 8) {
         MPIG_FUNC_ATTR((attend_dense_tokens_kernel<1, true>), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-        MPIG_CUDA(cudaLaunchKernelEx(&cfg, attend_dense_tokens_kernel<1, true>, p, T));
+        MPIG_CUDA(cudaLaunchKernelEx(&cfg, attend_dense_tokens_kernel<1, true>, p, T, (const int32_t *)step_masks(ctx->step_buf)));
     } else if (TG <= 16) {
         MPIG_FUNC_ATTR((attend_dense_tokens_kernel<1, false>), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-        MPIG_CUDA(cudaLaunchKernelEx(&cfg, attend_dense_tokens_kernel<1, false>, p, T));
+        MPIG_CUDA(cudaLaunchKernelEx(&cfg, attend_dense_tokens_kernel<1, false>, p, T, (const int32_t *)step_masks(ctx->step_buf)));
     } else {
         MPIG_FUNC_ATTR((attend_dense_tokens_kernel<2, false>), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-        MPIG_CUDA(cudaLaunchKernelEx(&cfg, attend_dense_tokens_kernel<2, false>, p, T));
+        MPIG_CUDA(cudaLaunchKernelEx(&cfg, attend_dense_tokens_kernel<2, false>, p, T, (const int32_t *)step_masks(ctx->step_buf)));
     }
     MPIG_LAUNCH_CHECK(ctx);
     ctx->last_tokens = T;

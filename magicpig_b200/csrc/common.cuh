@@ -59,7 +59,14 @@ int func_attr_once(const void *fn, cudaFuncAttribute attr, int value);
         if (_rc != MPIG_OK) return _rc;                                        \
     } while (0)
 
-constexpr int SEG_BITS = 16;       // table items are uint16 offsets inside key segments of at most 2^16 keys (tables.cu)
+constexpr int TREE_MAX = 8;        // nodes of a verification step (mpig_reserve_query_tokens caps t_max at this)
+
+// step_buf views (see mpig_ctx::step_buf): ancestor masks, parents, step bases; T = the pending step's node count
+template <typename I> __host__ __device__ inline I *step_masks(I *buf) { return buf; }
+template <typename I> __host__ __device__ inline I *step_parents(I *buf, int B) { return buf + (size_t)B * TREE_MAX; }
+template <typename I> __host__ __device__ inline I *step_bases(I *buf, int B) { return buf + (size_t)2 * B * TREE_MAX; }
+
+constexpr int SEG_BITS = 16;      // table items are uint16 offsets inside key segments of at most 2^16 keys (tables.cu)
 constexpr int SEG = 1 << SEG_BITS;
 
 struct LayerStore {
@@ -72,6 +79,14 @@ struct LayerStore {
     uint8_t *win = nullptr;      // window records
     __nv_bfloat16 *avg_k = nullptr;
     uint8_t *dense_kv = nullptr; // dense: full-context records
+};
+
+// one entry of the accept kernel's layer table: the REC-byte rows of a sparse window ([BG][cap], cap = Wcap) or of a dense KV
+// cache ([BG][cap], cap = max_length); dense = 1 selects dense_len and the dense step base
+struct AcceptLayer {
+    uint8_t *rows;
+    int cap;
+    int dense;
 };
 
 struct AttendTuning {
@@ -159,6 +174,14 @@ struct mpig_ctx {
     int last_tokens = 1;                     // rows of the readers (mpig_last_probe / _codes / _out_f32) = B * last_tokens * Hq
     bool plan_captured = false;              // a plan has been captured into a CUDA graph (the scratch addresses are baked in)
     int last_tokens_waves = 0;               // cluster waves of the last mpig_decode_tokens launch
+    // token trees (mpig_plan_tree / mpig_accept).  step_buf is allocated at create time for the largest step (8 nodes), so it never
+    // moves: int32 [B][T] ancestor masks (bit j of node t = node j is t or one of its ancestors) | int32 [B][T] parents | int32
+    // [B][2] step bases (window, dense length before the plan, after saturation).  Every plan writes it (chains for plan_tokens).
+    int32_t *step_buf = nullptr;
+    bool pending_tree = false;               // the pending step came from mpig_plan_tree (mpig_rewind is refused)
+    // device table of the layers that own rows (sparse windows and dense KV), for the one-launch accept kernel
+    void *accept_layers = nullptr;
+    int n_accept_layers = 0;
 };
 
 namespace mpig {
@@ -323,8 +346,7 @@ int launch_append_tokens(mpig_ctx *ctx, const AppendParams &ap, int T, cudaStrea
 int launch_fused_tokens(mpig_ctx *ctx, int layer, int T, const void *q, const void *k, const void *v, void *out, cudaStream_t s);
 // T-token dense decode (attend_dense.cu): q (B, T, Hq, d), rows already appended, causal over the last T rows
 int launch_attend_dense_tokens(mpig_ctx *ctx, const uint8_t *kv, const int32_t *len, int T, const void *q, void *out, cudaStream_t s,
-                               bool pdl);
-int launch_probe(mpig_ctx *ctx, int layer, const int32_t *query, int32_t *results, int32_t *nnz, cudaStream_t s, bool pdl);
+                               bool pdl);int launch_probe(mpig_ctx *ctx, int layer, const int32_t *query, int32_t *results, int32_t *nnz, cudaStream_t s, bool pdl);
 int launch_attend_mma(mpig_ctx *ctx, const AttendParams &p, cudaStream_t s, bool pdl);
 int launch_attend_dense(mpig_ctx *ctx, const uint8_t *kv, const int32_t *len, const void *q, void *out, cudaStream_t s, bool pdl);
 int launch_fused(mpig_ctx *ctx, int layer, const void *q, const void *k, const void *v, void *out, cudaStream_t s, bool pdl,

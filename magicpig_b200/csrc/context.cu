@@ -188,6 +188,24 @@ int mpig_create(const mpig_config *cfg, mpig_ctx **out) {
     TRY(dev_alloc(ctx, &ctx->counters, H * sizeof(int32_t)));
     TRY(dev_alloc(ctx, &ctx->mve, 2 * H * sizeof(float)));
     TRY(dev_alloc(ctx, &ctx->err_flag, 4 * sizeof(int32_t)));
+    TRY(dev_alloc(ctx, &ctx->step_buf, (size_t)cfg->batch_size * (2 * TREE_MAX + 2) * sizeof(int32_t), true));
+    {   // layer table of mpig_accept: every sparse window and every dense KV cache the context owns
+        std::vector<AcceptLayer> tab;
+        for (const LayerStore &ls : ctx->layers) {
+            if (ls.sparse && ctx->Wcap > 0) tab.push_back({ls.win, ctx->Wcap, 0});
+            if (ls.dense && ls.dense_kv) tab.push_back({ls.dense_kv, cfg->max_length, 1});
+        }
+        ctx->n_accept_layers = (int)tab.size();
+        if (!tab.empty()) {
+            TRY(dev_alloc(ctx, (uint8_t **)&ctx->accept_layers, tab.size() * sizeof(AcceptLayer)));
+            const cudaError_t e = cudaMemcpy(ctx->accept_layers, tab.data(), tab.size() * sizeof(AcceptLayer), cudaMemcpyHostToDevice);
+            if (e != cudaSuccess) {
+                set_error("mpig_create: accept table upload failed: %s", cudaGetErrorString(e));
+                mpig_destroy(ctx);
+                return MPIG_ECUDA;
+            }
+        }
+    }
     ctx->h_win_len.assign(cfg->batch_size, 0);
     ctx->h_dense_len.assign(cfg->batch_size, 0);
     // staging of the *_host entry points: q | k | v | out, one MAPPED pinned block the kernels read and write directly
@@ -235,6 +253,8 @@ void mpig_destroy(mpig_ctx *ctx) {
     cudaFree(ctx->counters);
     cudaFree(ctx->mve);
     cudaFree(ctx->err_flag);
+    cudaFree(ctx->step_buf);
+    cudaFree(ctx->accept_layers);
     cudaFree(ctx->out_f32);
     cudaFree(ctx->dbg_buf);
     cudaFree(ctx->fused_dbg);
@@ -276,8 +296,9 @@ int mpig_clear(mpig_ctx *ctx, void *stream) {
     for (auto &n : ctx->h_dense_len) n = 0;
     ctx->h_len_exact = true;
     ctx->last_tokens = 1;
-    ctx->pending_T = 0;     // no plan to decode or rewind since the clear
+    ctx->pending_T = 0;     // no plan to decode, rewind or accept since the clear
     ctx->rewound = true;
+    ctx->pending_tree = false;
     return MPIG_OK;
 }
 

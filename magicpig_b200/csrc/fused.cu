@@ -158,10 +158,13 @@ __device__ __forceinline__ int block_exclusive_scan_redux(int v, int *wtot, int 
 // instead of ~300 in two rounds.  KREG = false: whole 512-byte records through TMA + ldmatrix (the stand-alone kernel's way).
 // TOK = true: a verification step of T = gp.ntok tokens per request.  Cluster v serves VIRTUAL head v = (b*T + t)*Hq + h: q, out
 // and every per-head output are indexed by v (the (B, T, Hq, d) layout), the tables / records / window of group b*Hkv + h/G are
-// read, and the window ends T-1-t rows before win_len[b] (causal).  The T new rows were appended by append_tokens_kernel, so
-// k_new is null: no in-kernel row build.
+// read, and the window ends T-1-t rows before win_len[b].  The T new rows were appended by append_tokens_kernel, so k_new is null:
+// no in-kernel row build.  Of the step's rows the token sees those whose bit is set in its ancestor mask (gp.anc[b*T + t]; a chain
+// sets bits 0..t, so nothing is masked): the other rows score -inf.  `anc` is a kernel argument of its own (null for the
+// single-token instantiations) so that FusedParams, and with it their code, stays as it is.
 template <typename TagT, int THREADS, bool DBG, bool KREG, bool TOK = false>
-__global__ void __launch_bounds__(THREADS, (THREADS == 1024) ? 1 : 2) fused_decode_kernel(const __grid_constant__ FusedParams gp) {
+__global__ void __launch_bounds__(THREADS, (THREADS == 1024) ? 1 : 2) fused_decode_kernel(const __grid_constant__ FusedParams gp,
+                                                                                                   const int32_t *__restrict__ anc) {
     extern __shared__ __align__(128) uint8_t smem_raw[];
     __shared__ FusedParams p_s;   // parameters staged once (constant-bank misses were microseconds on the critical path)
     {
@@ -279,6 +282,11 @@ __global__ void __launch_bounds__(THREADS, (THREADS == 1024) ? 1 : 2) fused_deco
     } else if (warp == 1) {
         const int wl = p.win ? min(max(__ldg(p.win_len + bq) - (TOK ? s_geo[5] : 0), 0), p.Wcap) : 0;
         if (lane == 0) s_misc[1] = __int_as_float(wl);
+        if (TOK && lane == 0) {   // first window row of the step as this token sees it, and the token's ancestor mask
+            const int tk = p.ntok - 1 - s_geo[5], bt = bq * p.ntok + tk;
+            s_misc[2] = __int_as_float(wl - 1 - tk);
+            s_misc[3] = __int_as_float(__ldg(anc + bt));
+        }
         if (c == 0 && (h % p.G) == 0 && wl > 0 && p.k_new) {
             // centred key (bf16 arithmetic as torch: fp32 subtract, RNE) | value -> window row wl-1 (attnserver.py:275-290)
             const uint2 kk = __ldg(reinterpret_cast<const uint2 *>(p.k_new + (size_t)g * D) + lane);
@@ -782,12 +790,17 @@ __global__ void __launch_bounds__(THREADS, (THREADS == 1024) ? 1 : 2) fused_deco
                         const float w = sample_weight(proba, K, L, Lf);
                         z -= __logf(w + 1e-4f);
                     }
+                    if (TOK && is_win) {   // a step row of a node that is not this token or one of its ancestors
+                        const int o = row0 + lane - __float_as_int(s_misc[2]);
+                        if (o >= 0 && !((__float_as_uint(s_misc[3]) >> o) & 1u)) z = -CUDART_INF_F;
+                    }
                 }
                 if (DBG && wrec) wrec[11] = clk64() + (unsigned long long)(z == 123.456f);
                 // online softmax (base 2)
                 const float m_new = fmaxf(m_run, warp_max(z));
                 const float corr = (m_run == -CUDART_INF_F) ? 0.f : exp2f((m_run - m_new) * LOG2E_F);
-                const float pj = (lane < nrows) ? exp2f((z - m_new) * LOG2E_F) : 0.f;
+                // (TOK: a masked row is -inf, and so may be m_new for a tile with no visible row: its p must be 0, not NaN)
+                const float pj = (lane < nrows && (!TOK || z != -CUDART_INF_F)) ? exp2f((z - m_new) * LOG2E_F) : 0.f;
                 l_run = l_run * corr + pj;   // per-LANE partial sum (corr is warp-uniform): reduced once, before the state is stored
                 m_run = m_new;
 #pragma unroll
@@ -1068,7 +1081,7 @@ template <int THREADS, bool DBG, bool KREG>
 static int launch_variant(const cudaLaunchConfig_t &cfg, const FusedParams &p) {
     MPIG_FUNC_ATTR((fused_decode_kernel<uint8_t, THREADS, DBG, KREG>), cudaFuncAttributeMaxDynamicSharedMemorySize,
                    THREADS == 1024 ? 227 * 1024 - 1024 : 228 * 1024 / 2 - 2048);
-    MPIG_CUDA(cudaLaunchKernelEx(&cfg, fused_decode_kernel<uint8_t, THREADS, DBG, KREG>, p));
+    MPIG_CUDA(cudaLaunchKernelEx(&cfg, fused_decode_kernel<uint8_t, THREADS, DBG, KREG>, p, (const int32_t *)nullptr));
     return MPIG_OK;
 }
 
@@ -1169,10 +1182,10 @@ int launch_fused(mpig_ctx *ctx, int layer, const void *q, const void *k, const v
 }
 
 template <int THREADS, bool KREG>
-static int launch_tokens_variant(const cudaLaunchConfig_t &cfg, const FusedParams &p) {
+static int launch_tokens_variant(const cudaLaunchConfig_t &cfg, const FusedParams &p, const int32_t *anc) {
     MPIG_FUNC_ATTR((fused_decode_kernel<uint8_t, THREADS, false, KREG, true>), cudaFuncAttributeMaxDynamicSharedMemorySize,
                    THREADS == 1024 ? 227 * 1024 - 1024 : 228 * 1024 / 2 - 2048);
-    MPIG_CUDA(cudaLaunchKernelEx(&cfg, fused_decode_kernel<uint8_t, THREADS, false, KREG, true>, p));
+    MPIG_CUDA(cudaLaunchKernelEx(&cfg, fused_decode_kernel<uint8_t, THREADS, false, KREG, true>, p, anc));
     return MPIG_OK;
 }
 
@@ -1255,8 +1268,9 @@ int launch_fused_tokens(mpig_ctx *ctx, int layer, int T, const void *q, const vo
     attr[1].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 2;   // under PDL behind the append (or the SimHash kernel)
-    if (fp.threads == 1024) rc = ctx->fused_kreg ? launch_tokens_variant<1024, true>(cfg, p) : launch_tokens_variant<1024, false>(cfg, p);
-    else rc = ctx->fused_kreg ? launch_tokens_variant<512, true>(cfg, p) : launch_tokens_variant<512, false>(cfg, p);
+    const int32_t *anc = step_masks(ctx->step_buf);   // the pending step's ancestor masks (plan_kernel)
+    if (fp.threads == 1024) rc = ctx->fused_kreg ? launch_tokens_variant<1024, true>(cfg, p, anc) : launch_tokens_variant<1024, false>(cfg, p, anc);
+    else rc = ctx->fused_kreg ? launch_tokens_variant<512, true>(cfg, p, anc) : launch_tokens_variant<512, false>(cfg, p, anc);
     if (rc) return rc;
     MPIG_LAUNCH_CHECK(ctx);
     ctx->last_decode_fused = 1;

@@ -354,6 +354,55 @@ class LlamaDecodeRunner:
             self.pos.sub_(drop.long())
         return self.logits_tok[:, :T]
 
+    def step_tree(self, T: int, parents, nodes=None, count=None):
+        """A verification step over a token tree of T nodes: reads the candidates self.ids_tok[:, :T] in node order, writes
+        self.logits_tok[:, :T] (B, T, vocab), the logits after each node.  parents: device int32 (B, T) or (T,) (every request),
+        or a host sequence (parents[b][0] = -1, 0 <= parents[b][t] < t).  Node t sits at RoPE position pos + 1 + depth(t) and
+        attends to the context, its ancestors and itself; the depths are computed on the device.  Same eager-path math as
+        step_tokens.  With `nodes` / `count` (device int32 (B, T) / (B,), or host values) the step ends with server.accept(nodes,
+        count) and self.pos advances by count; without, every node stays in the caches (accept later) and self.pos advances by T.
+        Graph-capturable with device tensors."""
+        assert self.tp_world == 1, "verification steps are built for a single GPU"
+        assert 1 <= T <= self.max_query_tokens, f"T={T} outside [1, max_query_tokens={self.max_query_tokens}]"
+        sh, srv = self.shape, self.server
+        B, d, Hq, Hkv, hs, it = self.B, self.d, self.Hq_loc, self.Hkv_loc, sh.hidden_size, self.it_loc
+        if not (isinstance(parents, torch.Tensor) and parents.is_cuda):
+            parents = torch.as_tensor(parents, dtype=torch.int32).to(self.device)
+        parents = parents.to(torch.int32)
+        if parents.dim() == 1:
+            parents = parents[None].expand(B, T)
+        parents = parents.contiguous()
+        srv.plan(T, parents=parents)
+        # depth(t) = depth(parent(t)) + 1: T - 1 gathers settle every node of a topologically ordered tree
+        par = parents.long().clamp(min=0)
+        depth = torch.zeros((B, T), dtype=torch.long, device=self.device)
+        for _ in range(T - 1):
+            depth = torch.where(parents >= 0, depth.gather(1, par) + 1, 0)
+        pos = self.pos[:, None] + 1 + depth   # (B, T)
+        h = F.embedding(self.ids_tok[:, :T], self.embed)   # (B, T, hs)
+        for li, lw in enumerate(self.layers):
+            x = F.rms_norm(h, (hs,), lw["ln1"], sh.rms_norm_eps)
+            qkv = F.linear(x, lw["wqkv"])   # (B, T, (Hq+2Hkv)d)
+            q = self._rope_at(qkv[..., : Hq * d].reshape(B, T, Hq, d).transpose(1, 2), pos)
+            k = self._rope_at(qkv[..., Hq * d:(Hq + Hkv) * d].reshape(B, T, Hkv, d).transpose(1, 2), pos)
+            v = qkv[..., (Hq + Hkv) * d:].reshape(B, T, Hkv, d).transpose(1, 2)
+            a = srv.decode(q, k, v, li)   # (B, T, Hq*d), node t attending to its ancestors   <- the hot path
+            h = h + F.linear(a, lw["wo"])
+            x = F.rms_norm(h, (hs,), lw["ln2"], sh.rms_norm_eps)
+            gu = F.linear(x, lw["w_gate_up"])
+            h = h + F.linear(F.silu(gu[..., :it]) * gu[..., it:], lw["w_down"])
+        x = F.rms_norm(h, (hs,), self.norm, sh.rms_norm_eps)
+        self.logits_tok[:, :T].copy_(F.linear(x, self.lm_head).float())
+        if count is None:
+            self.pos.add_(T)
+        else:
+            srv.accept(nodes, count)
+            if isinstance(count, torch.Tensor):
+                self.pos.add_(count.to(self.device).long())
+            else:
+                self.pos.add_(torch.as_tensor(count if not isinstance(count, int) else [count] * B, device=self.device).long())
+        return self.logits_tok[:, :T]
+
     def _rope_at(self, x: torch.Tensor, pos: torch.Tensor) -> torch.Tensor:
         # x (B, H, T, d), pos (B, T): token t of request b rotated by its own position
         cos = self.cos[pos][:, None]

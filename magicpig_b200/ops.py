@@ -75,6 +75,7 @@ class Context:
         self._h = h
         self.max_query_tokens = 1
         self.last_tokens = 1   # T of the last decode: the readers return B*T*Hq rows
+        self.pending_tokens = 0   # T of the last plan (the shape accept() expects)
         if max_query_tokens > 1:
             self.reserve_query_tokens(max_query_tokens)
 
@@ -104,6 +105,7 @@ class Context:
     def clear(self):
         N.check(self.lib.mpig_clear(self._h, _stream()), "mpig_clear")
         self.last_tokens = 1
+        self.pending_tokens = 0
 
     def get_info(self, key: str) -> int:
         v = ctypes.c_int64(0)
@@ -111,7 +113,8 @@ class Context:
         return int(v.value)
 
     def error_flags(self) -> int:
-        """bit 0: a sparse window is full (generation_buffer exhausted), bit 1: a dense cache is full.  Synchronises."""
+        """bit 0: a sparse window is full (generation_buffer exhausted), bit 1: a dense cache is full, bit 2: a rewind drop was out
+        of range, bit 3: a malformed tree or accepted path.  Synchronises."""
         f = ctypes.c_int32(0)
         N.check(self.lib.mpig_error_flags(self._h, ctypes.byref(f), _stream()), "mpig_error_flags")
         return int(f.value)
@@ -243,12 +246,27 @@ class Context:
         N.check(self.lib.mpig_window_fill(self._h, layer, request, _ptr(avg_k), _ptr(k), _ptr(v), w, _stream()),
                 "mpig_window_fill")
 
-    def plan(self, tokens: int = 1):
-        """Advance every request's lengths by `tokens` (a verification step of that many tokens; reserve them first)."""
-        if tokens == 1:
+    def plan(self, tokens: int = 1, parents: Optional[torch.Tensor] = None):
+        """Advance every request's lengths by `tokens` (a verification step of that many tokens; reserve them first).  With
+        `parents` (device int32 (B, tokens): parents[b][0] = -1, 0 <= parents[b][t] < t) the step is a token tree: node t attends to
+        the context, its ancestors and itself.  Capturable; eager calls raise on a malformed tree without changing anything."""
+        if parents is not None:
+            self._chk(parents, torch.int32, (self.B, int(tokens)), "parents")
+            N.check(self.lib.mpig_plan_tree(self._h, int(tokens), _ptr(parents), _stream()), "mpig_plan_tree")
+        elif tokens == 1:
             N.check(self.lib.mpig_plan(self._h, _stream()), "mpig_plan")
         else:
             N.check(self.lib.mpig_plan_tokens(self._h, int(tokens), _stream()), "mpig_plan_tokens")
+        self.pending_tokens = int(tokens)
+
+    def accept(self, nodes: torch.Tensor, count: torch.Tensor):
+        """Commit the root path nodes[b][0 .. count[b]) of the pending step of request b: the path's rows move to the front of
+        the step in every sparse window and dense cache, and both lengths become base + count[b].  nodes: int32 (B, T), count: int32
+        (B,) on the device.  Capturable; eager calls raise on a path that is not a root path of the step without changing anything
+        (the call may be repeated)."""
+        self._chk(nodes, torch.int32, (self.B, self.pending_tokens), "nodes")
+        self._chk(count, torch.int32, (self.B,), "count")
+        N.check(self.lib.mpig_accept(self._h, _ptr(nodes), _ptr(count), _stream()), "mpig_accept")
 
     def reserve_query_tokens(self, t_max: int):
         """Allocate the per-step scratch for verification steps of up to t_max <= 8 tokens.  Not capturable, and refused once a

@@ -5,7 +5,7 @@
 Sizes are tiny (the tools slow kernels down 10-100x) but cover: the stand-alone SimHash / probe (uint8 tags, several clusters
 shapes, two key segments) / gather-attention kernels, the fused single-launch decode (cluster of 8, cluster of 4 over two
 segments, one CTA per head with codes from the SimHash kernel, several selection passes), the three-launch decode, the dense
-kernel, the tensor-core key hash, the table build, the window spill and verification steps of T tokens.  Results are also checked against each other so a tool run doubles as a test.
+kernel, the tensor-core key hash, the table build, the window spill, verification steps of T tokens and token trees with an accept.  Results are also checked against each other so a tool run doubles as a test.
 """
 import os
 import sys
@@ -238,8 +238,77 @@ def tokens_case(B, Hq, Hkv, n, K, L, T):
     print(f"tokens B={B} Hq={Hq} Hkv={Hkv} n={n} T={T}: waves {tok.get_info('tokens_cluster_waves')} ok")
 
 
+def tree_case(B, Hq, Hkv, n, K, L, parents, path):
+    """A token-tree step (the plan kernel's ancestor masks, the masked T-token fused and dense kernels, the accept kernel moving
+    rows in every layer): every node against a chain step over its root path on a twin context, then accept(path) on one and the
+    path as a chain step on the other, and one more token on both."""
+    T = len(parents)
+    assert path[-1] == T - 1, "the twin keeps the accepted path's chain step, so it must be the last one it runs"
+    M = n + 160
+    g = torch.Generator(device=dev).manual_seed(30 + T)
+    hf = torch.randn((d, K * L), generator=g, device=dev).bfloat16()
+    ctxs = []
+    for _ in range(2):
+        ctx = Context(K, L, 2, Hq, Hkv, d, B, M, generation_buffer=16, dense_layers=[0], alloc_dense_kv=True, device=dev,
+                      max_query_tokens=T)
+        ctx.set_option("out_f32", 1)
+        ctx.set_hash_func(hf)
+        ctxs.append(ctx)
+    g2 = torch.Generator(device=dev).manual_seed(31)
+    for b in range(B):
+        key = torch.randn((Hkv, n, d), generator=g2, device=dev).bfloat16()
+        val = torch.randn((Hkv, n, d), generator=g2, device=dev).bfloat16()
+        wk, wv = (torch.randn((Hkv, 68, d), generator=g2, device=dev).bfloat16() for _ in range(2))
+        dk, dv = (torch.randn((300, Hkv, d), generator=g2, device=dev).bfloat16() for _ in range(2))
+        for ctx in ctxs:
+            ctx.attn_fill(1, b, key, val, key.norm(p=2, dim=-1).float())
+            ctx.lsh_build(1, b, ctx.hash_keys(key))
+            ctx.window_fill(1, b, torch.zeros((Hkv, d), dtype=torch.bfloat16, device=dev), wk, wv)
+            ctx.dense_fill(0, b, dk, dv, 300)
+    q = torch.randn((B, T, Hq, d), generator=g, device=dev).bfloat16()
+    k, v = (torch.randn((B, T, Hkv, d), generator=g, device=dev).bfloat16() for _ in range(2))
+    tree, ref = ctxs
+
+    def root_path(t):
+        p = [t]
+        while parents[p[-1]] >= 0:
+            p.append(parents[p[-1]])
+        return p[::-1]
+
+    tree.plan(T, parents=torch.tensor([parents] * B, dtype=torch.int32, device=dev))
+    tree.decode_tokens(1, T, q, k, v)
+    o_s = tree.last_out_f32().reshape(B, T, Hq, d).clone()
+    tree.dense_decode_tokens(0, T, q, k, v)
+    o_d = tree.last_out_f32().reshape(B, T, Hq, d).clone()
+    tree.accept(torch.tensor([path + [0] * (T - len(path))] * B, dtype=torch.int32, device=dev),
+                torch.full((B,), len(path), dtype=torch.int32, device=dev))
+    for t in range(T):
+        p = root_path(t)
+        ref.plan(len(p))
+        ref.decode_tokens(1, len(p), q[:, p].contiguous(), k[:, p].contiguous(), v[:, p].contiguous())
+        r_s = ref.last_out_f32().reshape(B, len(p), Hq, d)[:, -1]
+        ref.dense_decode_tokens(0, len(p), q[:, p].contiguous(), k[:, p].contiguous(), v[:, p].contiguous())
+        r_d = ref.last_out_f32().reshape(B, len(p), Hq, d)[:, -1]
+        ref.rewind(torch.full((B,), 0 if p == path else len(p), dtype=torch.int32, device=dev))
+        for a, r in ((o_s[:, t], r_s), (o_d[:, t], r_d)):
+            assert float((a - r).abs().max()) <= 1e-5 * float(r.abs().max()), f"node {t} differs from its path's chain step"
+    q1 = torch.randn((B, 1, Hq, d), generator=g, device=dev).bfloat16()
+    k1, v1 = (torch.randn((B, 1, Hkv, d), generator=g, device=dev).bfloat16() for _ in range(2))
+    outs = []
+    for ctx in ctxs:
+        ctx.plan(1)
+        outs.append(ctx.decode_tokens(1, 1, q1, k1, v1).clone())
+        outs.append(ctx.dense_decode_tokens(0, 1, q1, k1, v1).clone())
+    assert torch.equal(outs[0], outs[2]) and torch.equal(outs[1], outs[3]), "state after accept differs from the path's chain"
+    assert tree.error_flags() == 0
+    torch.cuda.synchronize()
+    print(f"tree B={B} Hq={Hq} Hkv={Hkv} n={n} T={T}: ok")
+
+
 if __name__ == "__main__":
-    which = sys.argv[1:] or ["stages", "dense", "decode", "hostpeer", "spill", "tokens"]
+    which = sys.argv[1:] or ["stages", "dense", "decode", "hostpeer", "spill", "tokens", "tree"]
+    if "tree" in which:
+        tree_case(2, 4, 1, 800, 6, 24, [-1, 0, 0, 1, 1, 2], [0, 2, 5])   # clusters of 8 per node, dense T*G = 24 (two m-tiles)
     if "tokens" in which:
         tokens_case(2, 4, 1, 800, 6, 24, 3)              # clusters of 8 per virtual head, dense T*G = 12
         tokens_case(4, 32, 8, 400, 6, 24, 2)             # one CTA per virtual head (codes from the SimHash kernel), dense T*G = 8

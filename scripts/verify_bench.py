@@ -10,6 +10,11 @@ and, in the same process, the captured single-token step() that bench.py measure
 kernel and the algorithmic bytes of one step (weights, dense-layer KV records, the sparse layers' window + sampled records, counted
 from the nnz of an eager pass).  Sparse bytes grow with T; weights and dense KV do not.  step_T / step_1 (model) is the acceptance
 length a speculative loop needs to break even.  Prints one JSON line; --out also writes it to a file.
+
+--trees adds token-tree steps (plan_tree(T) -> layers -> accept(count = 0), so the lengths stay put) for a chain of 4 and of 8
+nodes, a binary tree of depth 3 (T = 7) and a star of 1 + 7 nodes (T = 8), with the same attention / model fields as the chain
+lines, plus the accept kernel alone (torch.profiler over graph replays) with a path of 7 nodes that moves 6 rows per layer and
+kv-head, and with count = 0.
 """
 import argparse
 import json
@@ -71,6 +76,7 @@ def main():
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--out", default=None)
+    ap.add_argument("--trees", action="store_true", help="also time token-tree steps and the accept kernel")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("verify_bench.py measures on the GPU; no CUDA device found")
@@ -78,7 +84,7 @@ def main():
     dev = "cuda:0"
     sh = LLAMA31_8B
     runner = LlamaDecodeRunner(sh, args.K, args.L, args.B, args.M, device=dev, seed=0, generation_buffer=256,
-                               max_query_tokens=max(Ts))
+                               max_query_tokens=8 if args.trees else max(Ts))
     t0 = time.time()
     runner.synthetic_prefill(args.P, seed=100)
     prefill_s = time.time() - t0
@@ -127,22 +133,101 @@ def main():
                             bytes=dict(weights=weight_bytes, dense_kv=dense_rows * REC, sparse_window=window_rows * REC,
                                        sparse_sampled=sampled * REC),
                             sparse_sampled_rows=sampled))
+    trees = dict(per_tree=tree_lines(runner, args, g)) if args.trees else None
     # the single-token step bench.py measures, in the same process
     runner.capture()
     step1_ms = replay_ms(runner.graph, args.iters, args.reps)
+    if trees:
+        trees["accept"] = accept_lines(runner, args)   # last: it grows the lengths
     base = next((r for r in results if r["T"] == 1), None)
-    for r in results:
+    for r in results + (trees["per_tree"] if trees else []):
         if base:
             r["break_even_accepted_tokens"] = round(r["model_ms"] / base["model_ms"], 3)
     line = dict(metric="verification step ms, Llama-3.1-8B @ P=98K, K10L150", B=B, P=args.P, K=args.K, L=args.L,
                 captured_step_ms=round(step1_ms, 4), per_T=results, gpu=gpu_identity(0), prefill_s=round(prefill_s, 1),
                 timing=f"CUDA events, median of {args.reps} blocks of {args.iters} graph replays")
+    if trees:
+        line.update(trees)
     text = json.dumps(line)
     print(text)
     if args.out:
         os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
         with open(args.out, "w") as f:
             f.write(text + "\n")
+
+
+TREES = {
+    "chain4": [-1, 0, 1, 2],
+    "chain8": [-1, 0, 1, 2, 3, 4, 5, 6],
+    "binary_depth3": [-1, 0, 0, 1, 1, 2, 2],
+    "star_1+7": [-1, 0, 0, 0, 0, 0, 0, 0],
+}
+
+
+def tree_lines(runner, args, g):
+    """Tree steps with accept(count = 0): the lengths stay where they are."""
+    srv, sh, dev = runner.server, runner.shape, runner.device
+    B, Hq, Hkv, d = args.B, sh.num_attention_heads, sh.num_key_value_heads, sh.head_dim
+    nl = runner.n_layers
+    nodes0 = torch.zeros((B, 8), dtype=torch.int32, device=dev)
+    count0 = torch.zeros((B,), dtype=torch.int32, device=dev)
+    out = []
+    for name, pars in TREES.items():
+        T = len(pars)
+        par = torch.tensor([pars] * B, dtype=torch.int32, device=dev)
+        q = torch.randn((B, Hq, T, d), generator=g, device=dev).bfloat16()
+        k = torch.randn((B, Hkv, T, d), generator=g, device=dev).bfloat16()
+        v = torch.randn((B, Hkv, T, d), generator=g, device=dev).bfloat16()
+        nodes = nodes0[:, :T].contiguous()
+
+        def attention(T=T, par=par, q=q, k=k, v=v, nodes=nodes):
+            srv.plan(T, parents=par)
+            for li in range(nl):
+                srv.decode(q, k, v, li)
+            srv.accept(nodes, count0)
+
+        ga = capture(attention)
+        att_ms = replay_ms(ga, args.iters, args.reps)
+        del ga
+        runner.ids_tok.random_(0, sh.vocab_size, generator=g)
+        gm = capture(lambda T=T, par=par, nodes=nodes: runner.step_tree(T, par, nodes, count0))
+        model_ms = replay_ms(gm, args.iters, args.reps)
+        del gm
+        out.append(dict(tree=name, T=T, parents=pars, attention_ms=round(att_ms, 4), model_ms=round(model_ms, 4),
+                        cluster_waves=srv.ctx.get_info("tokens_cluster_waves")))
+    return out
+
+
+def accept_lines(runner, args):
+    """The accept kernel alone, from profiled graph replays of plan_tree(8) -> accept.  The moving path grows the lengths by 7 per
+    replay, so this runs after every other measurement."""
+    srv, sh, dev = runner.server, runner.shape, runner.device
+    B, Hkv = args.B, sh.num_key_value_heads
+    # the accept kernel alone: a comb tree whose path of 7 nodes moves 6 rows per (layer, request, kv-head), and count = 0
+    comb = torch.tensor([[-1, 0, 0, 2, 3, 4, 5, 6]] * B, dtype=torch.int32, device=dev)
+    path = torch.tensor([[0, 2, 3, 4, 5, 6, 7, 0]] * B, dtype=torch.int32, device=dev)
+    accept = {}
+    for label, cnt in (("path7_moves6", 7), ("count0", 0)):
+        count = torch.full((B,), cnt, dtype=torch.int32, device=dev)
+        srv.plan(8, parents=comb)
+        srv.accept(path, count)   # eager warm-up
+        gr = torch.cuda.CUDAGraph()
+        s = torch.cuda.Stream()
+        s.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(s), torch.cuda.graph(gr, stream=s):
+            srv.plan(8, parents=comb)
+            srv.accept(path, count)
+        torch.cuda.synchronize()
+        reps = 8   # 8 x 7 rows of the 256-row generation buffer
+        with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+            for _ in range(reps):
+                gr.replay()
+            torch.cuda.synchronize()
+        us = [e.device_time_total for e in prof.events() if "accept_path_kernel" in e.name]
+        accept[label] = dict(kernel_us_median=round(statistics.median(us), 2) if us else None, samples=len(us),
+                             moved_bytes=runner.n_layers * B * Hkv * (6 if cnt else 0) * REC)
+        del gr
+    return accept
 
 
 if __name__ == "__main__":
