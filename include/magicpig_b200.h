@@ -77,6 +77,12 @@ typedef struct mpig_config {
     int32_t num_dense_layers;     /* entries used in dense_layers[] */
     int32_t dense_layers[16];     /* attnserver.py:18; tables/offload store are NOT allocated for these */
     int32_t alloc_dense_kv;       /* 1: also own the dense layers' full KV cache + dense decode kernel */
+    /* reserved[0]: 2 = plan the probing / fused clusters for two 512-thread CTAs per SM (experiment switch; otherwise one).
+     * reserved[1]: number of context slots C in [0, batch_size]; 0 means C = batch_size (every request owns its slot).  The
+     *   sampled store and the L hash tables of every sparse layer exist once per SLOT; the window, avg_k, the dense layers' KV,
+     *   the lengths and the per-step scratch stay per REQUEST.  Request b is bound to slot b mod C at creation and after
+     *   mpig_clear; mpig_fork_request / mpig_bind_request change the binding.  Requests bound to one slot decode over one copy of
+     *   the context (parallel sampling, several questions about one document). */
     int32_t reserved[8];
 } mpig_config;
 
@@ -117,7 +123,7 @@ int mpig_set_option(mpig_ctx *ctx, const char *key, int64_t value);
  * "fused_cluster_waves" (waves of thread-block clusters one fused launch takes on this device; 1 = all resident at once,
  * 0 = fused decode not applicable), "window_capacity" (sink + local + generation_buffer rows), "table_segments" (key segments S
  * of the tables, see mpig_lsh_table_ptrs), "query_tokens_max" (t_max of mpig_reserve_query_tokens, 1 without), "tokens_cluster_waves"
- * (waves of clusters the last mpig_decode_tokens launch with T > 1 took). */
+ * (waves of clusters the last mpig_decode_tokens launch with T > 1 took), "num_contexts" (context slots C, see reserved[1]). */
 int mpig_get_info(mpig_ctx *ctx, const char *key, int64_t *value);
 /* Capacity errors the DEVICE detected (the lengths saturate there): bit 0 = a sparse window is full (generation_buffer
  * exhausted: each further token overwrites the previous one's K/V), bit 1 = a dense cache reached max_length, bit 2 = mpig_rewind
@@ -135,9 +141,24 @@ int mpig_clear(mpig_ctx *ctx, void *stream);
 /* hash_func: bf16 (d, K*L) row-major, column l*K+i = bit i of table l (attnserver.py:55,268-270). */
 int mpig_set_hash_func(mpig_ctx *ctx, const void *hash_func_bf16, void *stream);
 
+/* ---- context slots (no reference equivalent; see mpig_config.reserved[1]) ------------------------------------------------------
+ * Both calls return MPIG_ESTATE when C = batch_size (the bindings are then fixed: request b reads slot b), are not capturable, and
+ * end the pending step: mpig_rewind / mpig_accept are refused (MPIG_ESTATE) until the next plan.  A step captured before either
+ * call replays with the new bindings (the kernels read the device map).
+ *
+ * Bind `dst` to the slot of `src` and make dst's per-request state a copy of src's: for every sparse layer window rows
+ * [0, win_len[src]) of every kv-head and avg_k, for every dense layer KV rows [0, dense_len[src]) of every kv-head, and both
+ * lengths (device and host mirror).  Reads the device lengths and synchronises `stream` (correct after replays of a captured
+ * plan); copy-engine calls only.  MPIG_EINVAL: src == dst or either outside [0, batch_size). */
+int mpig_fork_request(mpig_ctx *ctx, int src, int dst, void *stream);
+/* Bind `request` to `slot` (in [0, C)); its window and lengths are left alone: fill the slot (mpig_attn_fill + mpig_lsh_build /
+ * mpig_lsh_fill) and the window next.  Synchronises `stream`. */
+int mpig_bind_request(mpig_ctx *ctx, int request, int slot, void *stream);
+
 /* ---- lsh.LSH --------------------------------------------------------------------------------- */
 /* LSH::fill (lsh.cc:143-201): tables of one (layer, request) from codes already sorted per
- * (kv-head, table).  sorted_codes int16 (Hkv, L, n); sorted_indices int32 (Hkv, L, n). */
+ * (kv-head, table).  sorted_codes int16 (Hkv, L, n); sorted_indices int32 (Hkv, L, n).  The tables are those of the slot `request`
+ * is bound to (as for mpig_lsh_build and mpig_attn_fill): the fill changes the context of every request bound to that slot. */
 int mpig_lsh_fill(mpig_ctx *ctx, int layer, int request, const int16_t *sorted_codes,
                   const int32_t *sorted_indices, int n, void *stream);
 /* Key-side SimHash (attnserver.py:159-168): codes int16 (Hkv, L, n) of keys bf16 (Hkv, n, d) [already centred], with the
@@ -158,8 +179,9 @@ int mpig_lsh_get_mask(mpig_ctx *ctx, uint8_t *mask_out, void *stream);
  * Diagnostic used by the parity tests (library/lsh/test.py:43 computes the same sum). */
 int mpig_lsh_collision_counts(mpig_ctx *ctx, int layer, const int32_t *query, int32_t *counts, void *stream);
 /* raw views for tests.  Segmented compact CSR: keys are cut into S = ceil(max_length / 65536) segments of equal length
- * seg_len = ceil(max_length / S) rounded up to 64; offsets int32 (B, Hkv, L, S, NB+1) = absolute bucket starts inside the item
- * row, items uint16 (B, Hkv, L, M) = key index - seg_len * segment, segment s occupying [s * seg_len, ...) of its row. */
+ * seg_len = ceil(max_length / S) rounded up to 64; offsets int32 (C, Hkv, L, S, NB+1) = absolute bucket starts inside the item
+ * row, items uint16 (C, Hkv, L, M) = key index - seg_len * segment, segment s occupying [s * seg_len, ...) of its row (C context
+ * slots, the leading dimension). */
 int mpig_lsh_table_ptrs(mpig_ctx *ctx, int layer, const int32_t **offsets, const uint16_t **items);
 
 /* ---- sparse_attention_cpu.SparseAttentionServer ---------------------------------------------- */
@@ -175,7 +197,8 @@ int mpig_attention_wrapper(mpig_ctx *ctx, int layer, int K, int L, void *output_
                            const void *query_bf16, const float *query_norm, const int32_t *ind,
                            const int32_t *nnz, void *stream);
 /* get_key_cache / get_value_cache / get_key_norm (sparse_attention.cc:1213-1234), copied out
- * of the interleaved HBM layout: k, v bf16 (B, Hkv, M, d) and/or kn fp32 (B, Hkv, M); NULL skips. */
+ * of the interleaved HBM layout: k, v bf16 (C, Hkv, M, d) and/or kn fp32 (C, Hkv, M), one entry per context slot (C = B unless
+ * reserved[1] says otherwise; request b's store is entry slot-of-b); NULL skips. */
 int mpig_attn_read_cache(mpig_ctx *ctx, int layer, void *k_bf16, void *v_bf16, float *kn, void *stream);
 
 /* ---- the GPU-side glue of LSHSparseAttnServer.decode ------------------------------------------ */
@@ -198,8 +221,11 @@ int mpig_plan(mpig_ctx *ctx, void *stream);
  * P + g tokens would have, centred with the prefill's mean key.  spilled_out int32 [B] (host, may be NULL) receives g_b.
  * Reads the device window lengths (synchronises `stream`), so it is correct after eager plan() calls and after replays of a
  * captured step alike.  Not capturable.  A decode step captured before a spill stays valid after it.  Dense layers are
- * untouched.  MPIG_EINVAL: keep < 0 or sink + keep >= window capacity; MPIG_ESTATE: n_old + g_b > max_length for some sparse
- * layer, or no hash_func set.  On these errors nothing is modified. */
+ * untouched.  The spilled keys go into the store and tables of the request's slot, so a request with g_b > 0 must be alone on its
+ * slot among requests with a non-empty window: a request that shares its context generates at most generation_buffer tokens.
+ * MPIG_EINVAL: keep < 0 or sink + keep >= window capacity; MPIG_ESTATE: n_old + g_b > max_length for some sparse layer, a
+ * spilling request shares its slot with another request whose window is not empty, or no hash_func set.  On these errors
+ * nothing is modified. */
 int mpig_spill_window(mpig_ctx *ctx, int keep, int32_t *spilled_out, void *stream);
 /* Fused sparse-layer decode (attnserver.py:261-312): centre + append the new key/value to the
  * window, SimHash, probe, gather attention over window + sample with the LSE merge folded in -- one kernel launch.

@@ -41,7 +41,8 @@ class LSHSparseAttnServer:
                  key_hash: str = "tcgen05",
                  num_key_value_heads: Optional[int] = None,
                  num_attention_heads: Optional[int] = None,
-                 max_query_tokens: int = 1) -> None:
+                 max_query_tokens: int = 1,
+                 num_contexts: Optional[int] = None) -> None:
         """Keywords up to `dtype` are the reference's (attnserver.py:9-20).  Extras:
         hash_func   inject the (d, K*L) bf16 projection (the reference draws it unseeded, :55);
         table_build "device" = counting sort on the GPU (mpig_lsh_build); "sorted" = the reference's
@@ -52,6 +53,8 @@ class LSHSparseAttnServer:
         num_*_heads per-rank head counts under KV-head tensor parallelism (attnserver_dist.py:252-254);
         max_query_tokens  largest number of draft tokens a verification step may check (plan(num_tokens), decode of q_len > 1,
                     rewind); 1 = single-token decoding only.
+        num_contexts number of contexts (sampled stores + hash tables) the batch holds, 1..batch_size; None = batch_size.
+                    Request b starts on context b mod num_contexts; fork() and bind() change that.
         """
         self.K, self.L = K, L
         self.config = config
@@ -78,7 +81,7 @@ class LSHSparseAttnServer:
         self.ctx = Context(K, L, self.num_layers, self.num_attention_heads, self.num_key_value_heads, self.head_dim,
                            batch_size, max_length, num_sink_tokens, num_local_tokens, generation_buffer,
                            dense_layers=self.dense_layers, alloc_dense_kv=True, device=self.device,
-                           max_query_tokens=max_query_tokens)
+                           max_query_tokens=max_query_tokens, num_contexts=num_contexts or 0)
         if hash_func is None:
             hash_func = torch.randn((self.head_dim, K * L), device=self.device, dtype=torch.bfloat16)  # attnserver.py:55
         self.hash_func = hash_func.to(device=self.device, dtype=torch.bfloat16).contiguous()
@@ -137,6 +140,22 @@ class LSHSparseAttnServer:
             self.ctx.lsh_fill(layer_idx, request_id, sorted_codes.contiguous(), sorted_idx.int().contiguous())
         else:
             self.ctx.lsh_build(layer_idx, request_id, codes.contiguous())
+
+    def fork(self, src_request: int, dst_requests):
+        """Not in the reference.  Each request of dst_requests (an int or a sequence) continues from src_request's state: it
+        decodes over src_request's context (no copy of the sampled store or the tables) and gets a copy of its sink + local +
+        generated window, its dense-layer KV and its lengths.  The usual way to serve n answers to one prompt, or several
+        questions about one document: fill and build one request, then fork it.  Requests sharing a context generate at most
+        generation_buffer tokens (spill_window() refuses them).  Needs num_contexts < batch_size."""
+        for dst in ([dst_requests] if isinstance(dst_requests, int) else dst_requests):
+            self.ctx.fork(src_request, dst)
+            for a in self.avg_k:
+                a[dst].copy_(a[src_request])
+
+    def bind(self, request: int, context: int):
+        """Not in the reference.  Bind `request` to context slot `context` (0 <= context < num_contexts); fill() and
+        build_table() of the request then write that context, which every request bound to it reads."""
+        self.ctx.bind(request, context)
 
     def plan(self, num_tokens: int = 1, parents=None):
         """attnserver.py:196-224.  num_tokens > 1: a verification step of that many tokens per request (the decode calls of the

@@ -207,6 +207,7 @@ __global__ void __launch_bounds__(384, 1) attend_mma_kernel(const __grid_constan
         const int c_h = (T + w_h - 1) / w_h;
         const int r_lo = part * c_h, r_hi = min(r_lo + c_h, T);  // rows of this part inside the head's list
         const int g = ch / p.G;
+        const int sg = p.slot_of ? p.slot_of[ch / p.Hq] * (p.Hq / p.G) + (ch % p.Hq) / p.G : g;   // slot group of the sampled rows
         const int wlen = s_wlen[ch / p.Hq];
 
         DBG_STAMP_DEP(12, wlen);  // head / part resolved
@@ -242,10 +243,10 @@ __global__ void __launch_bounds__(384, 1) attend_mma_kernel(const __grid_constan
                     DBG_STAMP_DEP(15, (int)(size_t)ip);  // address ready
                     idx = __ldg(ip);
                     idx = min(max(idx, 0), p.M - 1);
-                    src = p.kv + ((size_t)g * p.M + idx) * REC;
+                    src = p.kv + ((size_t)sg * p.M + idx) * REC;
                 }
                 if (USE_TMA && do_fetch) bulk_g2s(slots + (size_t)lane * SLOT, src, REC, bar);
-                if (idx >= 0) meta = __ldg(p.kn + (size_t)g * p.M + idx);  // consumed in phase B: overlaps the row fetch
+                if (idx >= 0) meta = __ldg(p.kn + (size_t)sg * p.M + idx);  // consumed in phase B: overlaps the row fetch
             }
             if (!USE_TMA && do_fetch) {
                 const unsigned long long sp64 = (unsigned long long)src;

@@ -1,14 +1,15 @@
 // common.cuh -- context layout, error plumbing and PTX wrappers shared by the sm_90a kernels.
 //
-// HBM layout owned by a context (all per SPARSE layer unless noted; B requests, Hkv kv-heads,
-// M = max_length rows of capacity, d = head_dim, REC = 2*d bf16 = 512 B at d = 128):
+// HBM layout owned by a context (all per SPARSE layer unless noted; B requests, C context slots (mpig_config.reserved[1], 0 = B),
+// Hkv kv-heads, M = max_length rows of capacity, d = head_dim, REC = 2*d bf16 = 512 B at d = 128).  The sampled store and the
+// tables are per SLOT; request b reads slot slot_of[b] (slot group slot_of[b]*Hkv + h/G), its window and lengths are its own:
 //
-//   kv      [B][Hkv][M]      REC-byte records  { K row (d bf16) | V row (d bf16) }   one index -> one burst
-//   kn      [B][Hkv][M]      fp32 key norms (as given to fill; reference sparse_attention.h:45)
-//   offsets [B][Hkv][L][S][NB+1] int32 per-segment CSR bucket starts, absolute positions in the table's item row
+//   kv      [C][Hkv][M]      REC-byte records  { K row (d bf16) | V row (d bf16) }   one index -> one burst
+//   kn      [C][Hkv][M]      fp32 key norms (as given to fill; reference sparse_attention.h:45)
+//   offsets [C][Hkv][L][S][NB+1] int32 per-segment CSR bucket starts, absolute positions in the table's item row
 //                            (replaces table_start/table_end, lsh.h:38-39); S = nseg equal key segments of seg_len <= 65536
 //                            keys, sized to the probing cluster (DESIGN.md section 2)
-//   items   [B][Hkv][L][M]   uint16 key index - seg_len * segment, segment-major, then grouped by bucket (lsh.h:40 keeps int32)
+//   items   [C][Hkv][L][M]   uint16 key index - seg_len * segment, segment-major, then grouped by bucket (lsh.h:40 keeps int32)
 //   win     [B][Hkv][Wcap]   REC-byte records of the sink+local+generated window (keys centred)
 //   avg_k   [B][Hkv][d]      bf16 mean offloaded key (attnserver.py:142-148)
 //   dense   [B][Hkv][M]      REC-byte records (dense layers, only with alloc_dense_kv)
@@ -75,7 +76,7 @@ struct LayerStore {
     uint8_t *kv = nullptr;       // sparse: offloaded records
     float *kn = nullptr;
     int32_t *offsets = nullptr;
-    int32_t *items = nullptr;    // storage of the uint16 item rows [BG][L][M]
+    int32_t *items = nullptr;    // storage of the uint16 item rows [C*Hkv][L][M]
     uint8_t *win = nullptr;      // window records
     __nv_bfloat16 *avg_k = nullptr;
     uint8_t *dense_kv = nullptr; // dense: full-context records
@@ -109,7 +110,15 @@ struct mpig_ctx {
     int cta_per_sm = 1;    // probing / fused CTAs per SM the geometry is planned for (mpig_config.reserved[0] == 2 -> 2)
     int max_cluster = 8;   // largest probing / fused cluster whose B*Hq copies are all resident at once (mpig_create)
     std::vector<mpig::LayerStore> layers;
-    std::vector<std::vector<int>> n_off;  // [layer][request] offloaded key count (host bookkeeping)
+    std::vector<std::vector<int>> n_off;  // [layer][slot] offloaded key count (host bookkeeping)
+    // context slots: the sampled store and the tables exist once per slot, request b reads slot slot_of[b].  The device map is
+    // allocated at create time and never moves (a captured step reads the bindings of the replay); h_slot_of mirrors it.  Only
+    // copy-engine calls (mpig_clear, mpig_fork_request, mpig_bind_request) write it, never a kernel.
+    int C = 0;                            // number of slots (1..B)
+    int32_t *slot_of = nullptr;           // [B]
+    std::vector<int> h_slot_of;           // [B]
+    // the map the kernels get: null while every request owns its slot (C = B, bindings fixed), so that path addresses b itself
+    const int32_t *slot_map() const { return C < cfg.batch_size ? slot_of : nullptr; }
     // global state
     __nv_bfloat16 *hash_func = nullptr;   // (d, K*L) as given
     __nv_bfloat16 *hash_func_t = nullptr; // (K*L, d) transposed copy: K-major B operand for the SimHash GEMM
@@ -317,8 +326,9 @@ struct AppendParams {
 };
 
 struct AttendParams {
-    const uint8_t *kv;        // [BG][M] records           (sparse store; may be null if no sampled rows)
-    const float *kn;          // [BG][M]
+    const uint8_t *kv;        // [C*Hkv][M] records        (sparse store; may be null if no sampled rows)
+    const float *kn;          // [C*Hkv][M]
+    const int32_t *slot_of;   // [B] slot of each request, or null: request b reads slot b
     const uint8_t *win;       // [BG][Wcap] records         (null -> no window rows)
     const int32_t *win_len;   // [B]
     const int32_t *ind;       // [H][M]

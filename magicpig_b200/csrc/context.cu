@@ -93,6 +93,8 @@ int mpig_create(const mpig_config *cfg, mpig_ctx **out) {
     MPIG_REQUIRE(cfg->num_dense_layers >= 0 && cfg->num_dense_layers <= 16, MPIG_EINVAL, "mpig_create: num_dense_layers");
     MPIG_REQUIRE(cfg->num_sink_tokens >= 0 && cfg->num_local_tokens >= 0 && cfg->generation_buffer >= 0, MPIG_EINVAL,
                  "mpig_create: negative window size");
+    MPIG_REQUIRE(cfg->reserved[1] >= 0 && cfg->reserved[1] <= cfg->batch_size, MPIG_EINVAL,
+                 "mpig_create: num_contexts (reserved[1]) = %d outside [0, batch_size = %d]", cfg->reserved[1], cfg->batch_size);
     struct RestoreDevice {
         int prev = -1;
         RestoreDevice() { if (cudaGetDevice(&prev) != cudaSuccess) prev = -1; }
@@ -143,9 +145,13 @@ int mpig_create(const mpig_config *cfg, mpig_ctx **out) {
     ctx->max_cluster = ctx_max_cluster;
     ctx->bitmap_words = (cfg->max_length + 31) / 32;
     ctx->layers.resize(cfg->num_layers);
-    ctx->n_off.assign(cfg->num_layers, std::vector<int>(cfg->batch_size, 0));
+    ctx->C = cfg->reserved[1] > 0 ? cfg->reserved[1] : cfg->batch_size;
+    ctx->n_off.assign(cfg->num_layers, std::vector<int>(ctx->C, 0));
+    ctx->h_slot_of.resize(cfg->batch_size);
+    for (int b = 0; b < cfg->batch_size; ++b) ctx->h_slot_of[b] = b % ctx->C;
 
     const size_t M = (size_t)cfg->max_length, BG = (size_t)ctx->BG, L = (size_t)cfg->L, d = (size_t)cfg->head_dim;
+    const size_t SG = (size_t)ctx->C * cfg->num_key_value_heads;   // slot groups: the store and the tables are per slot
     int rc = MPIG_OK;
 #define TRY(x)                   \
     do {                         \
@@ -166,10 +172,10 @@ int mpig_create(const mpig_config *cfg, mpig_ctx **out) {
         }
         ls.sparse = true;
         // zero-initialised like the reference's caches (sparse_attention.cc:563-581): an index >= n reads zeros, not garbage
-        TRY(dev_alloc(ctx, &ls.kv, BG * M * ctx->rec_bytes, true));
-        TRY(dev_alloc(ctx, &ls.kn, BG * M * sizeof(float), true));
-        TRY(dev_alloc(ctx, &ls.offsets, BG * L * ctx->nseg * (size_t)(ctx->NB + 1) * sizeof(int32_t), true));
-        TRY(dev_alloc(ctx, &ls.items, ((BG * L * M * sizeof(uint16_t) + 15) & ~(size_t)15), false));
+        TRY(dev_alloc(ctx, &ls.kv, SG * M * ctx->rec_bytes, true));
+        TRY(dev_alloc(ctx, &ls.kn, SG * M * sizeof(float), true));
+        TRY(dev_alloc(ctx, &ls.offsets, SG * L * ctx->nseg * (size_t)(ctx->NB + 1) * sizeof(int32_t), true));
+        TRY(dev_alloc(ctx, &ls.items, ((SG * L * M * sizeof(uint16_t) + 15) & ~(size_t)15), false));
         TRY(dev_alloc(ctx, &ls.win, BG * (size_t)(ctx->Wcap > 0 ? ctx->Wcap : 1) * ctx->rec_bytes, true));
         TRY(dev_alloc(ctx, &ls.avg_k, BG * d * sizeof(__nv_bfloat16), true));
     }
@@ -178,6 +184,16 @@ int mpig_create(const mpig_config *cfg, mpig_ctx **out) {
     TRY(dev_alloc(ctx, &ctx->hash_func_t, d * cfg->K * L * sizeof(__nv_bfloat16)));
     TRY(dev_alloc(ctx, &ctx->win_len, (size_t)cfg->batch_size * sizeof(int32_t)));
     TRY(dev_alloc(ctx, &ctx->dense_len, (size_t)cfg->batch_size * sizeof(int32_t)));
+    TRY(dev_alloc(ctx, &ctx->slot_of, (size_t)cfg->batch_size * sizeof(int32_t)));
+    {
+        const cudaError_t e = cudaMemcpy(ctx->slot_of, ctx->h_slot_of.data(), (size_t)cfg->batch_size * sizeof(int32_t),
+                                         cudaMemcpyHostToDevice);
+        if (e != cudaSuccess) {
+            set_error("mpig_create: slot map upload failed: %s", cudaGetErrorString(e));
+            mpig_destroy(ctx);
+            return MPIG_ECUDA;
+        }
+    }
     TRY(dev_alloc(ctx, &ctx->codes, H * L * sizeof(int32_t)));
     TRY(dev_alloc(ctx, &ctx->qnorm, H * sizeof(float)));
     TRY(dev_alloc(ctx, &ctx->results, H * M * sizeof(int32_t)));
@@ -244,6 +260,7 @@ void mpig_destroy(mpig_ctx *ctx) {
     cudaFree(ctx->hash_func_t);
     cudaFree(ctx->win_len);
     cudaFree(ctx->dense_len);
+    cudaFree(ctx->slot_of);
     cudaFree(ctx->codes);
     cudaFree(ctx->qnorm);
     cudaFree(ctx->results);
@@ -274,12 +291,12 @@ int mpig_clear(mpig_ctx *ctx, void *stream) {
     mpig::DeviceGuard _dg(ctx);  // run on the context's device whatever the caller's current device is
     MPIG_REQUIRE(ctx, MPIG_EINVAL, "mpig_clear: null context");
     cudaStream_t s = as_stream(stream);
-    const size_t BG = ctx->BG, L = ctx->cfg.L;
+    const size_t BG = ctx->BG, SG = (size_t)ctx->C * ctx->cfg.num_key_value_heads, L = ctx->cfg.L;
     for (int l = 0; l < ctx->cfg.num_layers; ++l) {
         LayerStore &ls = ctx->layers[l];
         if (ls.sparse) {
             // an all-zero offsets array = every bucket empty; stale items/records are unreachable
-            MPIG_CUDA(cudaMemsetAsync(ls.offsets, 0, BG * L * ctx->nseg * (size_t)(ctx->NB + 1) * sizeof(int32_t), s));
+            MPIG_CUDA(cudaMemsetAsync(ls.offsets, 0, SG * L * ctx->nseg * (size_t)(ctx->NB + 1) * sizeof(int32_t), s));
             MPIG_CUDA(cudaMemsetAsync(ls.avg_k, 0, BG * ctx->cfg.head_dim * sizeof(__nv_bfloat16), s));
         }
         for (auto &n : ctx->n_off[l]) n = 0;
@@ -294,6 +311,9 @@ int mpig_clear(mpig_ctx *ctx, void *stream) {
     MPIG_CUDA(cudaMemsetAsync(ctx->err_flag, 0, 4 * sizeof(int32_t), s));
     for (auto &n : ctx->h_win_len) n = 0;
     for (auto &n : ctx->h_dense_len) n = 0;
+    // the initial binding b -> b mod C (the host mirror is a member: it outlives the copy)
+    for (int b = 0; b < ctx->cfg.batch_size; ++b) ctx->h_slot_of[b] = b % ctx->C;
+    MPIG_CUDA(cudaMemcpyAsync(ctx->slot_of, ctx->h_slot_of.data(), ctx->cfg.batch_size * sizeof(int32_t), cudaMemcpyHostToDevice, s));
     ctx->h_len_exact = true;
     ctx->last_tokens = 1;
     ctx->pending_T = 0;     // no plan to decode, rewind or accept since the clear
@@ -457,10 +477,79 @@ int mpig_get_info(mpig_ctx *ctx, const char *key, int64_t *value) {
     else if (k == "table_segments") *value = ctx->nseg;
     else if (k == "query_tokens_max") *value = ctx->tok_max;
     else if (k == "tokens_cluster_waves") *value = ctx->last_tokens_waves;
+    else if (k == "num_contexts") *value = ctx->C;
     else {
         set_error("mpig_get_info: unknown key '%s'", key);
         return MPIG_EINVAL;
     }
+    return MPIG_OK;
+}
+
+// shared checks of mpig_fork_request / mpig_bind_request
+static int binding_checks(mpig_ctx *ctx, int request, const char *who) {
+    MPIG_REQUIRE(ctx, MPIG_EINVAL, "%s: null context", who);
+    MPIG_REQUIRE(request >= 0 && request < ctx->cfg.batch_size, MPIG_EINVAL, "%s: request %d out of range [0, %d)", who, request,
+                 ctx->cfg.batch_size);
+    MPIG_REQUIRE(ctx->C < ctx->cfg.batch_size, MPIG_ESTATE,
+                 "%s: every request owns its context slot (num_contexts = batch_size); create the context with fewer slots to share one",
+                 who);
+    return MPIG_OK;
+}
+
+static int upload_slot_map(mpig_ctx *ctx, cudaStream_t s) {
+    MPIG_CUDA(cudaMemcpyAsync(ctx->slot_of, ctx->h_slot_of.data(), ctx->cfg.batch_size * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    MPIG_CUDA(cudaStreamSynchronize(s));
+    return MPIG_OK;
+}
+
+int mpig_fork_request(mpig_ctx *ctx, int src, int dst, void *stream) {
+    mpig::DeviceGuard _dg(ctx);
+    int rc = binding_checks(ctx, src, "mpig_fork_request");
+    if (rc) return rc;
+    rc = binding_checks(ctx, dst, "mpig_fork_request");
+    if (rc) return rc;
+    MPIG_REQUIRE(src != dst, MPIG_EINVAL, "mpig_fork_request: src == dst (%d)", src);
+    cudaStream_t s = as_stream(stream);
+    // the device lengths are the truth (replays of a captured plan() advance only them)
+    int32_t len[2] = {0, 0};
+    MPIG_CUDA(cudaMemcpyAsync(&len[0], ctx->win_len + src, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    MPIG_CUDA(cudaMemcpyAsync(&len[1], ctx->dense_len + src, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    MPIG_CUDA(cudaStreamSynchronize(s));
+    const size_t Hkv = ctx->cfg.num_key_value_heads, REC = ctx->rec_bytes;
+    for (const LayerStore &ls : ctx->layers) {
+        if (ls.sparse) {
+            const size_t pitch = (size_t)ctx->Wcap * REC;   // one kv-head's window
+            if (len[0] > 0)
+                MPIG_CUDA(cudaMemcpy2DAsync(ls.win + dst * Hkv * pitch, pitch, ls.win + src * Hkv * pitch, pitch, (size_t)len[0] * REC,
+                                            Hkv, cudaMemcpyDeviceToDevice, s));
+            const size_t avg = Hkv * ctx->cfg.head_dim;
+            MPIG_CUDA(cudaMemcpyAsync(ls.avg_k + dst * avg, ls.avg_k + src * avg, avg * sizeof(__nv_bfloat16), cudaMemcpyDeviceToDevice, s));
+        } else if (ls.dense_kv && len[1] > 0) {
+            const size_t pitch = (size_t)ctx->cfg.max_length * REC;   // one kv-head's cache
+            MPIG_CUDA(cudaMemcpy2DAsync(ls.dense_kv + dst * Hkv * pitch, pitch, ls.dense_kv + src * Hkv * pitch, pitch,
+                                        (size_t)len[1] * REC, Hkv, cudaMemcpyDeviceToDevice, s));
+        }
+    }
+    MPIG_CUDA(cudaMemcpyAsync(ctx->win_len + dst, ctx->win_len + src, sizeof(int32_t), cudaMemcpyDeviceToDevice, s));
+    MPIG_CUDA(cudaMemcpyAsync(ctx->dense_len + dst, ctx->dense_len + src, sizeof(int32_t), cudaMemcpyDeviceToDevice, s));
+    ctx->h_win_len[dst] = len[0];
+    ctx->h_dense_len[dst] = len[1];
+    ctx->h_slot_of[dst] = ctx->h_slot_of[src];
+    rc = upload_slot_map(ctx, s);
+    if (rc) return rc;
+    ctx->rewound = true;   // the pending step ends: its bases are stale for dst
+    return MPIG_OK;
+}
+
+int mpig_bind_request(mpig_ctx *ctx, int request, int slot, void *stream) {
+    mpig::DeviceGuard _dg(ctx);
+    int rc = binding_checks(ctx, request, "mpig_bind_request");
+    if (rc) return rc;
+    MPIG_REQUIRE(slot >= 0 && slot < ctx->C, MPIG_EINVAL, "mpig_bind_request: slot %d out of range [0, %d)", slot, ctx->C);
+    ctx->h_slot_of[request] = slot;
+    rc = upload_slot_map(ctx, as_stream(stream));
+    if (rc) return rc;
+    ctx->rewound = true;
     return MPIG_OK;
 }
 

@@ -39,6 +39,7 @@ static int decode_sparse(mpig_ctx *ctx, int layer, const void *q, const void *k,
     AttendParams p = {};
     p.kv = ls.kv;
     p.kn = ls.kn;
+    p.slot_of = ctx->slot_map();
     p.win = ls.win;
     p.win_len = ctx->win_len;
     p.ind = ctx->results;

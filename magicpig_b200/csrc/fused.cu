@@ -162,9 +162,12 @@ __device__ __forceinline__ int block_exclusive_scan_redux(int v, int *wtot, int 
 // no in-kernel row build.  Of the step's rows the token sees those whose bit is set in its ancestor mask (gp.anc[b*T + t]; a chain
 // sets bits 0..t, so nothing is masked): the other rows score -inf.  `anc` is a kernel argument of its own (null for the
 // single-token instantiations) so that FusedParams, and with it their code, stays as it is.
+// slot_of (B), or null: the tables, records and key norms are those of slot group slot_of[b]*Hkv + h/G (context slots shared by
+// several requests); the window, k_new and avg_k stay those of group b*Hkv + h/G.  Null reads group b*Hkv + h/G for both.
 template <typename TagT, int THREADS, bool DBG, bool KREG, bool TOK = false>
 __global__ void __launch_bounds__(THREADS, (THREADS == 1024) ? 1 : 2) fused_decode_kernel(const __grid_constant__ FusedParams gp,
-                                                                                                   const int32_t *__restrict__ anc) {
+                                                                                                   const int32_t *__restrict__ anc,
+                                                                                                   const int32_t *__restrict__ slot_of) {
     extern __shared__ __align__(128) uint8_t smem_raw[];
     __shared__ FusedParams p_s;   // parameters staged once (constant-bank misses were microseconds on the critical path)
     {
@@ -189,6 +192,9 @@ __global__ void __launch_bounds__(THREADS, (THREADS == 1024) ? 1 : 2) fused_deco
         }
         s_geo[3] = (int)c_ / gp.r;
         s_geo[4] = ((int)c_ % gp.r) * gp.Mc;
+        // slot group.  Read before griddepcontrol.wait: only copy-engine calls write the map (never a kernel), and a kernel starts
+        // after every copy ordered before it in the stream has completed (PDL overlaps a kernel with a preceding kernel only)
+        s_geo[6] = slot_of ? __ldg(slot_of + s_geo[2]) * (gp.Hq / gp.G) + (h_ % gp.Hq) / gp.G : s_geo[1];
     }
     unsigned long long t_dbg[12];
     if (DBG) {
@@ -202,7 +208,10 @@ __global__ void __launch_bounds__(THREADS, (THREADS == 1024) ? 1 : 2) fused_deco
     constexpr TagT EMPTY = (TagT)(SEL - 1);
     constexpr int NWARPS = THREADS / 32;
     const unsigned C = cluster_nctarank(), c = cluster_ctarank();
-    const int h = s_geo[0], g = s_geo[1], bq = s_geo[2];
+    const int h = s_geo[0], g = s_geo[1], bq = s_geo[2];   // g: the group of the window and the new row
+    // the slot group of the tables, records and key norms, re-read from shared memory where it is used (volatile: a value kept
+    // live across the kernel would add spills at the 64-register cap)
+    auto slot_group = [&]() -> size_t { return (size_t)*reinterpret_cast<volatile int *>(&s_geo[6]); };
     const int tid = threadIdx.x, lane = tid & 31;
     const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);   // the same value, but provably warp-uniform (uniform datapath: tile loop, request issue)
     constexpr int F_KEEP = FKeep<THREADS>::value;
@@ -370,7 +379,7 @@ __global__ void __launch_bounds__(THREADS, (THREADS == 1024) ? 1 : 2) fused_deco
                 const int code = s_codes[t];
                 int s = 0, e = 0;
                 if (seg_ok && code >= 0 && code < NB) {
-                    const int32_t *o = p.offsets + (((size_t)g * L + t) * S + seg) * (size_t)(NB + 1) + code;
+                    const int32_t *o = p.offsets + ((slot_group() * L + t) * S + seg) * (size_t)(NB + 1) + code;
                     s = __ldg(o);
                     e = __ldg(o + 1);
                 }
@@ -406,7 +415,7 @@ __global__ void __launch_bounds__(THREADS, (THREADS == 1024) ? 1 : 2) fused_deco
     }
     if (DBG) t_dbg[3] = clk64();
     {
-        const uint16_t *items_g = p.items + (size_t)g * L * (size_t)M;
+        const uint16_t *items_g = p.items + slot_group() * L * (size_t)M;
         const int nch = total_chunks;
         // record of chunk ch: from the array, or -- for pathologically long candidate streams -- rebuilt from the per-table data
         auto chunk_rec = [&](int ch) -> int2 {
@@ -636,12 +645,12 @@ __global__ void __launch_bounds__(THREADS, (THREADS == 1024) ? 1 : 2) fused_deco
                     auto rec_of = [&](int rr_) -> const uint8_t * {
                         const int r_ = (rr_ < nrows) ? rr_ : 0;
                         if (is_win) return p.win + ((size_t)g * p.Wcap + row0 + r_) * REC;
-                        return p.kv + ((size_t)g * M + (lo_key + (int)s_sel[row0 + r_])) * REC;
+                        return p.kv + (slot_group() * M + (lo_key + (int)s_sel[row0 + r_])) * REC;
                     };
                     if (lane < nrows) {
                         const uint8_t *rec = rec_of(lane);
                         if (lane != new_lane) bulk_g2s(slots + (size_t)lane * VSLOT, rec + D * 2, VSLOT, bar);
-                        if (!is_win) meta = __ldg(p.kn + (size_t)g * M + (lo_key + (int)s_sel[row0 + lane]));
+                        if (!is_win) meta = __ldg(p.kn + slot_group() * M + (lo_key + (int)s_sel[row0 + lane]));
                     }
                     // lane (grp, tig): 16 B = 8 consecutive k of rows grp and grp+8 per 32-k block (4 blocks): all 8 loads in flight
                     uint4 ka[4], kb[4];
@@ -711,8 +720,8 @@ __global__ void __launch_bounds__(THREADS, (THREADS == 1024) ? 1 : 2) fused_deco
                         src = p.win + ((size_t)g * p.Wcap + row0 + lane) * REC;
                     } else {
                         const int idx = lo_key + (int)s_sel[row0 + lane];
-                        src = p.kv + ((size_t)g * M + idx) * REC;
-                        meta = __ldg(p.kn + (size_t)g * M + idx);   // consumed after the scores: overlaps the row fetch
+                        src = p.kv + (slot_group() * M + idx) * REC;
+                        meta = __ldg(p.kn + slot_group() * M + idx);   // consumed after the scores: overlaps the row fetch
                     }
                 }
                 {
@@ -1078,10 +1087,10 @@ int fused_resident_clusters(int C, int threads) {
 int fused_cluster_waves(const mpig_ctx *ctx) { return fused_plan(ctx).ok ? fused_plan(ctx).cluster_waves : 0; }
 
 template <int THREADS, bool DBG, bool KREG>
-static int launch_variant(const cudaLaunchConfig_t &cfg, const FusedParams &p) {
+static int launch_variant(const cudaLaunchConfig_t &cfg, const FusedParams &p, const int32_t *slot_of) {
     MPIG_FUNC_ATTR((fused_decode_kernel<uint8_t, THREADS, DBG, KREG>), cudaFuncAttributeMaxDynamicSharedMemorySize,
                    THREADS == 1024 ? 227 * 1024 - 1024 : 228 * 1024 / 2 - 2048);
-    MPIG_CUDA(cudaLaunchKernelEx(&cfg, fused_decode_kernel<uint8_t, THREADS, DBG, KREG>, p, (const int32_t *)nullptr));
+    MPIG_CUDA(cudaLaunchKernelEx(&cfg, fused_decode_kernel<uint8_t, THREADS, DBG, KREG>, p, (const int32_t *)nullptr, slot_of));
     return MPIG_OK;
 }
 
@@ -1163,16 +1172,17 @@ int launch_fused(mpig_ctx *ctx, int layer, const void *q, const void *k, const v
     cfg.attrs = attr;
     cfg.numAttrs = (pdl && (ctx->pdl_first || !fp.hash_in_kernel)) ? 2 : 1;
     const int variant = (fp.threads == 1024 ? 0 : 4) + (p.dbg ? 2 : 0) + (ctx->fused_kreg ? 1 : 0);
+    const int32_t *sm = ctx->slot_map();
     int rc = MPIG_OK;
     switch (variant) {
-        case 0: rc = launch_variant<1024, false, false>(cfg, p); break;
-        case 1: rc = launch_variant<1024, false, true>(cfg, p); break;
-        case 2: rc = launch_variant<1024, true, false>(cfg, p); break;
-        case 3: rc = launch_variant<1024, true, true>(cfg, p); break;
-        case 4: rc = launch_variant<512, false, false>(cfg, p); break;
-        case 5: rc = launch_variant<512, false, true>(cfg, p); break;
-        case 6: rc = launch_variant<512, true, false>(cfg, p); break;
-        default: rc = launch_variant<512, true, true>(cfg, p); break;
+        case 0: rc = launch_variant<1024, false, false>(cfg, p, sm); break;
+        case 1: rc = launch_variant<1024, false, true>(cfg, p, sm); break;
+        case 2: rc = launch_variant<1024, true, false>(cfg, p, sm); break;
+        case 3: rc = launch_variant<1024, true, true>(cfg, p, sm); break;
+        case 4: rc = launch_variant<512, false, false>(cfg, p, sm); break;
+        case 5: rc = launch_variant<512, false, true>(cfg, p, sm); break;
+        case 6: rc = launch_variant<512, true, false>(cfg, p, sm); break;
+        default: rc = launch_variant<512, true, true>(cfg, p, sm); break;
     }
     if (rc) return rc;
     MPIG_LAUNCH_CHECK(ctx);
@@ -1182,10 +1192,10 @@ int launch_fused(mpig_ctx *ctx, int layer, const void *q, const void *k, const v
 }
 
 template <int THREADS, bool KREG>
-static int launch_tokens_variant(const cudaLaunchConfig_t &cfg, const FusedParams &p, const int32_t *anc) {
+static int launch_tokens_variant(const cudaLaunchConfig_t &cfg, const FusedParams &p, const int32_t *anc, const int32_t *slot_of) {
     MPIG_FUNC_ATTR((fused_decode_kernel<uint8_t, THREADS, false, KREG, true>), cudaFuncAttributeMaxDynamicSharedMemorySize,
                    THREADS == 1024 ? 227 * 1024 - 1024 : 228 * 1024 / 2 - 2048);
-    MPIG_CUDA(cudaLaunchKernelEx(&cfg, fused_decode_kernel<uint8_t, THREADS, false, KREG, true>, p, anc));
+    MPIG_CUDA(cudaLaunchKernelEx(&cfg, fused_decode_kernel<uint8_t, THREADS, false, KREG, true>, p, anc, slot_of));
     return MPIG_OK;
 }
 
@@ -1269,8 +1279,9 @@ int launch_fused_tokens(mpig_ctx *ctx, int layer, int T, const void *q, const vo
     cfg.attrs = attr;
     cfg.numAttrs = 2;   // under PDL behind the append (or the SimHash kernel)
     const int32_t *anc = step_masks(ctx->step_buf);   // the pending step's ancestor masks (plan_kernel)
-    if (fp.threads == 1024) rc = ctx->fused_kreg ? launch_tokens_variant<1024, true>(cfg, p, anc) : launch_tokens_variant<1024, false>(cfg, p, anc);
-    else rc = ctx->fused_kreg ? launch_tokens_variant<512, true>(cfg, p, anc) : launch_tokens_variant<512, false>(cfg, p, anc);
+    const int32_t *sm = ctx->slot_map();
+    if (fp.threads == 1024) rc = ctx->fused_kreg ? launch_tokens_variant<1024, true>(cfg, p, anc, sm) : launch_tokens_variant<1024, false>(cfg, p, anc, sm);
+    else rc = ctx->fused_kreg ? launch_tokens_variant<512, true>(cfg, p, anc, sm) : launch_tokens_variant<512, false>(cfg, p, anc, sm);
     if (rc) return rc;
     MPIG_LAUNCH_CHECK(ctx);
     ctx->last_decode_fused = 1;

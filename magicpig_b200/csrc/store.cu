@@ -57,7 +57,8 @@ __global__ void pack_records_nhd_kernel(const uint4 *__restrict__ k, const uint4
 }
 
 // Window spill, store side (mpig_spill_window): one CTA per (kv-head, request) of one sparse layer, 8 warps.  With g = spill_g[b]:
-//   window rows [sink, sink + g) -> records n_old .. n_old + g - 1 of the store (bitwise), their key norms
+//   window rows [sink, sink + g) -> records n_old .. n_old + g - 1 of the store of the request's slot (slot_of[b], or b when
+//   slot_of is null; the host lets only a request that is alone on its slot spill) (bitwise), their key norms
 //   kn = bf16(||k||_2) widened to fp32 (fp32 sum of squares, one rounding: what fill() stores), and their key halves -> stage
 //   (Hkv, g, d) bf16 at row spill_pre[b] * Hkv for the key hash;
 //   window rows [sink + g, sink + g + keep) -> [sink, sink + keep).
@@ -67,15 +68,16 @@ __global__ void pack_records_nhd_kernel(const uint4 *__restrict__ k, const uint4
 __global__ void __launch_bounds__(256) spill_move_kernel(uint4 *win, uint4 *__restrict__ rec, float *__restrict__ kn_store,
                                                          uint4 *__restrict__ stage, const int32_t *__restrict__ spill_g,
                                                          const int32_t *__restrict__ spill_pre, const int32_t *__restrict__ n_old_b,
-                                                         int Hkv, int M, int Wcap, int sink, int keep) {
+                                                         const int32_t *__restrict__ slot_of, int Hkv, int M, int Wcap, int sink, int keep) {
     constexpr int T = 256, UN = 4;
     const int gi = blockIdx.x, b = blockIdx.y, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int g = spill_g[b];
     if (g == 0) return;
     const size_t bg = (size_t)b * Hkv + gi;
+    const size_t sg = (size_t)(slot_of ? slot_of[b] : b) * Hkv + gi;   // store side: the request's slot
     uint4 *w = win + bg * Wcap * 32;
-    uint4 *r = rec + (bg * M + n_old_b[b]) * 32;
-    float *kns = kn_store + bg * M + n_old_b[b];
+    uint4 *r = rec + (sg * M + n_old_b[b]) * 32;
+    float *kns = kn_store + sg * M + n_old_b[b];
     uint4 *st = stage + ((size_t)spill_pre[b] * Hkv + (size_t)gi * g) * 16;
     for (int j = warp; j < g; j += T / 32) {
         const uint4 x = w[(size_t)(sink + j) * 32 + lane];
@@ -139,10 +141,11 @@ int mpig_attn_fill(mpig_ctx *ctx, int layer, int request, const void *k_bf16, co
     MPIG_REQUIRE(n == 0 || (k_bf16 && v_bf16 && kn), MPIG_EINVAL, "mpig_attn_fill: null input");
     const LayerStore &ls = ctx->layers[layer];
     const int Hkv = ctx->cfg.num_key_value_heads, M = ctx->cfg.max_length;
-    ctx->n_off[layer][request] = n;
+    const int slot = ctx->h_slot_of[request];   // every request bound to this slot sees the new context
+    ctx->n_off[layer][slot] = n;
     if (n == 0) return MPIG_OK;
-    uint4 *rec = reinterpret_cast<uint4 *>(ls.kv + (size_t)request * Hkv * M * ctx->rec_bytes);
-    float *kns = ls.kn + (size_t)request * Hkv * M;
+    uint4 *rec = reinterpret_cast<uint4 *>(ls.kv + (size_t)slot * Hkv * M * ctx->rec_bytes);
+    float *kns = ls.kn + (size_t)slot * Hkv * M;
     const size_t total = (size_t)Hkv * n * 32;
     const int blocks = (int)std::min<size_t>((total + 255) / 256, (size_t)ctx->num_sms * 16);
     pack_records_kernel<<<blocks, 256, 0, as_stream(stream)>>>((const uint4 *)k_bf16, (const uint4 *)v_bf16, kn, rec, kns, Hkv,
@@ -163,6 +166,7 @@ int mpig_attention_wrapper(mpig_ctx *ctx, int layer, int K, int L, void *output_
     AttendParams p = {};
     p.kv = ls.kv;
     p.kn = ls.kn;
+    p.slot_of = ctx->slot_map();
     p.win = nullptr;
     p.win_len = nullptr;
     p.ind = ind;
@@ -190,7 +194,7 @@ int mpig_attn_read_cache(mpig_ctx *ctx, int layer, void *k_bf16, void *v_bf16, f
     int rc = check_layer(ctx, layer, true, "mpig_attn_read_cache");
     if (rc) return rc;
     const LayerStore &ls = ctx->layers[layer];
-    const size_t rows = (size_t)ctx->BG * ctx->cfg.max_length;
+    const size_t rows = (size_t)ctx->C * ctx->cfg.num_key_value_heads * ctx->cfg.max_length;   // every slot
     if (k_bf16 || v_bf16) {
         const int blocks = (int)std::min<size_t>((rows * 32 + 255) / 256, (size_t)ctx->num_sms * 16);
         unpack_records_kernel<<<blocks, 256, 0, as_stream(stream)>>>((const uint4 *)ls.kv, (uint4 *)k_bf16, (uint4 *)v_bf16,
@@ -223,13 +227,22 @@ int mpig_spill_window(mpig_ctx *ctx, int keep, int32_t *spilled_out, void *strea
         meta[B + b] = tot;
         tot += g;
     }
+    // a shared slot's store and tables are every bound request's context: spilling one request's generated tokens into them would
+    // put those tokens into the others' samples
+    const std::vector<int> &slot = ctx->h_slot_of;
+    for (int b = 0; b < B; ++b)
+        for (int o = 0; o < B && meta[b] > 0; ++o)
+            MPIG_REQUIRE(o == b || slot[o] != slot[b] || wl[o] == 0, MPIG_ESTATE,
+                         "mpig_spill_window: request %d would spill %d rows into context slot %d, which request %d (window of %d rows) "
+                         "shares; a shared request generates at most generation_buffer tokens", b, meta[b], slot[b], o, wl[o]);
     for (int l = 0; l < nl; ++l) {
         if (!ctx->layers[l].sparse) continue;
         for (int b = 0; b < B; ++b) {
-            MPIG_REQUIRE(ctx->n_off[l][b] + meta[b] <= M, MPIG_ESTATE,
+            const int n_old = ctx->n_off[l][slot[b]];
+            MPIG_REQUIRE(n_old + meta[b] <= M, MPIG_ESTATE,
                          "mpig_spill_window: layer %d request %d: %d offloaded + %d spilled keys exceed max_length=%d", l, b,
-                         ctx->n_off[l][b], meta[b], M);
-            meta[(size_t)(2 + l) * B + b] = ctx->n_off[l][b];
+                         n_old, meta[b], M);
+            meta[(size_t)(2 + l) * B + b] = n_old;
         }
     }
     if (tot > 0) {
@@ -257,8 +270,8 @@ int mpig_spill_window(mpig_ctx *ctx, int keep, int32_t *spilled_out, void *strea
             if (!ls.sparse) continue;
             const int32_t *n_old = d_meta + (size_t)(2 + l) * B;
             spill_move_kernel<<<dim3(Hkv, B), 256, 0, s>>>(reinterpret_cast<uint4 *>(ls.win), reinterpret_cast<uint4 *>(ls.kv), ls.kn,
-                                                          reinterpret_cast<uint4 *>(keys), d_meta, d_meta + B, n_old, Hkv, M, ctx->Wcap,
-                                                          sink, keep);
+                                                          reinterpret_cast<uint4 *>(keys), d_meta, d_meta + B, n_old, ctx->slot_map(),
+                                                          Hkv, M, ctx->Wcap, sink, keep);
             MPIG_LAUNCH_CHECK(ctx);
             for (int b = 0; b < B; ++b) {
                 if (meta[b] == 0) continue;
@@ -276,7 +289,7 @@ int mpig_spill_window(mpig_ctx *ctx, int keep, int32_t *spilled_out, void *strea
         MPIG_CUDA(cudaStreamSynchronize(s));
         for (int l = 0; l < nl; ++l)
             if (ctx->layers[l].sparse)
-                for (int b = 0; b < B; ++b) ctx->n_off[l][b] += meta[b];
+                for (int b = 0; b < B; ++b) ctx->n_off[l][slot[b]] += meta[b];
         if (ctx->h_len_exact)
             for (int b = 0; b < B; ++b) ctx->h_win_len[b] = wl[b];
     }

@@ -7,7 +7,8 @@
 //   LSH::get_mask        :308-314  -> expand_mask_kernel
 // and, with no reference equivalent, the table side of a window spill (mpig_spill_window, store.cu) -> table_merge_kernel
 //
-// Table format (per request b, kv-head g, table l; row = (b*Hkv+g)*L + l): segmented compact CSR.
+// Table format (per context slot c, kv-head g, table l; row = (c*Hkv+g)*L + l): segmented compact CSR.  Request b reads the tables
+// of slot slot_of[b] (b itself when the map is null).
 //   Keys are cut into S = ceil(M / 65536) segments of EQUAL length seg_len = ceil(M / S) rounded up to 64 (<= 65536; equal so
 //   that the CTAs of a probing cluster own equal key ranges).  Segment s of a row owns the item region [s*seg_len, ...) of
 //   items[row][0..M) (uint16 = key index - s*seg_len, grouped by bucket) and its own bucket starts
@@ -130,13 +131,14 @@ __global__ void __launch_bounds__(1024) build_segments_kernel(const int16_t *__r
 // chunk read completely before any of it is written: a write lands only on positions already read.  No staging copy of the
 // segment is needed, so every K works in place (the old offsets are kept in shared memory when they fit beside the
 // histogram, K <= 14, and read from HBM otherwise).  A segment whose offsets are all equal has no old items, which covers a
-// segment beyond the old keys and tables that were never built (offsets still zero).  grid (L, Hkv, B * S), 512 threads;
+// segment beyond the old keys and tables that were never built (offsets still zero).  The tables are those of the request's slot
+// (slot_of[b], or b when slot_of is null; the host lets only a request that is alone on its slot spill).  grid (L, Hkv, B * S), 512 threads;
 // dynamic smem = (NB + 1 + 40 [+ NB + 1 when staged]) ints.
 // ---------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(512) table_merge_kernel(const int16_t *__restrict__ codes, int32_t *offsets, uint16_t *items,
                                                           const int32_t *__restrict__ spill_g, const int32_t *__restrict__ spill_pre,
-                                                          const int32_t *__restrict__ n_old_b, int Hkv, int L, int NB, int M, int S,
-                                                          int seg_len, int staged) {
+                                                          const int32_t *__restrict__ n_old_b, const int32_t *__restrict__ slot_of,
+                                                          int Hkv, int L, int NB, int M, int S, int seg_len, int staged) {
     extern __shared__ int smem_i[];
     constexpr int T = 512, UN = 4;
     int *ex = smem_i;                // NB + 1: histogram of the new codes -> exclusive prefix -> placement cursors
@@ -146,7 +148,7 @@ __global__ void __launch_bounds__(512) table_merge_kernel(const int16_t *__restr
     const int g = spill_g[b], n_old = n_old_b[b];
     const int seg_lo = seg * seg_len, seg_hi = min(seg_lo + seg_len, M);
     const int k0 = max(n_old, seg_lo), k1 = min(n_old + g, seg_hi);   // new keys of this segment
-    const size_t row = ((size_t)b * Hkv + gi) * L + l;
+    const size_t row = ((size_t)(slot_of ? slot_of[b] : b) * Hkv + gi) * L + l;
     int32_t *off = offsets + (row * S + seg) * (size_t)(NB + 1);
     if (k0 >= k1) {
         // a segment beyond all keys gets the offsets a build writes there (every bucket empty at seg_lo), so that tables that
@@ -248,7 +250,8 @@ __global__ void __launch_bounds__(THREADS) probe_kernel(const int32_t *__restric
                                                         int32_t *__restrict__ results,        // (H, M)
                                                         int32_t *__restrict__ nnz,            // (H)
                                                         uint32_t *__restrict__ bitmaps_out,   // (H,2,words) or null
-                                                        int L, int NB, int M, int G, int Mc, int words, int S, int r, int seg_len) {
+                                                        const int32_t *__restrict__ slot_of,  // (B) or null: request b reads slot b
+                                                        int L, int NB, int M, int G, int Hq, int Mc, int words, int S, int r, int seg_len) {
     extern __shared__ __align__(16) uint8_t smem_raw[];
     constexpr TagT SEL = (TagT)(~(TagT)0);
     constexpr TagT EMPTY = (TagT)(SEL - 1);
@@ -263,7 +266,10 @@ __global__ void __launch_bounds__(THREADS) probe_kernel(const int32_t *__restric
     uint16_t *s_ctab = reinterpret_cast<uint16_t *>(wsum + 40);
     constexpr int MAXCH = 2048;
     const unsigned C = cluster_nctarank(), c = cluster_ctarank();
-    const int h = blockIdx.x / C, g = h / G, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int h = blockIdx.x / C, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    // slot group of the head's tables.  The map may be read before griddepcontrol.wait: only copy-engine calls write it, and a
+    // kernel starts after every copy ordered before it in the stream has completed (PDL overlaps a kernel with a kernel only)
+    const int g = slot_of ? slot_of[h / Hq] * (Hq / G) + (h % Hq) / G : h / G;
     // CTA c of the cluster owns keys [lo_key, lo_key + Mc): sub-range (c % r) of key segment (c / r)
     const int seg = (int)c / r;
     const int lo_rel = ((int)c % r) * Mc;
@@ -438,9 +444,9 @@ __global__ void expand_mask_kernel(const uint32_t *__restrict__ bitmaps, uint8_t
 
 // diagnostic: full collision counts (library/lsh/test.py:43)
 __global__ void collision_counts_kernel(const int32_t *__restrict__ query, const int32_t *__restrict__ offsets,
-                                        const uint16_t *__restrict__ items, int32_t *__restrict__ counts, int L, int NB,
-                                        int M, int G, int S, int seg_len) {
-    const int h = blockIdx.x, g = h / G;
+                                        const uint16_t *__restrict__ items, int32_t *__restrict__ counts,
+                                        const int32_t *__restrict__ slot_of, int L, int NB, int M, int G, int Hq, int S, int seg_len) {
+    const int h = blockIdx.x, g = slot_of ? slot_of[h / Hq] * (Hq / G) + (h % Hq) / G : h / G;
     for (int t = 0; t < L; ++t) {
         const int code = query[(size_t)h * L + t];
         if (code < 0 || code >= NB) continue;
@@ -484,7 +490,8 @@ static int launch_probe_tt(mpig_ctx *ctx, const LayerStore &ls, const int32_t *q
     cfg.attrs = attr;
     cfg.numAttrs = pdl ? 2 : 1;
     MPIG_CUDA(cudaLaunchKernelEx(&cfg, probe_kernel<TagT, T>, query, (const int32_t *)ls.offsets, (const uint16_t *)ls.items,
-                                 results, nnz, bm, L, ctx->NB, M, ctx->G, Mc, ctx->bitmap_words, S, r, ctx->seg_len));
+                                 results, nnz, bm, ctx->slot_map(), L, ctx->NB, M, ctx->G, ctx->cfg.num_attention_heads, Mc,
+                                 ctx->bitmap_words, S, r, ctx->seg_len));
     MPIG_LAUNCH_CHECK(ctx);
     return MPIG_OK;
 }
@@ -533,8 +540,9 @@ int launch_probe(mpig_ctx *ctx, int layer, const int32_t *query, int32_t *result
 static int launch_build(mpig_ctx *ctx, int layer, int request, const int16_t *codes, const int32_t *idx, int n, cudaStream_t s) {
     const LayerStore &ls = ctx->layers[layer];
     const int Hkv = ctx->cfg.num_key_value_heads, L = ctx->cfg.L, S = ctx->nseg, M = ctx->cfg.max_length;
-    int32_t *off = ls.offsets + (size_t)request * Hkv * L * S * (size_t)(ctx->NB + 1);
-    uint16_t *it = reinterpret_cast<uint16_t *>(ls.items) + (size_t)request * Hkv * L * (size_t)M;
+    const size_t slot = ctx->h_slot_of[request];   // every request bound to this slot sees the new tables
+    int32_t *off = ls.offsets + slot * Hkv * L * S * (size_t)(ctx->NB + 1);
+    uint16_t *it = reinterpret_cast<uint16_t *>(ls.items) + slot * Hkv * L * (size_t)M;
     const size_t base = (size_t)(ctx->NB + 1 + 40) * sizeof(int);
     const int staged = base + (size_t)ctx->seg_len * 2 <= 200 * 1024;   // stage the sorted segment in shared memory when it fits
     const size_t smem = base + (staged ? (size_t)ctx->seg_len * 2 : 0);
@@ -557,8 +565,8 @@ int mpig::launch_table_merge(mpig_ctx *ctx, int layer, const int16_t *codes, con
     const size_t smem = base + (staged ? (size_t)(NB + 1) * sizeof(int) : 0);
     MPIG_FUNC_ATTR(table_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
     table_merge_kernel<<<dim3(L, Hkv, ctx->cfg.batch_size * S), 512, smem, s>>>(
-        codes, ls.offsets, reinterpret_cast<uint16_t *>(ls.items), g, pre, n_old, Hkv, L, NB, ctx->cfg.max_length, S, ctx->seg_len,
-        staged);
+        codes, ls.offsets, reinterpret_cast<uint16_t *>(ls.items), g, pre, n_old, ctx->slot_map(), Hkv, L, NB, ctx->cfg.max_length, S,
+        ctx->seg_len, staged);
     MPIG_LAUNCH_CHECK(ctx);
     return MPIG_OK;
 }
@@ -616,7 +624,8 @@ int mpig_lsh_collision_counts(mpig_ctx *ctx, int layer, const int32_t *query, in
     const LayerStore &ls = ctx->layers[layer];
     MPIG_CUDA(cudaMemsetAsync(counts, 0, (size_t)ctx->H * ctx->cfg.max_length * sizeof(int32_t), as_stream(stream)));
     collision_counts_kernel<<<ctx->H, 256, 0, as_stream(stream)>>>(query, ls.offsets, reinterpret_cast<const uint16_t *>(ls.items), counts,
-                                                                  ctx->cfg.L, ctx->NB, ctx->cfg.max_length, ctx->G, ctx->nseg, ctx->seg_len);
+                                                                  ctx->slot_map(), ctx->cfg.L, ctx->NB, ctx->cfg.max_length, ctx->G,
+                                                                  ctx->cfg.num_attention_heads, ctx->nseg, ctx->seg_len);
     MPIG_LAUNCH_CHECK(ctx);
     return MPIG_OK;
 }

@@ -57,14 +57,15 @@ class LlamaDecodeRunner:
     def __init__(self, shape: LlamaShape, K: int, L: int, batch_size: int, max_length: int, device: str = "cuda:0",
                  seed: int = 0, generation_buffer: int = 256, dense_layers=(0, 16, 32, 48, 64), num_layers: int | None = None,
                  tp_rank: int = 0, tp_world: int = 1, tp_group=None, fused: bool = True, tp_mode: str = "ag",
-                 tp_transport: str = "nccl", max_query_tokens: int = 1):
+                 tp_transport: str = "nccl", max_query_tokens: int = 1, num_contexts: int | None = None):
         """tp_mode (only with tp_world > 1; see magicpig_b200/tp.py):
              "ag"        attention sharded by KV head, one all-gather of head outputs per layer, wo / MLP replicated (north-star)
              "megatron"  + wo row-split, gate/up column-split, down row-split, two all-reduces per layer (llama_dist.py:49-70)
            tp_transport: "nccl" (torch.distributed collectives, captured in the CUDA graph) or "peer" (stores into the peers'
            buffers over NVLink: from the attention epilogue for "ag", one-shot all-reduce kernels for "megatron";
            magicpig_b200/peer.py).
-           max_query_tokens: largest T of step_tokens(T) (verification steps of speculative decoding; 1 = step() only)."""
+           max_query_tokens: largest T of step_tokens(T) (verification steps of speculative decoding; 1 = step() only).
+           num_contexts: contexts (sampled stores + hash tables) the batch holds; None = one per request."""
         assert tp_mode in ("ag", "megatron") and tp_transport in ("nccl", "peer")
         self.tp_mode, self.tp_transport = tp_mode, tp_transport
         self.shape = shape
@@ -101,7 +102,8 @@ class LlamaDecodeRunner:
         self.server = LSHSparseAttnServer(cfg, K=K, L=L, batch_size=batch_size, max_length=max_length,
                                           generation_buffer=generation_buffer, dense_layers=dense_layers, device=device,
                                           hash_func=hash_func, num_key_value_heads=self.Hkv_loc,
-                                          num_attention_heads=self.Hq_loc, max_query_tokens=max_query_tokens)
+                                          num_attention_heads=self.Hq_loc, max_query_tokens=max_query_tokens,
+                                          num_contexts=num_contexts)
 
         def w(*shape_):
             return (torch.randn(shape_, generator=g, device=self.device, dtype=torch.float32) * 0.02).to(torch.bfloat16)
@@ -159,12 +161,15 @@ class LlamaDecodeRunner:
         self.aux_launches_per_step = 0
 
     # ------------------------------------------------------------------------------------------
-    def synthetic_prefill(self, P: int, seed: int = 100, dist: str = "gauss"):
-        """Fill every layer's cache with a synthetic P-token context through fill()/build_table()."""
+    def synthetic_prefill(self, P: int, seed: int = 100, dist: str = "gauss", shared: bool = False):
+        """Fill every layer's cache with a synthetic P-token context through fill()/build_table().  shared=True: every request
+        holds the same context -- request 0 is filled and forked to the others when the server has fewer contexts than requests,
+        each request is filled with the same tensors otherwise."""
         srv = self.server
         g = torch.Generator(device=self.device).manual_seed(seed + 7919 * self.tp_rank)
         Hkv, d = self.Hkv_loc, self.d
-        for b in range(self.B):
+        fork = shared and srv.ctx.num_contexts < self.B
+        for b in range(1 if shared else self.B):
             srv.alloc_buffer(P)
             for layer in range(self.n_layers):
                 k = torch.randn((P, Hkv, d), generator=g, device=self.device, dtype=torch.float32)
@@ -175,11 +180,20 @@ class LlamaDecodeRunner:
                     k = k + torch.rand((P, 1, 1), generator=g, device=self.device) * 1.5 * centres[assign]
                 k = k.to(torch.bfloat16)
                 v = torch.randn((P, Hkv, d), generator=g, device=self.device, dtype=torch.float32).to(torch.bfloat16)
-                srv.fill(layer, b, k, v, P)
-                srv.build_table(layer, b, P)
+                for r in ([b] if fork or not shared else range(self.B)):
+                    srv.fill(layer, r, k, v, P)
+                    srv.build_table(layer, r, P)
                 del k, v
+        if fork:
+            srv.fork(0, range(1, self.B))
         self.pos.fill_(P - 1)
         torch.cuda.synchronize(self.device)
+
+    def fork(self, src: int, dst: int):
+        """Request dst continues from request src: the server's fork (shared context, copied window and dense KV) and src's
+        position."""
+        self.server.fork(src, dst)
+        self.pos[dst] = self.pos[src]
 
     # ------------------------------------------------------------------------------------------
     def _rope(self, x: torch.Tensor, pos: torch.Tensor) -> torch.Tensor:

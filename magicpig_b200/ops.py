@@ -41,7 +41,9 @@ class Context:
     def __init__(self, K: int, L: int, num_layers: int, num_attention_heads: int, num_key_value_heads: int,
                  head_dim: int, batch_size: int, max_length: int, num_sink_tokens: int = 4, num_local_tokens: int = 64,
                  generation_buffer: int = 256, dense_layers: Sequence[int] = (), alloc_dense_kv: bool = False,
-                 device: str | torch.device = "cuda:0", max_query_tokens: int = 1):
+                 device: str | torch.device = "cuda:0", max_query_tokens: int = 1, num_contexts: int = 0):
+        """num_contexts: context slots C in [0, batch_size] (0 = batch_size, every request owns its context).  The sampled store
+        and the hash tables exist once per slot; requests bound to one slot decode over one copy (fork(), bind())."""
         self.lib = N.load()
         self.device = torch.device(device)
         if self.device.type != "cuda":
@@ -69,10 +71,12 @@ class Context:
             cfg.dense_layers[i] = l
         cfg.alloc_dense_kv = 1 if alloc_dense_kv else 0
         cfg.reserved[0] = int(os.environ.get("MPIG_CTA_PER_SM", "1"))   # experiment switch: 2 = clusters of 512-thread CTAs, two per SM
+        cfg.reserved[1] = int(num_contexts)
         h = ctypes.c_void_p()
         with torch.cuda.device(self.device):
             N.check(self.lib.mpig_create(ctypes.byref(cfg), ctypes.byref(h)), "mpig_create")
         self._h = h
+        self.C = self.get_info("num_contexts")
         self.max_query_tokens = 1
         self.last_tokens = 1   # T of the last decode: the readers return B*T*Hq rows
         self.pending_tokens = 0   # T of the last plan (the shape accept() expects)
@@ -105,6 +109,23 @@ class Context:
     def clear(self):
         N.check(self.lib.mpig_clear(self._h, _stream()), "mpig_clear")
         self.last_tokens = 1
+        self.pending_tokens = 0
+
+    @property
+    def num_contexts(self) -> int:
+        return self.C
+
+    def fork(self, src: int, dst: int):
+        """Bind request dst to request src's context slot and copy src's window, avg_k, dense-layer KV and lengths into dst.
+        Synchronises; not capturable, but a step captured before it replays with the new binding.  Ends the pending step
+        (rewind / accept are refused until the next plan)."""
+        N.check(self.lib.mpig_fork_request(self._h, int(src), int(dst), _stream()), "mpig_fork_request")
+        self.pending_tokens = 0
+
+    def bind(self, request: int, slot: int):
+        """Bind `request` to context slot `slot` without touching its window or lengths (fill the slot and the window next).
+        Synchronises; ends the pending step like fork()."""
+        N.check(self.lib.mpig_bind_request(self._h, int(request), int(slot), _stream()), "mpig_bind_request")
         self.pending_tokens = 0
 
     def get_info(self, key: str) -> int:
@@ -223,9 +244,10 @@ class Context:
         self.last_tokens = 1
 
     def read_cache(self, layer: int, want_k=True, want_v=True, want_kn=True):
-        k = torch.empty((self.B, self.Hkv, self.M, self.d), dtype=torch.bfloat16, device=self.device) if want_k else None
-        v = torch.empty((self.B, self.Hkv, self.M, self.d), dtype=torch.bfloat16, device=self.device) if want_v else None
-        kn = torch.empty((self.B, self.Hkv, self.M), dtype=torch.float32, device=self.device) if want_kn else None
+        """k, v (C, Hkv, M, d) bf16 and kn (C, Hkv, M) fp32: the sampled store of every context slot (C = B by default)."""
+        k = torch.empty((self.C, self.Hkv, self.M, self.d), dtype=torch.bfloat16, device=self.device) if want_k else None
+        v = torch.empty((self.C, self.Hkv, self.M, self.d), dtype=torch.bfloat16, device=self.device) if want_v else None
+        kn = torch.empty((self.C, self.Hkv, self.M), dtype=torch.float32, device=self.device) if want_kn else None
         N.check(self.lib.mpig_attn_read_cache(self._h, layer, _ptr(k), _ptr(v), _ptr(kn), _stream()), "mpig_attn_read_cache")
         return k, v, kn
 

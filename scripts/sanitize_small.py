@@ -5,7 +5,8 @@
 Sizes are tiny (the tools slow kernels down 10-100x) but cover: the stand-alone SimHash / probe (uint8 tags, several clusters
 shapes, two key segments) / gather-attention kernels, the fused single-launch decode (cluster of 8, cluster of 4 over two
 segments, one CTA per head with codes from the SimHash kernel, several selection passes), the three-launch decode, the dense
-kernel, the tensor-core key hash, the table build, the window spill, verification steps of T tokens and token trees with an accept.  Results are also checked against each other so a tool run doubles as a test.
+kernel, the tensor-core key hash, the table build, the window spill, verification steps of T tokens, token trees with an accept and
+requests sharing one context slot.  Results are also checked against each other so a tool run doubles as a test.
 """
 import os
 import sys
@@ -305,8 +306,58 @@ def tree_case(B, Hq, Hkv, n, K, L, parents, path):
     print(f"tree B={B} Hq={Hq} Hkv={Hkv} n={n} T={T}: ok")
 
 
+def shared_case(B, Hq, Hkv, n, K, L):
+    """Context slots: request 0 filled and forked to the others over one slot (the fused kernel, the three-launch path's probe and
+    gather kernels reading the slot map), a bind, and a refused spill; every decode against a twin that holds B copies."""
+    M = n + 160
+    g = torch.Generator(device=dev).manual_seed(40)
+    hf = torch.randn((d, K * L), generator=g, device=dev).bfloat16()
+    ctxs = []
+    for C in (1, 0):
+        ctx = Context(K, L, 2, Hq, Hkv, d, B, M, generation_buffer=16, dense_layers=[0], alloc_dense_kv=True, device=dev,
+                      num_contexts=C)
+        ctx.set_option("out_f32", 1)
+        ctx.set_hash_func(hf)
+        ctxs.append(ctx)
+    sh, tw = ctxs
+    key = torch.randn((Hkv, n, d), generator=g, device=dev).bfloat16()
+    val = torch.randn((Hkv, n, d), generator=g, device=dev).bfloat16()
+    wk, wv = (torch.randn((Hkv, 68, d), generator=g, device=dev).bfloat16() for _ in range(2))
+    dk, dv = (torch.randn((300, Hkv, d), generator=g, device=dev).bfloat16() for _ in range(2))
+    for ctx, reqs in ((sh, [0]), (tw, range(B))):
+        for b in reqs:
+            ctx.attn_fill(1, b, key, val, key.norm(p=2, dim=-1).float())
+            ctx.lsh_build(1, b, ctx.hash_keys(key))
+            ctx.window_fill(1, b, torch.zeros((Hkv, d), dtype=torch.bfloat16, device=dev), wk, wv)
+            ctx.dense_fill(0, b, dk, dv, 300)
+    for b in range(1, B):
+        sh.fork(0, b)
+    sh.bind(B - 1, 0)
+    for impl in (1, 0):
+        q = torch.randn((B * Hq, d), generator=g, device=dev).bfloat16()
+        k, v = (torch.randn((B * Hkv, d), generator=g, device=dev).bfloat16() for _ in range(2))
+        outs = []
+        for ctx in ctxs:
+            ctx.set_option("decode_impl", impl)
+            ctx.plan()
+            ctx.decode(1, q, k, v)
+            outs.append(ctx.last_out_f32())
+            ctx.dense_decode(0, q, k, v)
+            outs.append(ctx.last_out_f32())
+        assert float((outs[0] - outs[2]).abs().max()) <= 1e-5 and torch.equal(outs[1], outs[3]), f"impl {impl}: shared != twin"
+    try:
+        sh.spill_window(0)
+        raise AssertionError("a spill into a shared slot was accepted")
+    except Exception as e:   # refused: the requests share slot 0 and their windows are not empty
+        assert "shares" in str(e), e
+    torch.cuda.synchronize()
+    print(f"shared B={B} Hq={Hq} Hkv={Hkv} n={n}: ok")
+
+
 if __name__ == "__main__":
-    which = sys.argv[1:] or ["stages", "dense", "decode", "hostpeer", "spill", "tokens", "tree"]
+    which = sys.argv[1:] or ["stages", "dense", "decode", "hostpeer", "spill", "tokens", "tree", "shared"]
+    if "shared" in which:
+        shared_case(3, 4, 2, 700, 6, 24)                 # clusters of several CTAs per head
     if "tree" in which:
         tree_case(2, 4, 1, 800, 6, 24, [-1, 0, 0, 1, 1, 2], [0, 2, 5])   # clusters of 8 per node, dense T*G = 24 (two m-tiles)
     if "tokens" in which:
