@@ -91,8 +91,7 @@ class LSHSparseAttnServer:
         # key codes of the layer whose table is being built (one layer in flight, as the reference)
         self.hash_code_buffer = torch.zeros((self.num_key_value_heads, L, max_length), dtype=torch.int16, device=self.device)
         self._out = {}   # layer (one token) or (layer, T) (T-token steps) -> decode output buffer (allocated on first use)
-        self._drop = None   # staging of host-side rewind counts
-        self._tree_stage = {}   # staging of host-side tree parents / accepted paths, per (name, T)
+        self._tree_stage = {}   # staging of host-side tree parents / accepted paths / rewind counts, per (name, shape)
 
     # ------------------------------------------------------------------------------------------
     def alloc_buffer(self, seq_len: int):
@@ -203,16 +202,9 @@ class LSHSparseAttnServer:
     def rewind(self, num_rejected):
         """Not in the reference.  Drops the last `num_rejected` tokens of the pending verification step: an int (every request),
         a sequence of B ints, or a device int32 (B,) tensor (capturable: acceptance can be decided on the GPU)."""
-        if isinstance(num_rejected, torch.Tensor) and num_rejected.is_cuda:
-            drop = num_rejected.to(torch.int32).contiguous()
-        else:
-            if isinstance(num_rejected, int):
-                num_rejected = [num_rejected] * self.batch_size
-            if self._drop is None:
-                self._drop = torch.zeros(self.batch_size, dtype=torch.int32, device=self.device)
-            self._drop.copy_(torch.as_tensor(list(num_rejected), dtype=torch.int32))
-            drop = self._drop
-        self.ctx.rewind(drop)
+        if isinstance(num_rejected, int):
+            num_rejected = [num_rejected] * self.batch_size
+        self.ctx.rewind(self._stage_int32("drop", num_rejected, (self.batch_size,)))
 
     def spill_window(self, keep: Optional[int] = None) -> torch.Tensor:
         """Not in the reference.  Moves the oldest generated tokens of every sparse layer's window into the sampled store and

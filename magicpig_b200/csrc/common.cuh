@@ -97,6 +97,27 @@ struct AttendTuning {
     int tma = 1;     // 1 = per-row cp.async.bulk (TMA engine), 0 = per-row 32 x 16 B cp.async (LSU path)
 };
 
+// The verification step between a plan and its rewind or accept.  Only begin() and end() write it: the plans begin a step
+// (step.cu); rewind and accept end it, and so do mpig_clear, mpig_fork_request and mpig_bind_request.
+struct PendingStep {
+    int T = 0;            // node count of the last plan (0 = no plan since create / clear); decode_tokens must match it
+    bool open = false;    // the step may still be rewound or accepted (at most once per plan)
+    bool tree = false;    // the step came from mpig_plan_tree (mpig_rewind is refused)
+    void begin(int t, bool is_tree) {
+        T = t;
+        open = true;
+        tree = is_tree;
+    }
+    // forget = true (mpig_clear): no step to decode either
+    void end(bool forget = false) {
+        open = false;
+        if (forget) {
+            T = 0;
+            tree = false;
+        }
+    }
+};
+
 }  // namespace mpig
 
 struct mpig_peer;
@@ -178,8 +199,7 @@ struct mpig_ctx {
     // multi-token verification steps (mpig_reserve_query_tokens / mpig_plan_tokens / mpig_decode_tokens / mpig_rewind).  After the
     // reservation the per-step scratch above (codes, qnorm, results, nnz, bitmaps, mve, out_f32) holds B*tok_max*Hq rows.
     int tok_max = 1;                         // largest T a step may verify (1 until mpig_reserve_query_tokens)
-    int pending_T = 0;                       // T of the last plan (0 = no plan yet); decode_tokens must match it
-    bool rewound = true;                     // the last plan has been rewound already (at most one rewind per plan)
+    mpig::PendingStep pending;               // the step of the last plan (step.cu)
     int last_tokens = 1;                     // rows of the readers (mpig_last_probe / _codes / _out_f32) = B * last_tokens * Hq
     bool plan_captured = false;              // a plan has been captured into a CUDA graph (the scratch addresses are baked in)
     int last_tokens_waves = 0;               // cluster waves of the last mpig_decode_tokens launch
@@ -187,7 +207,6 @@ struct mpig_ctx {
     // moves: int32 [B][T] ancestor masks (bit j of node t = node j is t or one of its ancestors) | int32 [B][T] parents | int32
     // [B][2] step bases (window, dense length before the plan, after saturation).  Every plan writes it (chains for plan_tokens).
     int32_t *step_buf = nullptr;
-    bool pending_tree = false;               // the pending step came from mpig_plan_tree (mpig_rewind is refused)
     // device table of the layers that own rows (sparse windows and dense KV), for the one-launch accept kernel
     void *accept_layers = nullptr;
     int n_accept_layers = 0;
@@ -345,10 +364,43 @@ struct AttendParams {
     int skip;                 // measurement aid (option "attend_skip"): 1 = no row fetch, 2 = no tile math, 4 = no merges
 };
 
+// The new rows of layer ls: its window (keys centred on avg_k) or, dense, its full KV cache.
+inline AppendParams append_params(const mpig_ctx *ctx, const LayerStore &ls, const void *k, const void *v, bool dense) {
+    AppendParams a = {};
+    a.k_new = (const __nv_bfloat16 *)k;
+    a.v_new = (const __nv_bfloat16 *)v;
+    a.avg_k = dense ? nullptr : ls.avg_k;
+    a.rows = dense ? ls.dense_kv : ls.win;
+    a.len = dense ? ctx->dense_len : ctx->win_len;
+    a.BG = ctx->BG;
+    a.Hkv = ctx->cfg.num_key_value_heads;
+    a.cap = dense ? ctx->cfg.max_length : ctx->Wcap;
+    return a;
+}
+
+// The fields of an attend_mma launch that every caller takes from the context.  The caller sets the rows to read (kv, kn,
+// slot_of, win, win_len, ind, nnz), mve, and Wcap / K / L where they differ.
+inline AttendParams attend_params(const mpig_ctx *ctx, const void *q, const float *qnorm, void *out) {
+    AttendParams p = {};
+    p.q = (const __nv_bfloat16 *)q;
+    p.qnorm = qnorm;
+    p.out = (__nv_bfloat16 *)out;
+    p.out_f32 = ctx->want_out_f32 ? ctx->out_f32 : nullptr;
+    p.partials = ctx->partials;
+    p.counters = ctx->counters;
+    p.H = ctx->H;
+    p.G = ctx->G;
+    p.Hq = ctx->cfg.num_attention_heads;
+    p.M = ctx->cfg.max_length;
+    p.Wcap = ctx->Wcap;
+    p.K = ctx->cfg.K;
+    p.L = ctx->cfg.L;
+    return p;
+}
+
 // rows = query rows to hash (0 = B*Hq)
 int launch_simhash(mpig_ctx *ctx, const void *query_bf16, int32_t *codes, float *qnorm, const AppendParams *ap,
                    cudaStream_t s, bool pdl, int rows = 0);
-int launch_append(mpig_ctx *ctx, const AppendParams &ap, cudaStream_t s);
 // the T new rows of every (request, kv-head): k/v (B, T, Hkv, d) -> rows len[b] - T + t (centred when ap.avg_k != null)
 int launch_append_tokens(mpig_ctx *ctx, const AppendParams &ap, int T, cudaStream_t s);
 // T-token sparse decode (fused.cu): append of the T window rows, then the T-token fused kernel; q (B, T, Hq, d), k / v
@@ -375,6 +427,9 @@ int launch_table_merge(mpig_ctx *ctx, int layer, const int16_t *codes, const int
 
 // ---- host helpers --------------------------------------------------------------------------
 int check_layer(mpig_ctx *ctx, int layer, bool need_sparse, const char *who);
+// the device lengths of requests [b0, b0 + n) into wl (win_len) and dl (dense_len), either may be null; synchronises s.  The
+// device lengths are the truth: replays of a captured plan advance only them (step.cu).
+int read_lengths(const mpig_ctx *ctx, int b0, int n, int32_t *wl, int32_t *dl, cudaStream_t s);
 inline cudaStream_t as_stream(void *s) { return (cudaStream_t)s; }
 
 }  // namespace mpig

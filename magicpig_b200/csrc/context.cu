@@ -316,9 +316,7 @@ int mpig_clear(mpig_ctx *ctx, void *stream) {
     MPIG_CUDA(cudaMemcpyAsync(ctx->slot_of, ctx->h_slot_of.data(), ctx->cfg.batch_size * sizeof(int32_t), cudaMemcpyHostToDevice, s));
     ctx->h_len_exact = true;
     ctx->last_tokens = 1;
-    ctx->pending_T = 0;     // no plan to decode, rewind or accept since the clear
-    ctx->rewound = true;
-    ctx->pending_tree = false;
+    ctx->pending.end(true);   // no plan to decode, rewind or accept since the clear
     return MPIG_OK;
 }
 
@@ -510,11 +508,9 @@ int mpig_fork_request(mpig_ctx *ctx, int src, int dst, void *stream) {
     if (rc) return rc;
     MPIG_REQUIRE(src != dst, MPIG_EINVAL, "mpig_fork_request: src == dst (%d)", src);
     cudaStream_t s = as_stream(stream);
-    // the device lengths are the truth (replays of a captured plan() advance only them)
     int32_t len[2] = {0, 0};
-    MPIG_CUDA(cudaMemcpyAsync(&len[0], ctx->win_len + src, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-    MPIG_CUDA(cudaMemcpyAsync(&len[1], ctx->dense_len + src, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-    MPIG_CUDA(cudaStreamSynchronize(s));
+    rc = read_lengths(ctx, src, 1, &len[0], &len[1], s);
+    if (rc) return rc;
     const size_t Hkv = ctx->cfg.num_key_value_heads, REC = ctx->rec_bytes;
     for (const LayerStore &ls : ctx->layers) {
         if (ls.sparse) {
@@ -537,7 +533,7 @@ int mpig_fork_request(mpig_ctx *ctx, int src, int dst, void *stream) {
     ctx->h_slot_of[dst] = ctx->h_slot_of[src];
     rc = upload_slot_map(ctx, s);
     if (rc) return rc;
-    ctx->rewound = true;   // the pending step ends: its bases are stale for dst
+    ctx->pending.end();   // its bases are stale for dst
     return MPIG_OK;
 }
 
@@ -549,7 +545,7 @@ int mpig_bind_request(mpig_ctx *ctx, int request, int slot, void *stream) {
     ctx->h_slot_of[request] = slot;
     rc = upload_slot_map(ctx, as_stream(stream));
     if (rc) return rc;
-    ctx->rewound = true;
+    ctx->pending.end();
     return MPIG_OK;
 }
 

@@ -17,15 +17,7 @@ static int decode_sparse(mpig_ctx *ctx, int layer, const void *q, const void *k,
     ctx->last_decode_fused = 0;
     ctx->last_tokens = 1;
     const LayerStore &ls = ctx->layers[layer];
-    AppendParams ap = {};
-    ap.k_new = (const __nv_bfloat16 *)k;
-    ap.v_new = (const __nv_bfloat16 *)v;
-    ap.avg_k = ls.avg_k;
-    ap.rows = ls.win;
-    ap.len = ctx->win_len;
-    ap.BG = ctx->BG;
-    ap.Hkv = ctx->cfg.num_key_value_heads;
-    ap.cap = ctx->Wcap;
+    const AppendParams ap = append_params(ctx, ls, k, v, false);
     const bool pdl = (ev == nullptr);
     if (ev) MPIG_CUDA(cudaEventRecord(ev[0], s));
     // PDL on the first kernel too: it may start (and prefetch its hash_func slice) while the caller's previous kernel drains;
@@ -36,7 +28,7 @@ static int decode_sparse(mpig_ctx *ctx, int layer, const void *q, const void *k,
     rc = launch_probe(ctx, layer, ctx->codes, ctx->results, ctx->nnz, s, pdl);
     if (rc) return rc;
     if (ev) MPIG_CUDA(cudaEventRecord(ev[2], s));
-    AttendParams p = {};
+    AttendParams p = attend_params(ctx, q, ctx->qnorm, out);
     p.kv = ls.kv;
     p.kn = ls.kn;
     p.slot_of = ctx->slot_map();
@@ -44,20 +36,7 @@ static int decode_sparse(mpig_ctx *ctx, int layer, const void *q, const void *k,
     p.win_len = ctx->win_len;
     p.ind = ctx->results;
     p.nnz = ctx->nnz;
-    p.q = (const __nv_bfloat16 *)q;
-    p.qnorm = ctx->qnorm;
-    p.out = (__nv_bfloat16 *)out;
     p.mve = ctx->mve;
-    p.partials = ctx->partials;
-    p.counters = ctx->counters;
-    p.H = ctx->H;
-    p.G = ctx->G;
-    p.Hq = ctx->cfg.num_attention_heads;
-    p.M = ctx->cfg.max_length;
-    p.Wcap = ctx->Wcap;
-    p.K = ctx->cfg.K;
-    p.L = ctx->cfg.L;
-    p.out_f32 = ctx->want_out_f32 ? ctx->out_f32 : nullptr;
     rc = launch_attend_mma(ctx, p, s, pdl);
     if (rc) return rc;
     if (ev) MPIG_CUDA(cudaEventRecord(ev[3], s));
@@ -190,39 +169,14 @@ int mpig_dense_decode(mpig_ctx *ctx, int layer, const void *query_bf16, const vo
     MPIG_REQUIRE(ls.dense && ls.dense_kv, MPIG_ESTATE, "mpig_dense_decode: layer %d has no dense KV", layer);
     MPIG_REQUIRE(query_bf16 && key_bf16 && value_bf16 && out_bf16, MPIG_EINVAL, "mpig_dense_decode: null argument");
     cudaStream_t s = as_stream(stream);
-    AppendParams ap = {};
-    ap.k_new = (const __nv_bfloat16 *)key_bf16;
-    ap.v_new = (const __nv_bfloat16 *)value_bf16;
-    ap.avg_k = nullptr;
-    ap.rows = ls.dense_kv;
-    ap.len = ctx->dense_len;
-    ap.BG = ctx->BG;
-    ap.Hkv = ctx->cfg.num_key_value_heads;
-    ap.cap = ctx->cfg.max_length;
-    rc = launch_append(ctx, ap, s);
+    rc = launch_append_tokens(ctx, append_params(ctx, ls, key_bf16, value_bf16, true), 1, s);
     if (rc) return rc;
     if (ctx->dense_impl == 1) return launch_attend_dense(ctx, ls.dense_kv, ctx->dense_len, query_bf16, out_bf16, s, false);
-    AttendParams p = {};
-    p.kv = nullptr;
-    p.kn = nullptr;
+    // the cache as window rows; qnorm is unused by window rows but must be a valid pointer
+    AttendParams p = attend_params(ctx, query_bf16, ctx->qnorm, out_bf16);
     p.win = ls.dense_kv;
     p.win_len = ctx->dense_len;
-    p.ind = nullptr;
-    p.nnz = nullptr;
-    p.q = (const __nv_bfloat16 *)query_bf16;
-    p.qnorm = ctx->qnorm;  // unused by window rows; must be a valid pointer
-    p.out = (__nv_bfloat16 *)out_bf16;
-    p.mve = nullptr;
-    p.partials = ctx->partials;
-    p.counters = ctx->counters;
-    p.H = ctx->H;
-    p.G = ctx->G;
-    p.Hq = ctx->cfg.num_attention_heads;
-    p.M = ctx->cfg.max_length;
     p.Wcap = ctx->cfg.max_length;
-    p.K = ctx->cfg.K;
-    p.L = ctx->cfg.L;
-    p.out_f32 = ctx->want_out_f32 ? ctx->out_f32 : nullptr;
     ctx->last_tokens = 1;
     return launch_attend_mma(ctx, p, s, false);
 }
@@ -235,7 +189,7 @@ static int tokens_checks(mpig_ctx *ctx, int layer, int T, const void *q, const v
     MPIG_REQUIRE(q && k && v && out, MPIG_EINVAL, "%s: null argument", who);
     MPIG_REQUIRE(T >= 1 && T <= ctx->tok_max, MPIG_EINVAL, "%s: T=%d outside [1, %d] (mpig_reserve_query_tokens sets the upper bound)",
                  who, T, ctx->tok_max);
-    MPIG_REQUIRE(T == ctx->pending_T, MPIG_ESTATE, "%s: T=%d but the last plan was for %d token(s)", who, T, ctx->pending_T);
+    MPIG_REQUIRE(T == ctx->pending.T, MPIG_ESTATE, "%s: T=%d but the last plan was for %d token(s)", who, T, ctx->pending.T);
     return MPIG_OK;
 }
 
@@ -259,16 +213,7 @@ int mpig_dense_decode_tokens(mpig_ctx *ctx, int layer, int T, const void *query_
     MPIG_REQUIRE(ctx->dense_impl == 1, MPIG_EUNSUPPORTED, "mpig_dense_decode_tokens: T=%d needs the GQA-shared dense kernel (dense_impl = 1)", T);
     MPIG_REQUIRE(T * ctx->G <= 32, MPIG_EUNSUPPORTED, "mpig_dense_decode_tokens: T*G = %d query rows per kv-group (at most 32)", T * ctx->G);
     cudaStream_t s = as_stream(stream);
-    AppendParams ap = {};
-    ap.k_new = (const __nv_bfloat16 *)key_bf16;
-    ap.v_new = (const __nv_bfloat16 *)value_bf16;
-    ap.avg_k = nullptr;
-    ap.rows = ls.dense_kv;
-    ap.len = ctx->dense_len;
-    ap.BG = ctx->BG;
-    ap.Hkv = ctx->cfg.num_key_value_heads;
-    ap.cap = ctx->cfg.max_length;
-    rc = launch_append_tokens(ctx, ap, T, s);
+    rc = launch_append_tokens(ctx, append_params(ctx, ls, key_bf16, value_bf16, true), T, s);
     if (rc) return rc;
     return launch_attend_dense_tokens(ctx, ls.dense_kv, ctx->dense_len, T, query_bf16, out_bf16, s, true);
 }

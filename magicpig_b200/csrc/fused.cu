@@ -988,26 +988,48 @@ struct FusedPlan {
     int cluster_waves;  // waves of clusters the grid needs (cudaOccupancyMaxActiveClusters; 0 = unknown)
 };
 
+using FusedKernel = void (*)(const FusedParams, const int32_t *, const int32_t *);
+
+// The fused_decode_kernel instantiation of a launch.  The T-token instantiations (tok) have no debug-clock variant.
+template <int THREADS> static FusedKernel fused_kernel_of(bool dbg, bool kreg, bool tok) {
+    if (tok) return kreg ? fused_decode_kernel<uint8_t, THREADS, false, true, true> : fused_decode_kernel<uint8_t, THREADS, false, false, true>;
+    if (dbg) return kreg ? fused_decode_kernel<uint8_t, THREADS, true, true> : fused_decode_kernel<uint8_t, THREADS, true, false>;
+    return kreg ? fused_decode_kernel<uint8_t, THREADS, false, true> : fused_decode_kernel<uint8_t, THREADS, false, false>;
+}
+static FusedKernel fused_kernel(int threads, bool dbg, bool kreg, bool tok) {
+    return threads == 1024 ? fused_kernel_of<1024>(dbg, kreg, tok) : fused_kernel_of<512>(dbg, kreg, tok);
+}
+
+// dynamic shared memory a CTA may use: per SM 228 KB, less the static parameter block and the 1 KB the system reserves per CTA
+static int fused_smem_cap(int threads) { return threads == 1024 ? 227 * 1024 - 1024 : 228 * 1024 / 2 - 2048; }
+
+// A grid of `clusters` clusters of the plan's C CTAs, with programmatic stream serialization when pdl.  attr[2] backs cfg.attrs.
+static cudaLaunchConfig_t fused_config(const FusedPlan &fp, int clusters, bool pdl, cudaStream_t s, cudaLaunchAttribute *attr) {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(clusters * fp.gm.C);
+    cfg.blockDim = dim3(fp.threads);
+    cfg.dynamicSmemBytes = fp.smem;
+    cfg.stream = s;
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = fp.gm.C;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[1].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = pdl ? 2 : 1;
+    return cfg;
+}
+
 // Clusters of this plan's variant that the device keeps resident at once.  A cluster occupies SMs of ONE GPC, and the
 // H100's GPCs have unequal SM counts, so #SMs / C over-counts; the runtime knows the real number.
-template <int THREADS, bool KREG, bool TOK = false>
-static int fused_max_active_clusters(const FusedPlan &fp) {
-    const void *fn = (const void *)fused_decode_kernel<uint8_t, THREADS, false, KREG, TOK>;
-    if (func_attr_once(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, THREADS == 1024 ? 227 * 1024 - 1024 : 228 * 1024 / 2 - 2048) != MPIG_OK)
-        return 0;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(fp.gm.C);
-    cfg.blockDim = dim3(THREADS);
-    cfg.dynamicSmemBytes = fp.smem;
-    cudaLaunchAttribute attr;
-    attr.id = cudaLaunchAttributeClusterDimension;
-    attr.val.clusterDim.x = fp.gm.C;
-    attr.val.clusterDim.y = 1;
-    attr.val.clusterDim.z = 1;
-    cfg.attrs = &attr;
-    cfg.numAttrs = 1;
+static int fused_max_active_clusters(const FusedPlan &fp, bool kreg, bool tok) {
+    const FusedKernel fn = fused_kernel(fp.threads, false, kreg, tok);
+    if (func_attr_once((const void *)fn, cudaFuncAttributeMaxDynamicSharedMemorySize, fused_smem_cap(fp.threads)) != MPIG_OK) return 0;
+    cudaLaunchAttribute attr[2];
+    const cudaLaunchConfig_t cfg = fused_config(fp, 1, false, 0, attr);
     int n = 0;
-    if (cudaOccupancyMaxActiveClusters(&n, fused_decode_kernel<uint8_t, THREADS, false, KREG, TOK>, &cfg) != cudaSuccess) {
+    if (cudaOccupancyMaxActiveClusters(&n, (const void *)fn, &cfg) != cudaSuccess) {
         cudaGetLastError();
         return 0;
     }
@@ -1029,7 +1051,7 @@ static FusedPlan fused_plan_compute(const mpig_ctx *ctx, int T = 1) {
     if (T == 1 && ctx->H * fp.gm.C > 2 * ctx->num_sms && fp.gm.C > 1) return fp;
     fp.threads = (HT * fp.gm.C > ctx->num_sms) ? 512 : 1024;
     // per CTA: dynamic + static (parameter block) + 1 KB the system reserves, out of 228 KB per SM
-    const size_t cap = (fp.threads == 1024) ? (227 * 1024 - 1024) : (size_t)(228 * 1024 / 2 - 2048);
+    const size_t cap = fused_smem_cap(fp.threads);
     const int stride = ctx->fused_kreg ? VSLOT : SLOT;
     const int max_warps = fp.threads / 32;
     int ncw = max_warps;
@@ -1043,13 +1065,7 @@ static FusedPlan fused_plan_compute(const mpig_ctx *ctx, int T = 1) {
     // the cluster splits the tables; with one CTA per head (large batches) every CTA would stream all of hash_func from L2:
     // those shapes hash in the separate tensor-core kernel (simhash.cu) and hand the codes over
     fp.hash_in_kernel = fp.gm.C >= 2;
-    int act;
-    if (T == 1)
-        act = fp.threads == 1024 ? (ctx->fused_kreg ? fused_max_active_clusters<1024, true>(fp) : fused_max_active_clusters<1024, false>(fp))
-                                 : (ctx->fused_kreg ? fused_max_active_clusters<512, true>(fp) : fused_max_active_clusters<512, false>(fp));
-    else
-        act = fp.threads == 1024 ? (ctx->fused_kreg ? fused_max_active_clusters<1024, true, true>(fp) : fused_max_active_clusters<1024, false, true>(fp))
-                                 : (ctx->fused_kreg ? fused_max_active_clusters<512, true, true>(fp) : fused_max_active_clusters<512, false, true>(fp));
+    const int act = fused_max_active_clusters(fp, ctx->fused_kreg, T > 1);
     fp.cluster_waves = act > 0 ? (HT + act - 1) / act : 0;
     fp.ok = true;
     return fp;
@@ -1081,33 +1097,18 @@ bool fused_applicable(const mpig_ctx *ctx) { return ctx->decode_impl == 1 && fus
 int fused_resident_clusters(int C, int threads) {
     FusedPlan fp = {};
     fp.gm.C = C;
-    fp.smem = threads == 1024 ? 227 * 1024 - 1024 : 228 * 1024 / 2 - 2048;   // the full carve-up the plan may use
-    return threads == 1024 ? fused_max_active_clusters<1024, false>(fp) : fused_max_active_clusters<512, false>(fp);
+    fp.threads = threads;
+    fp.smem = fused_smem_cap(threads);   // the full carve-up the plan may use
+    return fused_max_active_clusters(fp, false, false);
 }
 int fused_cluster_waves(const mpig_ctx *ctx) { return fused_plan(ctx).ok ? fused_plan(ctx).cluster_waves : 0; }
 
-template <int THREADS, bool DBG, bool KREG>
-static int launch_variant(const cudaLaunchConfig_t &cfg, const FusedParams &p, const int32_t *slot_of) {
-    MPIG_FUNC_ATTR((fused_decode_kernel<uint8_t, THREADS, DBG, KREG>), cudaFuncAttributeMaxDynamicSharedMemorySize,
-                   THREADS == 1024 ? 227 * 1024 - 1024 : 228 * 1024 / 2 - 2048);
-    MPIG_CUDA(cudaLaunchKernelEx(&cfg, fused_decode_kernel<uint8_t, THREADS, DBG, KREG>, p, (const int32_t *)nullptr, slot_of));
-    return MPIG_OK;
-}
-
-void peer_epilogue_view(const mpig_peer *p, uint8_t *const **blocks, unsigned long long **local, size_t *slot_bytes, size_t *data_bytes);
-
-int launch_fused(mpig_ctx *ctx, int layer, const void *q, const void *k, const void *v, void *out, cudaStream_t s, bool pdl,
-                 const mpig_peer *peer, int peer_rank, int peer_world, volatile uint32_t *host_flags, uint32_t host_epoch) {
-    const FusedPlan &fp = fused_plan(ctx);
-    MPIG_REQUIRE(fp.ok, MPIG_EUNSUPPORTED, "fused decode: shape not supported (L=%d, H=%d, segments=%d)", ctx->cfg.L, ctx->H, ctx->nseg);
+// The parameter block of a launch over the B*T*Hq (virtual) heads of T tokens per request; k / v = null: the rows were appended
+// before the launch.  Left zero here: the debug buffer, the host flags and the peer exchange (single-token launches set them) and
+// ntok (set by T-token launches).
+static FusedParams fused_params(const mpig_ctx *ctx, int layer, const FusedPlan &fp, int T, const void *q, const void *k,
+                                const void *v, void *out) {
     const LayerStore &ls = ctx->layers[layer];
-    ctx->last_probe_layer = layer;
-    if (!fp.hash_in_kernel) {
-        int rc = launch_simhash(ctx, q, ctx->codes, ctx->qnorm, nullptr, s, pdl && ctx->pdl_first);
-        if (rc) return rc;
-    } else {
-        MPIG_REQUIRE(ctx->hash_func_set, MPIG_ESTATE, "SimHash before mpig_set_hash_func: the projection has not been set");
-    }
     FusedParams p = {};
     p.q = (const __nv_bfloat16 *)q;
     p.k_new = (const __nv_bfloat16 *)k;
@@ -1128,9 +1129,58 @@ int launch_fused(mpig_ctx *ctx, int layer, const void *q, const void *k, const v
     p.results_out = ctx->save_mask ? ctx->results : nullptr;   // the index list goes to HBM only on request
     p.bitmaps_out = ctx->save_mask ? ctx->bitmaps : nullptr;
     p.codes_out = (ctx->save_mask && fp.hash_in_kernel) ? ctx->codes : nullptr;
+    p.issue_win = ctx->fused_issue_win;
+    p.H = ctx->H * T;
+    p.G = ctx->G;
+    p.Hq = ctx->cfg.num_attention_heads;
+    p.M = ctx->cfg.max_length;
+    p.Wcap = ctx->Wcap;
+    p.K = ctx->cfg.K;
+    p.L = ctx->cfg.L;
+    p.NB = ctx->NB;
+    p.S = ctx->nseg;
+    p.r = fp.gm.r;
+    p.Mc = fp.gm.Mc;
+    p.words = ctx->bitmap_words;
+    p.ncw = fp.ncw;
+    p.selcap = ctx->fused_selcap;
+    p.C = fp.gm.C;
+    p.seg_len = ctx->seg_len;
+    p.lay = fp.lay;
+    return p;
+}
+
+// One launch over p.H clusters.  The instantiation follows from the block: the debug-clock one when p.dbg is set, the T-token
+// one (with the pending step's ancestor masks, plan_kernel) when p.ntok is.
+static int fused_launch(mpig_ctx *ctx, const FusedPlan &fp, const FusedParams &p, bool pdl, cudaStream_t s) {
+    const bool tok = p.ntok > 0;
+    const FusedKernel fn = fused_kernel(fp.threads, p.dbg != nullptr, ctx->fused_kreg, tok);
+    MPIG_FUNC_ATTR(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, fused_smem_cap(fp.threads));
+    cudaLaunchAttribute attr[2];
+    const cudaLaunchConfig_t cfg = fused_config(fp, p.H, pdl, s, attr);
+    const int32_t *anc = tok ? step_masks(ctx->step_buf) : nullptr;
+    MPIG_CUDA(cudaLaunchKernelEx(&cfg, fn, p, anc, ctx->slot_map()));
+    MPIG_LAUNCH_CHECK(ctx);
+    ctx->last_decode_fused = 1;
+    return MPIG_OK;
+}
+
+void peer_epilogue_view(const mpig_peer *p, uint8_t *const **blocks, unsigned long long **local, size_t *slot_bytes, size_t *data_bytes);
+
+int launch_fused(mpig_ctx *ctx, int layer, const void *q, const void *k, const void *v, void *out, cudaStream_t s, bool pdl,
+                 const mpig_peer *peer, int peer_rank, int peer_world, volatile uint32_t *host_flags, uint32_t host_epoch) {
+    const FusedPlan &fp = fused_plan(ctx);
+    MPIG_REQUIRE(fp.ok, MPIG_EUNSUPPORTED, "fused decode: shape not supported (L=%d, H=%d, segments=%d)", ctx->cfg.L, ctx->H, ctx->nseg);
+    ctx->last_probe_layer = layer;
+    if (!fp.hash_in_kernel) {
+        int rc = launch_simhash(ctx, q, ctx->codes, ctx->qnorm, nullptr, s, pdl && ctx->pdl_first);
+        if (rc) return rc;
+    } else {
+        MPIG_REQUIRE(ctx->hash_func_set, MPIG_ESTATE, "SimHash before mpig_set_hash_func: the projection has not been set");
+    }
+    FusedParams p = fused_params(ctx, layer, fp, 1, q, k, v, out);
     p.dbg = ctx->fused_debug ? ctx->fused_dbg : nullptr;
     p.dbg_cap = ctx->num_sms * 8;
-    p.issue_win = ctx->fused_issue_win;
     p.host_flags = host_flags;
     p.host_epoch = host_epoch;
     if (peer) {
@@ -1140,62 +1190,9 @@ int launch_fused(mpig_ctx *ctx, int layer, const void *q, const void *k, const v
         p.peer_rank = peer_rank;
         p.peer_world = peer_world;
     }
-    p.H = ctx->H;
-    p.G = ctx->G;
-    p.Hq = ctx->cfg.num_attention_heads;
-    p.M = ctx->cfg.max_length;
-    p.Wcap = ctx->Wcap;
-    p.K = ctx->cfg.K;
-    p.L = ctx->cfg.L;
-    p.NB = ctx->NB;
-    p.S = ctx->nseg;
-    p.r = fp.gm.r;
-    p.Mc = fp.gm.Mc;
-    p.words = ctx->bitmap_words;
-    p.ncw = fp.ncw;
-    p.selcap = ctx->fused_selcap;
-    p.C = fp.gm.C;
-    p.seg_len = ctx->seg_len;
-    p.lay = fp.lay;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(ctx->H * fp.gm.C);
-    cfg.blockDim = dim3(fp.threads);
-    cfg.dynamicSmemBytes = fp.smem;
-    cfg.stream = s;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = fp.gm.C;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[1].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = (pdl && (ctx->pdl_first || !fp.hash_in_kernel)) ? 2 : 1;
-    const int variant = (fp.threads == 1024 ? 0 : 4) + (p.dbg ? 2 : 0) + (ctx->fused_kreg ? 1 : 0);
-    const int32_t *sm = ctx->slot_map();
-    int rc = MPIG_OK;
-    switch (variant) {
-        case 0: rc = launch_variant<1024, false, false>(cfg, p, sm); break;
-        case 1: rc = launch_variant<1024, false, true>(cfg, p, sm); break;
-        case 2: rc = launch_variant<1024, true, false>(cfg, p, sm); break;
-        case 3: rc = launch_variant<1024, true, true>(cfg, p, sm); break;
-        case 4: rc = launch_variant<512, false, false>(cfg, p, sm); break;
-        case 5: rc = launch_variant<512, false, true>(cfg, p, sm); break;
-        case 6: rc = launch_variant<512, true, false>(cfg, p, sm); break;
-        default: rc = launch_variant<512, true, true>(cfg, p, sm); break;
-    }
+    const int rc = fused_launch(ctx, fp, p, pdl && (ctx->pdl_first || !fp.hash_in_kernel), s);
     if (rc) return rc;
-    MPIG_LAUNCH_CHECK(ctx);
-    ctx->last_decode_fused = 1;
     ctx->last_tokens = 1;
-    return MPIG_OK;
-}
-
-template <int THREADS, bool KREG>
-static int launch_tokens_variant(const cudaLaunchConfig_t &cfg, const FusedParams &p, const int32_t *anc, const int32_t *slot_of) {
-    MPIG_FUNC_ATTR((fused_decode_kernel<uint8_t, THREADS, false, KREG, true>), cudaFuncAttributeMaxDynamicSharedMemorySize,
-                   THREADS == 1024 ? 227 * 1024 - 1024 : 228 * 1024 / 2 - 2048);
-    MPIG_CUDA(cudaLaunchKernelEx(&cfg, fused_decode_kernel<uint8_t, THREADS, false, KREG, true>, p, anc, slot_of));
     return MPIG_OK;
 }
 
@@ -1205,86 +1202,21 @@ int launch_fused_tokens(mpig_ctx *ctx, int layer, int T, const void *q, const vo
     MPIG_REQUIRE(fp.ok, MPIG_EUNSUPPORTED, "mpig_decode_tokens: shape not supported by the fused decode (L=%d, H=%d, T=%d, segments=%d)",
                  ctx->cfg.L, ctx->H, T, ctx->nseg);
     MPIG_REQUIRE(ctx->hash_func_set, MPIG_ESTATE, "SimHash before mpig_set_hash_func: the projection has not been set");
-    const LayerStore &ls = ctx->layers[layer];
-    const int HT = ctx->H * T;
     ctx->last_probe_layer = layer;
     int rc = MPIG_OK;
     if (ctx->Wcap > 0) {   // the T new rows (centred keys) go to the window first: the attention reads them from HBM
-        AppendParams ap = {};
-        ap.k_new = (const __nv_bfloat16 *)k;
-        ap.v_new = (const __nv_bfloat16 *)v;
-        ap.avg_k = ls.avg_k;
-        ap.rows = ls.win;
-        ap.len = ctx->win_len;
-        ap.BG = ctx->BG;
-        ap.Hkv = ctx->cfg.num_key_value_heads;
-        ap.cap = ctx->Wcap;
-        rc = launch_append_tokens(ctx, ap, T, s);
+        rc = launch_append_tokens(ctx, append_params(ctx, ctx->layers[layer], k, v, false), T, s);
         if (rc) return rc;
     }
     if (!fp.hash_in_kernel) {
         // one CTA per virtual head: the B*T*Hq query rows are hashed by the stand-alone tensor-core kernel
-        rc = launch_simhash(ctx, q, ctx->codes, ctx->qnorm, nullptr, s, true, HT);
+        rc = launch_simhash(ctx, q, ctx->codes, ctx->qnorm, nullptr, s, true, ctx->H * T);
         if (rc) return rc;
     }
-    FusedParams p = {};
-    p.q = (const __nv_bfloat16 *)q;
-    p.avg_k = ls.avg_k;
-    p.hf_t = ctx->hash_func_t;
-    p.codes_in = fp.hash_in_kernel ? nullptr : ctx->codes;
-    p.offsets = ls.offsets;
-    p.items = reinterpret_cast<const uint16_t *>(ls.items);
-    p.kv = ls.kv;
-    p.kn = ls.kn;
-    p.win = ctx->Wcap > 0 ? ls.win : nullptr;
-    p.win_len = ctx->win_len;
-    p.out = (__nv_bfloat16 *)out;
-    p.out_f32 = ctx->want_out_f32 ? ctx->out_f32 : nullptr;
-    p.mve = ctx->mve;
-    p.nnz_out = ctx->nnz;
-    p.results_out = ctx->save_mask ? ctx->results : nullptr;
-    p.bitmaps_out = ctx->save_mask ? ctx->bitmaps : nullptr;
-    p.codes_out = (ctx->save_mask && fp.hash_in_kernel) ? ctx->codes : nullptr;
-    p.issue_win = ctx->fused_issue_win;
-    p.H = HT;
-    p.G = ctx->G;
-    p.Hq = ctx->cfg.num_attention_heads;
-    p.M = ctx->cfg.max_length;
-    p.Wcap = ctx->Wcap;
-    p.K = ctx->cfg.K;
-    p.L = ctx->cfg.L;
-    p.NB = ctx->NB;
-    p.S = ctx->nseg;
-    p.r = fp.gm.r;
-    p.Mc = fp.gm.Mc;
-    p.words = ctx->bitmap_words;
-    p.ncw = fp.ncw;
-    p.selcap = ctx->fused_selcap;
-    p.C = fp.gm.C;
-    p.seg_len = ctx->seg_len;
-    p.lay = fp.lay;
+    FusedParams p = fused_params(ctx, layer, fp, T, q, nullptr, nullptr, out);
     p.ntok = T;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(HT * fp.gm.C);
-    cfg.blockDim = dim3(fp.threads);
-    cfg.dynamicSmemBytes = fp.smem;
-    cfg.stream = s;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = fp.gm.C;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[1].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 2;   // under PDL behind the append (or the SimHash kernel)
-    const int32_t *anc = step_masks(ctx->step_buf);   // the pending step's ancestor masks (plan_kernel)
-    const int32_t *sm = ctx->slot_map();
-    if (fp.threads == 1024) rc = ctx->fused_kreg ? launch_tokens_variant<1024, true>(cfg, p, anc, sm) : launch_tokens_variant<1024, false>(cfg, p, anc, sm);
-    else rc = ctx->fused_kreg ? launch_tokens_variant<512, true>(cfg, p, anc, sm) : launch_tokens_variant<512, false>(cfg, p, anc, sm);
+    rc = fused_launch(ctx, fp, p, true, s);   // under PDL behind the append (or the SimHash kernel)
     if (rc) return rc;
-    MPIG_LAUNCH_CHECK(ctx);
-    ctx->last_decode_fused = 1;
     ctx->last_tokens = T;
     ctx->last_tokens_waves = fp.cluster_waves;
     return MPIG_OK;

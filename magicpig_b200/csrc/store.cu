@@ -163,29 +163,16 @@ int mpig_attention_wrapper(mpig_ctx *ctx, int layer, int K, int L, void *output_
                  "mpig_attention_wrapper: null argument");
     MPIG_REQUIRE(K >= 1 && K <= 15 && L >= 1 && L <= 1024, MPIG_EINVAL, "mpig_attention_wrapper: K=%d L=%d outside [1,15] x [1,1024]", K, L);
     const LayerStore &ls = ctx->layers[layer];
-    AttendParams p = {};
+    AttendParams p = attend_params(ctx, query_bf16, query_norm, output_bf16);
     p.kv = ls.kv;
     p.kn = ls.kn;
     p.slot_of = ctx->slot_map();
-    p.win = nullptr;
-    p.win_len = nullptr;
     p.ind = ind;
     p.nnz = nnz;
-    p.q = (const __nv_bfloat16 *)query_bf16;
-    p.qnorm = query_norm;
-    p.out = (__nv_bfloat16 *)output_bf16;
-    p.out_f32 = ctx->want_out_f32 ? ctx->out_f32 : nullptr;
-    ctx->last_tokens = 1;
     p.mve = max_value_expsum;
-    p.partials = ctx->partials;
-    p.counters = ctx->counters;
-    p.H = ctx->H;
-    p.G = ctx->G;
-    p.Hq = ctx->cfg.num_attention_heads;
-    p.M = ctx->cfg.max_length;
-    p.Wcap = ctx->Wcap;
     p.K = K;
     p.L = L;
+    ctx->last_tokens = 1;
     return launch_attend_mma(ctx, p, as_stream(stream), false);
 }
 
@@ -214,10 +201,9 @@ int mpig_spill_window(mpig_ctx *ctx, int keep, int32_t *spilled_out, void *strea
                  "mpig_spill_window: keep=%d: sink (%d) + keep must leave a free row in the window (capacity %d)", keep, sink, ctx->Wcap);
     MPIG_REQUIRE(ctx->hash_func_set, MPIG_ESTATE, "mpig_spill_window before mpig_set_hash_func: the spilled keys cannot be hashed");
     cudaStream_t s = as_stream(stream);
-    // the device lengths are the truth (replays of a captured plan() advance only them)
     std::vector<int32_t> wl(B);
-    MPIG_CUDA(cudaMemcpyAsync(wl.data(), ctx->win_len, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-    MPIG_CUDA(cudaStreamSynchronize(s));
+    int rc = read_lengths(ctx, 0, B, wl.data(), nullptr, s);
+    if (rc) return rc;
     // meta = g[B] | pre[B] (exclusive prefix of g) | n_old[num_layers][B]
     std::vector<int32_t> meta((size_t)(2 + nl) * B, 0);
     int tot = 0;

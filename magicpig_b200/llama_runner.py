@@ -344,25 +344,11 @@ class LlamaDecodeRunner:
         request) the step ends with server.rewind(drop) and self.pos falls back by drop.  Graph-capturable; step() is separate."""
         assert self.tp_world == 1, "verification steps are built for a single GPU"
         assert 1 <= T <= self.max_query_tokens, f"T={T} outside [1, max_query_tokens={self.max_query_tokens}]"
-        sh, srv = self.shape, self.server
-        B, d, Hq, Hkv, hs, it = self.B, self.d, self.Hq_loc, self.Hkv_loc, sh.hidden_size, self.it_loc
+        srv = self.server
         srv.plan(T)
         pos = self.pos[:, None] + torch.arange(1, T + 1, device=self.device)   # (B, T)
         self.pos.add_(T)
-        h = F.embedding(self.ids_tok[:, :T], self.embed)   # (B, T, hs)
-        for li, lw in enumerate(self.layers):
-            x = F.rms_norm(h, (hs,), lw["ln1"], sh.rms_norm_eps)
-            qkv = F.linear(x, lw["wqkv"])   # (B, T, (Hq+2Hkv)d)
-            q = self._rope_at(qkv[..., : Hq * d].reshape(B, T, Hq, d).transpose(1, 2), pos)
-            k = self._rope_at(qkv[..., Hq * d:(Hq + Hkv) * d].reshape(B, T, Hkv, d).transpose(1, 2), pos)
-            v = qkv[..., (Hq + Hkv) * d:].reshape(B, T, Hkv, d).transpose(1, 2)
-            a = srv.decode(q, k, v, li)   # (B, T, Hq*d), token t attending causally   <- the hot path
-            h = h + F.linear(a, lw["wo"])
-            x = F.rms_norm(h, (hs,), lw["ln2"], sh.rms_norm_eps)
-            gu = F.linear(x, lw["w_gate_up"])
-            h = h + F.linear(F.silu(gu[..., :it]) * gu[..., it:], lw["w_down"])
-        x = F.rms_norm(h, (hs,), self.norm, sh.rms_norm_eps)
-        self.logits_tok[:, :T].copy_(F.linear(x, self.lm_head).float())
+        self._forward_tokens(T, pos)   # token t attending causally
         if drop is not None:
             srv.rewind(drop)
             self.pos.sub_(drop.long())
@@ -378,8 +364,7 @@ class LlamaDecodeRunner:
         Graph-capturable with device tensors."""
         assert self.tp_world == 1, "verification steps are built for a single GPU"
         assert 1 <= T <= self.max_query_tokens, f"T={T} outside [1, max_query_tokens={self.max_query_tokens}]"
-        sh, srv = self.shape, self.server
-        B, d, Hq, Hkv, hs, it = self.B, self.d, self.Hq_loc, self.Hkv_loc, sh.hidden_size, self.it_loc
+        srv, B = self.server, self.B
         if not (isinstance(parents, torch.Tensor) and parents.is_cuda):
             parents = torch.as_tensor(parents, dtype=torch.int32).to(self.device)
         parents = parents.to(torch.int32)
@@ -393,20 +378,7 @@ class LlamaDecodeRunner:
         for _ in range(T - 1):
             depth = torch.where(parents >= 0, depth.gather(1, par) + 1, 0)
         pos = self.pos[:, None] + 1 + depth   # (B, T)
-        h = F.embedding(self.ids_tok[:, :T], self.embed)   # (B, T, hs)
-        for li, lw in enumerate(self.layers):
-            x = F.rms_norm(h, (hs,), lw["ln1"], sh.rms_norm_eps)
-            qkv = F.linear(x, lw["wqkv"])   # (B, T, (Hq+2Hkv)d)
-            q = self._rope_at(qkv[..., : Hq * d].reshape(B, T, Hq, d).transpose(1, 2), pos)
-            k = self._rope_at(qkv[..., Hq * d:(Hq + Hkv) * d].reshape(B, T, Hkv, d).transpose(1, 2), pos)
-            v = qkv[..., (Hq + Hkv) * d:].reshape(B, T, Hkv, d).transpose(1, 2)
-            a = srv.decode(q, k, v, li)   # (B, T, Hq*d), node t attending to its ancestors   <- the hot path
-            h = h + F.linear(a, lw["wo"])
-            x = F.rms_norm(h, (hs,), lw["ln2"], sh.rms_norm_eps)
-            gu = F.linear(x, lw["w_gate_up"])
-            h = h + F.linear(F.silu(gu[..., :it]) * gu[..., it:], lw["w_down"])
-        x = F.rms_norm(h, (hs,), self.norm, sh.rms_norm_eps)
-        self.logits_tok[:, :T].copy_(F.linear(x, self.lm_head).float())
+        self._forward_tokens(T, pos)   # node t attending to its ancestors
         if count is None:
             self.pos.add_(T)
         else:
@@ -416,6 +388,26 @@ class LlamaDecodeRunner:
             else:
                 self.pos.add_(torch.as_tensor(count if not isinstance(count, int) else [count] * B, device=self.device).long())
         return self.logits_tok[:, :T]
+
+    def _forward_tokens(self, T: int, pos: torch.Tensor):
+        """The eager forward of the T rows of a verification step (after its plan): embeddings of self.ids_tok[:, :T] at RoPE
+        positions pos (B, T) through every layer into self.logits_tok[:, :T] (B, T, vocab)."""
+        sh, srv = self.shape, self.server
+        B, d, Hq, Hkv, hs, it = self.B, self.d, self.Hq_loc, self.Hkv_loc, sh.hidden_size, self.it_loc
+        h = F.embedding(self.ids_tok[:, :T], self.embed)   # (B, T, hs)
+        for li, lw in enumerate(self.layers):
+            x = F.rms_norm(h, (hs,), lw["ln1"], sh.rms_norm_eps)
+            qkv = F.linear(x, lw["wqkv"])   # (B, T, (Hq+2Hkv)d)
+            q = self._rope_at(qkv[..., : Hq * d].reshape(B, T, Hq, d).transpose(1, 2), pos)
+            k = self._rope_at(qkv[..., Hq * d:(Hq + Hkv) * d].reshape(B, T, Hkv, d).transpose(1, 2), pos)
+            v = qkv[..., (Hq + Hkv) * d:].reshape(B, T, Hkv, d).transpose(1, 2)
+            a = srv.decode(q, k, v, li)   # (B, T, Hq*d)   <- the hot path
+            h = h + F.linear(a, lw["wo"])
+            x = F.rms_norm(h, (hs,), lw["ln2"], sh.rms_norm_eps)
+            gu = F.linear(x, lw["w_gate_up"])
+            h = h + F.linear(F.silu(gu[..., :it]) * gu[..., it:], lw["w_down"])
+        x = F.rms_norm(h, (hs,), self.norm, sh.rms_norm_eps)
+        self.logits_tok[:, :T].copy_(F.linear(x, self.lm_head).float())
 
     def _rope_at(self, x: torch.Tensor, pos: torch.Tensor) -> torch.Tensor:
         # x (B, H, T, d), pos (B, T): token t of request b rotated by its own position

@@ -302,7 +302,9 @@ class Context:
         self._chk(drop, torch.int32, (self.B,), "drop")
         N.check(self.lib.mpig_rewind(self._h, _ptr(drop), _stream()), "mpig_rewind")
 
-    def _tokens_args(self, T: int, query, key, value, out):
+    def _decode_args(self, T: int, query, key, value, out, out_shape):
+        """The rows of a step of T tokens per request (T = 1: a single-token decode): query / key / value flattened to
+        (B*T*Hq, d) / (B*T*Hkv, d) and checked, and `out` checked, or allocated with out_shape when None."""
         q = query.reshape(self.B * T * self.Hq, self.d)
         k = key.reshape(self.B * T * self.Hkv, self.d)
         v = value.reshape(self.B * T * self.Hkv, self.d)
@@ -310,7 +312,7 @@ class Context:
         self._chk(k, torch.bfloat16, None, "key")
         self._chk(v, torch.bfloat16, None, "value")
         if out is None:
-            out = torch.empty((self.B, T, self.Hq * self.d), dtype=torch.bfloat16, device=self.device)
+            out = torch.empty(out_shape, dtype=torch.bfloat16, device=self.device)
         else:
             self._chk(out, torch.bfloat16, None, "out")
             if out.numel() != self.B * T * self.Hq * self.d:
@@ -320,7 +322,7 @@ class Context:
     def decode_tokens(self, layer: int, T: int, query: torch.Tensor, key: torch.Tensor, value: torch.Tensor,
                       out: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Sparse layer, verification step of T tokens: query (B,T,Hq,d), key/value (B,T,Hkv,d) bf16 -> out (B, T, Hq*d)."""
-        q, k, v, out = self._tokens_args(T, query, key, value, out)
+        q, k, v, out = self._decode_args(T, query, key, value, out, (self.B, T, self.Hq * self.d))
         N.check(self.lib.mpig_decode_tokens(self._h, layer, int(T), _ptr(q), _ptr(k), _ptr(v), _ptr(out), _stream()),
                 "mpig_decode_tokens")
         self.last_tokens = int(T)
@@ -329,7 +331,7 @@ class Context:
     def dense_decode_tokens(self, layer: int, T: int, query: torch.Tensor, key: torch.Tensor, value: torch.Tensor,
                             out: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Dense layer, same shapes as decode_tokens."""
-        q, k, v, out = self._tokens_args(T, query, key, value, out)
+        q, k, v, out = self._decode_args(T, query, key, value, out, (self.B, T, self.Hq * self.d))
         N.check(self.lib.mpig_dense_decode_tokens(self._h, layer, int(T), _ptr(q), _ptr(k), _ptr(v), _ptr(out), _stream()),
                 "mpig_dense_decode_tokens")
         self.last_tokens = int(T)
@@ -347,16 +349,7 @@ class Context:
     def decode(self, layer: int, query: torch.Tensor, key: torch.Tensor, value: torch.Tensor,
                out: Optional[torch.Tensor] = None) -> torch.Tensor:
         """query (B,Hq,1,d)|(B*Hq,d), key/value (B,Hkv,1,d)|(B*Hkv,d) bf16 -> out (B, Hq*d) bf16."""
-        q = query.reshape(self.H, self.d)
-        k = key.reshape(self.B * self.Hkv, self.d)
-        v = value.reshape(self.B * self.Hkv, self.d)
-        self._chk(q, torch.bfloat16, None, "query")
-        self._chk(k, torch.bfloat16, None, "key")
-        self._chk(v, torch.bfloat16, None, "value")
-        if out is None:
-            out = torch.empty((self.B, self.Hq * self.d), dtype=torch.bfloat16, device=self.device)
-        else:
-            self._chk(out, torch.bfloat16, None, "out")
+        q, k, v, out = self._decode_args(1, query, key, value, out, (self.B, self.Hq * self.d))
         N.check(self.lib.mpig_decode(self._h, layer, _ptr(q), _ptr(k), _ptr(v), _ptr(out), _stream()), "mpig_decode")
         self.last_tokens = 1
         return out
@@ -364,11 +357,7 @@ class Context:
     def decode_timed(self, layer: int, query: torch.Tensor, key: torch.Tensor, value: torch.Tensor, out: torch.Tensor):
         """decode() with CUDA events between the three kernels.  Asynchronous: read the times of all calls since the
         last collect with timing_collect()."""
-        q = query.reshape(self.H, self.d)
-        k = key.reshape(self.B * self.Hkv, self.d)
-        v = value.reshape(self.B * self.Hkv, self.d)
-        for t, nm in ((q, "query"), (k, "key"), (v, "value"), (out, "out")):
-            self._chk(t, torch.bfloat16, None, nm)
+        q, k, v, out = self._decode_args(1, query, key, value, out, (self.B, self.Hq * self.d))
         N.check(self.lib.mpig_decode_timed(self._h, layer, _ptr(q), _ptr(k), _ptr(v), _ptr(out), _stream()), "mpig_decode_timed")
         self.last_tokens = 1
 
@@ -413,14 +402,7 @@ class Context:
 
     def dense_decode(self, layer: int, query: torch.Tensor, key: torch.Tensor, value: torch.Tensor,
                      out: Optional[torch.Tensor] = None) -> torch.Tensor:
-        q = query.reshape(self.H, self.d)
-        k = key.reshape(self.B * self.Hkv, self.d)
-        v = value.reshape(self.B * self.Hkv, self.d)
-        self._chk(q, torch.bfloat16, None, "query")
-        self._chk(k, torch.bfloat16, None, "key")
-        self._chk(v, torch.bfloat16, None, "value")
-        if out is None:
-            out = torch.empty((self.B, self.Hq * self.d), dtype=torch.bfloat16, device=self.device)
+        q, k, v, out = self._decode_args(1, query, key, value, out, (self.B, self.Hq * self.d))
         N.check(self.lib.mpig_dense_decode(self._h, layer, _ptr(q), _ptr(k), _ptr(v), _ptr(out), _stream()),
                 "mpig_dense_decode")
         self.last_tokens = 1

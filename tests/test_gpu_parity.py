@@ -592,6 +592,32 @@ def test_dense_decode(cuda_lib, B, Hq, Hkv, P, impl):
         assert_1e3_before_rounding(out, o_ref)
 
 
+def test_dense_decode_checks_out(cuda_lib):
+    """A caller's `out` for dense_decode must be a contiguous bf16 tensor on the context's device with B*Hq*d elements: the
+    kernels write B*Hq*d bf16 values through its pointer."""
+    from magicpig_b200 import _native as N
+    from magicpig_b200.ops import Context
+    B, Hq, Hkv, d, P = 2, 8, 2, 128, 100
+    g = torch.Generator().manual_seed(11)
+    ctx = Context(4, 8, 1, Hq, Hkv, d, B, 512, dense_layers=[0], alloc_dense_kv=True, device=DEV)
+    for b in range(B):
+        ctx.dense_fill(0, b, torch.randn((P, Hkv, d), generator=g).bfloat16().to(DEV),
+                       torch.randn((P, Hkv, d), generator=g).bfloat16().to(DEV), P)
+    q = torch.randn((B, Hq, 1, d), generator=g).bfloat16().to(DEV)
+    k = torch.randn((B, Hkv, 1, d), generator=g).bfloat16().to(DEV)
+    v = torch.randn((B, Hkv, 1, d), generator=g).bfloat16().to(DEV)
+    bad = [torch.empty((B, Hq * d), dtype=torch.float32, device=DEV),        # dtype
+           torch.empty((B, Hq * d), dtype=torch.bfloat16),                    # device
+           torch.empty((Hq * d, B), dtype=torch.bfloat16, device=DEV).t(),    # contiguity
+           torch.empty((B, Hq * d // 2), dtype=torch.bfloat16, device=DEV)]   # size
+    for out in bad:
+        with pytest.raises(N.MagicPigError, match="^out: "):
+            ctx.dense_decode(0, q, k, v, out)
+    ctx.plan()
+    good = torch.empty((B, Hq * d), dtype=torch.bfloat16, device=DEV)
+    assert ctx.dense_decode(0, q, k, v, good) is good
+
+
 # ------------------------------------------------------------------------------------------------
 # the drop-in class on a small Llama-shaped config
 # ------------------------------------------------------------------------------------------------
