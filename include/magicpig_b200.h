@@ -82,7 +82,14 @@ typedef struct mpig_config {
      *   sampled store and the L hash tables of every sparse layer exist once per SLOT; the window, avg_k, the dense layers' KV,
      *   the lengths and the per-step scratch stay per REQUEST.  Request b is bound to slot b mod C at creation and after
      *   mpig_clear; mpig_fork_request / mpig_bind_request change the binding.  Requests bound to one slot decode over one copy of
-     *   the context (parallel sampling, several questions about one document). */
+     *   the context (parallel sampling, several questions about one document).
+     * reserved[2]: dense tail rows R; 0 (default) = every request owns a full dense KV cache [Hkv][max_length].  R > 0 (only
+     *   with 0 < C < batch_size, alloc_dense_kv = 1 and R <= max_length; otherwise MPIG_EINVAL) shares the dense layers' prompt
+     *   too: per dense layer a slot store [C][Hkv][max_length] and a tail [B][Hkv][R] per request.  mpig_dense_fill writes the
+     *   rows of the slot the request is bound to and makes seq_len the request's base; mpig_fork_request copies only src's rows
+     *   past its base; a request's dense capacity is min(max_length, base + R) (the plans refuse past it, a captured plan
+     *   saturates and raises mpig_error_flags bit 1); a rebound request must be dense-filled before its dense outputs mean
+     *   anything; dense_impl = 0 is MPIG_EUNSUPPORTED.  mpig_get_info("dense_tail_rows") reports R. */
     int32_t reserved[8];
 } mpig_config;
 
@@ -123,10 +130,10 @@ int mpig_set_option(mpig_ctx *ctx, const char *key, int64_t value);
  * "fused_cluster_waves" (waves of thread-block clusters one fused launch takes on this device; 1 = all resident at once,
  * 0 = fused decode not applicable), "window_capacity" (sink + local + generation_buffer rows), "table_segments" (key segments S
  * of the tables, see mpig_lsh_table_ptrs), "query_tokens_max" (t_max of mpig_reserve_query_tokens, 1 without), "tokens_cluster_waves"
- * (waves of clusters the last mpig_decode_tokens launch with T > 1 took), "num_contexts" (context slots C, see reserved[1]). */
+ * (waves of clusters the last mpig_decode_tokens launch with T > 1 took), "num_contexts" (context slots C, see reserved[1]), "dense_tail_rows" (R, see reserved[2]). */
 int mpig_get_info(mpig_ctx *ctx, const char *key, int64_t *value);
 /* Capacity errors the DEVICE detected (the lengths saturate there): bit 0 = a sparse window is full (generation_buffer
- * exhausted: each further token overwrites the previous one's K/V), bit 1 = a dense cache reached max_length, bit 2 = mpig_rewind
+ * exhausted: each further token overwrites the previous one's K/V), bit 1 = a dense cache reached its capacity (max_length, or base + R with reserved[2]), bit 2 = mpig_rewind
  * met a drop outside [0, T] (that request was left untouched), bit 3 = mpig_plan_tree met a malformed tree (that request ran as a
  * chain) or mpig_accept met a path that is not a root path of the step (that request was left untouched).  mpig_plan
  * itself returns MPIG_ESTATE for the same conditions as long as it has not been captured into a CUDA graph (replays advance

@@ -42,7 +42,8 @@ class LSHSparseAttnServer:
                  num_key_value_heads: Optional[int] = None,
                  num_attention_heads: Optional[int] = None,
                  max_query_tokens: int = 1,
-                 num_contexts: Optional[int] = None) -> None:
+                 num_contexts: Optional[int] = None,
+                 dense_tail_rows: Optional[int] = None) -> None:
         """Keywords up to `dtype` are the reference's (attnserver.py:9-20).  Extras:
         hash_func   inject the (d, K*L) bf16 projection (the reference draws it unseeded, :55);
         table_build "device" = counting sort on the GPU (mpig_lsh_build); "sorted" = the reference's
@@ -55,6 +56,8 @@ class LSHSparseAttnServer:
                     rewind); 1 = single-token decoding only.
         num_contexts number of contexts (sampled stores + hash tables) the batch holds, 1..batch_size; None = batch_size.
                     Request b starts on context b mod num_contexts; fork() and bind() change that.
+        dense_tail_rows R > 0: the dense layers' prompt rows are kept once per context too, and each request holds only the R
+                    rows it adds after its prompt (needs num_contexts < batch_size); None = a full dense cache per request.
         """
         self.K, self.L = K, L
         self.config = config
@@ -81,7 +84,8 @@ class LSHSparseAttnServer:
         self.ctx = Context(K, L, self.num_layers, self.num_attention_heads, self.num_key_value_heads, self.head_dim,
                            batch_size, max_length, num_sink_tokens, num_local_tokens, generation_buffer,
                            dense_layers=self.dense_layers, alloc_dense_kv=True, device=self.device,
-                           max_query_tokens=max_query_tokens, num_contexts=num_contexts or 0)
+                           max_query_tokens=max_query_tokens, num_contexts=num_contexts or 0,
+                           dense_tail_rows=dense_tail_rows or 0)
         if hash_func is None:
             hash_func = torch.randn((self.head_dim, K * L), device=self.device, dtype=torch.bfloat16)  # attnserver.py:55
         self.hash_func = hash_func.to(device=self.device, dtype=torch.bfloat16).contiguous()

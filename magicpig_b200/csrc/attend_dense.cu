@@ -65,30 +65,32 @@ __device__ __forceinline__ void finalize_dense_head(const DenseParams &p, int h,
 
 // Partition of the groups' rows over the nw warps of the grid (one warp runs it): s_prefix[bg] = first row of group bg in the
 // concatenation of all groups' rows, s_wpre[bg] = its first work item; a group of t rows gets max(1, t / Rp) items of >= TILE
-// rows, so the items number at most nw whenever nw > BG (a warp then takes at most one item).
-__device__ __forceinline__ void dense_partition(const DenseParams &p, int *s_prefix, int *s_wpre, int nw, int lane) {
+// rows, so the items number at most nw whenever nw > BG (a warp then takes at most one item).  rows_of(bg) = the rows of group bg
+// of the BG groups.
+template <class RowsOf>
+__device__ __forceinline__ void dense_partition_of(RowsOf rows_of, int BG, int *s_prefix, int *s_wpre, int nw, int lane) {
     int run = 0;
-    for (int g0 = 0; g0 < p.BG; g0 += 32) {
+    for (int g0 = 0; g0 < BG; g0 += 32) {
         const int bg = g0 + lane;
-        const int t = (bg < p.BG) ? min(max(p.len[bg / p.Hkv], 0), p.M) : 0;
+        const int t = (bg < BG) ? rows_of(bg) : 0;
         int inc = t;
 #pragma unroll
         for (int o = 1; o < 32; o <<= 1) {
             int v = __shfl_up_sync(0xffffffffu, inc, o);
             if (lane >= o) inc += v;
         }
-        if (bg < p.BG) s_prefix[bg] = run + inc - t;
+        if (bg < BG) s_prefix[bg] = run + inc - t;
         run += __shfl_sync(0xffffffffu, inc, 31);
     }
     const int total = run;
-    if (lane == 0) s_prefix[p.BG] = total;
-    const int Rp = (nw > p.BG) ? max(TILE, (total + (nw - p.BG) - 1) / (nw - p.BG)) : 0x3fffffff;
+    if (lane == 0) s_prefix[BG] = total;
+    const int Rp = (nw > BG) ? max(TILE, (total + (nw - BG) - 1) / (nw - BG)) : 0x3fffffff;
     __syncwarp();
     run = 0;
-    for (int g0 = 0; g0 < p.BG; g0 += 32) {
+    for (int g0 = 0; g0 < BG; g0 += 32) {
         const int bg = g0 + lane;
         int w = 0;
-        if (bg < p.BG) {
+        if (bg < BG) {
             const int t = s_prefix[bg + 1] - s_prefix[bg];
             w = (t > 0) ? max(1, t / Rp) : 0;
         }
@@ -98,10 +100,14 @@ __device__ __forceinline__ void dense_partition(const DenseParams &p, int *s_pre
             int v = __shfl_up_sync(0xffffffffu, inc, o);
             if (lane >= o) inc += v;
         }
-        if (bg < p.BG) s_wpre[bg] = run + inc - w;
+        if (bg < BG) s_wpre[bg] = run + inc - w;
         run += __shfl_sync(0xffffffffu, inc, 31);
     }
-    if (lane == 0) s_wpre[p.BG] = run;
+    if (lane == 0) s_wpre[BG] = run;
+}
+// one group per (request, kv-head) over its dense_len rows
+__device__ __forceinline__ void dense_partition(const DenseParams &p, int *s_prefix, int *s_wpre, int nw, int lane) {
+    dense_partition_of([&](int bg) { return min(max(p.len[bg / p.Hkv], 0), p.M); }, p.BG, s_prefix, s_wpre, nw, lane);
 }
 
 // the group work item `item` belongs to (s_wpre ascending)
@@ -357,8 +363,74 @@ __global__ void __launch_bounds__(384) attend_dense_kernel(const DenseParams p) 
 // States of the T*G rows fill a warp's whole ring (32 x 132 floats at T*G = 32): the CTA-level merge reads the other warps' rings in
 // place.  That is safe because a warp whose group is split (w_g > 1) never takes a second item (see the partition: then the items
 // number at most the warps).
-template <int NMT, bool PACK>
-__global__ void __launch_bounds__(256) attend_dense_tokens_kernel(const DenseParams p, int T, const int32_t *anc) {
+//
+// SLOTS (attend_dense_slot_kernel, shared dense mode): a group is (chunk, kv-head) instead, where a chunk is up to sl.cm requests
+// bound to one slot (dense_slot_chunks).  Its query rows are (member, t, j), member-major; its rows are the chunk's prefix in the
+// slot store, read once for all members, then each member's tail.  Prefix row k is visible to a member when k < its base; a
+// member's tail rows are visible to its own query rows only, the step rows among them by the ancestor mask as above.
+struct DenseSlots {
+    const int32_t *slot_of;  // [B] slot of each request
+    const int32_t *base;     // [B] dense_base: first row of each request in its tail
+    const uint8_t *tail;     // [BG][R] records
+    int B, R, cm;            // cm = requests per chunk: max(1, 32 / (T*G))
+};
+
+// Shared dense mode, warp 0: the chunks.  s_order = the requests by (slot, index); chunk c holds positions [s_cstart[c],
+// s_cstart[c + 1]) (at most sl.cm requests of one slot), s_cstart[B + 1] = the chunk count.  The rows of a chunk's group are its
+// prefix [0, max s_pre) of the slot store, then each member's tail: member m (a position) sees the prefix rows below s_pre[m] =
+// min(base, dense_len) and its tail at [s_tbeg[m], s_tend[m]), so the group has s_tend[last member] rows.  O(B^2 / 32)
+// shared-memory reads per lane (B at B <= 32).
+__device__ __forceinline__ void dense_slot_chunks(const DenseParams &p, const DenseSlots &sl, int *s_order, int *s_pre, int *s_tbeg,
+                                                  int *s_tend, int *s_cstart, int lane) {
+    const int B = sl.B;
+    int *s_slot = s_tend, *s_first = s_tbeg;   // scratch until the last pass writes them
+    for (int b = lane; b < B; b += 32) s_slot[b] = sl.slot_of[b];
+    __syncwarp();
+    for (int b = lane; b < B; b += 32) {
+        const int sb = s_slot[b];
+        int before = 0, rank = 0;
+        for (int j = 0; j < B; ++j) {
+            const int sj = s_slot[j];
+            before += (sj < sb);
+            rank += (sj == sb && j < b);
+        }
+        s_order[before + rank] = b;
+        s_first[before + rank] = (rank % sl.cm == 0);
+    }
+    __syncwarp();
+    int nc = 0;
+    for (int m0 = 0; m0 < B; m0 += 32) {
+        const int m = m0 + lane;
+        const bool f = m < B && s_first[m];
+        const unsigned bal = __ballot_sync(0xffffffffu, f);
+        if (f) s_cstart[nc + __popc(bal & ((1u << lane) - 1u))] = m;
+        nc += __popc(bal);
+    }
+    __syncwarp();
+    if (lane == 0) {
+        s_cstart[nc] = B;
+        s_cstart[B + 1] = nc;
+    }
+    __syncwarp();
+    for (int c = lane; c < nc; c += 32) {
+        const int cs = s_cstart[c], ce = s_cstart[c + 1];
+        int pc = 0;
+        for (int m = cs; m < ce; ++m) {
+            const int b = s_order[m];
+            s_pre[m] = min(max(min(sl.base[b], p.len[b]), 0), p.M);
+            pc = max(pc, s_pre[m]);
+        }
+        for (int m = cs; m < ce; ++m) {
+            const int b = s_order[m];
+            s_tbeg[m] = pc;
+            pc += min(max(p.len[b] - sl.base[b], 0), sl.R);
+            s_tend[m] = pc;
+        }
+    }
+}
+
+template <int NMT, bool PACK, bool SLOTS>
+__device__ __forceinline__ void dense_tokens_body(const DenseParams &p, int T, const int32_t *anc, const DenseSlots sl) {
     extern __shared__ __align__(128) uint8_t smem[];
     const int warps = blockDim.x >> 5, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     uint8_t *slots = smem + (size_t)warp * TILE * DSLOT;
@@ -369,9 +441,12 @@ __global__ void __launch_bounds__(256) attend_dense_tokens_kernel(const DensePar
     sp += (size_t)warps * sizeof(int);
     int *s_prefix = reinterpret_cast<int *>(sp);
     int *s_wpre = s_prefix + p.BG + 1;
+    // SLOTS: s_order [B] | s_pre [B] | s_tbeg [B] | s_tend [B] | s_cstart [B + 2] (dense_slot_chunks)
+    int *s_order = s_wpre + p.BG + 1, *s_pre = s_order + sl.B, *s_tbeg = s_pre + sl.B, *s_tend = s_tbeg + sl.B, *s_cstart = s_tend + sl.B;
     float *s_own = reinterpret_cast<float *>(slots);
     auto s_part_of = [&](int w) { return reinterpret_cast<float *>(smem + (size_t)w * TILE * DSLOT); };
     const int G = p.G, TG = T * G;
+    const int QS = SLOTS ? sl.cm * TG : TG;   // query rows a group may have: the stride of its states in the partial scratch
 
     if (lane == 0) {
         mbar_init(bar, 1);
@@ -381,20 +456,39 @@ __global__ void __launch_bounds__(256) attend_dense_tokens_kernel(const DensePar
     pdl_wait();
 
     const int nw = gridDim.x * warps;
-    if (warp == 0) dense_partition(p, s_prefix, s_wpre, nw, lane);   // the partition of attend_dense_kernel
+    if (warp == 0) {
+        if constexpr (SLOTS) {
+            dense_slot_chunks(p, sl, s_order, s_pre, s_tbeg, s_tend, s_cstart, lane);
+            __syncwarp();
+            dense_partition_of([&](int g) { return s_tend[s_cstart[g / p.Hkv + 1] - 1]; }, s_cstart[sl.B + 1] * p.Hkv, s_prefix, s_wpre,
+                               nw, lane);
+        } else {
+            dense_partition(p, s_prefix, s_wpre, nw, lane);   // the partition of attend_dense_kernel
+        }
+    }
     __syncthreads();
     pdl_launch_dependents();
 
+    const int NG = SLOTS ? s_cstart[sl.B + 1] * p.Hkv : p.BG;   // groups
     const int u = blockIdx.x * warps + warp;
-    const int n_items = s_wpre[p.BG];
+    const int n_items = s_wpre[NG];
     const int cta_w0 = blockIdx.x * warps;
     // output row of query row r of group bg: (B, T, Hq) order
-    auto out_row = [&](int bg, int r) { return ((bg / p.Hkv) * T + r / G) * p.Hq + (bg % p.Hkv) * G + r % G; };
+    auto out_row = [&](int bg, int r) {
+        if constexpr (SLOTS) {
+            const int rt = r % TG;
+            return (s_order[s_cstart[bg / p.Hkv] + r / TG] * T + rt / G) * p.Hq + (bg % p.Hkv) * G + rt % G;
+        } else {
+            return ((bg / p.Hkv) * T + r / G) * p.Hq + (bg % p.Hkv) * G + r % G;
+        }
+    };
+    // query rows of group bg
+    auto rows_q = [&](int bg) { return SLOTS ? (s_cstart[bg / p.Hkv + 1] - s_cstart[bg / p.Hkv]) * TG : TG; };
 
-    for (int bg = u; bg < p.BG; bg += nw) {
+    for (int bg = u; bg < NG; bg += nw) {
         if (s_prefix[bg + 1] == s_prefix[bg]) {
             const float z4[4] = {0.f, 0.f, 0.f, 0.f};
-            for (int r = 0; r < TG; ++r) finalize_dense_head(p, out_row(bg, r), 0.f, z4, lane);
+            for (int r = 0; r < rows_q(bg); ++r) finalize_dense_head(p, out_row(bg, r), 0.f, z4, lane);
         }
     }
 
@@ -408,28 +502,53 @@ __global__ void __launch_bounds__(256) attend_dense_tokens_kernel(const DensePar
     uint32_t phase = 0;
 
     for (int item = u; item < n_items; item += nw) {
-        const int bg = dense_item_group(s_wpre, p.BG, item);
+        const int bg = dense_item_group(s_wpre, NG, item);
         const int len = s_prefix[bg + 1] - s_prefix[bg];
         const int w_g = s_wpre[bg + 1] - s_wpre[bg];
         const int part = item - s_wpre[bg];
         const int c_g = (len + w_g - 1) / w_g;
         const int r_lo = part * c_g, r_hi = min(r_lo + c_g, len);
-        const uint8_t *rows = p.kv + (size_t)bg * p.M * REC;
+        const int qr = rows_q(bg);
+        // SLOTS: the chunk's first position, its prefix rows, and the slot store rows of this kv-head
+        const int cs = SLOTS ? s_cstart[bg / p.Hkv] : 0, pc = SLOTS ? s_tbeg[cs] : 0;
+        const uint8_t *rows = SLOTS ? p.kv + ((size_t)sl.slot_of[s_order[cs]] * p.Hkv + bg % p.Hkv) * p.M * REC
+                                    : p.kv + (size_t)bg * p.M * REC;
+        // the record of the group's row k
+        auto row_src = [&](int k) {
+            if constexpr (SLOTS) {
+                if (k < pc) return rows + (size_t)k * REC;
+                int m = cs;
+                while (s_tend[m] <= k) ++m;
+                return sl.tail + (((size_t)s_order[m] * p.Hkv + bg % p.Hkv) * sl.R + (k - s_tbeg[m])) * REC;
+            } else {
+                return rows + (size_t)k * REC;
+            }
+        };
 
         // this lane's query rows: r = mt*16 + i*8 + grp; rows past T*G are zero and unmasked.  Key row k is visible to query row r
-        // when k < lim or bit k - lim of vis is set (lim = the first row of the step, vis = the token's ancestor mask)
+        // when k < lim or bit k - lim of vis is set (lim = the first row of the step, vis = the token's ancestor mask); SLOTS: a
+        // prefix row (k < pc) when k < pre, a tail row when that holds and k >= tb (the member's tail starts at tb)
         const uint32_t *qrow[NMT][2];
         int lim[NMT][2];
         uint32_t vis[NMT][2];
+        int pre[SLOTS ? NMT : 1][2], tb[SLOTS ? NMT : 1][2];
 #pragma unroll
         for (int mt = 0; mt < NMT; ++mt)
 #pragma unroll
             for (int i = 0; i < 2; ++i) {
                 const int r = mt * 16 + i * 8 + grp;
-                const bool ok = r < TG && !(PACK && i == 1);
+                const bool ok = r < qr && !(PACK && i == 1);
                 qrow[mt][i] = ok ? reinterpret_cast<const uint32_t *>(p.q + (size_t)out_row(bg, r) * D) : nullptr;
-                lim[mt][i] = ok ? len - T : len;
-                vis[mt][i] = ok ? (uint32_t)__ldg(anc + (bg / p.Hkv) * T + r / G) : 0u;
+                if constexpr (SLOTS) {
+                    const int m = cs + r / TG;   // the member's position (valid when ok)
+                    lim[mt][i] = ok ? s_tend[m] - T : 0x3fffffff;
+                    vis[mt][i] = ok ? (anc ? (uint32_t)__ldg(anc + s_order[m] * T + (r % TG) / G) : 1u) : 0u;
+                    pre[mt][i] = ok ? s_pre[m] : 0x3fffffff;
+                    tb[mt][i] = ok ? s_tbeg[m] : 0;
+                } else {
+                    lim[mt][i] = ok ? len - T : len;
+                    vis[mt][i] = ok ? (uint32_t)__ldg(anc + (bg / p.Hkv) * T + r / G) : 0u;
+                }
             }
         auto q_frag = [&](int mt, int ks, uint32_t (&a)[4]) {
             a[0] = qrow[mt][0] ? __ldg(qrow[mt][0] + ks * 8 + tig) : 0u;
@@ -459,7 +578,7 @@ __global__ void __launch_bounds__(256) attend_dense_tokens_kernel(const DensePar
             if (lane == 0) mbar_arrive_expect_tx(bar, (uint32_t)nrows * REC);
             __syncwarp();
             if (lane < nrows) {
-                bulk_g2s(slots + (size_t)lane * DSLOT, rows + (size_t)(cr + lane) * REC, REC, bar);
+                bulk_g2s(slots + (size_t)lane * DSLOT, row_src(cr + lane), REC, bar);
             } else {
                 uint4 *vz = reinterpret_cast<uint4 *>(slots + (size_t)lane * DSLOT);
 #pragma unroll
@@ -512,7 +631,8 @@ __global__ void __launch_bounds__(256) attend_dense_tokens_kernel(const DensePar
                             const int r = nt * 8 + tig * 2 + e;
                             float &x = s[mt][nt][2 * i + e];
                             const int o = cr + r - lim[mt][i];
-                            const bool seen = o < 0 || ((unsigned)o < (unsigned)TREE_MAX && ((vis[mt][i] >> o) & 1u));
+                            bool seen = o < 0 || ((unsigned)o < (unsigned)TREE_MAX && ((vis[mt][i] >> o) & 1u));
+                            if constexpr (SLOTS) seen = (cr + r < pc) ? (cr + r < pre[mt][i]) : (cr + r >= tb[mt][i] && seen);
                             x = (r < nrows && seen) ? x * scale_log2 : -CUDART_INF_F;
                             mloc = fmaxf(mloc, x);
                         }
@@ -591,7 +711,7 @@ __global__ void __launch_bounds__(256) attend_dense_tokens_kernel(const DensePar
 #pragma unroll
             for (int i = 0; i < NI; ++i) {
                 const int r = mt * 16 + i * 8 + grp;
-                if (r < TG) {
+                if (r < qr) {
                     float *st = s_own + (size_t)r * PART_FLOATS;
                     if (tig == 0) {
                         st[0] = m_run[mt][i] * 0.6931471805599453f;
@@ -622,8 +742,8 @@ __global__ void __launch_bounds__(256) attend_dense_tokens_kernel(const DensePar
         const bool need_l1 = (w_g > 1 && wb > wa);
         const bool need_l2 = (w_g > 1 && cta_first != cta_last);
         int ticket2 = 0;
-        float *gslot = p.partials + ((size_t)blockIdx.x * 2 + ((i0 >= cta_w0) ? 1 : 0)) * (size_t)TG * PART_FLOATS;
-        for (int r = 0; r < TG; ++r) {
+        float *gslot = p.partials + ((size_t)blockIdx.x * 2 + ((i0 >= cta_w0) ? 1 : 0)) * (size_t)QS * PART_FLOATS;
+        for (int r = 0; r < qr; ++r) {
             float M_, L_, A[4];
             if (need_l1) {
                 merge_states<false>([&](int i) { return (const float *)(s_part_of(wa - cta_w0 + i) + (size_t)r * PART_FLOATS); },
@@ -643,12 +763,12 @@ __global__ void __launch_bounds__(256) attend_dense_tokens_kernel(const DensePar
         if (lane == 0) ticket2 = atom_add_acq_rel_gpu_d(p.counters + bg, 1);
         ticket2 = __shfl_sync(0xffffffffu, ticket2, 0);
         if (ticket2 == cta_last - cta_first) {
-            for (int r = 0; r < TG; ++r) {
+            for (int r = 0; r < qr; ++r) {
                 float M_, L_, A[4];
                 merge_states<true>(
                     [&](int i) {
                         const int c2 = cta_first + i;
-                        return (const float *)(p.partials + ((size_t)c2 * 2 + ((i0 >= c2 * warps) ? 1 : 0)) * (size_t)TG * PART_FLOATS +
+                        return (const float *)(p.partials + ((size_t)c2 * 2 + ((i0 >= c2 * warps) ? 1 : 0)) * (size_t)QS * PART_FLOATS +
                                                (size_t)r * PART_FLOATS);
                     },
                     cta_last - cta_first + 1, lane, M_, L_, A);
@@ -659,10 +779,18 @@ __global__ void __launch_bounds__(256) attend_dense_tokens_kernel(const DensePar
     }
 }
 
-int launch_attend_dense_tokens(mpig_ctx *ctx, const uint8_t *kv, const int32_t *len, int T, const void *q, void *out, cudaStream_t s,
-                               bool pdl) {
-    const int TG = T * ctx->G;
-    MPIG_REQUIRE(TG >= 1 && TG <= 32, MPIG_EUNSUPPORTED, "dense attention: T*G = %d query rows per group (at most 32)", TG);
+template <int NMT, bool PACK>
+__global__ void __launch_bounds__(256) attend_dense_tokens_kernel(const DenseParams p, int T, const int32_t *anc) {
+    dense_tokens_body<NMT, PACK, false>(p, T, anc, DenseSlots{});
+}
+
+// shared dense mode; anc = null: a single-token decode (each request's last row is its step row)
+template <int NMT, bool PACK>
+__global__ void __launch_bounds__(256) attend_dense_slot_kernel(const DenseParams p, int T, const int32_t *anc, const DenseSlots sl) {
+    dense_tokens_body<NMT, PACK, true>(p, T, anc, sl);
+}
+
+static DenseParams dense_params(const mpig_ctx *ctx, const uint8_t *kv, const int32_t *len, const void *q, void *out) {
     DenseParams p = {};
     p.kv = kv;
     p.len = len;
@@ -676,20 +804,72 @@ int launch_attend_dense_tokens(mpig_ctx *ctx, const uint8_t *kv, const int32_t *
     p.Hkv = ctx->cfg.num_key_value_heads;
     p.Hq = ctx->cfg.num_attention_heads;
     p.M = ctx->cfg.max_length;
-    const int warps = 8;
-    const size_t smem = (size_t)warps * TILE * DSLOT + (size_t)warps * 8 + (size_t)warps * 4 + 2 * (size_t)(p.BG + 1) * sizeof(int) + 16;
-    MPIG_REQUIRE(smem <= 227 * 1024, MPIG_EINVAL, "dense attention: %zu B shared memory", smem);
-    MPIG_REQUIRE((size_t)ctx->num_sms * 2 * TG <= (size_t)ctx->max_partial_warps * 2, MPIG_EINVAL, "dense attention: partial scratch too small");
+    return p;
+}
+
+static cudaLaunchConfig_t dense_config(const mpig_ctx *ctx, int warps, size_t smem, cudaStream_t s, bool pdl, cudaLaunchAttribute *attr) {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(ctx->num_sms);
     cfg.blockDim = dim3(warps * 32);
     cfg.dynamicSmemBytes = smem;
     cfg.stream = s;
-    cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = pdl ? 1 : 0;
+    return cfg;
+}
+
+int launch_attend_dense_slots(mpig_ctx *ctx, const LayerStore &ls, int T, const void *q, void *out, cudaStream_t s, bool pdl) {
+    const int B = ctx->cfg.batch_size, TG = T * ctx->G;
+    MPIG_REQUIRE(ctx->G >= 1 && TG <= 32, MPIG_EUNSUPPORTED, "dense attention: T*G = %d query rows per group (at most 32)", TG);
+    const DenseParams p = dense_params(ctx, ls.dense_kv, ctx->dense_len, q, out);
+    DenseSlots sl = {};
+    sl.slot_of = ctx->slot_of;
+    sl.base = ctx->dense_base;
+    sl.tail = ls.dense_tail;
+    sl.B = B;
+    sl.R = ctx->dense_tail_rows;
+    sl.cm = std::max(1, 32 / TG);
+    // the most query rows a group can have: a chunk of cm requests, or all B bound to one slot (the bindings may change after a
+    // capture, so the regime depends on B only)
+    const int rows = std::min(sl.cm, B) * TG;
+    const int warps = 8;
+    const size_t smem = (size_t)warps * TILE * DSLOT + (size_t)warps * 8 + (size_t)warps * 4 + 2 * (size_t)(p.BG + 1) * sizeof(int) +
+                        (size_t)(5 * B + 2) * sizeof(int) + 16;
+    MPIG_REQUIRE(smem <= 227 * 1024, MPIG_EINVAL, "dense attention: %zu B shared memory", smem);
+    // at most B*Hkv groups (a chunk holds at least one request), so partials and counters are those of the per-request kernels
+    MPIG_REQUIRE((size_t)ctx->num_sms * 2 * sl.cm * TG <= (size_t)ctx->max_partial_warps * 2, MPIG_EINVAL,
+                 "dense attention: partial scratch too small");
+    cudaLaunchAttribute attr[1];
+    cudaLaunchConfig_t cfg = dense_config(ctx, warps, smem, s, pdl, attr);
+    const int32_t *anc = (T > 1) ? (const int32_t *)step_masks(ctx->step_buf) : nullptr;
+    if (rows <= 8) {
+        MPIG_FUNC_ATTR((attend_dense_slot_kernel<1, true>), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+        MPIG_CUDA(cudaLaunchKernelEx(&cfg, attend_dense_slot_kernel<1, true>, p, T, anc, sl));
+    } else if (rows <= 16) {
+        MPIG_FUNC_ATTR((attend_dense_slot_kernel<1, false>), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+        MPIG_CUDA(cudaLaunchKernelEx(&cfg, attend_dense_slot_kernel<1, false>, p, T, anc, sl));
+    } else {
+        MPIG_FUNC_ATTR((attend_dense_slot_kernel<2, false>), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+        MPIG_CUDA(cudaLaunchKernelEx(&cfg, attend_dense_slot_kernel<2, false>, p, T, anc, sl));
+    }
+    MPIG_LAUNCH_CHECK(ctx);
+    ctx->last_tokens = T;
+    return MPIG_OK;
+}
+
+int launch_attend_dense_tokens(mpig_ctx *ctx, const uint8_t *kv, const int32_t *len, int T, const void *q, void *out, cudaStream_t s,
+                               bool pdl) {
+    const int TG = T * ctx->G;
+    MPIG_REQUIRE(TG >= 1 && TG <= 32, MPIG_EUNSUPPORTED, "dense attention: T*G = %d query rows per group (at most 32)", TG);
+    const DenseParams p = dense_params(ctx, kv, len, q, out);
+    const int warps = 8;
+    const size_t smem = (size_t)warps * TILE * DSLOT + (size_t)warps * 8 + (size_t)warps * 4 + 2 * (size_t)(p.BG + 1) * sizeof(int) + 16;
+    MPIG_REQUIRE(smem <= 227 * 1024, MPIG_EINVAL, "dense attention: %zu B shared memory", smem);
+    MPIG_REQUIRE((size_t)ctx->num_sms * 2 * TG <= (size_t)ctx->max_partial_warps * 2, MPIG_EINVAL, "dense attention: partial scratch too small");
+    cudaLaunchAttribute attr[1];
+    cudaLaunchConfig_t cfg = dense_config(ctx, warps, smem, s, pdl, attr);
     if (TG <= 8) {
         MPIG_FUNC_ATTR((attend_dense_tokens_kernel<1, true>), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
         MPIG_CUDA(cudaLaunchKernelEx(&cfg, attend_dense_tokens_kernel<1, true>, p, T, (const int32_t *)step_masks(ctx->step_buf)));
@@ -708,35 +888,15 @@ int launch_attend_dense_tokens(mpig_ctx *ctx, const uint8_t *kv, const int32_t *
 int launch_attend_dense(mpig_ctx *ctx, const uint8_t *kv, const int32_t *len, const void *q, void *out, cudaStream_t s, bool pdl) {
     MPIG_REQUIRE(ctx->G >= 1 && ctx->G <= GMAX, MPIG_EUNSUPPORTED, "dense attention: group size %d > %d", ctx->G, GMAX);
     ctx->last_tokens = 1;
-    DenseParams p = {};
-    p.kv = kv;
-    p.len = len;
-    p.q = (const __nv_bfloat16 *)q;
-    p.out = (__nv_bfloat16 *)out;
-    p.out_f32 = ctx->want_out_f32 ? ctx->out_f32 : nullptr;
-    p.partials = ctx->partials;
-    p.counters = ctx->counters;
-    p.BG = ctx->BG;
-    p.G = ctx->G;
-    p.Hkv = ctx->cfg.num_key_value_heads;
-    p.Hq = ctx->cfg.num_attention_heads;
-    p.M = ctx->cfg.max_length;
+    const DenseParams p = dense_params(ctx, kv, len, q, out);
     const int warps = 12;
     const size_t smem = (size_t)warps * TILE * DSLOT + (size_t)warps * 8 + (size_t)warps * 4 + 2 * (size_t)(p.BG + 1) * sizeof(int) + 16;
     MPIG_REQUIRE(smem <= 227 * 1024, MPIG_EINVAL, "dense attention: %zu B shared memory", smem);
     MPIG_REQUIRE((size_t)ctx->num_sms * 2 * GPART <= (size_t)ctx->max_partial_warps * 2 * PART_FLOATS, MPIG_EINVAL,
                  "dense attention: partial scratch too small");
     MPIG_FUNC_ATTR(attend_dense_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(ctx->num_sms);
-    cfg.blockDim = dim3(warps * 32);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = s;
     cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = pdl ? 1 : 0;
+    cudaLaunchConfig_t cfg = dense_config(ctx, warps, smem, s, pdl, attr);
     MPIG_CUDA(cudaLaunchKernelEx(&cfg, attend_dense_kernel, p));
     MPIG_LAUNCH_CHECK(ctx);
     return MPIG_OK;

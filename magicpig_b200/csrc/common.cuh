@@ -13,6 +13,12 @@
 //   win     [B][Hkv][Wcap]   REC-byte records of the sink+local+generated window (keys centred)
 //   avg_k   [B][Hkv][d]      bf16 mean offloaded key (attnserver.py:142-148)
 //   dense   [B][Hkv][M]      REC-byte records (dense layers, only with alloc_dense_kv)
+//
+// Shared dense mode (mpig_config.reserved[2] = R tail rows > 0, only with C < B): per dense layer the prompt rows live once per
+// slot and the rows a request adds after its prompt in a tail of its own.  Row r of request b is row r of slot slot_of[b]'s store
+// when r < dense_base[b], else row r - dense_base[b] of b's tail:
+//   dense   [C][Hkv][M]      REC-byte records (the slot store)
+//   tail    [B][Hkv][R]      REC-byte records (the request tail)
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -20,6 +26,7 @@
 #include <stdio.h>
 #include <string.h>
 
+#include <algorithm>
 #include <string>
 #include <vector>
 
@@ -79,11 +86,13 @@ struct LayerStore {
     int32_t *items = nullptr;    // storage of the uint16 item rows [C*Hkv][L][M]
     uint8_t *win = nullptr;      // window records
     __nv_bfloat16 *avg_k = nullptr;
-    uint8_t *dense_kv = nullptr; // dense: full-context records
+    uint8_t *dense_kv = nullptr; // dense: full-context records ([B][Hkv][M]), or the slot store ([C][Hkv][M]) in shared dense mode
+    uint8_t *dense_tail = nullptr; // dense, shared dense mode only: the request tails [B][Hkv][R]
 };
 
 // one entry of the accept kernel's layer table: the REC-byte rows of a sparse window ([BG][cap], cap = Wcap) or of a dense KV
-// cache ([BG][cap], cap = max_length); dense = 1 selects dense_len and the dense step base
+// cache ([BG][cap], cap = max_length, or the request tails with cap = R in shared dense mode); dense = 1 selects dense_len and the
+// dense step base
 struct AcceptLayer {
     uint8_t *rows;
     int cap;
@@ -140,6 +149,18 @@ struct mpig_ctx {
     std::vector<int> h_slot_of;           // [B]
     // the map the kernels get: null while every request owns its slot (C = B, bindings fixed), so that path addresses b itself
     const int32_t *slot_map() const { return C < cfg.batch_size ? slot_of : nullptr; }
+    // shared dense mode (R = dense_tail_rows > 0): the prompt rows of the dense layers live once per slot, each request's later
+    // rows in its own tail of R rows.  dense_base[b] = the first row of request b that lies in its tail (set by mpig_dense_fill and
+    // mpig_fork_request, zeroed by mpig_clear); allocated at create time and never moved, h_dense_base mirrors it exactly.
+    int dense_tail_rows = 0;
+    int32_t *dense_base = nullptr;        // [B], shared dense mode only
+    std::vector<int> h_dense_base;        // [B]
+    // the base map the kernels get: null in the default layout
+    const int32_t *dense_base_map() const { return dense_tail_rows > 0 ? dense_base : nullptr; }
+    // the dense capacity of request b: max_length, or min(max_length, base + R) in shared dense mode
+    int dense_cap(int b) const {
+        return dense_tail_rows > 0 ? std::min(cfg.max_length, h_dense_base[b] + dense_tail_rows) : cfg.max_length;
+    }
     // global state
     __nv_bfloat16 *hash_func = nullptr;   // (d, K*L) as given
     __nv_bfloat16 *hash_func_t = nullptr; // (K*L, d) transposed copy: K-major B operand for the SimHash GEMM
@@ -188,7 +209,7 @@ struct mpig_ctx {
     float *out_f32 = nullptr;                // [H][d]
     // capacity bookkeeping (the window / the dense cache saturate silently on the device): a device flag raised by
     // plan_kernel plus a host mirror that is exact as long as plan() is not replayed from a CUDA graph
-    int32_t *err_flag = nullptr;             // bit 0: sparse window full, bit 1: dense cache full
+    int32_t *err_flag = nullptr;             // bit 0: sparse window full, bit 1: a dense cache reached its capacity
     std::vector<int> h_win_len, h_dense_len; // [B]
     bool h_len_exact = true;
     void *host_stage_dev = nullptr;          // device-side address of the mapped pinned block host_stage
@@ -364,17 +385,19 @@ struct AttendParams {
     int skip;                 // measurement aid (option "attend_skip"): 1 = no row fetch, 2 = no tile math, 4 = no merges
 };
 
-// The new rows of layer ls: its window (keys centred on avg_k) or, dense, its full KV cache.
+// The new rows of layer ls: its window (keys centred on avg_k) or, dense, its full KV cache (in shared dense mode its request
+// tails, addressed from ctx->dense_base_map() -- see launch_append_tokens).
 inline AppendParams append_params(const mpig_ctx *ctx, const LayerStore &ls, const void *k, const void *v, bool dense) {
     AppendParams a = {};
     a.k_new = (const __nv_bfloat16 *)k;
     a.v_new = (const __nv_bfloat16 *)v;
     a.avg_k = dense ? nullptr : ls.avg_k;
-    a.rows = dense ? ls.dense_kv : ls.win;
+    const bool tail = dense && ctx->dense_tail_rows > 0;
+    a.rows = dense ? (tail ? ls.dense_tail : ls.dense_kv) : ls.win;
     a.len = dense ? ctx->dense_len : ctx->win_len;
     a.BG = ctx->BG;
     a.Hkv = ctx->cfg.num_key_value_heads;
-    a.cap = dense ? ctx->cfg.max_length : ctx->Wcap;
+    a.cap = dense ? (tail ? ctx->dense_tail_rows : ctx->cfg.max_length) : ctx->Wcap;
     return a;
 }
 
@@ -401,14 +424,19 @@ inline AttendParams attend_params(const mpig_ctx *ctx, const void *q, const floa
 // rows = query rows to hash (0 = B*Hq)
 int launch_simhash(mpig_ctx *ctx, const void *query_bf16, int32_t *codes, float *qnorm, const AppendParams *ap,
                    cudaStream_t s, bool pdl, int rows = 0);
-// the T new rows of every (request, kv-head): k/v (B, T, Hkv, d) -> rows len[b] - T + t (centred when ap.avg_k != null)
-int launch_append_tokens(mpig_ctx *ctx, const AppendParams &ap, int T, cudaStream_t s);
+// the T new rows of every (request, kv-head): k/v (B, T, Hkv, d) -> rows len[b] - T + t (centred when ap.avg_k != null); with a
+// base map (shared dense mode) row len[b] - T + t - base[b] of the request's tail
+int launch_append_tokens(mpig_ctx *ctx, const AppendParams &ap, int T, cudaStream_t s, const int32_t *base = nullptr);
 // T-token sparse decode (fused.cu): append of the T window rows, then the T-token fused kernel; q (B, T, Hq, d), k / v
 // (B, T, Hkv, d), out (B, T, Hq*d).  Refuses (nothing launched) when the fused decode does not apply.
 int launch_fused_tokens(mpig_ctx *ctx, int layer, int T, const void *q, const void *k, const void *v, void *out, cudaStream_t s);
 // T-token dense decode (attend_dense.cu): q (B, T, Hq, d), rows already appended, causal over the last T rows
 int launch_attend_dense_tokens(mpig_ctx *ctx, const uint8_t *kv, const int32_t *len, int T, const void *q, void *out, cudaStream_t s,
-                               bool pdl);int launch_probe(mpig_ctx *ctx, int layer, const int32_t *query, int32_t *results, int32_t *nnz, cudaStream_t s, bool pdl);
+                               bool pdl);
+// shared dense mode (attend_dense.cu): the dense layer ls over the slot stores and the request tails, T = 1 (single-token decode,
+// causal) or the pending step's T (ancestor masks); q (B, T, Hq, d), rows already appended
+int launch_attend_dense_slots(mpig_ctx *ctx, const LayerStore &ls, int T, const void *q, void *out, cudaStream_t s, bool pdl);
+int launch_probe(mpig_ctx *ctx, int layer, const int32_t *query, int32_t *results, int32_t *nnz, cudaStream_t s, bool pdl);
 int launch_attend_mma(mpig_ctx *ctx, const AttendParams &p, cudaStream_t s, bool pdl);
 int launch_attend_dense(mpig_ctx *ctx, const uint8_t *kv, const int32_t *len, const void *q, void *out, cudaStream_t s, bool pdl);
 int launch_fused(mpig_ctx *ctx, int layer, const void *q, const void *k, const void *v, void *out, cudaStream_t s, bool pdl,

@@ -95,6 +95,16 @@ int mpig_create(const mpig_config *cfg, mpig_ctx **out) {
                  "mpig_create: negative window size");
     MPIG_REQUIRE(cfg->reserved[1] >= 0 && cfg->reserved[1] <= cfg->batch_size, MPIG_EINVAL,
                  "mpig_create: num_contexts (reserved[1]) = %d outside [0, batch_size = %d]", cfg->reserved[1], cfg->batch_size);
+    if (cfg->reserved[2] != 0) {   // shared dense mode: R tail rows per request, the prompt rows once per slot
+        MPIG_REQUIRE(cfg->reserved[2] >= 1 && cfg->reserved[2] <= cfg->max_length, MPIG_EINVAL,
+                     "mpig_create: dense_tail_rows (reserved[2]) = %d outside [1, max_length = %d]", cfg->reserved[2], cfg->max_length);
+        MPIG_REQUIRE(cfg->reserved[1] > 0 && cfg->reserved[1] < cfg->batch_size, MPIG_EINVAL,
+                     "mpig_create: dense_tail_rows (reserved[2]) = %d needs fewer context slots than requests (num_contexts = "
+                     "reserved[1] = %d, batch_size = %d)", cfg->reserved[2], cfg->reserved[1], cfg->batch_size);
+        MPIG_REQUIRE(cfg->alloc_dense_kv, MPIG_EINVAL,
+                     "mpig_create: dense_tail_rows (reserved[2]) = %d needs alloc_dense_kv = 1 (the context owns the dense KV)",
+                     cfg->reserved[2]);
+    }
     struct RestoreDevice {
         int prev = -1;
         RestoreDevice() { if (cudaGetDevice(&prev) != cudaSuccess) prev = -1; }
@@ -149,6 +159,8 @@ int mpig_create(const mpig_config *cfg, mpig_ctx **out) {
     ctx->n_off.assign(cfg->num_layers, std::vector<int>(ctx->C, 0));
     ctx->h_slot_of.resize(cfg->batch_size);
     for (int b = 0; b < cfg->batch_size; ++b) ctx->h_slot_of[b] = b % ctx->C;
+    ctx->dense_tail_rows = cfg->reserved[2];
+    ctx->h_dense_base.assign(cfg->batch_size, 0);
 
     const size_t M = (size_t)cfg->max_length, BG = (size_t)ctx->BG, L = (size_t)cfg->L, d = (size_t)cfg->head_dim;
     const size_t SG = (size_t)ctx->C * cfg->num_key_value_heads;   // slot groups: the store and the tables are per slot
@@ -167,7 +179,12 @@ int mpig_create(const mpig_config *cfg, mpig_ctx **out) {
         LayerStore &ls = ctx->layers[l];
         if (dense) {
             ls.dense = true;
-            if (cfg->alloc_dense_kv) TRY(dev_alloc(ctx, &ls.dense_kv, BG * M * ctx->rec_bytes, false));
+            if (cfg->alloc_dense_kv && ctx->dense_tail_rows > 0) {   // the slot stores and the request tails
+                TRY(dev_alloc(ctx, &ls.dense_kv, SG * M * ctx->rec_bytes, false));
+                TRY(dev_alloc(ctx, &ls.dense_tail, BG * (size_t)ctx->dense_tail_rows * ctx->rec_bytes, false));
+            } else if (cfg->alloc_dense_kv) {
+                TRY(dev_alloc(ctx, &ls.dense_kv, BG * M * ctx->rec_bytes, false));
+            }
             continue;
         }
         ls.sparse = true;
@@ -185,6 +202,7 @@ int mpig_create(const mpig_config *cfg, mpig_ctx **out) {
     TRY(dev_alloc(ctx, &ctx->win_len, (size_t)cfg->batch_size * sizeof(int32_t)));
     TRY(dev_alloc(ctx, &ctx->dense_len, (size_t)cfg->batch_size * sizeof(int32_t)));
     TRY(dev_alloc(ctx, &ctx->slot_of, (size_t)cfg->batch_size * sizeof(int32_t)));
+    if (ctx->dense_tail_rows > 0) TRY(dev_alloc(ctx, &ctx->dense_base, (size_t)cfg->batch_size * sizeof(int32_t)));
     {
         const cudaError_t e = cudaMemcpy(ctx->slot_of, ctx->h_slot_of.data(), (size_t)cfg->batch_size * sizeof(int32_t),
                                          cudaMemcpyHostToDevice);
@@ -209,7 +227,8 @@ int mpig_create(const mpig_config *cfg, mpig_ctx **out) {
         std::vector<AcceptLayer> tab;
         for (const LayerStore &ls : ctx->layers) {
             if (ls.sparse && ctx->Wcap > 0) tab.push_back({ls.win, ctx->Wcap, 0});
-            if (ls.dense && ls.dense_kv) tab.push_back({ls.dense_kv, cfg->max_length, 1});
+            if (ls.dense && ls.dense_tail) tab.push_back({ls.dense_tail, ctx->dense_tail_rows, 1});
+            else if (ls.dense && ls.dense_kv) tab.push_back({ls.dense_kv, cfg->max_length, 1});
         }
         ctx->n_accept_layers = (int)tab.size();
         if (!tab.empty()) {
@@ -255,12 +274,14 @@ void mpig_destroy(mpig_ctx *ctx) {
         cudaFree(ls.win);
         cudaFree(ls.avg_k);
         cudaFree(ls.dense_kv);
+        cudaFree(ls.dense_tail);
     }
     cudaFree(ctx->hash_func);
     cudaFree(ctx->hash_func_t);
     cudaFree(ctx->win_len);
     cudaFree(ctx->dense_len);
     cudaFree(ctx->slot_of);
+    cudaFree(ctx->dense_base);
     cudaFree(ctx->codes);
     cudaFree(ctx->qnorm);
     cudaFree(ctx->results);
@@ -303,6 +324,8 @@ int mpig_clear(mpig_ctx *ctx, void *stream) {
     }
     MPIG_CUDA(cudaMemsetAsync(ctx->win_len, 0, ctx->cfg.batch_size * sizeof(int32_t), s));
     MPIG_CUDA(cudaMemsetAsync(ctx->dense_len, 0, ctx->cfg.batch_size * sizeof(int32_t), s));
+    if (ctx->dense_base) MPIG_CUDA(cudaMemsetAsync(ctx->dense_base, 0, ctx->cfg.batch_size * sizeof(int32_t), s));
+    for (auto &n : ctx->h_dense_base) n = 0;
     const size_t rows = (size_t)ctx->H * ctx->tok_max;   // the per-step scratch holds B*t_max*Hq rows after a reservation
     MPIG_CUDA(cudaMemsetAsync(ctx->nnz, 0, rows * sizeof(int32_t), s));
     MPIG_CUDA(cudaMemsetAsync(ctx->counters, 0, ctx->H * sizeof(int32_t), s));
@@ -476,6 +499,7 @@ int mpig_get_info(mpig_ctx *ctx, const char *key, int64_t *value) {
     else if (k == "query_tokens_max") *value = ctx->tok_max;
     else if (k == "tokens_cluster_waves") *value = ctx->last_tokens_waves;
     else if (k == "num_contexts") *value = ctx->C;
+    else if (k == "dense_tail_rows") *value = ctx->dense_tail_rows;
     else {
         set_error("mpig_get_info: unknown key '%s'", key);
         return MPIG_EINVAL;
@@ -520,11 +544,22 @@ int mpig_fork_request(mpig_ctx *ctx, int src, int dst, void *stream) {
                                             Hkv, cudaMemcpyDeviceToDevice, s));
             const size_t avg = Hkv * ctx->cfg.head_dim;
             MPIG_CUDA(cudaMemcpyAsync(ls.avg_k + dst * avg, ls.avg_k + src * avg, avg * sizeof(__nv_bfloat16), cudaMemcpyDeviceToDevice, s));
+        } else if (ls.dense_tail) {
+            // shared dense mode: the prompt stays in the slot store; only src's tail rows [0, len - base) are copied
+            const size_t pitch = (size_t)ctx->dense_tail_rows * REC;   // one kv-head's tail
+            const int rows = std::min(std::max(len[1] - ctx->h_dense_base[src], 0), ctx->dense_tail_rows);
+            if (rows > 0)
+                MPIG_CUDA(cudaMemcpy2DAsync(ls.dense_tail + dst * Hkv * pitch, pitch, ls.dense_tail + src * Hkv * pitch, pitch,
+                                            (size_t)rows * REC, Hkv, cudaMemcpyDeviceToDevice, s));
         } else if (ls.dense_kv && len[1] > 0) {
             const size_t pitch = (size_t)ctx->cfg.max_length * REC;   // one kv-head's cache
             MPIG_CUDA(cudaMemcpy2DAsync(ls.dense_kv + dst * Hkv * pitch, pitch, ls.dense_kv + src * Hkv * pitch, pitch,
                                         (size_t)len[1] * REC, Hkv, cudaMemcpyDeviceToDevice, s));
         }
+    }
+    if (ctx->dense_base) {
+        MPIG_CUDA(cudaMemcpyAsync(ctx->dense_base + dst, ctx->dense_base + src, sizeof(int32_t), cudaMemcpyDeviceToDevice, s));
+        ctx->h_dense_base[dst] = ctx->h_dense_base[src];
     }
     MPIG_CUDA(cudaMemcpyAsync(ctx->win_len + dst, ctx->win_len + src, sizeof(int32_t), cudaMemcpyDeviceToDevice, s));
     MPIG_CUDA(cudaMemcpyAsync(ctx->dense_len + dst, ctx->dense_len + src, sizeof(int32_t), cudaMemcpyDeviceToDevice, s));

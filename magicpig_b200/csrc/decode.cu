@@ -149,14 +149,19 @@ int mpig_dense_fill(mpig_ctx *ctx, int layer, int request, const void *k_bf16, c
     MPIG_REQUIRE(seq_len >= 0 && seq_len <= ctx->cfg.max_length, MPIG_EINVAL, "mpig_dense_fill: seq_len=%d exceeds max_length",
                  seq_len);
     const int Hkv = ctx->cfg.num_key_value_heads, M = ctx->cfg.max_length;
-    uint4 *rec = reinterpret_cast<uint4 *>(ls.dense_kv + (size_t)request * Hkv * M * ctx->rec_bytes);
+    // shared dense mode: the rows go to the slot the request is bound to (as the sparse fills), and they become its base
+    const bool shared = ctx->dense_tail_rows > 0;
+    const size_t owner = shared ? (size_t)ctx->h_slot_of[request] : (size_t)request;
+    uint4 *rec = reinterpret_cast<uint4 *>(ls.dense_kv + owner * Hkv * M * ctx->rec_bytes);
     if (seq_len > 0) {
         rc = launch_pack_nhd(ctx, k_bf16, v_bf16, (uint8_t *)rec, Hkv, seq_len, M, as_stream(stream));
         if (rc) return rc;
     }
     MPIG_CUDA(cudaMemcpyAsync(ctx->dense_len + request, &seq_len, sizeof(int), cudaMemcpyHostToDevice, as_stream(stream)));
+    if (shared) MPIG_CUDA(cudaMemcpyAsync(ctx->dense_base + request, &seq_len, sizeof(int), cudaMemcpyHostToDevice, as_stream(stream)));
     MPIG_CUDA(cudaStreamSynchronize(as_stream(stream)));  // seq_len is a stack variable
     ctx->h_dense_len[request] = seq_len;
+    if (shared) ctx->h_dense_base[request] = seq_len;
     return MPIG_OK;
 }
 
@@ -169,6 +174,13 @@ int mpig_dense_decode(mpig_ctx *ctx, int layer, const void *query_bf16, const vo
     MPIG_REQUIRE(ls.dense && ls.dense_kv, MPIG_ESTATE, "mpig_dense_decode: layer %d has no dense KV", layer);
     MPIG_REQUIRE(query_bf16 && key_bf16 && value_bf16 && out_bf16, MPIG_EINVAL, "mpig_dense_decode: null argument");
     cudaStream_t s = as_stream(stream);
+    if (ctx->dense_tail_rows > 0) {
+        MPIG_REQUIRE(ctx->dense_impl == 1, MPIG_EUNSUPPORTED,
+                     "mpig_dense_decode: the shared dense layout (dense_tail_rows > 0) needs the GQA-shared dense kernel (dense_impl = 1)");
+        rc = launch_append_tokens(ctx, append_params(ctx, ls, key_bf16, value_bf16, true), 1, s, ctx->dense_base);
+        if (rc) return rc;
+        return launch_attend_dense_slots(ctx, ls, 1, query_bf16, out_bf16, s, false);
+    }
     rc = launch_append_tokens(ctx, append_params(ctx, ls, key_bf16, value_bf16, true), 1, s);
     if (rc) return rc;
     if (ctx->dense_impl == 1) return launch_attend_dense(ctx, ls.dense_kv, ctx->dense_len, query_bf16, out_bf16, s, false);
@@ -213,8 +225,9 @@ int mpig_dense_decode_tokens(mpig_ctx *ctx, int layer, int T, const void *query_
     MPIG_REQUIRE(ctx->dense_impl == 1, MPIG_EUNSUPPORTED, "mpig_dense_decode_tokens: T=%d needs the GQA-shared dense kernel (dense_impl = 1)", T);
     MPIG_REQUIRE(T * ctx->G <= 32, MPIG_EUNSUPPORTED, "mpig_dense_decode_tokens: T*G = %d query rows per kv-group (at most 32)", T * ctx->G);
     cudaStream_t s = as_stream(stream);
-    rc = launch_append_tokens(ctx, append_params(ctx, ls, key_bf16, value_bf16, true), T, s);
+    rc = launch_append_tokens(ctx, append_params(ctx, ls, key_bf16, value_bf16, true), T, s, ctx->dense_base_map());
     if (rc) return rc;
+    if (ctx->dense_tail_rows > 0) return launch_attend_dense_slots(ctx, ls, T, query_bf16, out_bf16, s, true);
     return launch_attend_dense_tokens(ctx, ls.dense_kv, ctx->dense_len, T, query_bf16, out_bf16, s, true);
 }
 

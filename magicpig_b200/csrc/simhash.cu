@@ -170,15 +170,16 @@ __global__ void __launch_bounds__(SH_THREADS) simhash_kernel(const __nv_bfloat16
 }
 
 // T new rows per (request, kv-head): one warp per (b, t, kv-head).  k_new / v_new are (B, T, Hkv, D); row t of request b goes to
-// position len[b] - T + t (len already advanced by the plan).  The attention launch that reads the rows follows under
-// programmatic dependent launch.
-__global__ void append_tokens_kernel(AppendParams a, int T) {
+// position len[b] - T + t (len already advanced by the plan); with a base map (shared dense mode: a.rows are the request tails)
+// to position len[b] - T + t - base[b] of the tail.  The attention launch that reads the rows follows under programmatic
+// dependent launch.
+__global__ void append_tokens_kernel(AppendParams a, int T, const int32_t *base) {
     pdl_launch_dependents();
     const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if (warp >= a.BG * T) return;
     const int kh = warp % a.Hkv, bt = warp / a.Hkv, b = bt / T, t = bt % T;
     const int bg = b * a.Hkv + kh;
-    const int pos = a.len[b] - T + t;
+    const int pos = a.len[b] - T + t - (base ? base[b] : 0);
     if (pos < 0 || pos >= a.cap) return;
     store_row(a, bg, pos, warp, lane);   // warp = (b*T + t)*Hkv + kh: the row of the (B, T, Hkv, D) input
 }
@@ -227,9 +228,9 @@ int launch_simhash(mpig_ctx *ctx, const void *query_bf16, int32_t *codes, float 
     return MPIG_OK;
 }
 
-int launch_append_tokens(mpig_ctx *ctx, const AppendParams &ap, int T, cudaStream_t s) {
+int launch_append_tokens(mpig_ctx *ctx, const AppendParams &ap, int T, cudaStream_t s, const int32_t *base) {
     const int warps = ap.BG * T;
-    append_tokens_kernel<<<(warps + 7) / 8, 256, 0, s>>>(ap, T);
+    append_tokens_kernel<<<(warps + 7) / 8, 256, 0, s>>>(ap, T, base);
     MPIG_LAUNCH_CHECK(ctx);
     return MPIG_OK;
 }

@@ -26,15 +26,16 @@ __global__ void rewind_kernel(const int32_t *drop, int32_t *win_len, int32_t *de
 }
 
 // Lengths advance by T (1 for mpig_plan) and saturate at the capacity (the append then overwrites the last row); saturation of a
-// store that is in use raises the context's device error flag (bit 0: sparse window = generation_buffer exhausted, bit 1: dense
-// cache = max_length exhausted), readable with mpig_error_flags -- the host-side check in mpig_plan cannot see replays of a
-// captured graph.
+// store that is in use raises the context's device error flag (bit 0: sparse window = generation_buffer exhausted, bit 1: a dense
+// cache reached its capacity: dcap = max_length, or min(dcap, dense_base[b] + tail_rows) with a base map in shared dense mode),
+// readable with mpig_error_flags -- the host-side check in mpig_plan cannot see replays of a captured graph.
 // The step's node records go to step_buf: the bases (lengths after the plan minus T), the parents and the ancestor masks (bit j of
 // mask t: node j is node t or one of its ancestors).  parents == null: a chain (node t's parent is t - 1).  A malformed tree
 // (parents[b][0] != -1 or parents[b][t] outside [0, t)) raises bit 3 and request b runs as a chain.  apply = 0: only that check
 // (an eager mpig_plan_tree that refuses changes nothing).
 __global__ void plan_kernel(int32_t *win_len, int32_t *dense_len, int32_t *err_flag, int B, int T, int wcap, int dcap,
-                            int has_window, int has_dense, int32_t *step_buf, const int32_t *parents, int apply) {
+                            int has_window, int has_dense, int32_t *step_buf, const int32_t *parents, int apply,
+                            const int32_t *dense_base, int tail_rows) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b < B) {
         int par[TREE_MAX];
@@ -49,6 +50,7 @@ __global__ void plan_kernel(int32_t *win_len, int32_t *dense_len, int32_t *err_f
         }
         if (!apply) return;
         int w = win_len[b] + T, dl = dense_len[b] + T;
+        if (dense_base) dcap = min(dcap, dense_base[b] + tail_rows);
         if (w > wcap) {
             w = wcap;
             if (has_window) atomicOr(err_flag, 1);
@@ -75,12 +77,13 @@ __global__ void plan_kernel(int32_t *win_len, int32_t *dense_len, int32_t *err_f
 // warp per (row-owning layer, request, kv-head); lane l moves 16-byte chunk l (+32, ...) of each record, and reads every chunk of
 // the path before it writes any, so the in-place move needs no staging.  A path is valid when 0 <= count <= T, nodes[0] = 0 and
 // parents[nodes[i]] = nodes[i-1]; an invalid one leaves request b untouched and raises bit 3.  Rows are addressed from the step
-// bases plan_kernel recorded (never from the lengths this kernel rewrites) and stay inside each store's capacity.  The warp of
+// bases plan_kernel recorded (never from the lengths this kernel rewrites) and stay inside each store's capacity; with a base map
+// (shared dense mode) the dense entries are the request tails, where the step starts at row base - dense_base[b].  The warp of
 // (table entry 0, b, kv-head 0) sets both lengths to base + count.  apply = 0: only the check.
 __global__ void __launch_bounds__(256) accept_path_kernel(const AcceptLayer *layers, int n_layers, const int32_t *nodes,
                                                           const int32_t *count, const int32_t *step_buf, int32_t *win_len,
                                                           int32_t *dense_len, int32_t *err_flag, int B, int Hkv, int T, int rec16,
-                                                          int apply) {
+                                                          int apply, const int32_t *dense_base) {
     const int wid = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
     const int nl = max(n_layers, 1);
     if (wid >= nl * B * Hkv) return;
@@ -108,7 +111,7 @@ __global__ void __launch_bounds__(256) accept_path_kernel(const AcceptLayer *lay
     const int32_t *bases = step_bases(step_buf, B);
     if (li < n_layers) {
         const AcceptLayer ly = layers[li];
-        const int base = bases[2 * b + ly.dense];
+        const int base = bases[2 * b + ly.dense] - ((ly.dense && dense_base) ? dense_base[b] : 0);
         uint4 *rows = reinterpret_cast<uint4 *>(ly.rows + ((size_t)b * Hkv + head) * (size_t)ly.cap * rec16 * 16);
         for (int ch = lane; ch < rec16; ch += 32) {
             uint4 v[TREE_MAX];
@@ -143,8 +146,9 @@ static int plan_checks(mpig_ctx *ctx, int T, bool has_window, bool has_dense, co
         MPIG_REQUIRE(!has_window || ctx->h_win_len[b] + T <= ctx->Wcap, MPIG_ESTATE,
                      "%s: request %d: the sparse window is full (%d rows = sink + local + generation_buffer); "
                      "raise generation_buffer or clear()", who, b, ctx->Wcap);
-        MPIG_REQUIRE(!has_dense || ctx->h_dense_len[b] == 0 || ctx->h_dense_len[b] + T <= ctx->cfg.max_length, MPIG_ESTATE,
-                     "%s: request %d: the dense KV cache is full (max_length = %d)", who, b, ctx->cfg.max_length);
+        MPIG_REQUIRE(!has_dense || ctx->h_dense_len[b] == 0 || ctx->h_dense_len[b] + T <= ctx->dense_cap(b), MPIG_ESTATE,
+                     "%s: request %d: the dense KV cache is full (capacity %d rows: %s)", who, b, ctx->dense_cap(b),
+                     ctx->dense_tail_rows > 0 ? "the prompt base + dense_tail_rows, or max_length" : "max_length");
     }
     return MPIG_OK;
 }
@@ -169,11 +173,12 @@ static int plan_step(mpig_ctx *ctx, int T, cudaStream_t s, const char *who, cons
         if (rc) return rc;
         for (int b = 0; b < B; ++b) {
             ctx->h_win_len[b] = std::min(ctx->h_win_len[b] + T, ctx->Wcap);
-            ctx->h_dense_len[b] = std::min(ctx->h_dense_len[b] + T, ctx->cfg.max_length);
+            ctx->h_dense_len[b] = std::min(ctx->h_dense_len[b] + T, ctx->dense_cap(b));
         }
     }
     plan_kernel<<<(B + 127) / 128, 128, 0, s>>>(ctx->win_len, ctx->dense_len, ctx->err_flag, B, T, ctx->Wcap, ctx->cfg.max_length,
-                                               has_window, has_dense, ctx->step_buf, parents, 1);
+                                               has_window, has_dense, ctx->step_buf, parents, 1, ctx->dense_base_map(),
+                                               ctx->dense_tail_rows);
     MPIG_LAUNCH_CHECK(ctx);
     ctx->pending.begin(T, parents != nullptr);
     return MPIG_OK;
@@ -199,7 +204,7 @@ static int launch_accept(mpig_ctx *ctx, const int32_t *nodes, const int32_t *cou
     const int warps = std::max(ctx->n_accept_layers, 1) * B * Hkv;
     accept_path_kernel<<<(warps + 7) / 8, 256, 0, s>>>((const AcceptLayer *)ctx->accept_layers, ctx->n_accept_layers, nodes, count,
                                                        ctx->step_buf, ctx->win_len, ctx->dense_len, ctx->err_flag, B, Hkv, T,
-                                                       ctx->rec_bytes / 16, apply);
+                                                       ctx->rec_bytes / 16, apply, ctx->dense_base_map());
     MPIG_LAUNCH_CHECK(ctx);
     return MPIG_OK;
 }
@@ -309,7 +314,7 @@ int mpig_plan_tree(mpig_ctx *ctx, int T, const int32_t *parents, void *stream) {
         [&](int apply) -> int {
             if (apply) return plan_step(ctx, T, s, "mpig_plan_tree", parents);
             plan_kernel<<<(B + 127) / 128, 128, 0, s>>>(ctx->win_len, ctx->dense_len, ctx->err_flag, B, T, ctx->Wcap,
-                                                       ctx->cfg.max_length, 0, 0, ctx->step_buf, parents, 0);
+                                                       ctx->cfg.max_length, 0, 0, ctx->step_buf, parents, 0, nullptr, 0);
             MPIG_LAUNCH_CHECK(ctx);
             return MPIG_OK;
         });
