@@ -77,7 +77,7 @@ __device__ __forceinline__ int atom_add_acq_rel_cta_shared(int *addr, int v) {
 // contributor to arrive (acq_rel ticket counters, no barrier, no second kernel):
 //   level 1  parts inside one CTA      -> shared-memory slots + shared-memory ticket
 //   level 2  CTAs that share the head  -> global scratch slots (2 per CTA: head entering / head leaving) + ticket
-// smem: ring [warps][32][528] | bars [warps] u64 | s_part [warps][132] f32 | s_own [warps][132] f32
+// smem: ring [warps][32][528] | bars [warps rounded up to even] u64 | s_part [warps][132] f32 | s_own [warps][132] f32
 //       | s_cnt [warps] | s_wlen [B] | s_prefix [H+1] | s_wpre [H+1]
 template <bool USE_TMA, bool DBG>
 __global__ void __launch_bounds__(384, 1) attend_mma_kernel(const __grid_constant__ AttendParams gp) {
@@ -97,7 +97,7 @@ __global__ void __launch_bounds__(384, 1) attend_mma_kernel(const __grid_constan
     uint8_t *slots = smem + (size_t)warp * TILE * SLOT;
     uint8_t *sp = smem + (size_t)warps * TILE * SLOT;
     uint64_t *bar = reinterpret_cast<uint64_t *>(sp) + warp;
-    sp += (size_t)warps * sizeof(uint64_t);
+    sp += (size_t)((warps + 1) & ~1) * sizeof(uint64_t);   // padded to 16 bytes: the state slots below are read / written as float4
     float *s_part = reinterpret_cast<float *>(sp);
     sp += (size_t)warps * PART_FLOATS * sizeof(float);
     float *s_own = reinterpret_cast<float *>(sp) + (size_t)warp * PART_FLOATS;
@@ -446,7 +446,7 @@ int launch_attend_mma(mpig_ctx *ctx, const AttendParams &p_in, cudaStream_t s, b
     p.dbg = ctx->attend_debug ? ctx->dbg_buf : nullptr;
     p.skip = ctx->attend_skip;
     if (p.dbg) MPIG_CUDA(cudaMemsetAsync(p.dbg, 0, (size_t)ctx->max_partial_warps * 16 * sizeof(unsigned long long), s));
-    const size_t smem = (size_t)warps * TILE * SLOT + (size_t)warps * 8 + (size_t)warps * 2 * PART_FLOATS * 4 + (size_t)warps * 4 +
+    const size_t smem = (size_t)warps * TILE * SLOT + (size_t)((warps + 1) & ~1) * 8 + (size_t)warps * 2 * PART_FLOATS * 4 + (size_t)warps * 4 +
                         (size_t)(p.H / p.Hq) * 4 + 2 * (size_t)(p.H + 1) * sizeof(int) + 16;
     MPIG_REQUIRE(smem <= 226 * 1024, MPIG_EINVAL, "attend(mma): warps=%d H=%d needs %zu B shared memory (> 227 KB)", warps, p.H, smem);
     MPIG_FUNC_ATTR((attend_mma_kernel<true, false>), cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024);
