@@ -338,6 +338,7 @@ int mpig_accept(mpig_ctx *ctx, const int32_t *nodes, const int32_t *count, void 
 /* k, v bf16 (P, Hkv, d) -- the prefill cache in NHD layout as models/llama.py:282 passes it. */
 int mpig_dense_fill(mpig_ctx *ctx, int layer, int request, const void *k_bf16, const void *v_bf16,
                     int seq_len, void *stream);
+/* Single-token dense decode.  MPIG_EUNSUPPORTED for G = Hq / Hkv > 32 with dense_impl = 1. */
 int mpig_dense_decode(mpig_ctx *ctx, int layer, const void *query_bf16, const void *key_bf16,
                       const void *value_bf16, void *out_bf16, void *stream);
 

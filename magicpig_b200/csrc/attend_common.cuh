@@ -29,6 +29,20 @@ __device__ __forceinline__ void mma_16816(float &c0, float &c1, float &c2, float
                  : "+f"(c0), "+f"(c1), "+f"(c2), "+f"(c3)
                  : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
+__device__ __forceinline__ void mma_16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+    mma_16816(c[0], c[1], c[2], c[3], a, b0, b1);
+}
+// tickets of the last-arriver merges
+__device__ __forceinline__ int atom_add_acq_rel_gpu(int *addr, int v) {
+    int old;
+    asm volatile("atom.acq_rel.gpu.global.add.s32 %0, [%1], %2;" : "=r"(old) : "l"(addr), "r"(v) : "memory");
+    return old;
+}
+__device__ __forceinline__ int atom_add_acq_rel_cta_shared(int *addr, int v) {
+    int old;
+    asm volatile("atom.acq_rel.cta.shared.add.s32 %0, [%1], %2;" : "=r"(old) : "r"(smem_u32(addr)), "r"(v) : "memory");
+    return old;
+}
 // x^n, 0 <= n < 2^NBITS, by repeated squaring in fp64 (error ~n_mults * 1e-16), rounded once to fp32.  The trip count is a
 // compile-time constant and the multiply is predicated, so the (uniform) exponent costs no loop control: 2 * NBITS - 1 DMUL.
 template <int NBITS>

@@ -2,57 +2,30 @@
 // context (prefill rows + generated rows), the part the reference hands to FlashInfer's paged decode.
 //
 // Unlike the sampled layers, all G q-heads of a kv-group read the SAME rows, so the kernel is organised per
-// (request, kv-head) group: each fetched 512-byte K|V record is used for all G heads (G <= 8), i.e. HBM and L2 see
-// every record once (the generic gather kernel in range mode fetched it G times and was L2-bound).  Heads sit on the
-// M axis of the tensor-core tiles:
-//     S^T (heads x 32 rows) = Q_g (16 x 128, rows >= G zero) . K_tile^T      A = Q fragments (registers), B = K rows (ldmatrix)
-//     O   (heads x 128)    += P (16 x 32) . V_tile                            rows 0..7 of A = bf16(p), rows 8..15 = bf16(p - bf16(p))
-// so the score accumulators of one lane are exactly the A fragment of the second product (no shuffles), and the
-// hi/lo split of the probabilities rides in the otherwise unused rows 8..15.
+// (request, kv-head) group: each fetched 512-byte K|V record is used for all T*G <= 32 query rows of the group (G heads for
+// each of the step's T tokens), i.e. HBM and L2 see every record once (the generic gather kernel in range mode fetched it G
+// times and was L2-bound), and dense KV bytes per step do not grow with T.  Query rows sit on the M axis of the tensor-core
+// tiles:
+//     S^T (rows x 32 keys) = Q_g (16 x 128) . K_tile^T      A = Q fragments (registers), B = K rows (ldmatrix)
+//     O   (rows x 128)    += P (16 x 32) . V_tile           P as bf16(p) + bf16(p - bf16(p))
+// so the score accumulators of one lane are exactly the A fragment of the second product (no shuffles).
 // Work decomposition, fetch (one cp.async.bulk per row, 528-byte slots) and the two-level last-arriver merge are the
 // ones of attend_mma.cu with "kv-group" in place of "head".
 #include "attend_common.cuh"
 
 namespace mpig {
 
-constexpr int DSLOT = REC + 16;          // 528 B
-constexpr int GMAX = 8;
-constexpr int GPART = GMAX * PART_FLOATS;  // floats per partial state of a group
-
 struct DenseParams {
     const uint8_t *kv;       // [BG][M] records
     const int32_t *len;      // [B]
-    const __nv_bfloat16 *q;  // [H][D]
-    __nv_bfloat16 *out;      // [H][D]
-    float *out_f32;          // [H][D] or null: the output before the bf16 rounding (option "out_f32")
-    float *partials;         // [grid][2][GPART]
+    const __nv_bfloat16 *q;  // [B][T][Hq][D]
+    __nv_bfloat16 *out;      // [B][T][Hq][D]
+    float *out_f32;          // [B][T][Hq][D] or null: the output before the bf16 rounding (option "out_f32")
+    float *partials;         // [grid][2][query rows per group][PART_FLOATS]
     int32_t *counters;       // [BG]
     int BG, G, Hkv, Hq, M;
 };
 
-__device__ __forceinline__ void ldsm4(uint32_t (&r)[4], uint32_t saddr) {
-    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(saddr));
-}
-__device__ __forceinline__ void ldsm4t(uint32_t (&r)[4], uint32_t saddr) {
-    asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
-                 : "r"(saddr));
-}
-__device__ __forceinline__ void mma16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ int atom_add_acq_rel_gpu_d(int *addr, int v) {
-    int old;
-    asm volatile("atom.acq_rel.gpu.global.add.s32 %0, [%1], %2;" : "=r"(old) : "l"(addr), "r"(v) : "memory");
-    return old;
-}
-__device__ __forceinline__ int atom_add_acq_rel_cta_shared_d(int *addr, int v) {
-    int old;
-    asm volatile("atom.acq_rel.cta.shared.add.s32 %0, [%1], %2;" : "=r"(old) : "r"(smem_u32(addr)), "r"(v) : "memory");
-    return old;
-}
 __device__ __forceinline__ void finalize_dense_head(const DenseParams &p, int h, float l, const float acc[4], int lane) {
     __nv_bfloat16 *out = p.out;
     const float inv = (l > 0.f) ? 1.0f / l : 0.f;
@@ -105,10 +78,6 @@ __device__ __forceinline__ void dense_partition_of(RowsOf rows_of, int BG, int *
     }
     if (lane == 0) s_wpre[BG] = run;
 }
-// one group per (request, kv-head) over its dense_len rows
-__device__ __forceinline__ void dense_partition(const DenseParams &p, int *s_prefix, int *s_wpre, int nw, int lane) {
-    dense_partition_of([&](int bg) { return min(max(p.len[bg / p.Hkv], 0), p.M); }, p.BG, s_prefix, s_wpre, nw, lane);
-}
 
 // the group work item `item` belongs to (s_wpre ascending)
 __device__ __forceinline__ int dense_item_group(const int *s_wpre, int BG, int item) {
@@ -121,250 +90,18 @@ __device__ __forceinline__ int dense_item_group(const int *s_wpre, int BG, int i
     return a;
 }
 
-// smem: ring [warps][32][528] (reused as merge scratch once a warp's rows are done) | bars [warps] u64 | s_cnt [warps]
-//       | s_prefix [BG+1] | s_wpre [BG+1]
-__global__ void __launch_bounds__(384) attend_dense_kernel(const DenseParams p) {
-    extern __shared__ __align__(128) uint8_t smem[];
-    const int warps = blockDim.x >> 5, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    uint8_t *slots = smem + (size_t)warp * TILE * DSLOT;
-    uint8_t *sp = smem + (size_t)warps * TILE * DSLOT;
-    uint64_t *bar = reinterpret_cast<uint64_t *>(sp) + warp;
-    sp += (size_t)warps * sizeof(uint64_t);
-    int *s_cnt = reinterpret_cast<int *>(sp);
-    sp += (size_t)warps * sizeof(int);
-    int *s_prefix = reinterpret_cast<int *>(sp);
-    int *s_wpre = s_prefix + p.BG + 1;
-    // merge scratch inside each warp's (by then idle) ring: own state at +0, level-1 slot at +GPART floats
-    float *s_own = reinterpret_cast<float *>(slots);
-    auto s_part_of = [&](int w) { return reinterpret_cast<float *>(smem + (size_t)w * TILE * DSLOT) + GPART; };
-
-    if (lane == 0) {
-        mbar_init(bar, 1);
-        fence_proxy_async();  // init visible to the async proxy (a cluster-scope mbarrier_init fence costs an L1 invalidate: ~4.7 us measured)
-    }
-    if (threadIdx.x < warps) s_cnt[threadIdx.x] = 0;
-    pdl_wait();
-
-    const int nw = gridDim.x * warps;
-    if (warp == 0) dense_partition(p, s_prefix, s_wpre, nw, lane);
-    __syncthreads();
-    pdl_launch_dependents();
-
-    const int u = blockIdx.x * warps + warp;
-    const int n_items = s_wpre[p.BG];
-    const int cta_w0 = blockIdx.x * warps;
-    const int G = p.G;
-
-    // groups without rows: zero outputs
-    for (int bg = u; bg < p.BG; bg += nw) {
-        if (s_prefix[bg + 1] == s_prefix[bg]) {
-            const float z4[4] = {0.f, 0.f, 0.f, 0.f};
-            for (int hh = 0; hh < G; ++hh) finalize_dense_head(p, (bg / p.Hkv) * p.Hq + (bg % p.Hkv) * G + hh, 0.f, z4, lane);
-        }
-    }
-
-    const float scale_log2 = rsqrtf((float)D) * LOG2E_F;
-    const int grp = lane >> 2, tig = lane & 3;
-    const uint32_t slots_s = smem_u32(slots);
-    // ldmatrix lane offsets: K rows as the B operand of S^T (non-transposed), V rows as the B operand of O (transposed)
-    const uint32_t k_lane_off = (uint32_t)(((lane & 7) + (lane >> 4) * 8) * DSLOT + ((lane >> 3) & 1) * 16);
-    const uint32_t v_lane_off = (uint32_t)(((lane & 7) + ((lane >> 3) & 1) * 8) * DSLOT + D * 2 + (lane >> 4) * 16);
-    uint32_t phase = 0;
-
-    for (int item = u; item < n_items; item += nw) {
-        const int bg = dense_item_group(s_wpre, p.BG, item);
-        const int T = s_prefix[bg + 1] - s_prefix[bg];
-        const int w_g = s_wpre[bg + 1] - s_wpre[bg];
-        const int part = item - s_wpre[bg];
-        const int c_g = (T + w_g - 1) / w_g;
-        const int r_lo = part * c_g, r_hi = min(r_lo + c_g, T);
-        const int h_base = (bg / p.Hkv) * p.Hq + (bg % p.Hkv) * G;
-        const uint8_t *rows = p.kv + (size_t)bg * p.M * REC;
-
-        // Q fragments: row grp of the A operand = head h_base + grp (zero rows for grp >= G)
-        uint32_t qa[8][2];
-        {
-            const uint32_t *q32 = reinterpret_cast<const uint32_t *>(p.q + (size_t)(h_base + min(grp, G - 1)) * D);
-#pragma unroll
-            for (int ks = 0; ks < 8; ++ks) {
-                qa[ks][0] = (grp < G) ? __ldg(q32 + ks * 8 + tig) : 0u;
-                qa[ks][1] = (grp < G) ? __ldg(q32 + ks * 8 + 4 + tig) : 0u;
-            }
-        }
-        __syncwarp();
-        fence_proxy_async();  // merge scratch of a previous item lives in the ring the next copies will overwrite
-        float m_run = -CUDART_INF_F, l_run = 0.f;  // of head grp (replicated over tig)
-        float acc[16][4];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) acc[i][0] = acc[i][1] = acc[i][2] = acc[i][3] = 0.f;
-
-        for (int cr = r_lo; cr < r_hi; cr += TILE) {
-            const int nrows = min(TILE, r_hi - cr);
-            if (lane == 0) mbar_arrive_expect_tx(bar, (uint32_t)nrows * REC);
-            __syncwarp();
-            if (lane < nrows) {
-                bulk_g2s(slots + (size_t)lane * DSLOT, rows + (size_t)(cr + lane) * REC, REC, bar);
-            } else {
-                uint4 *vz = reinterpret_cast<uint4 *>(slots + (size_t)lane * DSLOT);  // K and V bytes must be finite
-#pragma unroll
-                for (int i = 0; i < 32; ++i) vz[i] = make_uint4(0, 0, 0, 0);
-            }
-            __syncwarp();
-            mbar_wait(bar, phase);
-            phase ^= 1;
-
-            // ---- S^T = Q_g . K_tile^T : 4 n-tiles of 8 rows ---------------------------------------------------
-            float s[4][4];
-#pragma unroll
-            for (int nt = 0; nt < 4; ++nt) s[nt][0] = s[nt][1] = s[nt][2] = s[nt][3] = 0.f;
-#pragma unroll
-            for (int ks = 0; ks < 8; ++ks) {
-                const uint32_t a[4] = {qa[ks][0], 0u, qa[ks][1], 0u};
-#pragma unroll
-                for (int j = 0; j < 2; ++j) {
-                    uint32_t b[4];
-                    ldsm4(b, slots_s + (uint32_t)(j * 16 * DSLOT + ks * 32) + k_lane_off);
-                    mma16816(s[2 * j], a, b[0], b[1]);
-                    mma16816(s[2 * j + 1], a, b[2], b[3]);
-                }
-            }
-            // ---- online softmax of head grp over this tile's rows (lane holds rows nt*8 + tig*2 + {0,1}) --------
-            float mloc = -CUDART_INF_F;
-#pragma unroll
-            for (int nt = 0; nt < 4; ++nt)
-#pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                    const int r = nt * 8 + tig * 2 + e;
-                    s[nt][e] = (r < nrows) ? s[nt][e] * scale_log2 : -CUDART_INF_F;
-                    mloc = fmaxf(mloc, s[nt][e]);
-                }
-            mloc = fmaxf(mloc, __shfl_xor_sync(0xffffffffu, mloc, 1));
-            mloc = fmaxf(mloc, __shfl_xor_sync(0xffffffffu, mloc, 2));
-            const float m_new = fmaxf(m_run, mloc);
-            const float corr = (m_run == -CUDART_INF_F) ? 0.f : exp2f(m_run - m_new);
-            float lsum = 0.f;
-#pragma unroll
-            for (int nt = 0; nt < 4; ++nt)
-#pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                    s[nt][e] = exp2f(s[nt][e] - m_new);  // exp2f(-inf) = 0 for masked rows
-                    lsum += s[nt][e];
-                }
-            lsum += __shfl_xor_sync(0xffffffffu, lsum, 1);
-            lsum += __shfl_xor_sync(0xffffffffu, lsum, 2);
-            l_run = l_run * corr + lsum;
-            m_run = m_new;
-            if (cr > r_lo) {
-#pragma unroll
-                for (int i = 0; i < 16; ++i) {
-                    acc[i][0] *= corr; acc[i][1] *= corr; acc[i][2] *= corr; acc[i][3] *= corr;
-                }
-            }
-            // ---- O += P . V : the score accumulators ARE the A fragment; lo parts go to rows 8..15 --------------
-#pragma unroll
-            for (int ks = 0; ks < 2; ++ks) {
-                uint32_t a[4];
-#pragma unroll
-                for (int half = 0; half < 2; ++half) {
-                    const float p0 = s[2 * ks + half][0], p1 = s[2 * ks + half][1];
-                    const uint32_t h0 = f32_to_bf16_rne(p0), h1 = f32_to_bf16_rne(p1);
-                    const uint32_t l0 = f32_to_bf16_rne(p0 - bf16_bits_to_f32(h0)), l1 = f32_to_bf16_rne(p1 - bf16_bits_to_f32(h1));
-                    a[2 * half] = h0 | (h1 << 16);      // a0 / a2: row grp      (hi)
-                    a[2 * half + 1] = l0 | (l1 << 16);  // a1 / a3: row grp + 8  (lo)
-                }
-#pragma unroll
-                for (int n2 = 0; n2 < 8; ++n2) {
-                    uint32_t b[4];
-                    ldsm4t(b, slots_s + (uint32_t)(ks * 16 * DSLOT + n2 * 32) + v_lane_off);
-                    mma16816(acc[2 * n2], a, b[0], b[1]);
-                    mma16816(acc[2 * n2 + 1], a, b[2], b[3]);
-                }
-            }
-            __syncwarp();
-            fence_proxy_async();
-        }
-
-        // ---- part done: states of the G heads -> [G][132] floats in the warp's idle ring --------------------------
-        __syncwarp();
-        if (grp < G) {
-            float *st = s_own + (size_t)grp * PART_FLOATS;
-            if (tig == 0) {
-                st[0] = m_run * 0.6931471805599453f;  // running max is kept in base-2 units here; states carry natural units
-                st[1] = l_run;
-            }
-#pragma unroll
-            for (int nt = 0; nt < 16; ++nt)
-                *reinterpret_cast<float2 *>(st + 4 + nt * 8 + tig * 2) = make_float2(acc[nt][0] + acc[nt][2], acc[nt][1] + acc[nt][3]);
-        }
-        __syncwarp();
-
-        const int i0 = s_wpre[bg], i1 = i0 + w_g - 1;
-        const int wa = max(i0, cta_w0), wb = min(i1, cta_w0 + warps - 1);
-        bool carry = true;
-        if (w_g > 1 && wb > wa) {
-            // level 1: publish own states into the level-1 slot, last arriver of this CTA combines
-            float *mine = s_part_of(warp);
-            for (int t = lane; t < G * PART_FLOATS; t += 32) mine[t] = s_own[t];
-            __syncwarp();
-            int ticket = 0;
-            if (lane == 0) ticket = atom_add_acq_rel_cta_shared_d(&s_cnt[wa - cta_w0], 1);
-            ticket = __shfl_sync(0xffffffffu, ticket, 0);
-            carry = (ticket == wb - wa);
-        }
-        if (!carry) continue;
-        const int cta_first = i0 / warps, cta_last = i1 / warps;
-        const bool need_l1 = (w_g > 1 && wb > wa);
-        const bool need_l2 = (w_g > 1 && cta_first != cta_last);
-        int ticket2 = 0;
-        float *gslot = p.partials + ((size_t)blockIdx.x * 2 + ((i0 >= cta_w0) ? 1 : 0)) * GPART;
-        // combine level 1 per head, then either finalise or publish for level 2
-        for (int hh = 0; hh < G; ++hh) {
-            float M_, L_, A[4];
-            if (need_l1) {
-                merge_states<false>([&](int i) { return (const float *)(s_part_of(wa - cta_w0 + i) + (size_t)hh * PART_FLOATS); },
-                                    wb - wa + 1, lane, M_, L_, A);
-            } else {
-                const float *st = s_own + (size_t)hh * PART_FLOATS;
-                M_ = st[0];
-                L_ = st[1];
-                const float4 o4 = *reinterpret_cast<const float4 *>(st + 4 + 4 * lane);
-                A[0] = o4.x; A[1] = o4.y; A[2] = o4.z; A[3] = o4.w;
-            }
-            if (!need_l2) finalize_dense_head(p, h_base + hh, L_, A, lane);
-            else store_state(gslot + (size_t)hh * PART_FLOATS, M_, L_, A, lane);
-        }
-        if (!need_l2) continue;
-        __syncwarp();
-        if (lane == 0) ticket2 = atom_add_acq_rel_gpu_d(p.counters + bg, 1);
-        ticket2 = __shfl_sync(0xffffffffu, ticket2, 0);
-        if (ticket2 == cta_last - cta_first) {
-            for (int hh = 0; hh < G; ++hh) {
-                float M_, L_, A[4];
-                merge_states<true>(
-                    [&](int i) {
-                        const int c2 = cta_first + i;
-                        return (const float *)(p.partials + ((size_t)c2 * 2 + ((i0 >= c2 * warps) ? 1 : 0)) * GPART + (size_t)hh * PART_FLOATS);
-                    },
-                    cta_last - cta_first + 1, lane, M_, L_, A);
-                finalize_dense_head(p, h_base + hh, L_, A, lane);
-            }
-            if (lane == 0) p.counters[bg] = 0;
-        }
-    }
-}
-
-// ---- verification step of T tokens ------------------------------------------------------------------------------------------
-// The same per-(request, kv-head) organisation for the T*G <= 32 query rows of a group: row r = t*G + j is q-head j of the group
-// for token t, the rows sit on the M axis of NMT m16 tiles, and every K|V record is fetched ONCE for all of them (dense KV bytes per
-// step do not grow with T).  Token t sees the rows [0, len - T) before the step and those of the step's rows len - T + j whose bit j
-// is set in its ancestor mask anc[b*T + t] (plan_kernel; a chain sets bits 0..t, i.e. rows [0, len - (T-1-t)): causal).
-//   PACK (T*G <= 8): one m-tile whose rows 8..15 are free carry the lo halves of the bf16 hi/lo split of P, as above;
+// ---- query rows, masks, merge ------------------------------------------------------------------------------------------------
+// Row r = t*G + j of a group is q-head j of the group for token t; the rows sit on the M axis of NMT m16 tiles.  Token t sees the
+// rows [0, len - T) before the step and those of the step's rows len - T + j whose bit j is set in its ancestor mask anc[b*T + t]
+// (plan_kernel; a chain sets bits 0..t, i.e. rows [0, len - (T-1-t)): causal).  anc = null is a single-token decode: the step row
+// is visible, and the step buffer is not read.
+//   PACK (T*G <= 8): one m-tile whose rows 8..15 are free carry the lo halves of the bf16 hi/lo split of P;
 //   otherwise the lo halves are a second pass of MMAs over each m-tile into the same accumulators.
 // States of the T*G rows fill a warp's whole ring (32 x 132 floats at T*G = 32): the CTA-level merge reads the other warps' rings in
 // place.  That is safe because a warp whose group is split (w_g > 1) never takes a second item (see the partition: then the items
 // number at most the warps).
 //
-// SLOTS (attend_dense_slot_kernel, shared dense mode): a group is (chunk, kv-head) instead, where a chunk is up to sl.cm requests
+// SLOTS (shared dense mode): a group is (chunk, kv-head) instead, where a chunk is up to sl.cm requests
 // bound to one slot (dense_slot_chunks).  Its query rows are (member, t, j), member-major; its rows are the chunk's prefix in the
 // slot store, read once for all members, then each member's tail.  Prefix row k is visible to a member when k < its base; a
 // member's tail rows are visible to its own query rows only, the step rows among them by the ancestor mask as above.
@@ -429,12 +166,17 @@ __device__ __forceinline__ void dense_slot_chunks(const DenseParams &p, const De
     }
 }
 
+// smem: ring [warps][32][528] (reused as merge scratch once a warp's rows are done) | bars [warps] u64 | s_cnt [warps]
+//       | s_prefix [BG+1] | s_wpre [BG+1] | SLOTS: the chunks (below)
+// Up to 384 threads for the packed default-layout instantiation, which single-token decode launches with 12 warps (168 registers);
+// the other instantiations need more than the 168 registers a 384-thread bound allows, or spill under it.
 template <int NMT, bool PACK, bool SLOTS>
-__device__ __forceinline__ void dense_tokens_body(const DenseParams &p, int T, const int32_t *anc, const DenseSlots sl) {
+__global__ void __launch_bounds__((PACK && !SLOTS) ? 384 : 256)
+    attend_dense_kernel(const DenseParams p, int T, const int32_t *anc, const DenseSlots sl) {
     extern __shared__ __align__(128) uint8_t smem[];
     const int warps = blockDim.x >> 5, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    uint8_t *slots = smem + (size_t)warp * TILE * DSLOT;
-    uint8_t *sp = smem + (size_t)warps * TILE * DSLOT;
+    uint8_t *slots = smem + (size_t)warp * TILE * SLOT;
+    uint8_t *sp = smem + (size_t)warps * TILE * SLOT;
     uint64_t *bar = reinterpret_cast<uint64_t *>(sp) + warp;
     sp += (size_t)warps * sizeof(uint64_t);
     int *s_cnt = reinterpret_cast<int *>(sp);
@@ -444,7 +186,7 @@ __device__ __forceinline__ void dense_tokens_body(const DenseParams &p, int T, c
     // SLOTS: s_order [B] | s_pre [B] | s_tbeg [B] | s_tend [B] | s_cstart [B + 2] (dense_slot_chunks)
     int *s_order = s_wpre + p.BG + 1, *s_pre = s_order + sl.B, *s_tbeg = s_pre + sl.B, *s_tend = s_tbeg + sl.B, *s_cstart = s_tend + sl.B;
     float *s_own = reinterpret_cast<float *>(slots);
-    auto s_part_of = [&](int w) { return reinterpret_cast<float *>(smem + (size_t)w * TILE * DSLOT); };
+    auto s_part_of = [&](int w) { return reinterpret_cast<float *>(smem + (size_t)w * TILE * SLOT); };
     const int G = p.G, TG = T * G;
     const int QS = SLOTS ? sl.cm * TG : TG;   // query rows a group may have: the stride of its states in the partial scratch
 
@@ -463,7 +205,7 @@ __device__ __forceinline__ void dense_tokens_body(const DenseParams &p, int T, c
             dense_partition_of([&](int g) { return s_tend[s_cstart[g / p.Hkv + 1] - 1]; }, s_cstart[sl.B + 1] * p.Hkv, s_prefix, s_wpre,
                                nw, lane);
         } else {
-            dense_partition(p, s_prefix, s_wpre, nw, lane);   // the partition of attend_dense_kernel
+            dense_partition_of([&](int g) { return min(max(p.len[g / p.Hkv], 0), p.M); }, p.BG, s_prefix, s_wpre, nw, lane);
         }
     }
     __syncthreads();
@@ -495,10 +237,14 @@ __device__ __forceinline__ void dense_tokens_body(const DenseParams &p, int T, c
     const float scale_log2 = rsqrtf((float)D) * LOG2E_F;
     const int grp = lane >> 2, tig = lane & 3;
     const uint32_t slots_s = smem_u32(slots);
-    const uint32_t k_lane_off = (uint32_t)(((lane & 7) + (lane >> 4) * 8) * DSLOT + ((lane >> 3) & 1) * 16);
-    const uint32_t v_lane_off = (uint32_t)(((lane & 7) + ((lane >> 3) & 1) * 8) * DSLOT + D * 2 + (lane >> 4) * 16);
+    const uint32_t k_lane_off = (uint32_t)(((lane & 7) + (lane >> 4) * 8) * SLOT + ((lane >> 3) & 1) * 16);
+    const uint32_t v_lane_off = (uint32_t)(((lane & 7) + ((lane >> 3) & 1) * 8) * SLOT + D * 2 + (lane >> 4) * 16);
     constexpr int NI = PACK ? 1 : 2;   // query rows a lane holds per m-tile: grp (and grp + 8)
     constexpr bool QREG = (NMT == 1);  // one m-tile: the q fragments stay in registers; two: re-read per tile (L1)
+    // the instantiation single-token decode runs: output rows read from one lane each, tile visibility as a bitmask (a division by
+    // G per row and a branch per score measurably slow it; the other instantiations keep the per-row and per-score forms, which
+    // cost them fewer registers and spills)
+    constexpr bool FAST = PACK && !SLOTS;
     uint32_t phase = 0;
 
     for (int item = u; item < n_items; item += nw) {
@@ -509,6 +255,8 @@ __device__ __forceinline__ void dense_tokens_body(const DenseParams &p, int T, c
         const int c_g = (len + w_g - 1) / w_g;
         const int r_lo = part * c_g, r_hi = min(r_lo + c_g, len);
         const int qr = rows_q(bg);
+        // FAST: lane r computes the output row of query row r, for the q rows below and the merge
+        const int lane_row = FAST ? out_row(bg, min(lane, qr - 1)) : 0;
         // SLOTS: the chunk's first position, its prefix rows, and the slot store rows of this kv-head
         const int cs = SLOTS ? s_cstart[bg / p.Hkv] : 0, pc = SLOTS ? s_tbeg[cs] : 0;
         const uint8_t *rows = SLOTS ? p.kv + ((size_t)sl.slot_of[s_order[cs]] * p.Hkv + bg % p.Hkv) * p.M * REC
@@ -538,7 +286,8 @@ __device__ __forceinline__ void dense_tokens_body(const DenseParams &p, int T, c
             for (int i = 0; i < 2; ++i) {
                 const int r = mt * 16 + i * 8 + grp;
                 const bool ok = r < qr && !(PACK && i == 1);
-                qrow[mt][i] = ok ? reinterpret_cast<const uint32_t *>(p.q + (size_t)out_row(bg, r) * D) : nullptr;
+                const int row = FAST ? __shfl_sync(0xffffffffu, lane_row, r) : 0;
+                qrow[mt][i] = ok ? reinterpret_cast<const uint32_t *>(p.q + (size_t)(FAST ? row : out_row(bg, r)) * D) : nullptr;
                 if constexpr (SLOTS) {
                     const int m = cs + r / TG;   // the member's position (valid when ok)
                     lim[mt][i] = ok ? s_tend[m] - T : 0x3fffffff;
@@ -547,7 +296,7 @@ __device__ __forceinline__ void dense_tokens_body(const DenseParams &p, int T, c
                     tb[mt][i] = ok ? s_tbeg[m] : 0;
                 } else {
                     lim[mt][i] = ok ? len - T : len;
-                    vis[mt][i] = ok ? (uint32_t)__ldg(anc + (bg / p.Hkv) * T + r / G) : 0u;
+                    vis[mt][i] = ok ? (anc ? (uint32_t)__ldg(anc + (bg / p.Hkv) * T + r / G) & ((1u << TREE_MAX) - 1u) : 1u) : 0u;
                 }
             }
         auto q_frag = [&](int mt, int ks, uint32_t (&a)[4]) {
@@ -578,9 +327,9 @@ __device__ __forceinline__ void dense_tokens_body(const DenseParams &p, int T, c
             if (lane == 0) mbar_arrive_expect_tx(bar, (uint32_t)nrows * REC);
             __syncwarp();
             if (lane < nrows) {
-                bulk_g2s(slots + (size_t)lane * DSLOT, row_src(cr + lane), REC, bar);
+                bulk_g2s(slots + (size_t)lane * SLOT, row_src(cr + lane), REC, bar);
             } else {
-                uint4 *vz = reinterpret_cast<uint4 *>(slots + (size_t)lane * DSLOT);
+                uint4 *vz = reinterpret_cast<uint4 *>(slots + (size_t)lane * SLOT);
 #pragma unroll
                 for (int i = 0; i < 32; ++i) vz[i] = make_uint4(0, 0, 0, 0);
             }
@@ -609,11 +358,11 @@ __device__ __forceinline__ void dense_tokens_body(const DenseParams &p, int T, c
 #pragma unroll
                 for (int j = 0; j < 2; ++j) {
                     uint32_t b[4];
-                    ldsm4(b, slots_s + (uint32_t)(j * 16 * DSLOT + ks * 32) + k_lane_off);
+                    ldsm_x4(b, slots_s + (uint32_t)(j * 16 * SLOT + ks * 32) + k_lane_off);
 #pragma unroll
                     for (int mt = 0; mt < NMT; ++mt) {
-                        mma16816(s[mt][2 * j], a[mt], b[0], b[1]);
-                        mma16816(s[mt][2 * j + 1], a[mt], b[2], b[3]);
+                        mma_16816(s[mt][2 * j], a[mt], b[0], b[1]);
+                        mma_16816(s[mt][2 * j + 1], a[mt], b[2], b[3]);
                     }
                 }
             }
@@ -623,6 +372,15 @@ __device__ __forceinline__ void dense_tokens_body(const DenseParams &p, int T, c
             for (int mt = 0; mt < NMT; ++mt)
 #pragma unroll
                 for (int i = 0; i < NI; ++i) {
+                    // FAST: bit r of `seen` = tile row r is visible, once per tile.  It must agree with the per-score rule
+                    // below (key cr + r visible when r < nrows and (cr + r < lim or bit cr + r - lim of vis is set)).
+                    uint32_t seen = 0;
+                    if constexpr (FAST) {
+                        const int o = lim[mt][i] - cr;   // tile row of the step's first row
+                        seen = (o >= 32) ? ~0u : (o > 0 ? ~0u >> (32 - o) : 0u);
+                        if (o > -TREE_MAX && o < 32) seen |= (o >= 0) ? vis[mt][i] << o : vis[mt][i] >> -o;
+                        seen = (seen & (~0u >> (32 - nrows))) >> (tig * 2);
+                    }
                     float mloc = -CUDART_INF_F;
 #pragma unroll
                     for (int nt = 0; nt < 4; ++nt)
@@ -630,10 +388,14 @@ __device__ __forceinline__ void dense_tokens_body(const DenseParams &p, int T, c
                         for (int e = 0; e < 2; ++e) {
                             const int r = nt * 8 + tig * 2 + e;
                             float &x = s[mt][nt][2 * i + e];
-                            const int o = cr + r - lim[mt][i];
-                            bool seen = o < 0 || ((unsigned)o < (unsigned)TREE_MAX && ((vis[mt][i] >> o) & 1u));
-                            if constexpr (SLOTS) seen = (cr + r < pc) ? (cr + r < pre[mt][i]) : (cr + r >= tb[mt][i] && seen);
-                            x = (r < nrows && seen) ? x * scale_log2 : -CUDART_INF_F;
+                            if constexpr (FAST) {
+                                x = ((seen >> (nt * 8 + e)) & 1u) ? x * scale_log2 : -CUDART_INF_F;
+                            } else {
+                                const int o = cr + r - lim[mt][i];
+                                bool vis_r = o < 0 || ((unsigned)o < (unsigned)TREE_MAX && ((vis[mt][i] >> o) & 1u));
+                                if constexpr (SLOTS) vis_r = (cr + r < pc) ? (cr + r < pre[mt][i]) : (cr + r >= tb[mt][i] && vis_r);
+                                x = (r < nrows && vis_r) ? x * scale_log2 : -CUDART_INF_F;
+                            }
                             mloc = fmaxf(mloc, x);
                         }
                     mloc = fmaxf(mloc, __shfl_xor_sync(0xffffffffu, mloc, 1));
@@ -691,12 +453,12 @@ __device__ __forceinline__ void dense_tokens_body(const DenseParams &p, int T, c
 #pragma unroll
                     for (int n2 = 0; n2 < 8; ++n2) {
                         uint32_t b[4];
-                        ldsm4t(b, slots_s + (uint32_t)(ks * 16 * DSLOT + n2 * 32) + v_lane_off);
-                        mma16816(acc[mt][2 * n2], ahi, b[0], b[1]);
-                        mma16816(acc[mt][2 * n2 + 1], ahi, b[2], b[3]);
+                        ldsm_x4_trans(b, slots_s + (uint32_t)(ks * 16 * SLOT + n2 * 32) + v_lane_off);
+                        mma_16816(acc[mt][2 * n2], ahi, b[0], b[1]);
+                        mma_16816(acc[mt][2 * n2 + 1], ahi, b[2], b[3]);
                         if (!PACK) {
-                            mma16816(acc[mt][2 * n2], alo, b[0], b[1]);
-                            mma16816(acc[mt][2 * n2 + 1], alo, b[2], b[3]);
+                            mma_16816(acc[mt][2 * n2], alo, b[0], b[1]);
+                            mma_16816(acc[mt][2 * n2 + 1], alo, b[2], b[3]);
                         }
                     }
                 }
@@ -733,11 +495,12 @@ __device__ __forceinline__ void dense_tokens_body(const DenseParams &p, int T, c
         if (w_g > 1 && wb > wa) {
             // level 1: the states stay in each warp's ring; the last arriver of this CTA combines them
             int ticket = 0;
-            if (lane == 0) ticket = atom_add_acq_rel_cta_shared_d(&s_cnt[wa - cta_w0], 1);
+            if (lane == 0) ticket = atom_add_acq_rel_cta_shared(&s_cnt[wa - cta_w0], 1);
             ticket = __shfl_sync(0xffffffffu, ticket, 0);
             carry = (ticket == wb - wa);
         }
         if (!carry) continue;
+        auto row_of = [&](int r) { return FAST ? __shfl_sync(0xffffffffu, lane_row, r) : out_row(bg, r); };
         const int cta_first = i0 / warps, cta_last = i1 / warps;
         const bool need_l1 = (w_g > 1 && wb > wa);
         const bool need_l2 = (w_g > 1 && cta_first != cta_last);
@@ -755,12 +518,12 @@ __device__ __forceinline__ void dense_tokens_body(const DenseParams &p, int T, c
                 const float4 o4 = *reinterpret_cast<const float4 *>(st + 4 + 4 * lane);
                 A[0] = o4.x; A[1] = o4.y; A[2] = o4.z; A[3] = o4.w;
             }
-            if (!need_l2) finalize_dense_head(p, out_row(bg, r), L_, A, lane);
+            if (!need_l2) finalize_dense_head(p, row_of(r), L_, A, lane);
             else store_state(gslot + (size_t)r * PART_FLOATS, M_, L_, A, lane);
         }
         if (!need_l2) continue;
         __syncwarp();
-        if (lane == 0) ticket2 = atom_add_acq_rel_gpu_d(p.counters + bg, 1);
+        if (lane == 0) ticket2 = atom_add_acq_rel_gpu(p.counters + bg, 1);
         ticket2 = __shfl_sync(0xffffffffu, ticket2, 0);
         if (ticket2 == cta_last - cta_first) {
             for (int r = 0; r < qr; ++r) {
@@ -772,28 +535,19 @@ __device__ __forceinline__ void dense_tokens_body(const DenseParams &p, int T, c
                                                (size_t)r * PART_FLOATS);
                     },
                     cta_last - cta_first + 1, lane, M_, L_, A);
-                finalize_dense_head(p, out_row(bg, r), L_, A, lane);
+                finalize_dense_head(p, row_of(r), L_, A, lane);
             }
             if (lane == 0) p.counters[bg] = 0;
         }
     }
 }
 
-template <int NMT, bool PACK>
-__global__ void __launch_bounds__(256) attend_dense_tokens_kernel(const DenseParams p, int T, const int32_t *anc) {
-    dense_tokens_body<NMT, PACK, false>(p, T, anc, DenseSlots{});
-}
-
-// shared dense mode; anc = null: a single-token decode (each request's last row is its step row)
-template <int NMT, bool PACK>
-__global__ void __launch_bounds__(256) attend_dense_slot_kernel(const DenseParams p, int T, const int32_t *anc, const DenseSlots sl) {
-    dense_tokens_body<NMT, PACK, true>(p, T, anc, sl);
-}
-
-static DenseParams dense_params(const mpig_ctx *ctx, const uint8_t *kv, const int32_t *len, const void *q, void *out) {
+int launch_attend_dense(mpig_ctx *ctx, const LayerStore &ls, int T, const void *q, void *out, cudaStream_t s, bool pdl) {
+    const bool slots = ctx->dense_tail_rows > 0;
+    const int B = ctx->cfg.batch_size, TG = T * ctx->G;
     DenseParams p = {};
-    p.kv = kv;
-    p.len = len;
+    p.kv = ls.dense_kv;
+    p.len = ctx->dense_len;
     p.q = (const __nv_bfloat16 *)q;
     p.out = (__nv_bfloat16 *)out;
     p.out_f32 = ctx->want_out_f32 ? ctx->out_f32 : nullptr;
@@ -804,101 +558,45 @@ static DenseParams dense_params(const mpig_ctx *ctx, const uint8_t *kv, const in
     p.Hkv = ctx->cfg.num_key_value_heads;
     p.Hq = ctx->cfg.num_attention_heads;
     p.M = ctx->cfg.max_length;
-    return p;
-}
-
-static cudaLaunchConfig_t dense_config(const mpig_ctx *ctx, int warps, size_t smem, cudaStream_t s, bool pdl, cudaLaunchAttribute *attr) {
+    DenseSlots sl = {};
+    if (slots) {
+        sl.slot_of = ctx->slot_of;
+        sl.base = ctx->dense_base;
+        sl.tail = ls.dense_tail;
+        sl.B = B;
+        sl.R = ctx->dense_tail_rows;
+        sl.cm = std::max(1, 32 / TG);
+    }
+    // the most query rows a group can have: T*G, or in slot mode a chunk of cm requests or all B bound to one slot (the bindings
+    // may change after a capture, so the regime depends on B only); the partial scratch holds states of cm*T*G rows
+    const int rows = slots ? std::min(sl.cm, B) * TG : TG;
+    const int qs = slots ? sl.cm * TG : TG;
+    // 12 warps for single-token decode in the default layout, 8 for every other launch: the warp count sets the row partition
+    const int warps = (!slots && T == 1 && rows <= 8) ? 12 : 8;
+    const size_t smem = (size_t)warps * (TILE * SLOT + 8 + 4) + 2 * (size_t)(p.BG + 1) * sizeof(int) +
+                        (slots ? (size_t)(5 * B + 2) * sizeof(int) : 0) + 16;
+    MPIG_REQUIRE(smem <= 227 * 1024, MPIG_EINVAL, "dense attention: %zu B shared memory", smem);
+    // slot mode has at most B*Hkv groups (a chunk holds at least one request), so the counters suffice in both modes
+    MPIG_REQUIRE((size_t)ctx->num_sms * 2 * qs <= (size_t)ctx->max_partial_warps * 2, MPIG_EINVAL, "dense attention: partial scratch too small");
+    void (*kernel)(DenseParams, int, const int32_t *, DenseSlots);
+    if (rows <= 8) kernel = slots ? attend_dense_kernel<1, true, true> : attend_dense_kernel<1, true, false>;
+    else if (rows <= 16) kernel = slots ? attend_dense_kernel<1, false, true> : attend_dense_kernel<1, false, false>;
+    else kernel = slots ? attend_dense_kernel<2, false, true> : attend_dense_kernel<2, false, false>;
+    MPIG_FUNC_ATTR(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(ctx->num_sms);
     cfg.blockDim = dim3(warps * 32);
     cfg.dynamicSmemBytes = smem;
     cfg.stream = s;
+    cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = pdl ? 1 : 0;
-    return cfg;
-}
-
-int launch_attend_dense_slots(mpig_ctx *ctx, const LayerStore &ls, int T, const void *q, void *out, cudaStream_t s, bool pdl) {
-    const int B = ctx->cfg.batch_size, TG = T * ctx->G;
-    MPIG_REQUIRE(ctx->G >= 1 && TG <= 32, MPIG_EUNSUPPORTED, "dense attention: T*G = %d query rows per group (at most 32)", TG);
-    const DenseParams p = dense_params(ctx, ls.dense_kv, ctx->dense_len, q, out);
-    DenseSlots sl = {};
-    sl.slot_of = ctx->slot_of;
-    sl.base = ctx->dense_base;
-    sl.tail = ls.dense_tail;
-    sl.B = B;
-    sl.R = ctx->dense_tail_rows;
-    sl.cm = std::max(1, 32 / TG);
-    // the most query rows a group can have: a chunk of cm requests, or all B bound to one slot (the bindings may change after a
-    // capture, so the regime depends on B only)
-    const int rows = std::min(sl.cm, B) * TG;
-    const int warps = 8;
-    const size_t smem = (size_t)warps * TILE * DSLOT + (size_t)warps * 8 + (size_t)warps * 4 + 2 * (size_t)(p.BG + 1) * sizeof(int) +
-                        (size_t)(5 * B + 2) * sizeof(int) + 16;
-    MPIG_REQUIRE(smem <= 227 * 1024, MPIG_EINVAL, "dense attention: %zu B shared memory", smem);
-    // at most B*Hkv groups (a chunk holds at least one request), so partials and counters are those of the per-request kernels
-    MPIG_REQUIRE((size_t)ctx->num_sms * 2 * sl.cm * TG <= (size_t)ctx->max_partial_warps * 2, MPIG_EINVAL,
-                 "dense attention: partial scratch too small");
-    cudaLaunchAttribute attr[1];
-    cudaLaunchConfig_t cfg = dense_config(ctx, warps, smem, s, pdl, attr);
     const int32_t *anc = (T > 1) ? (const int32_t *)step_masks(ctx->step_buf) : nullptr;
-    if (rows <= 8) {
-        MPIG_FUNC_ATTR((attend_dense_slot_kernel<1, true>), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-        MPIG_CUDA(cudaLaunchKernelEx(&cfg, attend_dense_slot_kernel<1, true>, p, T, anc, sl));
-    } else if (rows <= 16) {
-        MPIG_FUNC_ATTR((attend_dense_slot_kernel<1, false>), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-        MPIG_CUDA(cudaLaunchKernelEx(&cfg, attend_dense_slot_kernel<1, false>, p, T, anc, sl));
-    } else {
-        MPIG_FUNC_ATTR((attend_dense_slot_kernel<2, false>), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-        MPIG_CUDA(cudaLaunchKernelEx(&cfg, attend_dense_slot_kernel<2, false>, p, T, anc, sl));
-    }
+    MPIG_CUDA(cudaLaunchKernelEx(&cfg, kernel, p, T, anc, sl));
     MPIG_LAUNCH_CHECK(ctx);
     ctx->last_tokens = T;
-    return MPIG_OK;
-}
-
-int launch_attend_dense_tokens(mpig_ctx *ctx, const uint8_t *kv, const int32_t *len, int T, const void *q, void *out, cudaStream_t s,
-                               bool pdl) {
-    const int TG = T * ctx->G;
-    MPIG_REQUIRE(TG >= 1 && TG <= 32, MPIG_EUNSUPPORTED, "dense attention: T*G = %d query rows per group (at most 32)", TG);
-    const DenseParams p = dense_params(ctx, kv, len, q, out);
-    const int warps = 8;
-    const size_t smem = (size_t)warps * TILE * DSLOT + (size_t)warps * 8 + (size_t)warps * 4 + 2 * (size_t)(p.BG + 1) * sizeof(int) + 16;
-    MPIG_REQUIRE(smem <= 227 * 1024, MPIG_EINVAL, "dense attention: %zu B shared memory", smem);
-    MPIG_REQUIRE((size_t)ctx->num_sms * 2 * TG <= (size_t)ctx->max_partial_warps * 2, MPIG_EINVAL, "dense attention: partial scratch too small");
-    cudaLaunchAttribute attr[1];
-    cudaLaunchConfig_t cfg = dense_config(ctx, warps, smem, s, pdl, attr);
-    if (TG <= 8) {
-        MPIG_FUNC_ATTR((attend_dense_tokens_kernel<1, true>), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-        MPIG_CUDA(cudaLaunchKernelEx(&cfg, attend_dense_tokens_kernel<1, true>, p, T, (const int32_t *)step_masks(ctx->step_buf)));
-    } else if (TG <= 16) {
-        MPIG_FUNC_ATTR((attend_dense_tokens_kernel<1, false>), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-        MPIG_CUDA(cudaLaunchKernelEx(&cfg, attend_dense_tokens_kernel<1, false>, p, T, (const int32_t *)step_masks(ctx->step_buf)));
-    } else {
-        MPIG_FUNC_ATTR((attend_dense_tokens_kernel<2, false>), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-        MPIG_CUDA(cudaLaunchKernelEx(&cfg, attend_dense_tokens_kernel<2, false>, p, T, (const int32_t *)step_masks(ctx->step_buf)));
-    }
-    MPIG_LAUNCH_CHECK(ctx);
-    ctx->last_tokens = T;
-    return MPIG_OK;
-}
-
-int launch_attend_dense(mpig_ctx *ctx, const uint8_t *kv, const int32_t *len, const void *q, void *out, cudaStream_t s, bool pdl) {
-    MPIG_REQUIRE(ctx->G >= 1 && ctx->G <= GMAX, MPIG_EUNSUPPORTED, "dense attention: group size %d > %d", ctx->G, GMAX);
-    ctx->last_tokens = 1;
-    const DenseParams p = dense_params(ctx, kv, len, q, out);
-    const int warps = 12;
-    const size_t smem = (size_t)warps * TILE * DSLOT + (size_t)warps * 8 + (size_t)warps * 4 + 2 * (size_t)(p.BG + 1) * sizeof(int) + 16;
-    MPIG_REQUIRE(smem <= 227 * 1024, MPIG_EINVAL, "dense attention: %zu B shared memory", smem);
-    MPIG_REQUIRE((size_t)ctx->num_sms * 2 * GPART <= (size_t)ctx->max_partial_warps * 2 * PART_FLOATS, MPIG_EINVAL,
-                 "dense attention: partial scratch too small");
-    MPIG_FUNC_ATTR(attend_dense_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    cudaLaunchAttribute attr[1];
-    cudaLaunchConfig_t cfg = dense_config(ctx, warps, smem, s, pdl, attr);
-    MPIG_CUDA(cudaLaunchKernelEx(&cfg, attend_dense_kernel, p));
-    MPIG_LAUNCH_CHECK(ctx);
     return MPIG_OK;
 }
 

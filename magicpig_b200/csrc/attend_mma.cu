@@ -55,17 +55,6 @@ __device__ __forceinline__ uint32_t clk32_after(int dep) {
         }                                                                                                \
     } while (0)
 
-__device__ __forceinline__ int atom_add_acq_rel_gpu(int *addr, int v) {
-    int old;
-    asm volatile("atom.acq_rel.gpu.global.add.s32 %0, [%1], %2;" : "=r"(old) : "l"(addr), "r"(v) : "memory");
-    return old;
-}
-__device__ __forceinline__ int atom_add_acq_rel_cta_shared(int *addr, int v) {
-    int old;
-    asm volatile("atom.acq_rel.cta.shared.add.s32 %0, [%1], %2;" : "=r"(old) : "r"(smem_u32(addr)), "r"(v) : "memory");
-    return old;
-}
-
 // Work decomposition (head-aligned stream-K).  Head h owns T_h = W_b + nnz_h rows.  With nw warps in the grid,
 //   Rp  = max(32, ceil(total / (nw - H)))            rows a warp should take
 //   w_h = max(1, floor(T_h / Rp))                    warps ("parts") of head h;  sum_h w_h <= nw

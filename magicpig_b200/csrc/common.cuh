@@ -430,15 +430,12 @@ int launch_append_tokens(mpig_ctx *ctx, const AppendParams &ap, int T, cudaStrea
 // T-token sparse decode (fused.cu): append of the T window rows, then the T-token fused kernel; q (B, T, Hq, d), k / v
 // (B, T, Hkv, d), out (B, T, Hq*d).  Refuses (nothing launched) when the fused decode does not apply.
 int launch_fused_tokens(mpig_ctx *ctx, int layer, int T, const void *q, const void *k, const void *v, void *out, cudaStream_t s);
-// T-token dense decode (attend_dense.cu): q (B, T, Hq, d), rows already appended, causal over the last T rows
-int launch_attend_dense_tokens(mpig_ctx *ctx, const uint8_t *kv, const int32_t *len, int T, const void *q, void *out, cudaStream_t s,
-                               bool pdl);
-// shared dense mode (attend_dense.cu): the dense layer ls over the slot stores and the request tails, T = 1 (single-token decode,
-// causal) or the pending step's T (ancestor masks); q (B, T, Hq, d), rows already appended
-int launch_attend_dense_slots(mpig_ctx *ctx, const LayerStore &ls, int T, const void *q, void *out, cudaStream_t s, bool pdl);
+// dense decode (attend_dense.cu) of the dense layer ls, T*G <= 32: T = 1 (single-token decode, causal) or the pending step's T
+// (ancestor masks); q / out (B, T, Hq, d), rows already appended.  Shared dense mode (dense_tail_rows > 0) reads the slot stores
+// and the request tails.
+int launch_attend_dense(mpig_ctx *ctx, const LayerStore &ls, int T, const void *q, void *out, cudaStream_t s, bool pdl);
 int launch_probe(mpig_ctx *ctx, int layer, const int32_t *query, int32_t *results, int32_t *nnz, cudaStream_t s, bool pdl);
 int launch_attend_mma(mpig_ctx *ctx, const AttendParams &p, cudaStream_t s, bool pdl);
-int launch_attend_dense(mpig_ctx *ctx, const uint8_t *kv, const int32_t *len, const void *q, void *out, cudaStream_t s, bool pdl);
 int launch_fused(mpig_ctx *ctx, int layer, const void *q, const void *k, const void *v, void *out, cudaStream_t s, bool pdl,
                  const mpig_peer *peer = nullptr, int peer_rank = 0, int peer_world = 1, volatile uint32_t *host_flags = nullptr,
                  uint32_t host_epoch = 0);

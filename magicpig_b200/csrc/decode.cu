@@ -165,32 +165,37 @@ int mpig_dense_fill(mpig_ctx *ctx, int layer, int request, const void *k_bf16, c
     return MPIG_OK;
 }
 
-int mpig_dense_decode(mpig_ctx *ctx, int layer, const void *query_bf16, const void *key_bf16, const void *value_bf16,
-                      void *out_bf16, void *stream) {
-    mpig::DeviceGuard _dg(ctx);  // run on the context's device whatever the caller's current device is
-    int rc = check_layer(ctx, layer, false, "mpig_dense_decode");
-    if (rc) return rc;
+// the body of the two dense entry points: append the T new rows, then attend over the layer's dense KV
+static int dense_decode(mpig_ctx *ctx, int layer, int T, const void *q, const void *k, const void *v, void *out, cudaStream_t s,
+                        const char *who) {
     const LayerStore &ls = ctx->layers[layer];
-    MPIG_REQUIRE(ls.dense && ls.dense_kv, MPIG_ESTATE, "mpig_dense_decode: layer %d has no dense KV", layer);
-    MPIG_REQUIRE(query_bf16 && key_bf16 && value_bf16 && out_bf16, MPIG_EINVAL, "mpig_dense_decode: null argument");
-    cudaStream_t s = as_stream(stream);
-    if (ctx->dense_tail_rows > 0) {
-        MPIG_REQUIRE(ctx->dense_impl == 1, MPIG_EUNSUPPORTED,
-                     "mpig_dense_decode: the shared dense layout (dense_tail_rows > 0) needs the GQA-shared dense kernel (dense_impl = 1)");
-        rc = launch_append_tokens(ctx, append_params(ctx, ls, key_bf16, value_bf16, true), 1, s, ctx->dense_base);
-        if (rc) return rc;
-        return launch_attend_dense_slots(ctx, ls, 1, query_bf16, out_bf16, s, false);
+    MPIG_REQUIRE(ls.dense && ls.dense_kv, MPIG_ESTATE, "%s: layer %d has no dense KV", who, layer);
+    if (ctx->dense_impl == 1) {
+        MPIG_REQUIRE(T * ctx->G <= 32, MPIG_EUNSUPPORTED, "%s: T*G = %d query rows per kv-group (at most 32)", who, T * ctx->G);
+    } else {
+        MPIG_REQUIRE(T == 1, MPIG_EUNSUPPORTED, "%s: T=%d needs the GQA-shared dense kernel (dense_impl = 1)", who, T);
+        MPIG_REQUIRE(ctx->dense_tail_rows == 0, MPIG_EUNSUPPORTED,
+                     "%s: the shared dense layout (dense_tail_rows > 0) needs the GQA-shared dense kernel (dense_impl = 1)", who);
     }
-    rc = launch_append_tokens(ctx, append_params(ctx, ls, key_bf16, value_bf16, true), 1, s);
+    int rc = launch_append_tokens(ctx, append_params(ctx, ls, k, v, true), T, s, ctx->dense_base_map());
     if (rc) return rc;
-    if (ctx->dense_impl == 1) return launch_attend_dense(ctx, ls.dense_kv, ctx->dense_len, query_bf16, out_bf16, s, false);
+    if (ctx->dense_impl == 1) return launch_attend_dense(ctx, ls, T, q, out, s, T > 1);
     // the cache as window rows; qnorm is unused by window rows but must be a valid pointer
-    AttendParams p = attend_params(ctx, query_bf16, ctx->qnorm, out_bf16);
+    AttendParams p = attend_params(ctx, q, ctx->qnorm, out);
     p.win = ls.dense_kv;
     p.win_len = ctx->dense_len;
     p.Wcap = ctx->cfg.max_length;
     ctx->last_tokens = 1;
     return launch_attend_mma(ctx, p, s, false);
+}
+
+int mpig_dense_decode(mpig_ctx *ctx, int layer, const void *query_bf16, const void *key_bf16, const void *value_bf16,
+                      void *out_bf16, void *stream) {
+    mpig::DeviceGuard _dg(ctx);  // run on the context's device whatever the caller's current device is
+    int rc = check_layer(ctx, layer, false, "mpig_dense_decode");
+    if (rc) return rc;
+    MPIG_REQUIRE(query_bf16 && key_bf16 && value_bf16 && out_bf16, MPIG_EINVAL, "mpig_dense_decode: null argument");
+    return dense_decode(ctx, layer, 1, query_bf16, key_bf16, value_bf16, out_bf16, as_stream(stream), "mpig_dense_decode");
 }
 
 // shared checks of the two T-token entry points
@@ -219,16 +224,7 @@ int mpig_dense_decode_tokens(mpig_ctx *ctx, int layer, int T, const void *query_
     mpig::DeviceGuard _dg(ctx);
     int rc = tokens_checks(ctx, layer, T, query_bf16, key_bf16, value_bf16, out_bf16, false, "mpig_dense_decode_tokens");
     if (rc) return rc;
-    const LayerStore &ls = ctx->layers[layer];
-    MPIG_REQUIRE(ls.dense && ls.dense_kv, MPIG_ESTATE, "mpig_dense_decode_tokens: layer %d has no dense KV", layer);
-    if (T == 1) return mpig_dense_decode(ctx, layer, query_bf16, key_bf16, value_bf16, out_bf16, stream);
-    MPIG_REQUIRE(ctx->dense_impl == 1, MPIG_EUNSUPPORTED, "mpig_dense_decode_tokens: T=%d needs the GQA-shared dense kernel (dense_impl = 1)", T);
-    MPIG_REQUIRE(T * ctx->G <= 32, MPIG_EUNSUPPORTED, "mpig_dense_decode_tokens: T*G = %d query rows per kv-group (at most 32)", T * ctx->G);
-    cudaStream_t s = as_stream(stream);
-    rc = launch_append_tokens(ctx, append_params(ctx, ls, key_bf16, value_bf16, true), T, s, ctx->dense_base_map());
-    if (rc) return rc;
-    if (ctx->dense_tail_rows > 0) return launch_attend_dense_slots(ctx, ls, T, query_bf16, out_bf16, s, true);
-    return launch_attend_dense_tokens(ctx, ls.dense_kv, ctx->dense_len, T, query_bf16, out_bf16, s, true);
+    return dense_decode(ctx, layer, T, query_bf16, key_bf16, value_bf16, out_bf16, as_stream(stream), "mpig_dense_decode_tokens");
 }
 
 }  // extern "C"

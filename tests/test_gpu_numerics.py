@@ -634,11 +634,15 @@ DENSE_P = [1, 31, 32, 33, 4095, 4097, 60000]
 
 @pytest.mark.parametrize("impl", [1, 0])
 @pytest.mark.parametrize("P", DENSE_P)
-@pytest.mark.parametrize("regime", ["R2", "R4"])
-def test_dense_single(cuda_lib, regime, P, impl):
+@pytest.mark.parametrize("regime,G", [("R2", None), ("R4", None), ("R2", 16), ("R4", 16), ("R2", 32), ("R4", 32)],
+                         ids=["R2", "R4", "R2-G16", "R4-G16", "R2-G32", "R4-G32"])
+def test_dense_single(cuda_lib, regime, G, P, impl):
     """Single-token dense decode (dense_impl 1: GQA-shared kernel, 0: generic gather) at tile edges, and at a P whose groups
-    are split over several CTAs (level-2 merge)."""
+    are split over several CTAs (level-2 merge).  G = 16 / 32: more query heads per kv-head than one packed m-tile holds, on
+    one m-tile or two."""
     B, Hq, Hkv = (1, 8, 1) if P > 5000 else (2, 8, 2)
+    if G:
+        Hq = G * Hkv
     c = make_dense(regime, B, Hq, Hkv, P, 1, seed=P + 3, place="new" if P == 1 else ("first" if P % 2 else "last"))
     o = check_dense(c)
     ctx = dense_ctx(B, Hq, Hkv, P + 256, impl=impl)
