@@ -89,7 +89,15 @@ typedef struct mpig_config {
      *   rows of the slot the request is bound to and makes seq_len the request's base; mpig_fork_request copies only src's rows
      *   past its base; a request's dense capacity is min(max_length, base + R) (the plans refuse past it, a captured plan
      *   saturates and raises mpig_error_flags bit 1); a rebound request must be dense-filled before its dense outputs mean
-     *   anything; dense_impl = 0 is MPIG_EUNSUPPORTED.  mpig_get_info("dense_tail_rows") reports R. */
+     *   anything; dense_impl = 0 is MPIG_EUNSUPPORTED.  mpig_get_info("dense_tail_rows") reports R.
+     * reserved[3]: 1 = shared spill (only with 0 < C < batch_size <= 32; otherwise MPIG_EINVAL).  mpig_spill_window accepts
+     *   requests that share a slot: their rows go into the slot's store and tables in request order, and every spilled key is
+     *   PRIVATE: request b samples the slot's prompt keys plus the private keys it spilled itself or inherited through
+     *   mpig_fork_request, so its result equals that of an exclusive slot holding those keys (codes, nnz and index sets equal after
+     *   renumbering, fp32 outputs up to summation order).  The capacity is shared (prompt + all private keys of a slot <=
+     *   max_length).  A fill of a slot (mpig_attn_fill, mpig_lsh_build / mpig_lsh_fill) and mpig_clear drop its private keys;
+     *   private keys nobody sees any more keep their rows until then.  mpig_lsh_collision_counts stays unfiltered.
+     *   mpig_get_info("shared_spill") reports the flag. */
     int32_t reserved[8];
 } mpig_config;
 
@@ -130,7 +138,8 @@ int mpig_set_option(mpig_ctx *ctx, const char *key, int64_t value);
  * "fused_cluster_waves" (waves of thread-block clusters one fused launch takes on this device; 1 = all resident at once,
  * 0 = fused decode not applicable), "window_capacity" (sink + local + generation_buffer rows), "table_segments" (key segments S
  * of the tables, see mpig_lsh_table_ptrs), "query_tokens_max" (t_max of mpig_reserve_query_tokens, 1 without), "tokens_cluster_waves"
- * (waves of clusters the last mpig_decode_tokens launch with T > 1 took), "num_contexts" (context slots C, see reserved[1]), "dense_tail_rows" (R, see reserved[2]). */
+ * (waves of clusters the last mpig_decode_tokens launch with T > 1 took), "num_contexts" (context slots C, see reserved[1]), "dense_tail_rows" (R, see reserved[2]),
+ * "shared_spill" (0 / 1, see reserved[3]). */
 int mpig_get_info(mpig_ctx *ctx, const char *key, int64_t *value);
 /* Capacity errors the DEVICE detected (the lengths saturate there): bit 0 = a sparse window is full (generation_buffer
  * exhausted: each further token overwrites the previous one's K/V), bit 1 = a dense cache reached its capacity (max_length, or base + R with reserved[2]), bit 2 = mpig_rewind
@@ -156,10 +165,12 @@ int mpig_set_hash_func(mpig_ctx *ctx, const void *hash_func_bf16, void *stream);
  * Bind `dst` to the slot of `src` and make dst's per-request state a copy of src's: for every sparse layer window rows
  * [0, win_len[src]) of every kv-head and avg_k, for every dense layer KV rows [0, dense_len[src]) of every kv-head, and both
  * lengths (device and host mirror).  Reads the device lengths and synchronises `stream` (correct after replays of a captured
- * plan); copy-engine calls only.  MPIG_EINVAL: src == dst or either outside [0, batch_size). */
+ * plan); copy-engine calls only, plus in shared spill mode (reserved[3]) one kernel: dst then sees exactly the private keys src
+ * sees, and no longer its own.  MPIG_EINVAL: src == dst or either outside [0, batch_size). */
 int mpig_fork_request(mpig_ctx *ctx, int src, int dst, void *stream);
 /* Bind `request` to `slot` (in [0, C)); its window and lengths are left alone: fill the slot (mpig_attn_fill + mpig_lsh_build /
- * mpig_lsh_fill) and the window next.  Synchronises `stream`. */
+ * mpig_lsh_fill) and the window next.  In shared spill mode the request sees no private key until it spills again.  Synchronises
+ * `stream`. */
 int mpig_bind_request(mpig_ctx *ctx, int request, int slot, void *stream);
 
 /* ---- lsh.LSH --------------------------------------------------------------------------------- */
@@ -229,10 +240,13 @@ int mpig_plan(mpig_ctx *ctx, void *stream);
  * Reads the device window lengths (synchronises `stream`), so it is correct after eager plan() calls and after replays of a
  * captured step alike.  Not capturable.  A decode step captured before a spill stays valid after it.  Dense layers are
  * untouched.  The spilled keys go into the store and tables of the request's slot, so a request with g_b > 0 must be alone on its
- * slot among requests with a non-empty window: a request that shares its context generates at most generation_buffer tokens.
- * MPIG_EINVAL: keep < 0 or sink + keep >= window capacity; MPIG_ESTATE: n_old + g_b > max_length for some sparse layer, a
- * spilling request shares its slot with another request whose window is not empty, or no hash_func set.  On these errors
- * nothing is modified. */
+ * slot among requests with a non-empty window: a request that shares its context generates at most generation_buffer tokens --
+ * unless the context is in shared spill mode (reserved[3]), where the requests of a slot spill into it in request order, n_old is
+ * the slot's count plus the rows of the slot's earlier requests, and each spilled key is private to its request.
+ * MPIG_EINVAL: keep < 0 or sink + keep >= window capacity; MPIG_ESTATE: n_old + g_b (shared spill: the slot's count plus all its
+ * requests' rows) > max_length for some sparse layer, a spilling request shares its slot with another request whose window is not
+ * empty (not in shared spill mode), the sparse layers of a slot disagree on its private key count (shared spill mode, after a
+ * partial refill), or no hash_func set.  On these errors nothing is modified. */
 int mpig_spill_window(mpig_ctx *ctx, int keep, int32_t *spilled_out, void *stream);
 /* Fused sparse-layer decode (attnserver.py:261-312): centre + append the new key/value to the
  * window, SimHash, probe, gather attention over window + sample with the LSE merge folded in -- one kernel launch.

@@ -43,7 +43,8 @@ class LSHSparseAttnServer:
                  num_attention_heads: Optional[int] = None,
                  max_query_tokens: int = 1,
                  num_contexts: Optional[int] = None,
-                 dense_tail_rows: Optional[int] = None) -> None:
+                 dense_tail_rows: Optional[int] = None,
+                 shared_spill: bool = False) -> None:
         """Keywords up to `dtype` are the reference's (attnserver.py:9-20).  Extras:
         hash_func   inject the (d, K*L) bf16 projection (the reference draws it unseeded, :55);
         table_build "device" = counting sort on the GPU (mpig_lsh_build); "sorted" = the reference's
@@ -58,6 +59,9 @@ class LSHSparseAttnServer:
                     Request b starts on context b mod num_contexts; fork() and bind() change that.
         dense_tail_rows R > 0: the dense layers' prompt rows are kept once per context too, and each request holds only the R
                     rows it adds after its prompt (needs num_contexts < batch_size); None = a full dense cache per request.
+        shared_spill  requests that share a context may spill_window() into it (needs num_contexts < batch_size <= 32): each
+                    spilled token is private to the request that spilled it and to requests later forked from it.  Size max_length
+                    for the prompt plus every request's spilled tokens.
         """
         self.K, self.L = K, L
         self.config = config
@@ -85,7 +89,7 @@ class LSHSparseAttnServer:
                            batch_size, max_length, num_sink_tokens, num_local_tokens, generation_buffer,
                            dense_layers=self.dense_layers, alloc_dense_kv=True, device=self.device,
                            max_query_tokens=max_query_tokens, num_contexts=num_contexts or 0,
-                           dense_tail_rows=dense_tail_rows or 0)
+                           dense_tail_rows=dense_tail_rows or 0, shared_spill=shared_spill)
         if hash_func is None:
             hash_func = torch.randn((self.head_dim, K * L), device=self.device, dtype=torch.bfloat16)  # attnserver.py:55
         self.hash_func = hash_func.to(device=self.device, dtype=torch.bfloat16).contiguous()
@@ -149,7 +153,9 @@ class LSHSparseAttnServer:
         decodes over src_request's context (no copy of the sampled store or the tables) and gets a copy of its sink + local +
         generated window, its dense-layer KV and its lengths.  The usual way to serve n answers to one prompt, or several
         questions about one document: fill and build one request, then fork it.  Requests sharing a context generate at most
-        generation_buffer tokens (spill_window() refuses them).  Needs num_contexts < batch_size."""
+        generation_buffer tokens (spill_window() refuses them) unless the server was made with shared_spill=True: then each dst
+        sees exactly the tokens src spilled before the fork, and each request's later spills stay its own.  Needs num_contexts <
+        batch_size."""
         for dst in ([dst_requests] if isinstance(dst_requests, int) else dst_requests):
             self.ctx.fork(src_request, dst)
             for a in self.avg_k:
@@ -157,7 +163,8 @@ class LSHSparseAttnServer:
 
     def bind(self, request: int, context: int):
         """Not in the reference.  Bind `request` to context slot `context` (0 <= context < num_contexts); fill() and
-        build_table() of the request then write that context, which every request bound to it reads."""
+        build_table() of the request then write that context, which every request bound to it reads.  With shared_spill the
+        request sees none of the tokens spilled into a context until it spills again."""
         self.ctx.bind(request, context)
 
     def plan(self, num_tokens: int = 1, parents=None):
@@ -214,7 +221,9 @@ class LSHSparseAttnServer:
         """Not in the reference.  Moves the oldest generated tokens of every sparse layer's window into the sampled store and
         the hash tables, keeping the newest `keep` (default num_local_tokens) in the window, so that a generation can run past
         generation_buffer tokens.  Call it between tokens, never inside a captured step (it synchronises); plan() does not
-        spill on its own.  Returns the spilled token count per request, int32 (B,) on the host."""
+        spill on its own.  Returns the spilled token count per request, int32 (B,) on the host.  Requests that share a context
+        may spill only with shared_spill=True; their spilled tokens then go to the shared context but each request samples only
+        its own (and those inherited through fork())."""
         return self.ctx.spill_window(keep)
 
     def decode(self, query_states: torch.Tensor, key_states: torch.Tensor, value_states: torch.Tensor, layer_idx: int):

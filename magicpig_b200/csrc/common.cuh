@@ -161,6 +161,18 @@ struct mpig_ctx {
     int dense_cap(int b) const {
         return dense_tail_rows > 0 ? std::min(cfg.max_length, h_dense_base[b] + dense_tail_rows) : cfg.max_length;
     }
+    // shared spill mode (mpig_config.reserved[3] = 1, DESIGN.md section 3.12): requests that share a slot spill into it, and each
+    // spilled key is private.  Keys [private_lo[layer][slot], ...) of a slot's store are private; the private key at offset p is
+    // seen by request b iff bit b of vis[slot][p] is set.  Both arrays are allocated at create time and never move (a captured
+    // step reads the current ones).  Kernels write them (fills, spill, fork, bind) as well as mpig_clear's memsets, so the decode
+    // kernels read them only after griddepcontrol.wait.
+    bool shared_spill = false;
+    uint32_t *vis = nullptr;              // [C][max_length]
+    int32_t *private_lo = nullptr;        // [num_layers][C]
+    std::vector<std::vector<int>> h_private_lo;   // [layer][slot], mirrors private_lo
+    // the maps the kernels get: null unless in shared spill mode
+    const uint32_t *vis_map() const { return shared_spill ? vis : nullptr; }
+    const int32_t *private_lo_map(int layer) const { return shared_spill ? private_lo + (size_t)layer * C : nullptr; }
     // global state
     __nv_bfloat16 *hash_func = nullptr;   // (d, K*L) as given
     __nv_bfloat16 *hash_func_t = nullptr; // (K*L, d) transposed copy: K-major B operand for the SimHash GEMM
@@ -449,6 +461,14 @@ int launch_pack_nhd(mpig_ctx *ctx, const void *k, const void *v, uint8_t *rec, i
 // are device arrays [B].
 int launch_table_merge(mpig_ctx *ctx, int layer, const int16_t *codes, const int32_t *g, const int32_t *pre, const int32_t *n_old,
                        cudaStream_t s);
+// the same merge over n entries of slot-indexed arrays (entry i merges into slot i): shared spill mode merges once per slot
+int launch_table_merge_slots(mpig_ctx *ctx, int layer, const int16_t *codes, const int32_t *g, const int32_t *pre,
+                             const int32_t *n_old, cudaStream_t s);
+// shared spill mode: a request's place in the visibility map changes (store.cu).  src >= 0: dst sees exactly the private keys src
+// sees (a fork); src < 0: dst sees no private key (a bind).  Every slot's map is rewritten.
+int launch_vis_rebind(mpig_ctx *ctx, int src, int dst, cudaStream_t s);
+// shared spill mode: a fill of `layer` through request `request` (n prompt keys) empties the private region of its slot
+int reset_private(mpig_ctx *ctx, int layer, int request, int n, cudaStream_t s);
 
 // ---- host helpers --------------------------------------------------------------------------
 int check_layer(mpig_ctx *ctx, int layer, bool need_sparse, const char *who);

@@ -105,6 +105,12 @@ int mpig_create(const mpig_config *cfg, mpig_ctx **out) {
                      "mpig_create: dense_tail_rows (reserved[2]) = %d needs alloc_dense_kv = 1 (the context owns the dense KV)",
                      cfg->reserved[2]);
     }
+    if (cfg->reserved[3] != 0) {   // shared spill: requests that share a slot spill into it, each seeing only its own spilled keys
+        MPIG_REQUIRE(cfg->reserved[3] == 1, MPIG_EINVAL, "mpig_create: shared_spill (reserved[3]) = %d is not 0 or 1", cfg->reserved[3]);
+        MPIG_REQUIRE(cfg->reserved[1] > 0 && cfg->reserved[1] < cfg->batch_size && cfg->batch_size <= 32, MPIG_EINVAL,
+                     "mpig_create: shared_spill (reserved[3]) needs fewer context slots than requests and at most 32 requests (one "
+                     "visibility bit each): num_contexts = reserved[1] = %d, batch_size = %d", cfg->reserved[1], cfg->batch_size);
+    }
     struct RestoreDevice {
         int prev = -1;
         RestoreDevice() { if (cudaGetDevice(&prev) != cudaSuccess) prev = -1; }
@@ -161,6 +167,8 @@ int mpig_create(const mpig_config *cfg, mpig_ctx **out) {
     for (int b = 0; b < cfg->batch_size; ++b) ctx->h_slot_of[b] = b % ctx->C;
     ctx->dense_tail_rows = cfg->reserved[2];
     ctx->h_dense_base.assign(cfg->batch_size, 0);
+    ctx->shared_spill = cfg->reserved[3] == 1;
+    ctx->h_private_lo.assign(cfg->num_layers, std::vector<int>(ctx->C, 0));
 
     const size_t M = (size_t)cfg->max_length, BG = (size_t)ctx->BG, L = (size_t)cfg->L, d = (size_t)cfg->head_dim;
     const size_t SG = (size_t)ctx->C * cfg->num_key_value_heads;   // slot groups: the store and the tables are per slot
@@ -203,6 +211,10 @@ int mpig_create(const mpig_config *cfg, mpig_ctx **out) {
     TRY(dev_alloc(ctx, &ctx->dense_len, (size_t)cfg->batch_size * sizeof(int32_t)));
     TRY(dev_alloc(ctx, &ctx->slot_of, (size_t)cfg->batch_size * sizeof(int32_t)));
     if (ctx->dense_tail_rows > 0) TRY(dev_alloc(ctx, &ctx->dense_base, (size_t)cfg->batch_size * sizeof(int32_t)));
+    if (ctx->shared_spill) {
+        TRY(dev_alloc(ctx, &ctx->vis, (size_t)ctx->C * M * sizeof(uint32_t)));
+        TRY(dev_alloc(ctx, &ctx->private_lo, (size_t)cfg->num_layers * ctx->C * sizeof(int32_t)));
+    }
     {
         const cudaError_t e = cudaMemcpy(ctx->slot_of, ctx->h_slot_of.data(), (size_t)cfg->batch_size * sizeof(int32_t),
                                          cudaMemcpyHostToDevice);
@@ -282,6 +294,8 @@ void mpig_destroy(mpig_ctx *ctx) {
     cudaFree(ctx->dense_len);
     cudaFree(ctx->slot_of);
     cudaFree(ctx->dense_base);
+    cudaFree(ctx->vis);
+    cudaFree(ctx->private_lo);
     cudaFree(ctx->codes);
     cudaFree(ctx->qnorm);
     cudaFree(ctx->results);
@@ -326,6 +340,12 @@ int mpig_clear(mpig_ctx *ctx, void *stream) {
     MPIG_CUDA(cudaMemsetAsync(ctx->dense_len, 0, ctx->cfg.batch_size * sizeof(int32_t), s));
     if (ctx->dense_base) MPIG_CUDA(cudaMemsetAsync(ctx->dense_base, 0, ctx->cfg.batch_size * sizeof(int32_t), s));
     for (auto &n : ctx->h_dense_base) n = 0;
+    if (ctx->shared_spill) {   // no private keys: every slot's store is empty again
+        MPIG_CUDA(cudaMemsetAsync(ctx->vis, 0, (size_t)ctx->C * ctx->cfg.max_length * sizeof(uint32_t), s));
+        MPIG_CUDA(cudaMemsetAsync(ctx->private_lo, 0, (size_t)ctx->cfg.num_layers * ctx->C * sizeof(int32_t), s));
+        for (auto &v : ctx->h_private_lo)
+            for (auto &n : v) n = 0;
+    }
     const size_t rows = (size_t)ctx->H * ctx->tok_max;   // the per-step scratch holds B*t_max*Hq rows after a reservation
     MPIG_CUDA(cudaMemsetAsync(ctx->nnz, 0, rows * sizeof(int32_t), s));
     MPIG_CUDA(cudaMemsetAsync(ctx->counters, 0, ctx->H * sizeof(int32_t), s));
@@ -500,6 +520,7 @@ int mpig_get_info(mpig_ctx *ctx, const char *key, int64_t *value) {
     else if (k == "tokens_cluster_waves") *value = ctx->last_tokens_waves;
     else if (k == "num_contexts") *value = ctx->C;
     else if (k == "dense_tail_rows") *value = ctx->dense_tail_rows;
+    else if (k == "shared_spill") *value = ctx->shared_spill ? 1 : 0;
     else {
         set_error("mpig_get_info: unknown key '%s'", key);
         return MPIG_EINVAL;
@@ -566,6 +587,8 @@ int mpig_fork_request(mpig_ctx *ctx, int src, int dst, void *stream) {
     ctx->h_win_len[dst] = len[0];
     ctx->h_dense_len[dst] = len[1];
     ctx->h_slot_of[dst] = ctx->h_slot_of[src];
+    rc = launch_vis_rebind(ctx, src, dst, s);   // shared spill mode: dst sees exactly the private keys src sees
+    if (rc) return rc;
     rc = upload_slot_map(ctx, s);
     if (rc) return rc;
     ctx->pending.end();   // its bases are stale for dst
@@ -578,6 +601,8 @@ int mpig_bind_request(mpig_ctx *ctx, int request, int slot, void *stream) {
     if (rc) return rc;
     MPIG_REQUIRE(slot >= 0 && slot < ctx->C, MPIG_EINVAL, "mpig_bind_request: slot %d out of range [0, %d)", slot, ctx->C);
     ctx->h_slot_of[request] = slot;
+    rc = launch_vis_rebind(ctx, -1, request, as_stream(stream));   // shared spill mode: no private key until it spills again
+    if (rc) return rc;
     rc = upload_slot_map(ctx, as_stream(stream));
     if (rc) return rc;
     ctx->pending.end();

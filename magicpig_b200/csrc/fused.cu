@@ -164,10 +164,17 @@ __device__ __forceinline__ int block_exclusive_scan_redux(int v, int *wtot, int 
 // single-token instantiations) so that FusedParams, and with it their code, stays as it is.
 // slot_of (B), or null: the tables, records and key norms are those of slot group slot_of[b]*Hkv + h/G (context slots shared by
 // several requests); the window, k_new and avg_k stay those of group b*Hkv + h/G.  Null reads group b*Hkv + h/G for both.
-template <typename TagT, int THREADS, bool DBG, bool KREG, bool TOK = false>
+// SPILL (shared spill mode): vis / plo are the slots' visibility maps [C][M] and this layer's private starts [C]; the private keys
+// of the slot that request b does not see leave the tags before SELECT (filter_private).  Kernel arguments of their own, like anc
+// and slot_of, so that FusedParams stays as it is, and null in the instantiations without SPILL, which never read them: at the
+// 64-register cap any reference to them, even a test for null, moved the allocator's choices and added spills to the default
+// instantiation (DESIGN.md section 3.12).
+template <typename TagT, int THREADS, bool DBG, bool KREG, bool TOK = false, bool SPILL = false>
 __global__ void __launch_bounds__(THREADS, (THREADS == 1024) ? 1 : 2) fused_decode_kernel(const __grid_constant__ FusedParams gp,
                                                                                                    const int32_t *__restrict__ anc,
-                                                                                                   const int32_t *__restrict__ slot_of) {
+                                                                                                   const int32_t *__restrict__ slot_of,
+                                                                                                   const uint32_t *__restrict__ vis,
+                                                                                                   const int32_t *__restrict__ plo) {
     extern __shared__ __align__(128) uint8_t smem_raw[];
     __shared__ FusedParams p_s;   // parameters staged once (constant-bank misses were microseconds on the critical path)
     {
@@ -195,6 +202,7 @@ __global__ void __launch_bounds__(THREADS, (THREADS == 1024) ? 1 : 2) fused_deco
         // slot group.  Read before griddepcontrol.wait: only copy-engine calls write the map (never a kernel), and a kernel starts
         // after every copy ordered before it in the stream has completed (PDL overlaps a kernel with a preceding kernel only)
         s_geo[6] = slot_of ? __ldg(slot_of + s_geo[2]) * (gp.Hq / gp.G) + (h_ % gp.Hq) / gp.G : s_geo[1];
+        if (SPILL) s_geo[7] = __ldg(slot_of + s_geo[2]);   // shared spill mode (C < B: the map exists): the slot itself
     }
     unsigned long long t_dbg[12];
     if (DBG) {
@@ -542,6 +550,13 @@ __global__ void __launch_bounds__(THREADS, (THREADS == 1024) ? 1 : 2) fused_deco
                 __syncthreads();
             }
         }
+    }
+    // shared spill mode: the other requests' private keys leave the tags (after the last sweep's barrier; vis is kernel-written
+    // data, and this is long after griddepcontrol.wait).  The slot comes from shared memory: nothing stays live in registers.
+    if (SPILL) {
+        const volatile int *vg = s_geo;
+        const int sl = vg[7];
+        filter_private(tag, vis + (size_t)sl * p.M, __ldg(plo + sl), vg[3] * p.seg_len + vg[4], p.Mc, vg[2]);
     }
     if (DBG) t_dbg[4] = clk64();
 
@@ -988,16 +1003,18 @@ struct FusedPlan {
     int cluster_waves;  // waves of clusters the grid needs (cudaOccupancyMaxActiveClusters; 0 = unknown)
 };
 
-using FusedKernel = void (*)(const FusedParams, const int32_t *, const int32_t *);
+using FusedKernel = void (*)(const FusedParams, const int32_t *, const int32_t *, const uint32_t *, const int32_t *);
 
-// The fused_decode_kernel instantiation of a launch.  The T-token instantiations (tok) have no debug-clock variant.
-template <int THREADS> static FusedKernel fused_kernel_of(bool dbg, bool kreg, bool tok) {
-    if (tok) return kreg ? fused_decode_kernel<uint8_t, THREADS, false, true, true> : fused_decode_kernel<uint8_t, THREADS, false, false, true>;
-    if (dbg) return kreg ? fused_decode_kernel<uint8_t, THREADS, true, true> : fused_decode_kernel<uint8_t, THREADS, true, false>;
-    return kreg ? fused_decode_kernel<uint8_t, THREADS, false, true> : fused_decode_kernel<uint8_t, THREADS, false, false>;
+// The fused_decode_kernel instantiation of a launch.  The T-token instantiations (tok) have no debug-clock variant; every variant
+// has a shared spill twin (spill).
+template <int THREADS, bool SPILL> static FusedKernel fused_kernel_of(bool dbg, bool kreg, bool tok) {
+    if (tok) return kreg ? fused_decode_kernel<uint8_t, THREADS, false, true, true, SPILL> : fused_decode_kernel<uint8_t, THREADS, false, false, true, SPILL>;
+    if (dbg) return kreg ? fused_decode_kernel<uint8_t, THREADS, true, true, false, SPILL> : fused_decode_kernel<uint8_t, THREADS, true, false, false, SPILL>;
+    return kreg ? fused_decode_kernel<uint8_t, THREADS, false, true, false, SPILL> : fused_decode_kernel<uint8_t, THREADS, false, false, false, SPILL>;
 }
-static FusedKernel fused_kernel(int threads, bool dbg, bool kreg, bool tok) {
-    return threads == 1024 ? fused_kernel_of<1024>(dbg, kreg, tok) : fused_kernel_of<512>(dbg, kreg, tok);
+static FusedKernel fused_kernel(int threads, bool dbg, bool kreg, bool tok, bool spill = false) {
+    if (spill) return threads == 1024 ? fused_kernel_of<1024, true>(dbg, kreg, tok) : fused_kernel_of<512, true>(dbg, kreg, tok);
+    return threads == 1024 ? fused_kernel_of<1024, false>(dbg, kreg, tok) : fused_kernel_of<512, false>(dbg, kreg, tok);
 }
 
 // dynamic shared memory a CTA may use: per SM 228 KB, less the static parameter block and the 1 KB the system reserves per CTA
@@ -1023,8 +1040,8 @@ static cudaLaunchConfig_t fused_config(const FusedPlan &fp, int clusters, bool p
 
 // Clusters of this plan's variant that the device keeps resident at once.  A cluster occupies SMs of ONE GPC, and the
 // H100's GPCs have unequal SM counts, so #SMs / C over-counts; the runtime knows the real number.
-static int fused_max_active_clusters(const FusedPlan &fp, bool kreg, bool tok) {
-    const FusedKernel fn = fused_kernel(fp.threads, false, kreg, tok);
+static int fused_max_active_clusters(const FusedPlan &fp, bool kreg, bool tok, bool spill) {
+    const FusedKernel fn = fused_kernel(fp.threads, false, kreg, tok, spill);
     if (func_attr_once((const void *)fn, cudaFuncAttributeMaxDynamicSharedMemorySize, fused_smem_cap(fp.threads)) != MPIG_OK) return 0;
     cudaLaunchAttribute attr[2];
     const cudaLaunchConfig_t cfg = fused_config(fp, 1, false, 0, attr);
@@ -1065,7 +1082,7 @@ static FusedPlan fused_plan_compute(const mpig_ctx *ctx, int T = 1) {
     // the cluster splits the tables; with one CTA per head (large batches) every CTA would stream all of hash_func from L2:
     // those shapes hash in the separate tensor-core kernel (simhash.cu) and hand the codes over
     fp.hash_in_kernel = fp.gm.C >= 2;
-    const int act = fused_max_active_clusters(fp, ctx->fused_kreg, T > 1);
+    const int act = fused_max_active_clusters(fp, ctx->fused_kreg, T > 1, ctx->shared_spill);
     fp.cluster_waves = act > 0 ? (HT + act - 1) / act : 0;
     fp.ok = true;
     return fp;
@@ -1099,7 +1116,7 @@ int fused_resident_clusters(int C, int threads) {
     fp.gm.C = C;
     fp.threads = threads;
     fp.smem = fused_smem_cap(threads);   // the full carve-up the plan may use
-    return fused_max_active_clusters(fp, false, false);
+    return fused_max_active_clusters(fp, false, false, false);
 }
 int fused_cluster_waves(const mpig_ctx *ctx) { return fused_plan(ctx).ok ? fused_plan(ctx).cluster_waves : 0; }
 
@@ -1152,14 +1169,14 @@ static FusedParams fused_params(const mpig_ctx *ctx, int layer, const FusedPlan 
 
 // One launch over p.H clusters.  The instantiation follows from the block: the debug-clock one when p.dbg is set, the T-token
 // one (with the pending step's ancestor masks, plan_kernel) when p.ntok is.
-static int fused_launch(mpig_ctx *ctx, const FusedPlan &fp, const FusedParams &p, bool pdl, cudaStream_t s) {
+static int fused_launch(mpig_ctx *ctx, int layer, const FusedPlan &fp, const FusedParams &p, bool pdl, cudaStream_t s) {
     const bool tok = p.ntok > 0;
-    const FusedKernel fn = fused_kernel(fp.threads, p.dbg != nullptr, ctx->fused_kreg, tok);
+    const FusedKernel fn = fused_kernel(fp.threads, p.dbg != nullptr, ctx->fused_kreg, tok, ctx->shared_spill);
     MPIG_FUNC_ATTR(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, fused_smem_cap(fp.threads));
     cudaLaunchAttribute attr[2];
     const cudaLaunchConfig_t cfg = fused_config(fp, p.H, pdl, s, attr);
     const int32_t *anc = tok ? step_masks(ctx->step_buf) : nullptr;
-    MPIG_CUDA(cudaLaunchKernelEx(&cfg, fn, p, anc, ctx->slot_map()));
+    MPIG_CUDA(cudaLaunchKernelEx(&cfg, fn, p, anc, ctx->slot_map(), ctx->vis_map(), ctx->private_lo_map(layer)));
     MPIG_LAUNCH_CHECK(ctx);
     ctx->last_decode_fused = 1;
     return MPIG_OK;
@@ -1190,7 +1207,7 @@ int launch_fused(mpig_ctx *ctx, int layer, const void *q, const void *k, const v
         p.peer_rank = peer_rank;
         p.peer_world = peer_world;
     }
-    const int rc = fused_launch(ctx, fp, p, pdl && (ctx->pdl_first || !fp.hash_in_kernel), s);
+    const int rc = fused_launch(ctx, layer, fp, p, pdl && (ctx->pdl_first || !fp.hash_in_kernel), s);
     if (rc) return rc;
     ctx->last_tokens = 1;
     return MPIG_OK;
@@ -1215,7 +1232,7 @@ int launch_fused_tokens(mpig_ctx *ctx, int layer, int T, const void *q, const vo
     }
     FusedParams p = fused_params(ctx, layer, fp, T, q, nullptr, nullptr, out);
     p.ntok = T;
-    rc = fused_launch(ctx, fp, p, true, s);   // under PDL behind the append (or the SimHash kernel)
+    rc = fused_launch(ctx, layer, fp, p, true, s);   // under PDL behind the append (or the SimHash kernel)
     if (rc) return rc;
     ctx->last_tokens = T;
     ctx->last_tokens_waves = fp.cluster_waves;

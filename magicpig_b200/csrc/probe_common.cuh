@@ -89,6 +89,19 @@ __device__ __forceinline__ void st_shared_cluster_f4(const void *local_smem_addr
     asm volatile("st.shared::cluster.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(remote), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
 }
 
+// Shared spill mode (DESIGN.md section 3.12): drop from the tags of this CTA's key range [lo_key, lo_key + Mc) the private keys of
+// the slot that request b does not see.  Keys >= plo (the slot's prompt key count) are private; private key k is seen by b iff bit
+// b of vis_slot[k - plo] is set.  Every tag of such a key that is not EMPTY (one collision or SEL) becomes EMPTY, so the selection,
+// nnz, the index list and the collision bitmaps all see the request's own context.  vis is written by kernels (spill, fork, bind):
+// call it after griddepcontrol.wait.  Ends with a barrier.
+template <typename TagT>
+__device__ __noinline__ void filter_private(TagT *tag, const uint32_t *vis_slot, int plo, int lo_key, int Mc, int b) {
+    constexpr TagT EMPTY = (TagT)((TagT)(~(TagT)0) - 1);
+    for (int i = max(plo - lo_key, 0) + (int)threadIdx.x; i < Mc; i += (int)blockDim.x)
+        if (tag[i] != EMPTY && !((__ldcg(vis_slot + (lo_key + i - plo)) >> b) & 1u)) tag[i] = EMPTY;
+    __syncthreads();
+}
+
 // cluster geometry of a probe: S key segments (padded to a power of two Sp) x r CTAs per segment, C = Sp*r <= 8 CTAs per
 // q-head, each owning Mc keys (one tag each) of one segment
 struct ProbeGeom {

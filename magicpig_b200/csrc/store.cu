@@ -58,27 +58,36 @@ __global__ void pack_records_nhd_kernel(const uint4 *__restrict__ k, const uint4
 
 // Window spill, store side (mpig_spill_window): one CTA per (kv-head, request) of one sparse layer, 8 warps.  With g = spill_g[b]:
 //   window rows [sink, sink + g) -> records n_old .. n_old + g - 1 of the store of the request's slot (slot_of[b], or b when
-//   slot_of is null; the host lets only a request that is alone on its slot spill) (bitwise), their key norms
-//   kn = bf16(||k||_2) widened to fp32 (fp32 sum of squares, one rounding: what fill() stores), and their key halves -> stage
-//   (Hkv, g, d) bf16 at row spill_pre[b] * Hkv for the key hash;
+//   slot_of is null) (bitwise), their key norms kn = bf16(||k||_2) widened to fp32 (fp32 sum of squares, one rounding: what fill()
+//   stores), and their key halves -> the staging for the key hash: a block (Hkv, g, d) bf16 at row spill_pre[b] * Hkv;
 //   window rows [sink + g, sink + g + keep) -> [sink, sink + keep).
+// Shared spill mode (blk != null, [3][B]): the requests of one slot stage into ONE block (Hkv, blk[b], d) at row spill_pre[b] * Hkv,
+// request b's rows at offset blk[B + b] of every kv-head's run, so that the slot's new keys are hashed and merged together; with
+// vis != null (one sparse layer's launch: the map is the same for every layer) the CTAs of kv-head 0 also make private keys
+// blk[2B + b] .. + g - 1 of the slot visible to b alone.
 // The kept rows move down in place, so they are copied in chunks of ascending rows, each chunk read completely before any of
 // it is written (a row is only ever written after every row it lands on has been read).  One CTA owns the whole window of its
 // (request, kv-head): no ordering between CTAs is involved.
 __global__ void __launch_bounds__(256) spill_move_kernel(uint4 *win, uint4 *__restrict__ rec, float *__restrict__ kn_store,
                                                          uint4 *__restrict__ stage, const int32_t *__restrict__ spill_g,
                                                          const int32_t *__restrict__ spill_pre, const int32_t *__restrict__ n_old_b,
-                                                         const int32_t *__restrict__ slot_of, int Hkv, int M, int Wcap, int sink, int keep) {
+                                                         const int32_t *__restrict__ slot_of, int Hkv, int M, int Wcap, int sink, int keep,
+                                                         const int32_t *__restrict__ blk, uint32_t *__restrict__ vis) {
     constexpr int T = 256, UN = 4;
     const int gi = blockIdx.x, b = blockIdx.y, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int g = spill_g[b];
     if (g == 0) return;
     const size_t bg = (size_t)b * Hkv + gi;
-    const size_t sg = (size_t)(slot_of ? slot_of[b] : b) * Hkv + gi;   // store side: the request's slot
+    const int slot = slot_of ? slot_of[b] : b;
+    const size_t sg = (size_t)slot * Hkv + gi;   // store side: the request's slot
     uint4 *w = win + bg * Wcap * 32;
     uint4 *r = rec + (sg * M + n_old_b[b]) * 32;
     float *kns = kn_store + sg * M + n_old_b[b];
-    uint4 *st = stage + ((size_t)spill_pre[b] * Hkv + (size_t)gi * g) * 16;
+    const int B = gridDim.y;
+    const size_t st_rows = blk ? blk[b] : g, st_off = blk ? blk[B + b] : 0;
+    uint4 *st = stage + ((size_t)spill_pre[b] * Hkv + (size_t)gi * st_rows + st_off) * 16;
+    if (vis && gi == 0)
+        for (int j = tid; j < g; j += T) vis[(size_t)slot * M + blk[2 * B + b] + j] = 1u << b;
     for (int j = warp; j < g; j += T / 32) {
         const uint4 x = w[(size_t)(sink + j) * 32 + lane];
         r[(size_t)j * 32 + lane] = x;
@@ -116,6 +125,39 @@ __global__ void __launch_bounds__(256) spill_move_kernel(uint4 *win, uint4 *__re
     }
 }
 
+// shared spill mode, mpig_fork_request (src >= 0: dst sees exactly what src sees) and mpig_bind_request (src < 0: dst sees nothing)
+__global__ void vis_rebind_kernel(uint32_t *vis, size_t words, int src, int dst) {
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < words; i += (size_t)gridDim.x * blockDim.x) {
+        const uint32_t v = vis[i];
+        vis[i] = (v & ~(1u << dst)) | (src >= 0 ? ((v >> src) & 1u) << dst : 0u);
+    }
+}
+
+// shared spill mode, a fill: the slot's map is emptied and its private keys start at n in this layer
+__global__ void reset_private_kernel(uint32_t *vis_slot, int M, int32_t *plo, int n) {
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < M; i += gridDim.x * blockDim.x) vis_slot[i] = 0u;
+    if (blockIdx.x == 0 && threadIdx.x == 0) *plo = n;
+}
+
+int launch_vis_rebind(mpig_ctx *ctx, int src, int dst, cudaStream_t s) {
+    if (!ctx->shared_spill) return MPIG_OK;
+    const size_t words = (size_t)ctx->C * ctx->cfg.max_length;
+    const int blocks = (int)std::min<size_t>((words + 255) / 256, (size_t)ctx->num_sms * 4);
+    vis_rebind_kernel<<<blocks, 256, 0, s>>>(ctx->vis, words, src, dst);
+    MPIG_LAUNCH_CHECK(ctx);
+    return MPIG_OK;
+}
+
+int reset_private(mpig_ctx *ctx, int layer, int request, int n, cudaStream_t s) {
+    if (!ctx->shared_spill) return MPIG_OK;
+    const int slot = ctx->h_slot_of[request], M = ctx->cfg.max_length;
+    const int blocks = std::min((M + 255) / 256, ctx->num_sms * 4);
+    reset_private_kernel<<<blocks, 256, 0, s>>>(ctx->vis + (size_t)slot * M, M, ctx->private_lo + (size_t)layer * ctx->C + slot, n);
+    MPIG_LAUNCH_CHECK(ctx);
+    ctx->h_private_lo[layer][slot] = n;
+    return MPIG_OK;
+}
+
 int launch_pack_nhd(mpig_ctx *ctx, const void *k, const void *v, uint8_t *rec, int Hkv, int n, int rows_cap, cudaStream_t s) {
     const size_t total = (size_t)Hkv * n * 32;
     const int blocks = (int)std::min<size_t>((total + 255) / 256, (size_t)ctx->num_sms * 16);
@@ -142,6 +184,8 @@ int mpig_attn_fill(mpig_ctx *ctx, int layer, int request, const void *k_bf16, co
     const LayerStore &ls = ctx->layers[layer];
     const int Hkv = ctx->cfg.num_key_value_heads, M = ctx->cfg.max_length;
     const int slot = ctx->h_slot_of[request];   // every request bound to this slot sees the new context
+    rc = reset_private(ctx, layer, request, n, as_stream(stream));
+    if (rc) return rc;
     ctx->n_off[layer][slot] = n;
     if (n == 0) return MPIG_OK;
     uint4 *rec = reinterpret_cast<uint4 *>(ls.kv + (size_t)slot * Hkv * M * ctx->rec_bytes);
@@ -204,36 +248,76 @@ int mpig_spill_window(mpig_ctx *ctx, int keep, int32_t *spilled_out, void *strea
     std::vector<int32_t> wl(B);
     int rc = read_lengths(ctx, 0, B, wl.data(), nullptr, s);
     if (rc) return rc;
-    // meta = g[B] | pre[B] (exclusive prefix of g) | n_old[num_layers][B]
-    std::vector<int32_t> meta((size_t)(2 + nl) * B, 0);
+    // meta = g[B] | pre[B] (staging block of each request) | n_old[num_layers][B]; shared spill mode appends blk[3][B] (rows of
+    // the request's staging block, the request's offset in it, its first private offset) | g[C] | pre[C] | n_old[num_layers][C]
+    // per slot.  Exclusive requests stage in request order; in shared spill mode the requests of a slot stage in request order
+    // inside one block per slot, the blocks in slot order, so each slot's new keys are contiguous in the staging and the store.
+    const bool shared = ctx->shared_spill;
+    const int C = ctx->C;
+    const size_t o_blk = (size_t)(2 + nl) * B, o_sg = o_blk + 3 * (size_t)B, o_spre = o_sg + C, o_sn = o_spre + C;
+    std::vector<int32_t> meta(shared ? o_sn + (size_t)nl * C : o_blk, 0);
+    const std::vector<int> &slot = ctx->h_slot_of;
     int tot = 0;
     for (int b = 0; b < B; ++b) {
         const int g = std::max(0, wl[b] - sink - keep);
         meta[b] = g;
-        meta[B + b] = tot;
-        tot += g;
+        if (!shared) {
+            meta[B + b] = tot;
+            tot += g;
+        } else {
+            meta[o_blk + B + b] = meta[o_sg + slot[b]];   // offset inside the slot's block
+            meta[o_sg + slot[b]] += g;
+        }
     }
-    // a shared slot's store and tables are every bound request's context: spilling one request's generated tokens into them would
-    // put those tokens into the others' samples
-    const std::vector<int> &slot = ctx->h_slot_of;
-    for (int b = 0; b < B; ++b)
-        for (int o = 0; o < B && meta[b] > 0; ++o)
-            MPIG_REQUIRE(o == b || slot[o] != slot[b] || wl[o] == 0, MPIG_ESTATE,
-                         "mpig_spill_window: request %d would spill %d rows into context slot %d, which request %d (window of %d rows) "
-                         "shares; a shared request generates at most generation_buffer tokens", b, meta[b], slot[b], o, wl[o]);
+    if (shared) {
+        for (int c = 0; c < C; ++c) {
+            meta[o_spre + c] = tot;
+            tot += meta[o_sg + c];
+        }
+        // private keys have the same offsets in every sparse layer only while the layers agree on the slot's private count
+        std::vector<int> priv(C, -1);
+        for (int l = 0; l < nl; ++l) {
+            if (!ctx->layers[l].sparse) continue;
+            for (int c = 0; c < C; ++c) {
+                if (meta[o_sg + c] == 0) continue;
+                const int pc = ctx->n_off[l][c] - ctx->h_private_lo[l][c];
+                MPIG_REQUIRE(priv[c] < 0 || priv[c] == pc, MPIG_ESTATE,
+                             "mpig_spill_window: context slot %d holds %d private keys in layer %d but %d in an earlier sparse layer "
+                             "(a partial refill?); refill every sparse layer of the slot", c, pc, l, priv[c]);
+                priv[c] = pc;
+            }
+        }
+        for (int b = 0; b < B; ++b) {
+            meta[B + b] = meta[o_spre + slot[b]];
+            meta[o_blk + b] = meta[o_sg + slot[b]];
+            meta[o_blk + 2 * B + b] = std::max(priv[slot[b]], 0) + meta[o_blk + B + b];
+        }
+    } else {
+        // a shared slot's store and tables are every bound request's context: spilling one request's generated tokens into them
+        // would put those tokens into the others' samples
+        for (int b = 0; b < B; ++b)
+            for (int o = 0; o < B && meta[b] > 0; ++o)
+                MPIG_REQUIRE(o == b || slot[o] != slot[b] || wl[o] == 0, MPIG_ESTATE,
+                             "mpig_spill_window: request %d would spill %d rows into context slot %d, which request %d (window of %d rows) "
+                             "shares; a shared request generates at most generation_buffer tokens unless the context was created "
+                             "with shared spill (reserved[3])", b, meta[b], slot[b], o, wl[o]);
+    }
     for (int l = 0; l < nl; ++l) {
         if (!ctx->layers[l].sparse) continue;
         for (int b = 0; b < B; ++b) {
             const int n_old = ctx->n_off[l][slot[b]];
-            MPIG_REQUIRE(n_old + meta[b] <= M, MPIG_ESTATE,
+            const int add = shared ? meta[o_sg + slot[b]] : meta[b];   // shared spill: the capacity is the slot's
+            MPIG_REQUIRE(n_old + add <= M, MPIG_ESTATE,
                          "mpig_spill_window: layer %d request %d: %d offloaded + %d spilled keys exceed max_length=%d", l, b,
-                         n_old, meta[b], M);
-            meta[(size_t)(2 + l) * B + b] = n_old;
+                         n_old, add, M);
+            meta[(size_t)(2 + l) * B + b] = n_old + (shared ? meta[o_blk + B + b] : 0);
         }
+        if (shared)
+            for (int c = 0; c < C; ++c) meta[o_sn + (size_t)l * C + c] = ctx->n_off[l][c];
     }
     if (tot > 0) {
         // scratch for the worst case (every request spills all its non-sink rows), allocated once
-        const size_t meta_bytes = (((size_t)(2 + nl) * B * sizeof(int32_t)) + 255) & ~(size_t)255;
+        const size_t meta_bytes = ((meta.size() * sizeof(int32_t)) + 255) & ~(size_t)255;
         const size_t rows_cap = (size_t)B * std::max(ctx->Wcap - sink, 1);
         const size_t key_bytes = rows_cap * Hkv * d * sizeof(__nv_bfloat16);
         if (!ctx->spill_buf) {
@@ -251,21 +335,28 @@ int mpig_spill_window(mpig_ctx *ctx, int keep, int32_t *spilled_out, void *strea
         __nv_bfloat16 *keys = reinterpret_cast<__nv_bfloat16 *>(ctx->spill_buf + meta_bytes);
         int16_t *codes = reinterpret_cast<int16_t *>(ctx->spill_buf + meta_bytes + key_bytes);
         MPIG_CUDA(cudaMemcpyAsync(d_meta, meta.data(), meta.size() * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+        bool vis_done = false;
         for (int l = 0; l < nl; ++l) {
             LayerStore &ls = ctx->layers[l];
             if (!ls.sparse) continue;
             const int32_t *n_old = d_meta + (size_t)(2 + l) * B;
             spill_move_kernel<<<dim3(Hkv, B), 256, 0, s>>>(reinterpret_cast<uint4 *>(ls.win), reinterpret_cast<uint4 *>(ls.kv), ls.kn,
                                                           reinterpret_cast<uint4 *>(keys), d_meta, d_meta + B, n_old, ctx->slot_map(),
-                                                          Hkv, M, ctx->Wcap, sink, keep);
+                                                          Hkv, M, ctx->Wcap, sink, keep, shared ? d_meta + o_blk : nullptr,
+                                                          shared && !vis_done ? ctx->vis : nullptr);
             MPIG_LAUNCH_CHECK(ctx);
-            for (int b = 0; b < B; ++b) {
-                if (meta[b] == 0) continue;
-                const int rc = mpig_hash_keys(ctx, keys + (size_t)meta[B + b] * Hkv * d, meta[b], codes + (size_t)meta[B + b] * Hkv * L,
+            vis_done = true;
+            // the key hash and the merge: per request, or per slot in shared spill mode
+            const int nb = shared ? C : B;
+            const int32_t *g_of = shared ? meta.data() + o_sg : meta.data(), *pre_of = shared ? meta.data() + o_spre : meta.data() + B;
+            for (int i = 0; i < nb; ++i) {
+                if (g_of[i] == 0) continue;
+                const int rc = mpig_hash_keys(ctx, keys + (size_t)pre_of[i] * Hkv * d, g_of[i], codes + (size_t)pre_of[i] * Hkv * L,
                                               stream);
                 if (rc) return rc;
             }
-            const int rc = launch_table_merge(ctx, l, codes, d_meta, d_meta + B, n_old, s);
+            const int rc = shared ? launch_table_merge_slots(ctx, l, codes, d_meta + o_sg, d_meta + o_spre, d_meta + o_sn + (size_t)l * C, s)
+                                  : launch_table_merge(ctx, l, codes, d_meta, d_meta + B, n_old, s);
             if (rc) return rc;
         }
         for (int b = 0; b < B; ++b)

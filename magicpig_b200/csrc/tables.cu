@@ -251,6 +251,8 @@ __global__ void __launch_bounds__(THREADS) probe_kernel(const int32_t *__restric
                                                         int32_t *__restrict__ nnz,            // (H)
                                                         uint32_t *__restrict__ bitmaps_out,   // (H,2,words) or null
                                                         const int32_t *__restrict__ slot_of,  // (B) or null: request b reads slot b
+                                                        const uint32_t *__restrict__ vis,     // [C][M] shared spill mode, else null
+                                                        const int32_t *__restrict__ plo,      // [C] this layer's private starts
                                                         int L, int NB, int M, int G, int Hq, int Mc, int words, int S, int r, int seg_len) {
     extern __shared__ __align__(16) uint8_t smem_raw[];
     constexpr TagT SEL = (TagT)(~(TagT)0);
@@ -381,6 +383,10 @@ __global__ void __launch_bounds__(THREADS) probe_kernel(const int32_t *__restric
         }
     }
     __syncthreads();
+    if (vis) {   // shared spill mode: the private keys of the slot that this head's request does not see (after pdl_wait above)
+        const int sl = slot_of[h / Hq];
+        filter_private(tag, vis + (size_t)sl * M, plo[sl], lo_key, Mc, h / Hq);
+    }
 
     // compaction of this CTA's key range, ascending.  Each thread owns a run of `pw` 32-bit words of tags; pw is odd so the
     // lanes of a warp start in 32 different banks (an even word stride made every sweep load a 2..8-way bank conflict).
@@ -469,8 +475,9 @@ using namespace mpig;
 namespace mpig {
 // shared with decode.cu
 template <typename TagT, int T>
-static int launch_probe_tt(mpig_ctx *ctx, const LayerStore &ls, const int32_t *query, int32_t *results, int32_t *nnz,
+static int launch_probe_tt(mpig_ctx *ctx, int layer, const int32_t *query, int32_t *results, int32_t *nnz,
                            cudaStream_t s, bool pdl, int C, int r, int Mc, size_t smem) {
+    const LayerStore &ls = ctx->layers[layer];
     const int M = ctx->cfg.max_length, L = ctx->cfg.L, S = ctx->nseg;
     MPIG_FUNC_ATTR((probe_kernel<TagT, T>), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     MPIG_FUNC_ATTR((probe_kernel<TagT, T>), cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
@@ -490,7 +497,8 @@ static int launch_probe_tt(mpig_ctx *ctx, const LayerStore &ls, const int32_t *q
     cfg.attrs = attr;
     cfg.numAttrs = pdl ? 2 : 1;
     MPIG_CUDA(cudaLaunchKernelEx(&cfg, probe_kernel<TagT, T>, query, (const int32_t *)ls.offsets, (const uint16_t *)ls.items,
-                                 results, nnz, bm, ctx->slot_map(), L, ctx->NB, M, ctx->G, ctx->cfg.num_attention_heads, Mc,
+                                 results, nnz, bm, ctx->slot_map(), ctx->vis_map(), ctx->private_lo_map(layer), L,
+                                 ctx->NB, M, ctx->G, ctx->cfg.num_attention_heads, Mc,
                                  ctx->bitmap_words, S, r, ctx->seg_len));
     MPIG_LAUNCH_CHECK(ctx);
     return MPIG_OK;
@@ -511,7 +519,7 @@ ProbeGeom probe_geometry(const mpig_ctx *ctx) {
 }
 
 template <typename TagT>
-static int launch_probe_t(mpig_ctx *ctx, const LayerStore &ls, const int32_t *query, int32_t *results, int32_t *nnz,
+static int launch_probe_t(mpig_ctx *ctx, int layer, const int32_t *query, int32_t *results, int32_t *nnz,
                           cudaStream_t s, bool pdl) {
     const int M = ctx->cfg.max_length, L = ctx->cfg.L;
     const ProbeGeom gm = probe_geometry(ctx);
@@ -522,16 +530,15 @@ static int launch_probe_t(mpig_ctx *ctx, const LayerStore &ls, const int32_t *qu
     // more clusters than the GPU holds at once (1024-thread CTAs are one per SM): halve the CTA so two share an SM and the
     // whole grid is resident in one wave
     if (ctx->H * C > ctx->num_sms && smem <= 110 * 1024)
-        return launch_probe_tt<TagT, 512>(ctx, ls, query, results, nnz, s, pdl, C, r, Mc, smem);
-    return launch_probe_tt<TagT, 1024>(ctx, ls, query, results, nnz, s, pdl, C, r, Mc, smem);
+        return launch_probe_tt<TagT, 512>(ctx, layer, query, results, nnz, s, pdl, C, r, Mc, smem);
+    return launch_probe_tt<TagT, 1024>(ctx, layer, query, results, nnz, s, pdl, C, r, Mc, smem);
 }
 
 int launch_probe(mpig_ctx *ctx, int layer, const int32_t *query, int32_t *results, int32_t *nnz, cudaStream_t s, bool pdl) {
-    const LayerStore &ls = ctx->layers[layer];
     ctx->last_probe_layer = layer;
     // table ids 0..L-1 must stay clear of the two reserved tag values
-    if (ctx->cfg.L <= 254) return launch_probe_t<uint8_t>(ctx, ls, query, results, nnz, s, pdl);
-    return launch_probe_t<uint16_t>(ctx, ls, query, results, nnz, s, pdl);
+    if (ctx->cfg.L <= 254) return launch_probe_t<uint8_t>(ctx, layer, query, results, nnz, s, pdl);
+    return launch_probe_t<uint16_t>(ctx, layer, query, results, nnz, s, pdl);
 }
 }  // namespace mpig
 
@@ -571,6 +578,24 @@ int mpig::launch_table_merge(mpig_ctx *ctx, int layer, const int16_t *codes, con
     return MPIG_OK;
 }
 
+// shared spill mode: entry c of g / pre / n_old ([C] each) merges the keys the requests of slot c spilled, contiguous in the
+// slot's store and in the staging, into slot c's tables -- one CTA per (table, kv-head, slot x segment), so no two CTAs write
+// the same table row
+int mpig::launch_table_merge_slots(mpig_ctx *ctx, int layer, const int16_t *codes, const int32_t *g, const int32_t *pre,
+                                   const int32_t *n_old, cudaStream_t s) {
+    const LayerStore &ls = ctx->layers[layer];
+    const int Hkv = ctx->cfg.num_key_value_heads, L = ctx->cfg.L, S = ctx->nseg, NB = ctx->NB;
+    const size_t base = (size_t)(NB + 1 + 40) * sizeof(int);
+    const int staged = base + (size_t)(NB + 1) * sizeof(int) <= 200 * 1024;
+    const size_t smem = base + (staged ? (size_t)(NB + 1) * sizeof(int) : 0);
+    MPIG_FUNC_ATTR(table_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    table_merge_kernel<<<dim3(L, Hkv, ctx->C * S), 512, smem, s>>>(codes, ls.offsets, reinterpret_cast<uint16_t *>(ls.items), g, pre,
+                                                                   n_old, nullptr, Hkv, L, NB, ctx->cfg.max_length, S, ctx->seg_len,
+                                                                   staged);
+    MPIG_LAUNCH_CHECK(ctx);
+    return MPIG_OK;
+}
+
 extern "C" {
 
 int mpig_lsh_fill(mpig_ctx *ctx, int layer, int request, const int16_t *sorted_codes, const int32_t *sorted_indices,
@@ -582,6 +607,8 @@ int mpig_lsh_fill(mpig_ctx *ctx, int layer, int request, const int16_t *sorted_c
     MPIG_REQUIRE(n >= 0 && n <= ctx->cfg.max_length, MPIG_EINVAL, "mpig_lsh_fill: n=%d exceeds max_length=%d", n,
                  ctx->cfg.max_length);
     MPIG_REQUIRE(n == 0 || (sorted_codes && sorted_indices), MPIG_EINVAL, "mpig_lsh_fill: null input");
+    rc = reset_private(ctx, layer, request, n, as_stream(stream));
+    if (rc) return rc;
     return launch_build(ctx, layer, request, sorted_codes, sorted_indices, n, as_stream(stream));
 }
 
@@ -593,6 +620,8 @@ int mpig_lsh_build(mpig_ctx *ctx, int layer, int request, const int16_t *key_cod
     MPIG_REQUIRE(n >= 0 && n <= ctx->cfg.max_length, MPIG_EINVAL, "mpig_lsh_build: n=%d exceeds max_length=%d", n,
                  ctx->cfg.max_length);
     MPIG_REQUIRE(n == 0 || key_codes, MPIG_EINVAL, "mpig_lsh_build: null input");
+    rc = reset_private(ctx, layer, request, n, as_stream(stream));
+    if (rc) return rc;
     return launch_build(ctx, layer, request, key_codes, nullptr, n, as_stream(stream));
 }
 

@@ -58,7 +58,7 @@ class LlamaDecodeRunner:
                  seed: int = 0, generation_buffer: int = 256, dense_layers=(0, 16, 32, 48, 64), num_layers: int | None = None,
                  tp_rank: int = 0, tp_world: int = 1, tp_group=None, fused: bool = True, tp_mode: str = "ag",
                  tp_transport: str = "nccl", max_query_tokens: int = 1, num_contexts: int | None = None,
-                 dense_tail_rows: int | None = None):
+                 dense_tail_rows: int | None = None, shared_spill: bool = False):
         """tp_mode (only with tp_world > 1; see magicpig_b200/tp.py):
              "ag"        attention sharded by KV head, one all-gather of head outputs per layer, wo / MLP replicated (north-star)
              "megatron"  + wo row-split, gate/up column-split, down row-split, two all-reduces per layer (llama_dist.py:49-70)
@@ -68,7 +68,9 @@ class LlamaDecodeRunner:
            max_query_tokens: largest T of step_tokens(T) (verification steps of speculative decoding; 1 = step() only).
            num_contexts: contexts (sampled stores + hash tables) the batch holds; None = one per request.
            dense_tail_rows: R > 0 keeps the dense layers' prompt once per context, R rows per request after it; None = a full
-           dense cache per request."""
+           dense cache per request.
+           shared_spill: requests forked from one prompt may spill their windows into the shared context (spill_window()), each
+           seeing only its own spilled tokens; needs num_contexts < batch_size <= 32."""
         assert tp_mode in ("ag", "megatron") and tp_transport in ("nccl", "peer")
         self.tp_mode, self.tp_transport = tp_mode, tp_transport
         self.shape = shape
@@ -106,7 +108,7 @@ class LlamaDecodeRunner:
                                           generation_buffer=generation_buffer, dense_layers=dense_layers, device=device,
                                           hash_func=hash_func, num_key_value_heads=self.Hkv_loc,
                                           num_attention_heads=self.Hq_loc, max_query_tokens=max_query_tokens,
-                                          num_contexts=num_contexts, dense_tail_rows=dense_tail_rows)
+                                          num_contexts=num_contexts, dense_tail_rows=dense_tail_rows, shared_spill=shared_spill)
 
         def w(*shape_):
             return (torch.randn(shape_, generator=g, device=self.device, dtype=torch.float32) * 0.02).to(torch.bfloat16)

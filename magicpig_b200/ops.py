@@ -42,12 +42,16 @@ class Context:
                  head_dim: int, batch_size: int, max_length: int, num_sink_tokens: int = 4, num_local_tokens: int = 64,
                  generation_buffer: int = 256, dense_layers: Sequence[int] = (), alloc_dense_kv: bool = False,
                  device: str | torch.device = "cuda:0", max_query_tokens: int = 1, num_contexts: int = 0,
-                 dense_tail_rows: int = 0):
+                 dense_tail_rows: int = 0, shared_spill: bool = False):
         """num_contexts: context slots C in [0, batch_size] (0 = batch_size, every request owns its context).  The sampled store
         and the hash tables exist once per slot; requests bound to one slot decode over one copy (fork(), bind()).
         dense_tail_rows: R > 0 keeps the dense layers' prompt rows once per slot as well (needs C < batch_size and alloc_dense_kv);
         each request holds only the R rows it adds after its prompt, so it may generate at most R tokens past the prompt it was
-        filled or forked with.  0 = one full dense cache per request."""
+        filled or forked with.  0 = one full dense cache per request.
+        shared_spill: requests that share a slot may spill_window() into it (needs 0 < C < batch_size <= 32).  Each spilled key is
+        private: it is seen by the request that spilled it and by requests later forked from it, so every request decodes as if
+        it had the slot to itself.  Private keys nobody sees any more keep their place in the slot until it is refilled: size
+        max_length for the prompt plus every request's spilled tokens."""
         self.lib = N.load()
         self.device = torch.device(device)
         if self.device.type != "cuda":
@@ -77,12 +81,14 @@ class Context:
         cfg.reserved[0] = int(os.environ.get("MPIG_CTA_PER_SM", "1"))   # experiment switch: 2 = clusters of 512-thread CTAs, two per SM
         cfg.reserved[1] = int(num_contexts)
         cfg.reserved[2] = int(dense_tail_rows)
+        cfg.reserved[3] = 1 if shared_spill else 0
         h = ctypes.c_void_p()
         with torch.cuda.device(self.device):
             N.check(self.lib.mpig_create(ctypes.byref(cfg), ctypes.byref(h)), "mpig_create")
         self._h = h
         self.C = self.get_info("num_contexts")
         self.dense_tail_rows = self.get_info("dense_tail_rows")
+        self.shared_spill = bool(self.get_info("shared_spill"))
         self.max_query_tokens = 1
         self.last_tokens = 1   # T of the last decode: the readers return B*T*Hq rows
         self.pending_tokens = 0   # T of the last plan (the shape accept() expects)
@@ -123,7 +129,8 @@ class Context:
 
     def fork(self, src: int, dst: int):
         """Bind request dst to request src's context slot and copy src's window, avg_k, dense-layer KV and lengths into dst
-        (with dense_tail_rows > 0 only the dense rows past src's prompt: the prompt stays in the slot).
+        (with dense_tail_rows > 0 only the dense rows past src's prompt: the prompt stays in the slot).  With shared_spill dst
+        sees exactly the spilled keys src sees.
         Synchronises; not capturable, but a step captured before it replays with the new binding.  Ends the pending step
         (rewind / accept are refused until the next plan)."""
         N.check(self.lib.mpig_fork_request(self._h, int(src), int(dst), _stream()), "mpig_fork_request")
@@ -131,7 +138,8 @@ class Context:
 
     def bind(self, request: int, slot: int):
         """Bind `request` to context slot `slot` without touching its window or lengths (fill the slot and the window next; with
-        dense_tail_rows > 0 dense-fill it too before its dense outputs mean anything).
+        dense_tail_rows > 0 dense-fill it too before its dense outputs mean anything).  With shared_spill it sees no spilled key
+        until it spills again.
         Synchronises; ends the pending step like fork()."""
         N.check(self.lib.mpig_bind_request(self._h, int(request), int(slot), _stream()), "mpig_bind_request")
         self.pending_tokens = 0

@@ -5,8 +5,8 @@
 Sizes are tiny (the tools slow kernels down 10-100x) but cover: the stand-alone SimHash / probe (uint8 tags, several clusters
 shapes, two key segments) / gather-attention kernels, the fused single-launch decode (cluster of 8, cluster of 4 over two
 segments, one CTA per head with codes from the SimHash kernel, several selection passes), the three-launch decode, the dense
-kernel, the tensor-core key hash, the table build, the window spill, verification steps of T tokens, token trees with an accept and
-requests sharing one context slot.  Results are also checked against each other so a tool run doubles as a test.
+kernel, the tensor-core key hash, the table build, the window spill, verification steps of T tokens, token trees with an accept,
+requests sharing one context slot, and shared spill (several requests of one slot spill, a fork, single-token and T-token decodes).  Results are also checked against each other so a tool run doubles as a test.
 """
 import os
 import sys
@@ -354,8 +354,78 @@ def shared_case(B, Hq, Hkv, n, K, L):
     print(f"shared B={B} Hq={Hq} Hkv={Hkv} n={n}: ok")
 
 
+def shared_spill_case(B, Hq, Hkv, n, K, L, T):
+    """B requests on one slot in shared spill mode against a twin with one slot per request: every request spills (the visibility
+    writes of spill_move_kernel, the per-slot merge), single-token and T-token decodes (the filter of the fused and probe kernels),
+    then a fork (vis_rebind_kernel) after which the forked request, fed the same inputs as its source, decodes exactly like it."""
+    M = n + 400
+    g = torch.Generator(device=dev).manual_seed(11)
+    hf = torch.randn((d, K * L), generator=g, device=dev).bfloat16()
+    key = torch.randn((Hkv, n, d), generator=g, device=dev).bfloat16()
+    val = torch.randn((Hkv, n, d), generator=g, device=dev).bfloat16()
+    ctxs = []
+    for C, shared in ((1, True), (0, False)):
+        ctx = Context(K, L, 1, Hq, Hkv, d, B, M, num_local_tokens=64, generation_buffer=24, device=dev, max_query_tokens=T,
+                      num_contexts=C, shared_spill=shared)
+        ctx.set_option("save_mask", 1)
+        ctx.set_option("out_f32", 1)
+        ctx.set_hash_func(hf)
+        for b in (range(1) if shared else range(B)):
+            ctx.attn_fill(0, b, key, val, key.norm(p=2, dim=-1).float())
+            ctx.lsh_build(0, b, ctx.hash_keys(key))
+        g2 = torch.Generator(device=dev).manual_seed(12)
+        for b in range(B):
+            w = 68 + 4 * b   # different window lengths: different spill sizes
+            ctx.window_fill(0, b, torch.zeros((Hkv, d), dtype=torch.bfloat16, device=dev),
+                            torch.randn((Hkv, w, d), generator=g2, device=dev).bfloat16(),
+                            torch.randn((Hkv, w, d), generator=g2, device=dev).bfloat16())
+        ctxs.append(ctx)
+    sh, tw = ctxs
+    for step in range(4):
+        if step == 2:
+            spilled = [c.spill_window(48).tolist() for c in ctxs]
+            assert spilled[0] == spilled[1] and min(spilled[0]) > 0, spilled
+        for impl in (1, 0):
+            q = torch.randn((B * Hq, d), generator=g, device=dev).bfloat16()
+            kv = torch.randn((B * Hkv, d), generator=g, device=dev).bfloat16()
+            nz = []
+            for c in ctxs:
+                c.set_option("decode_impl", impl)
+                c.plan()
+                c.decode(0, q, kv, kv)
+                nz.append((c.last_probe()[0], c.last_out_f32()))
+            assert torch.equal(nz[0][0], nz[1][0]) and float((nz[0][1] - nz[1][1]).abs().max()) <= 1e-5 * float(nz[1][1].abs().max()), \
+                f"step {step} impl {impl}: shared != twin"
+    q = torch.randn((B, T, Hq, d), generator=g, device=dev).bfloat16()
+    kv = torch.randn((B, T, Hkv, d), generator=g, device=dev).bfloat16()
+    nz = []
+    for c in ctxs:
+        c.set_option("decode_impl", 1)
+        c.plan(T)
+        c.decode_tokens(0, T, q, kv, kv)
+        nz.append(c.last_probe()[0])
+        c.rewind(torch.zeros(B, dtype=torch.int32, device=dev))
+    assert torch.equal(nz[0], nz[1]), "T-token step: shared != twin"
+    sh.fork(0, B - 1)
+    q = torch.randn((B, Hq, d), generator=g, device=dev).bfloat16()
+    kv = torch.randn((B, Hkv, d), generator=g, device=dev).bfloat16()
+    q[B - 1], kv[B - 1] = q[0], kv[0]
+    sh.plan()
+    sh.decode(0, q, kv, kv)
+    nnz, res = sh.last_probe(want_results=True)
+    o = sh.last_out_f32()
+    torch.cuda.synchronize()
+    a, b_ = slice(0, Hq), slice((B - 1) * Hq, B * Hq)
+    valid = torch.arange(M, device=dev)[None] < nnz[a, None]
+    assert torch.equal(nnz[a], nnz[b_]) and torch.equal(torch.where(valid, res[a], -1), torch.where(valid, res[b_], -1)) \
+        and torch.equal(o[a], o[b_]), "fork: dst != src"
+    print(f"shared spill B={B} Hq={Hq} Hkv={Hkv} n={n} T={T}: ok")
+
+
 if __name__ == "__main__":
-    which = sys.argv[1:] or ["stages", "dense", "decode", "hostpeer", "spill", "tokens", "tree", "shared"]
+    which = sys.argv[1:] or ["stages", "dense", "decode", "hostpeer", "spill", "tokens", "tree", "shared", "shared_spill"]
+    if "shared_spill" in which:
+        shared_spill_case(3, 4, 2, 700, 6, 24, 3)
     if "shared" in which:
         shared_case(3, 4, 2, 700, 6, 24)                 # clusters of several CTAs per head
     if "tree" in which:
