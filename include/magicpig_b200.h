@@ -144,7 +144,8 @@ int mpig_get_info(mpig_ctx *ctx, const char *key, int64_t *value);
 /* Capacity errors the DEVICE detected (the lengths saturate there): bit 0 = a sparse window is full (generation_buffer
  * exhausted: each further token overwrites the previous one's K/V), bit 1 = a dense cache reached its capacity (max_length, or base + R with reserved[2]), bit 2 = mpig_rewind
  * met a drop outside [0, T] (that request was left untouched), bit 3 = mpig_plan_tree met a malformed tree (that request ran as a
- * chain) or mpig_accept met a path that is not a root path of the step (that request was left untouched).  mpig_plan
+ * chain) or mpig_accept met a path that is not a root path of the step (that request was left untouched), bit 4 =
+ * mpig_reorder_requests met a map that breaks its rule (every request was left untouched).  mpig_plan
  * itself returns MPIG_ESTATE for the same conditions as long as it has not been captured into a CUDA graph (replays advance
  * only the device-side lengths).  mpig_spill_window is the way out of a full sparse window.  Synchronises `stream`.  The
  * reference has no such check (flashinfer append past the page). */
@@ -158,7 +159,8 @@ int mpig_clear(mpig_ctx *ctx, void *stream);
 int mpig_set_hash_func(mpig_ctx *ctx, const void *hash_func_bf16, void *stream);
 
 /* ---- context slots (no reference equivalent; see mpig_config.reserved[1]) ------------------------------------------------------
- * Both calls return MPIG_ESTATE when C = batch_size (the bindings are then fixed: request b reads slot b), are not capturable, and
+ * Fork and bind return MPIG_ESTATE when C = batch_size (the bindings are then fixed: request b reads slot b), are not capturable
+ * (mpig_reorder_requests is the capturable form of a batch of forks), and
  * end the pending step: mpig_rewind / mpig_accept are refused (MPIG_ESTATE) until the next plan.  A step captured before either
  * call replays with the new bindings (the kernels read the device map).
  *
@@ -172,6 +174,24 @@ int mpig_fork_request(mpig_ctx *ctx, int src, int dst, void *stream);
  * mpig_lsh_fill) and the window next.  In shared spill mode the request sees no private key until it spills again.  Synchronises
  * `stream`. */
 int mpig_bind_request(mpig_ctx *ctx, int request, int slot, void *stream);
+/* Request b continues request src_of[b]'s sequence (device int32 [B]; src_of[b] == b leaves b as it is).  The device-side,
+ * capturable form of mpig_fork_request(src_of[b], b) for every b with src_of[b] != b, all at once (beam search: each step, each new
+ * beam continues some old beam).  For every moved request b, with s = src_of[b]: window rows [0, win_len[s]) of every sparse layer
+ * and kv-head and avg_k; dense rows [0, dense_len[s]) (reserved[2] = R > 0: tail rows [0, min(dense_len[s] - dense_base[s], R))
+ * and the base); both lengths; the slot binding; in shared spill mode (reserved[3]) b then sees exactly the private keys s sees.
+ * Every later decode output equals the output after those forks, bitwise.  One kernel launch plus one device-to-device copy of
+ * the slot map (the decode kernels read the map before they wait on their predecessor, so no kernel writes it).
+ * The map's rule: 0 <= src_of[b] < B and src_of[src_of[b]] == src_of[b] for every b -- a request that is a source keeps its own
+ * sequence, so no request is both read and written and the copy runs in place.  Any beam step can be put in this form
+ * (magicpig_b200.attnserver.beam_sources).  A map that breaks the rule changes nothing and raises mpig_error_flags bit 4; outside
+ * a capture the call reads the map first (synchronises `stream`) and then also returns MPIG_EINVAL (the call may be repeated).
+ * Capturable: a replay applies whatever the map holds then.  Capturing it makes the host mirror of the lengths inexact until
+ * mpig_clear (as a captured plan does), and makes every later host path that needs a request's binding or dense base (fills,
+ * mpig_spill_window, fork, bind) read the device maps first, for the rest of the context's life (the graph may be replayed at
+ * any time).  Eager calls leave the mirrors exact.  Ends the pending step (mpig_rewind / mpig_accept are refused until the next plan).  MPIG_ESTATE when
+ * C = batch_size, MPIG_EINVAL on a null argument.  With R = 0 a moved request copies its whole dense cache: correct but slow at long
+ * contexts (see DESIGN.md section 3.13). */
+int mpig_reorder_requests(mpig_ctx *ctx, const int32_t *src_of, void *stream);
 
 /* ---- lsh.LSH --------------------------------------------------------------------------------- */
 /* LSH::fill (lsh.cc:143-201): tables of one (layer, request) from codes already sorted per

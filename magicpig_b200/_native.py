@@ -87,6 +87,7 @@ _SIGNATURES = {
     "mpig_accept": (_i, [_vp, _vp, _vp, _vp]),
     "mpig_fork_request": (_i, [_vp, _i, _i, _vp]),
     "mpig_bind_request": (_i, [_vp, _i, _i, _vp]),
+    "mpig_reorder_requests": (_i, [_vp, _vp, _vp]),
     "mpig_launch_count": (ctypes.c_uint64, [_vp]),
     "mpig_get_info": (_i, [_vp, ctypes.c_char_p, ctypes.POINTER(ctypes.c_int64)]),
     "mpig_error_flags": (_i, [_vp, ctypes.POINTER(ctypes.c_int32), _vp]),

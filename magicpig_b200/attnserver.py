@@ -23,6 +23,30 @@ from .ops import Context
 from . import synth
 
 
+def beam_sources(parents: torch.Tensor):
+    """Where the new beams of a beam-search step live.  parents (B,) int: new beam i continues old beam parents[i], old beam j
+    being held by request j.  Returns (src_of, request_of), both int32 (B,) on parents' device:
+      request_of[i]  the request that holds new beam i: each chosen parent keeps its own request for its first child (in i order),
+                     the other children take the requests of the unchosen parents in ascending order (a permutation);
+      src_of         the map for LSHSparseAttnServer.reorder: src_of[request_of[i]] = parents[i].  Every source keeps its own
+                     request, so src_of[src_of[b]] == src_of[b] by construction.
+    Device torch ops only (B x B comparisons): no host synchronisation and no data-dependent shapes, so it can be captured."""
+    p = parents.long().reshape(-1)
+    B = p.numel()
+    ar = torch.arange(B, device=p.device)
+    same = p[:, None] == p[None, :]                                    # [i, j]: beams i and j have one parent
+    first = ~(same & (ar[None, :] < ar[:, None])).any(dim=1)          # i is its parent's first child
+    chosen = (p[None, :] == ar[:, None]).any(dim=1)                   # [r]: request r holds a parent
+    free_rank = torch.cumsum((~chosen).long(), 0) - 1                 # rank of an unchosen request among the unchosen
+    free = ((~chosen[None, :]) & (free_rank[None, :] == ar[:, None])).long()   # [k, r]: r is the k-th unchosen request
+    free_req = (free * ar[None, :]).sum(dim=1)                        # the k-th unchosen request (k < their count)
+    child_rank = (torch.cumsum((~first).long(), 0) - 1).clamp(min=0)  # rank of a later child among the later children
+    request_of = torch.where(first, p, free_req[child_rank])
+    src_of = torch.empty_like(p)
+    src_of[request_of] = p
+    return src_of.to(torch.int32), request_of.to(torch.int32)
+
+
 class LSHSparseAttnServer:
     def __init__(self,
                  config,
@@ -160,6 +184,16 @@ class LSHSparseAttnServer:
             self.ctx.fork(src_request, dst)
             for a in self.avg_k:
                 a[dst].copy_(a[src_request])
+
+    def reorder(self, src_of: torch.Tensor):
+        """Not in the reference.  Request b continues request src_of[b]'s sequence: fork(src_of[b], b) for every b with
+        src_of[b] != b, done on the device (the server's avg_k copies are gathered with device ops too).  src_of: device int32
+        (B,) whose sources are fixed points (src_of[src_of[b]] == src_of[b]); beam_sources() builds one from a beam step's
+        parents.  CUDA-graph capturable.  Needs num_contexts < batch_size."""
+        self.ctx.reorder(src_of)
+        idx = src_of.long()
+        for a in self.avg_k:
+            a.copy_(a.index_select(0, idx))
 
     def bind(self, request: int, context: int):
         """Not in the reference.  Bind `request` to context slot `context` (0 <= context < num_contexts); fill() and

@@ -92,12 +92,16 @@ struct LayerStore {
 
 // one entry of the accept kernel's layer table: the REC-byte rows of a sparse window ([BG][cap], cap = Wcap) or of a dense KV
 // cache ([BG][cap], cap = max_length, or the request tails with cap = R in shared dense mode); dense = 1 selects dense_len and the
-// dense step base
+// dense step base.  The reorder kernel walks the same table: a sparse entry also carries the layer's avg_k ([BG][d], null for a
+// dense entry), and x0 is the entry's first CTA column in the reorder grid (Hkv * ceil(cap / REORDER_ROWS) columns per entry).
 struct AcceptLayer {
     uint8_t *rows;
     int cap;
     int dense;
+    __nv_bfloat16 *avg_k;
+    int x0;
 };
+constexpr int REORDER_ROWS = 64;   // rows one CTA of the reorder kernel copies (32 KB of records)
 
 struct AttendTuning {
     int ctas = 0;    // 0 = one per SM * occupancy
@@ -107,7 +111,7 @@ struct AttendTuning {
 };
 
 // The verification step between a plan and its rewind or accept.  Only begin() and end() write it: the plans begin a step
-// (step.cu); rewind and accept end it, and so do mpig_clear, mpig_fork_request and mpig_bind_request.
+// (step.cu); rewind and accept end it, and so do mpig_clear, mpig_fork_request, mpig_bind_request and mpig_reorder_requests.
 struct PendingStep {
     int T = 0;            // node count of the last plan (0 = no plan since create / clear); decode_tokens must match it
     bool open = false;    // the step may still be rewound or accepted (at most once per plan)
@@ -143,21 +147,32 @@ struct mpig_ctx {
     std::vector<std::vector<int>> n_off;  // [layer][slot] offloaded key count (host bookkeeping)
     // context slots: the sampled store and the tables exist once per slot, request b reads slot slot_of[b].  The device map is
     // allocated at create time and never moves (a captured step reads the bindings of the replay); h_slot_of mirrors it.  Only
-    // copy-engine calls (mpig_clear, mpig_fork_request, mpig_bind_request) write it, never a kernel.
+    // copy-engine calls write it, never a kernel: mpig_clear, mpig_fork_request and mpig_bind_request upload it, and
+    // mpig_reorder_requests has its kernel write the new map into slot_stage and then copies that into slot_of with a
+    // device-to-device memcpy (a memcpy node under capture).  So the decode kernels may read it before griddepcontrol.wait.
     int C = 0;                            // number of slots (1..B)
     int32_t *slot_of = nullptr;           // [B]
+    int32_t *slot_stage = nullptr;        // [B] the reorder kernel's new map, copied into slot_of after it
     std::vector<int> h_slot_of;           // [B]
+    // h_slot_of and h_dense_base equal the device maps unless a reorder was captured into a CUDA graph (its replays change only
+    // the device maps): while false, every host path that reads them refreshes them first (refresh_maps).  mpig_clear sets it
+    // again, unless a reorder has ever been captured: that graph may be replayed after the clear.
+    bool h_map_exact = true;
+    bool reorder_captured = false;
     // the map the kernels get: null while every request owns its slot (C = B, bindings fixed), so that path addresses b itself
     const int32_t *slot_map() const { return C < cfg.batch_size ? slot_of : nullptr; }
     // shared dense mode (R = dense_tail_rows > 0): the prompt rows of the dense layers live once per slot, each request's later
-    // rows in its own tail of R rows.  dense_base[b] = the first row of request b that lies in its tail (set by mpig_dense_fill and
-    // mpig_fork_request, zeroed by mpig_clear); allocated at create time and never moved, h_dense_base mirrors it exactly.
+    // rows in its own tail of R rows.  dense_base[b] = the first row of request b that lies in its tail (set by mpig_dense_fill,
+    // mpig_fork_request and the reorder kernel, zeroed by mpig_clear); allocated at create time and never moved, h_dense_base
+    // mirrors it (exactly while h_map_exact).  The decode kernels read it only after griddepcontrol.wait.
     int dense_tail_rows = 0;
     int32_t *dense_base = nullptr;        // [B], shared dense mode only
     std::vector<int> h_dense_base;        // [B]
     // the base map the kernels get: null in the default layout
     const int32_t *dense_base_map() const { return dense_tail_rows > 0 ? dense_base : nullptr; }
-    // the dense capacity of request b: max_length, or min(max_length, base + R) in shared dense mode
+    // the dense capacity of request b: max_length, or min(max_length, base + R) in shared dense mode.  Read only by the plans'
+    // host-mirror checks, which run only while h_len_exact; a captured reorder clears h_len_exact with h_map_exact and only
+    // mpig_clear sets both again, so h_dense_base is exact wherever this is read.
     int dense_cap(int b) const {
         return dense_tail_rows > 0 ? std::min(cfg.max_length, h_dense_base[b] + dense_tail_rows) : cfg.max_length;
     }
@@ -221,7 +236,7 @@ struct mpig_ctx {
     float *out_f32 = nullptr;                // [H][d]
     // capacity bookkeeping (the window / the dense cache saturate silently on the device): a device flag raised by
     // plan_kernel plus a host mirror that is exact as long as plan() is not replayed from a CUDA graph
-    int32_t *err_flag = nullptr;             // bit 0: sparse window full, bit 1: a dense cache reached its capacity
+    int32_t *err_flag = nullptr;             // bits: see mpig_error_flags (0 window full, 1 dense full, 2 rewind, 3 tree, 4 reorder)
     std::vector<int> h_win_len, h_dense_len; // [B]
     bool h_len_exact = true;
     void *host_stage_dev = nullptr;          // device-side address of the mapped pinned block host_stage
@@ -240,9 +255,10 @@ struct mpig_ctx {
     // moves: int32 [B][T] ancestor masks (bit j of node t = node j is t or one of its ancestors) | int32 [B][T] parents | int32
     // [B][2] step bases (window, dense length before the plan, after saturation).  Every plan writes it (chains for plan_tokens).
     int32_t *step_buf = nullptr;
-    // device table of the layers that own rows (sparse windows and dense KV), for the one-launch accept kernel
+    // device table of the layers that own rows (sparse windows and dense KV), for the one-launch accept and reorder kernels
     void *accept_layers = nullptr;
     int n_accept_layers = 0;
+    int reorder_cols = 0;                    // CTA columns of the reorder kernel's copy grid (the last entry's x0 + its columns)
 };
 
 namespace mpig {
@@ -475,6 +491,9 @@ int check_layer(mpig_ctx *ctx, int layer, bool need_sparse, const char *who);
 // the device lengths of requests [b0, b0 + n) into wl (win_len) and dl (dense_len), either may be null; synchronises s.  The
 // device lengths are the truth: replays of a captured plan advance only them (step.cu).
 int read_lengths(const mpig_ctx *ctx, int b0, int n, int32_t *wl, int32_t *dl, cudaStream_t s);
+// h_slot_of / h_dense_base from the device maps when a captured reorder may have changed them (!h_map_exact; synchronises s),
+// a no-op otherwise.  Every host path that reads either mirror calls it first (context.cu).
+int refresh_maps(mpig_ctx *ctx, cudaStream_t s);
 inline cudaStream_t as_stream(void *s) { return (cudaStream_t)s; }
 
 }  // namespace mpig

@@ -235,13 +235,20 @@ int mpig_create(const mpig_config *cfg, mpig_ctx **out) {
     TRY(dev_alloc(ctx, &ctx->mve, 2 * H * sizeof(float)));
     TRY(dev_alloc(ctx, &ctx->err_flag, 4 * sizeof(int32_t)));
     TRY(dev_alloc(ctx, &ctx->step_buf, (size_t)cfg->batch_size * (2 * TREE_MAX + 2) * sizeof(int32_t), true));
-    {   // layer table of mpig_accept: every sparse window and every dense KV cache the context owns
+    TRY(dev_alloc(ctx, &ctx->slot_stage, (size_t)cfg->batch_size * sizeof(int32_t)));
+    {   // layer table of mpig_accept and mpig_reorder_requests: every sparse window and every dense KV cache the context owns
         std::vector<AcceptLayer> tab;
         for (const LayerStore &ls : ctx->layers) {
-            if (ls.sparse && ctx->Wcap > 0) tab.push_back({ls.win, ctx->Wcap, 0});
-            if (ls.dense && ls.dense_tail) tab.push_back({ls.dense_tail, ctx->dense_tail_rows, 1});
-            else if (ls.dense && ls.dense_kv) tab.push_back({ls.dense_kv, cfg->max_length, 1});
+            if (ls.sparse && ctx->Wcap > 0) tab.push_back({ls.win, ctx->Wcap, 0, ls.avg_k, 0});
+            if (ls.dense && ls.dense_tail) tab.push_back({ls.dense_tail, ctx->dense_tail_rows, 1, nullptr, 0});
+            else if (ls.dense && ls.dense_kv) tab.push_back({ls.dense_kv, cfg->max_length, 1, nullptr, 0});
         }
+        int x0 = 0;
+        for (AcceptLayer &e : tab) {
+            e.x0 = x0;
+            x0 += cfg->num_key_value_heads * ((e.cap + REORDER_ROWS - 1) / REORDER_ROWS);
+        }
+        ctx->reorder_cols = x0;
         ctx->n_accept_layers = (int)tab.size();
         if (!tab.empty()) {
             TRY(dev_alloc(ctx, (uint8_t **)&ctx->accept_layers, tab.size() * sizeof(AcceptLayer)));
@@ -274,6 +281,24 @@ int mpig_create(const mpig_config *cfg, mpig_ctx **out) {
     return MPIG_OK;
 }
 
+}  // extern "C"
+
+int mpig::refresh_maps(mpig_ctx *ctx, cudaStream_t s) {
+    if (ctx->h_map_exact) return MPIG_OK;
+    const int B = ctx->cfg.batch_size;
+    std::vector<int32_t> so(B), db(B, 0);
+    MPIG_CUDA(cudaMemcpyAsync(so.data(), ctx->slot_of, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    if (ctx->dense_base) MPIG_CUDA(cudaMemcpyAsync(db.data(), ctx->dense_base, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    MPIG_CUDA(cudaStreamSynchronize(s));
+    for (int b = 0; b < B; ++b) {
+        ctx->h_slot_of[b] = so[b];
+        ctx->h_dense_base[b] = db[b];
+    }
+    return MPIG_OK;   // h_map_exact stays false: a later replay of the captured reorder changes the device maps again
+}
+
+extern "C" {
+
 void mpig_destroy(mpig_ctx *ctx) {
     if (!ctx) return;
     {
@@ -293,6 +318,7 @@ void mpig_destroy(mpig_ctx *ctx) {
     cudaFree(ctx->win_len);
     cudaFree(ctx->dense_len);
     cudaFree(ctx->slot_of);
+    cudaFree(ctx->slot_stage);
     cudaFree(ctx->dense_base);
     cudaFree(ctx->vis);
     cudaFree(ctx->private_lo);
@@ -358,6 +384,7 @@ int mpig_clear(mpig_ctx *ctx, void *stream) {
     for (int b = 0; b < ctx->cfg.batch_size; ++b) ctx->h_slot_of[b] = b % ctx->C;
     MPIG_CUDA(cudaMemcpyAsync(ctx->slot_of, ctx->h_slot_of.data(), ctx->cfg.batch_size * sizeof(int32_t), cudaMemcpyHostToDevice, s));
     ctx->h_len_exact = true;
+    ctx->h_map_exact = !ctx->reorder_captured;
     ctx->last_tokens = 1;
     ctx->pending.end(true);   // no plan to decode, rewind or accept since the clear
     return MPIG_OK;
@@ -553,6 +580,8 @@ int mpig_fork_request(mpig_ctx *ctx, int src, int dst, void *stream) {
     if (rc) return rc;
     MPIG_REQUIRE(src != dst, MPIG_EINVAL, "mpig_fork_request: src == dst (%d)", src);
     cudaStream_t s = as_stream(stream);
+    rc = refresh_maps(ctx, s);
+    if (rc) return rc;
     int32_t len[2] = {0, 0};
     rc = read_lengths(ctx, src, 1, &len[0], &len[1], s);
     if (rc) return rc;
@@ -600,6 +629,8 @@ int mpig_bind_request(mpig_ctx *ctx, int request, int slot, void *stream) {
     int rc = binding_checks(ctx, request, "mpig_bind_request");
     if (rc) return rc;
     MPIG_REQUIRE(slot >= 0 && slot < ctx->C, MPIG_EINVAL, "mpig_bind_request: slot %d out of range [0, %d)", slot, ctx->C);
+    rc = refresh_maps(ctx, as_stream(stream));   // the whole host map is uploaded below
+    if (rc) return rc;
     ctx->h_slot_of[request] = slot;
     rc = launch_vis_rebind(ctx, -1, request, as_stream(stream));   // shared spill mode: no private key until it spills again
     if (rc) return rc;

@@ -151,6 +151,8 @@ int mpig_dense_fill(mpig_ctx *ctx, int layer, int request, const void *k_bf16, c
     const int Hkv = ctx->cfg.num_key_value_heads, M = ctx->cfg.max_length;
     // shared dense mode: the rows go to the slot the request is bound to (as the sparse fills), and they become its base
     const bool shared = ctx->dense_tail_rows > 0;
+    rc = refresh_maps(ctx, as_stream(stream));
+    if (rc) return rc;
     const size_t owner = shared ? (size_t)ctx->h_slot_of[request] : (size_t)request;
     uint4 *rec = reinterpret_cast<uint4 *>(ls.dense_kv + owner * Hkv * M * ctx->rec_bytes);
     if (seq_len > 0) {

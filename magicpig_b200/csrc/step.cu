@@ -1,5 +1,6 @@
 // step.cu -- the lifecycle of a decode step: plan (lengths advance by T, the step's node records), then at most one rewind or
-// accept per plan, and the host mirror of the lengths that the eager checks of the plans read.
+// accept per plan, and the host mirror of the lengths that the eager checks of the plans read; and the device-side reorder of
+// requests that a beam-search step ends with (mpig_reorder_requests).
 //
 // Replaces attnserver.py:196-198 (plan(): kv_last_page_len += 1) and, beyond the reference, the verification steps of
 // speculative decoding: chains of T tokens (mpig_plan_tokens / mpig_rewind) and token trees (mpig_plan_tree / mpig_accept).
@@ -133,6 +134,98 @@ __global__ void __launch_bounds__(256) accept_path_kernel(const AcceptLayer *lay
     }
 }
 
+// mpig_reorder_requests: request b continues request s = src_of[b]'s sequence.  The map's rule -- 0 <= src_of[b] < B and
+// src_of[src_of[b]] == src_of[b] -- is checked in full by every CTA before it writes anything; a bad map leaves every request
+// untouched and raises bit 4.  The rule means no request the call reads from is written, so the copy runs in place, in one pass.
+//   Rows b < B: one CTA per (table entry, kv-head, chunk of REORDER_ROWS rows) in column x (entry e owns columns
+//   [x0_e, x0_e + Hkv * ceil(cap_e / REORDER_ROWS))); CTAs of a request that stays (s == b), or past s's rows, exit at once.  The
+//   rows are s's window rows [0, win_len[s]), dense rows [0, dense_len[s]) or, with a base map (shared dense mode), tail rows
+//   [0, dense_len[s] - dense_base[s]), each capped at the entry's capacity; chunk 0 of a sparse entry also copies s's avg_k.
+//   The CTA of column 0 sets b's lengths and dense base to s's (one thread per request, as the accept kernel's leader), and
+//   writes slot_of[s] into slot_stage[b] for every b: the host copies the staging into slot_of after the kernel, so that no
+//   kernel writes the slot map (mpig_ctx::slot_of).
+//   Row B (shared spill mode): every vis word is rewritten in a register by the one thread that owns it: bit b becomes bit
+//   src_of[b] of the word's old value for every moved b (vis_rebind_kernel(src_of[b], b) for all of them at once).
+// apply = 0: only the check (an eager call that refuses).
+__global__ void __launch_bounds__(256) reorder_requests_kernel(const AcceptLayer *layers, int n_layers, const int32_t *src_of,
+                                                               int32_t *win_len, int32_t *dense_len, int32_t *dense_base,
+                                                               const int32_t *slot_of, int32_t *slot_stage, uint32_t *vis,
+                                                               size_t vis_words, int32_t *err_flag, int B, int Hkv, int rec16,
+                                                               int d16, int apply) {
+    constexpr int T = 256, UN = REORDER_ROWS * 32 / T;
+    const int tid = threadIdx.x, x = blockIdx.x, b = blockIdx.y;
+    bool ok = true;
+    for (int i = tid; i < B; i += T) {
+        const int s = src_of[i];
+        ok &= (s >= 0 && s < B) && src_of[s] == s;
+    }
+    ok = __syncthreads_and(ok);
+    if (!ok) {
+        if (x == 0 && b == 0 && tid == 0) atomicOr(err_flag, 16);
+        if (x == 0 && b < B && tid == 0) slot_stage[b] = slot_of[b];   // the copy after the kernel leaves the map as it was
+        return;
+    }
+    if (!apply) return;
+    if (b == B) {   // the visibility map (B <= 32 in shared spill mode)
+        __shared__ int s_src[32];
+        if (tid < B) s_src[tid] = src_of[tid];
+        __syncthreads();
+        uint32_t moved = 0;
+        for (int r = 0; r < B; ++r) moved |= (s_src[r] != r ? 1u : 0u) << r;
+        for (size_t i = (size_t)x * T + tid; i < vis_words; i += (size_t)gridDim.x * T) {
+            const uint32_t v = vis[i];
+            uint32_t w = v & ~moved;
+            for (uint32_t m = moved; m; m &= m - 1) {
+                const int r = __ffs(m) - 1;
+                w |= ((v >> s_src[r]) & 1u) << r;
+            }
+            vis[i] = w;
+        }
+        return;
+    }
+    const int s = src_of[b];
+    if (x == 0 && tid == 0) {
+        slot_stage[b] = slot_of[s];
+        if (s != b) {
+            win_len[b] = win_len[s];
+            dense_len[b] = dense_len[s];
+            if (dense_base) dense_base[b] = dense_base[s];
+        }
+    }
+    if (s == b || n_layers == 0) return;
+    __shared__ int s_entry;
+    for (int e = tid; e < n_layers; e += T)
+        if (layers[e].x0 <= x && (e + 1 == n_layers || layers[e + 1].x0 > x)) s_entry = e;
+    __syncthreads();
+    const AcceptLayer ly = layers[s_entry];
+    const int nch = (ly.cap + REORDER_ROWS - 1) / REORDER_ROWS;
+    const int head = (x - ly.x0) / nch, ch = (x - ly.x0) % nch;
+    if (ly.avg_k && ch == 0 && tid < d16) {
+        const uint4 *a = reinterpret_cast<const uint4 *>(ly.avg_k);
+        reinterpret_cast<uint4 *>(ly.avg_k)[((size_t)b * Hkv + head) * d16 + tid] = a[((size_t)s * Hkv + head) * d16 + tid];
+    }
+    int n = ly.dense ? dense_len[s] - (dense_base ? dense_base[s] : 0) : win_len[s];
+    n = min(max(n, 0), ly.cap);
+    const int r0 = ch * REORDER_ROWS;
+    if (r0 >= n) return;
+    const int total = min(REORDER_ROWS, n - r0) * rec16;   // 16-byte chunks of the CTA's rows, contiguous in both requests
+    const uint4 *src = reinterpret_cast<const uint4 *>(ly.rows) + (((size_t)s * Hkv + head) * ly.cap + r0) * rec16;
+    uint4 *dst = reinterpret_cast<uint4 *>(ly.rows) + (((size_t)b * Hkv + head) * ly.cap + r0) * rec16;
+    for (int c0 = 0; c0 < total; c0 += T * UN) {
+        uint4 v[UN];
+#pragma unroll
+        for (int u = 0; u < UN; ++u) {
+            const int i = c0 + u * T + tid;
+            if (i < total) v[u] = src[i];
+        }
+#pragma unroll
+        for (int u = 0; u < UN; ++u) {
+            const int i = c0 + u * T + tid;
+            if (i < total) dst[i] = v[u];
+        }
+    }
+}
+
 int read_lengths(const mpig_ctx *ctx, int b0, int n, int32_t *wl, int32_t *dl, cudaStream_t s) {
     if (wl) MPIG_CUDA(cudaMemcpyAsync(wl, ctx->win_len + b0, n * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
     if (dl) MPIG_CUDA(cudaMemcpyAsync(dl, ctx->dense_len + b0, n * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
@@ -225,6 +318,30 @@ static int checked_launch(cudaStream_t s, bool *eager, bool *refused, HostCheck 
     }
     *refused = !ok;
     return launch(ok ? 1 : 0);
+}
+
+// apply = 1: the reorder kernel, then the new slot map from its staging into slot_of (a copy-engine call, a memcpy node under
+// capture); apply = 0: one CTA that only raises the flag bit
+static int launch_reorder(mpig_ctx *ctx, const int32_t *src_of, int apply, cudaStream_t s) {
+    const int B = ctx->cfg.batch_size, Hkv = ctx->cfg.num_key_value_heads;
+    const size_t words = ctx->shared_spill ? (size_t)ctx->C * ctx->cfg.max_length : 0;
+    const dim3 grid(apply ? std::max(ctx->reorder_cols, 1) : 1, apply ? B + (words ? 1 : 0) : 1);
+    reorder_requests_kernel<<<grid, 256, 0, s>>>((const AcceptLayer *)ctx->accept_layers, ctx->n_accept_layers, src_of, ctx->win_len,
+                                                 ctx->dense_len, ctx->dense_base_map() ? ctx->dense_base : nullptr, ctx->slot_of,
+                                                 ctx->slot_stage, ctx->vis, words, ctx->err_flag, B, Hkv, ctx->rec_bytes / 16,
+                                                 ctx->cfg.head_dim / 8, apply);
+    MPIG_LAUNCH_CHECK(ctx);
+    if (apply) MPIG_CUDA(cudaMemcpyAsync(ctx->slot_of, ctx->slot_stage, B * sizeof(int32_t), cudaMemcpyDeviceToDevice, s));
+    return MPIG_OK;
+}
+
+// the host restatement of the reorder kernel's check
+static bool reorder_map_ok(const int32_t *src_of, int B) {
+    for (int b = 0; b < B; ++b) {
+        const int s = src_of[b];
+        if (s < 0 || s >= B || src_of[s] != s) return false;
+    }
+    return true;
 }
 
 // after an applied rewind / accept: the step ends, and the host mirror follows the device lengths (an eager call: they are the
@@ -351,6 +468,44 @@ int mpig_accept(mpig_ctx *ctx, const int32_t *nodes, const int32_t *count, void 
                  "mpig_accept: a path that is not a root path of the pending step (count outside [0, %d], nodes[0] != 0 or "
                  "parents[nodes[i]] != nodes[i-1]); nothing was changed (error flag bit 3)", T);
     return end_step(ctx, eager, s);
+}
+
+int mpig_reorder_requests(mpig_ctx *ctx, const int32_t *src_of, void *stream) {
+    mpig::DeviceGuard _dg(ctx);
+    MPIG_REQUIRE(ctx && src_of, MPIG_EINVAL, "mpig_reorder_requests: null argument");
+    MPIG_REQUIRE(ctx->C < ctx->cfg.batch_size, MPIG_ESTATE,
+                 "mpig_reorder_requests: every request owns its context slot (num_contexts = batch_size); create the context with "
+                 "fewer slots to share one");
+    const int B = ctx->cfg.batch_size;
+    cudaStream_t s = as_stream(stream);
+    bool eager = true, refused = false;
+    std::vector<int32_t> sh(B);
+    int rc = checked_launch(
+        s, &eager, &refused,
+        [&](bool &ok) -> int {
+            MPIG_CUDA(cudaMemcpyAsync(sh.data(), src_of, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+            MPIG_CUDA(cudaStreamSynchronize(s));
+            ok = reorder_map_ok(sh.data(), B);
+            return MPIG_OK;
+        },
+        [&](int apply) { return launch_reorder(ctx, src_of, apply, s); });
+    if (rc) return rc;
+    MPIG_REQUIRE(!refused, MPIG_EINVAL,
+                 "mpig_reorder_requests: a map whose sources are not all fixed points (src_of[b] outside [0, %d) or "
+                 "src_of[src_of[b]] != src_of[b]); nothing was changed (error flag bit 4)", B);
+    if (!eager) {   // replays change the device maps only
+        ctx->h_map_exact = false;
+        ctx->reorder_captured = true;
+    }
+    rc = end_step(ctx, eager, s);   // the lengths' mirror, as after a rewind; the bases of the pending step are stale
+    if (rc || !eager) return rc;
+    if (!ctx->h_map_exact) return refresh_maps(ctx, s);
+    std::vector<int> so = ctx->h_slot_of, db = ctx->h_dense_base;
+    for (int b = 0; b < B; ++b) {
+        ctx->h_slot_of[b] = so[sh[b]];
+        ctx->h_dense_base[b] = db[sh[b]];
+    }
+    return MPIG_OK;
 }
 
 }  // extern "C"

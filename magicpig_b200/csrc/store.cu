@@ -183,6 +183,8 @@ int mpig_attn_fill(mpig_ctx *ctx, int layer, int request, const void *k_bf16, co
     MPIG_REQUIRE(n == 0 || (k_bf16 && v_bf16 && kn), MPIG_EINVAL, "mpig_attn_fill: null input");
     const LayerStore &ls = ctx->layers[layer];
     const int Hkv = ctx->cfg.num_key_value_heads, M = ctx->cfg.max_length;
+    rc = refresh_maps(ctx, as_stream(stream));
+    if (rc) return rc;
     const int slot = ctx->h_slot_of[request];   // every request bound to this slot sees the new context
     rc = reset_private(ctx, layer, request, n, as_stream(stream));
     if (rc) return rc;
@@ -247,6 +249,8 @@ int mpig_spill_window(mpig_ctx *ctx, int keep, int32_t *spilled_out, void *strea
     cudaStream_t s = as_stream(stream);
     std::vector<int32_t> wl(B);
     int rc = read_lengths(ctx, 0, B, wl.data(), nullptr, s);
+    if (rc) return rc;
+    rc = refresh_maps(ctx, s);   // each request's keys go to the slot it is bound to now
     if (rc) return rc;
     // meta = g[B] | pre[B] (staging block of each request) | n_old[num_layers][B]; shared spill mode appends blk[3][B] (rows of
     // the request's staging block, the request's offset in it, its first private offset) | g[C] | pre[C] | n_old[num_layers][C]

@@ -607,6 +607,8 @@ int mpig_lsh_fill(mpig_ctx *ctx, int layer, int request, const int16_t *sorted_c
     MPIG_REQUIRE(n >= 0 && n <= ctx->cfg.max_length, MPIG_EINVAL, "mpig_lsh_fill: n=%d exceeds max_length=%d", n,
                  ctx->cfg.max_length);
     MPIG_REQUIRE(n == 0 || (sorted_codes && sorted_indices), MPIG_EINVAL, "mpig_lsh_fill: null input");
+    rc = refresh_maps(ctx, as_stream(stream));   // the tables of the slot the request is bound to now
+    if (rc) return rc;
     rc = reset_private(ctx, layer, request, n, as_stream(stream));
     if (rc) return rc;
     return launch_build(ctx, layer, request, sorted_codes, sorted_indices, n, as_stream(stream));
@@ -620,6 +622,8 @@ int mpig_lsh_build(mpig_ctx *ctx, int layer, int request, const int16_t *key_cod
     MPIG_REQUIRE(n >= 0 && n <= ctx->cfg.max_length, MPIG_EINVAL, "mpig_lsh_build: n=%d exceeds max_length=%d", n,
                  ctx->cfg.max_length);
     MPIG_REQUIRE(n == 0 || key_codes, MPIG_EINVAL, "mpig_lsh_build: null input");
+    rc = refresh_maps(ctx, as_stream(stream));   // the tables of the slot the request is bound to now
+    if (rc) return rc;
     rc = reset_private(ctx, layer, request, n, as_stream(stream));
     if (rc) return rc;
     return launch_build(ctx, layer, request, key_codes, nullptr, n, as_stream(stream));

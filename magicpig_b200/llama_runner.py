@@ -24,7 +24,7 @@ import torch.nn.functional as F
 
 from . import _native as N
 from . import tp
-from .attnserver import LSHSparseAttnServer
+from .attnserver import LSHSparseAttnServer, beam_sources
 
 
 @dataclass
@@ -199,6 +199,36 @@ class LlamaDecodeRunner:
         position."""
         self.server.fork(src, dst)
         self.pos[dst] = self.pos[src]
+
+    def reorder(self, src_of: torch.Tensor):
+        """Request b continues request src_of[b]: the server's reorder (device int32 (B,), sources are fixed points) and the
+        sources' positions.  Capturable."""
+        assert self.tp_world == 1, "reorder is built for a single GPU"
+        self.server.reorder(src_of)
+        self.pos.copy_(self.pos.index_select(0, src_of.long()))
+
+    def beam_select(self, scores: torch.Tensor):
+        """The choice of one beam-search step from self.logits (after step()): scores (B,) fp32 are the beams' log-probabilities.
+        Returns (parents, tokens, new_scores), each (B,): new beam i extends beam parents[i] by tokens[i], with log-probability
+        new_scores[i] = scores[parents[i]] + log_softmax(logits[parents[i]])[tokens[i]], the B best of the B * vocab candidates."""
+        V = self.logits.shape[1]
+        cand = torch.log_softmax(self.logits, dim=-1) + scores[:, None]
+        new_scores, flat = cand.reshape(-1).topk(self.B)
+        return flat // V, flat % V, new_scores
+
+    def beam_step(self, scores: torch.Tensor):
+        """One beam-search step after step(), all on the device (capturable; capture(beam_scores=scores) puts step() and this into
+        one graph): beam_select, then the new beams move into their requests (beam_sources + reorder), self.ids[request_of[i]] =
+        tokens[i] and scores[request_of[i]] = new_scores[i] in place.  From one prompt held by every request, start with scores
+        [0, -inf, ...]: the B beams then start from distinct tokens of beam 0.  Returns (parents, tokens, request_of)."""
+        assert self.tp_world == 1, "beam search is built for a single GPU"
+        parents, tokens, new_scores = self.beam_select(scores)
+        src_of, request_of = beam_sources(parents)
+        self.reorder(src_of)
+        req = request_of.long()
+        self.ids[req, 0] = tokens
+        scores[req] = new_scores
+        return parents, tokens, request_of
 
     # ------------------------------------------------------------------------------------------
     def _rope(self, x: torch.Tensor, pos: torch.Tensor) -> torch.Tensor:
@@ -421,18 +451,25 @@ class LlamaDecodeRunner:
         x1, x2 = x[..., : self.d // 2], x[..., self.d // 2:]
         return x * cos + torch.cat([-x2, x1], dim=-1) * sin
 
-    def capture(self, warm: int = 3):
-        """Capture step() into a CUDA graph (launch-bound otherwise: ~600 small kernels per token)."""
+    def capture(self, warm: int = 3, beam_scores: torch.Tensor | None = None):
+        """Capture step() into a CUDA graph (launch-bound otherwise: ~600 small kernels per token).  With beam_scores (a device
+        fp32 (B,) tensor that stays in place) the graph is step() followed by beam_step(beam_scores); the warm-up steps run it too,
+        so reset the beams' state (clear and prefill) before the first replay."""
+        def body():
+            self.step()
+            if beam_scores is not None:
+                self.beam_step(beam_scores)
+
         s = torch.cuda.Stream(device=self.device)
         s.wait_stream(torch.cuda.current_stream(self.device))
         with torch.cuda.stream(s):
             for _ in range(warm):
-                self.step()
+                body()
         torch.cuda.current_stream(self.device).wait_stream(s)
         torch.cuda.synchronize(self.device)
         self.graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(self.graph):
-            self.step()
+            body()
         return warm + 1  # decode steps consumed (window slots used)
 
     def replay(self):

@@ -144,6 +144,16 @@ class Context:
         N.check(self.lib.mpig_bind_request(self._h, int(request), int(slot), _stream()), "mpig_bind_request")
         self.pending_tokens = 0
 
+    def reorder(self, src_of: torch.Tensor):
+        """Request b continues request src_of[b]'s sequence: fork(src_of[b], b) for every b with src_of[b] != b, in one kernel
+        on the device.  src_of: int32 (B,) on the device; every source must keep its own sequence (src_of[src_of[b]] ==
+        src_of[b]).  Capturable: a replay reorders by whatever src_of holds then.  Eager calls synchronise and raise on a map that
+        breaks the rule without changing anything; under capture such a map changes nothing and raises error_flags() bit 4.
+        Ends the pending step like fork()."""
+        self._chk(src_of, torch.int32, (self.B,), "src_of")
+        N.check(self.lib.mpig_reorder_requests(self._h, _ptr(src_of), _stream()), "mpig_reorder_requests")
+        self.pending_tokens = 0
+
     def get_info(self, key: str) -> int:
         v = ctypes.c_int64(0)
         N.check(self.lib.mpig_get_info(self._h, key.encode(), ctypes.byref(v)), "mpig_get_info")
@@ -151,7 +161,7 @@ class Context:
 
     def error_flags(self) -> int:
         """bit 0: a sparse window is full (generation_buffer exhausted), bit 1: a dense cache reached its capacity, bit 2: a rewind drop was out
-        of range, bit 3: a malformed tree or accepted path.  Synchronises."""
+        of range, bit 3: a malformed tree or accepted path, bit 4: a reorder map that breaks its rule.  Synchronises."""
         f = ctypes.c_int32(0)
         N.check(self.lib.mpig_error_flags(self._h, ctypes.byref(f), _stream()), "mpig_error_flags")
         return int(f.value)

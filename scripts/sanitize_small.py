@@ -6,7 +6,9 @@ Sizes are tiny (the tools slow kernels down 10-100x) but cover: the stand-alone 
 shapes, two key segments) / gather-attention kernels, the fused single-launch decode (cluster of 8, cluster of 4 over two
 segments, one CTA per head with codes from the SimHash kernel, several selection passes), the three-launch decode, the dense
 kernel, the tensor-core key hash, the table build, the window spill, verification steps of T tokens, token trees with an accept,
-requests sharing one context slot, and shared spill (several requests of one slot spill, a fork, single-token and T-token decodes).  Results are also checked against each other so a tool run doubles as a test.
+requests sharing one context slot, shared spill (several requests of one slot spill, a fork, single-token and T-token decodes), and
+the device-side reorder of requests (`reorder`: the in-place copy between requests, eager, refused and captured).  Results are also
+checked against each other so a tool run doubles as a test.
 """
 import os
 import sys
@@ -422,8 +424,84 @@ def shared_spill_case(B, Hq, Hkv, n, K, L, T):
     print(f"shared spill B={B} Hq={Hq} Hkv={Hkv} n={n} T={T}: ok")
 
 
+def reorder_case(B, Hq, Hkv, n, K, L, R):
+    """mpig_reorder_requests: the in-place copy of windows, avg_k and dense tails between requests of one slot (shared dense mode,
+    shared spill: the visibility rewrite of the same launch) and the slot-map staging, against a twin that forks request by request;
+    then a bad map (nothing changes), and a reorder captured into a graph and replayed."""
+    M = n + 400
+    g = torch.Generator(device=dev).manual_seed(21)
+    hf = torch.randn((d, K * L), generator=g, device=dev).bfloat16()
+    key = torch.randn((Hkv, n, d), generator=g, device=dev).bfloat16()
+    val = torch.randn((Hkv, n, d), generator=g, device=dev).bfloat16()
+    dk, dv = (torch.randn((300, Hkv, d), generator=g, device=dev).bfloat16() for _ in range(2))
+    ctxs = []
+    for _ in range(2):
+        ctx = Context(K, L, 2, Hq, Hkv, d, B, M, generation_buffer=24, dense_layers=[0], alloc_dense_kv=True, device=dev,
+                      num_contexts=2, dense_tail_rows=R, shared_spill=True)
+        ctx.set_option("out_f32", 1)
+        ctx.set_hash_func(hf)
+        g2 = torch.Generator(device=dev).manual_seed(22)
+        for c in range(2):
+            ctx.attn_fill(1, c, key, val, key.norm(p=2, dim=-1).float())
+            ctx.lsh_build(1, c, ctx.hash_keys(key))
+        for b in range(B):
+            ctx.window_fill(1, b, torch.zeros((Hkv, d), dtype=torch.bfloat16, device=dev),
+                            torch.randn((Hkv, 68, d), generator=g2, device=dev).bfloat16(),
+                            torch.randn((Hkv, 68, d), generator=g2, device=dev).bfloat16())
+            ctx.dense_fill(0, b, dk, dv, 300)
+        ctxs.append(ctx)
+    sh, tw = ctxs
+
+    def step():
+        q = torch.randn((B * Hq, d), generator=g, device=dev).bfloat16()
+        kv = torch.randn((B * Hkv, d), generator=g, device=dev).bfloat16()
+        outs = []
+        for c in ctxs:
+            c.plan()
+            c.dense_decode(0, q, kv, kv)
+            outs.append(c.last_out_f32())
+            c.decode(1, q, kv, kv)
+            outs.append(c.last_out_f32())
+        assert torch.equal(outs[0], outs[2]) and torch.equal(outs[1], outs[3]), "reorder != forks"
+
+    def forks(m):
+        for b, s_ in enumerate(m):
+            if s_ != b:
+                tw.fork(s_, b)
+
+    for _ in range(3):
+        step()
+    assert sh.spill_window(64).tolist() == tw.spill_window(64).tolist()
+    m = [0, 0, 2, 0][:B]
+    sh.reorder(torch.tensor(m, dtype=torch.int32, device=dev))
+    forks(m)
+    step()
+    try:
+        sh.reorder(torch.tensor([1, 2, 2, 3][:B], dtype=torch.int32, device=dev))
+        raise AssertionError("a map whose source is moved was accepted")
+    except Exception as e:
+        assert "code -1" in str(e), e
+    step()
+    src = torch.tensor([2, 1, 2, 2][:B], dtype=torch.int32, device=dev)
+    s = torch.cuda.Stream()
+    s.wait_stream(torch.cuda.current_stream())
+    graph = torch.cuda.CUDAGraph()
+    with torch.cuda.stream(s):
+        with torch.cuda.graph(graph, stream=s):
+            sh.reorder(src)
+    torch.cuda.synchronize()
+    graph.replay()
+    forks(src.tolist())
+    step()
+    assert sh.error_flags() == 16 and tw.error_flags() == 0
+    torch.cuda.synchronize()
+    print(f"reorder B={B} Hq={Hq} Hkv={Hkv} n={n} R={R}: ok")
+
+
 if __name__ == "__main__":
-    which = sys.argv[1:] or ["stages", "dense", "decode", "hostpeer", "spill", "tokens", "tree", "shared", "shared_spill"]
+    which = sys.argv[1:] or ["stages", "dense", "decode", "hostpeer", "spill", "tokens", "tree", "shared", "shared_spill", "reorder"]
+    if "reorder" in which:
+        reorder_case(4, 4, 2, 700, 6, 24, 40)
     if "shared_spill" in which:
         shared_spill_case(3, 4, 2, 700, 6, 24, 3)
     if "shared" in which:
