@@ -48,6 +48,15 @@ LLAMA31_8B = LlamaShape()
 LLAMA31_70B = LlamaShape("Llama-3.1-70B-Instruct", 80, 8192, 28672, 64, 8, 128256, 500000.0, 1e-5)
 
 
+def rope_tables(theta: float, d: int, rows: int, device) -> tuple[torch.Tensor, torch.Tensor]:
+    """The (rows, d) bf16 cos / sin tables of rotate-half RoPE for positions 0 .. rows - 1 (llama.py:111-124)."""
+    inv_freq = 1.0 / (theta ** (torch.arange(0, d, 2, device=device, dtype=torch.float32) / d))
+    t = torch.arange(rows, device=device, dtype=torch.float32)
+    freqs = torch.outer(t, inv_freq)
+    emb = torch.cat([freqs, freqs], dim=-1)
+    return emb.cos().to(torch.bfloat16), emb.sin().to(torch.bfloat16)
+
+
 class LlamaDecodeRunner:
     # The CUDA-core GEMV issues 24*rows + 16 instructions per KB of weights per warp; at the HBM rate an SM has ~23 clocks per
     # KB (4 issue slots each), so it streams at the memory rate for rows <= 2 and is ALU-bound beyond (measured at rows = 8:
@@ -138,12 +147,7 @@ class LlamaDecodeRunner:
         self.embed = w(shape.vocab_size, hs)
         self.lm_head = w(shape.vocab_size, hs)
         self.norm = torch.ones(hs, device=self.device, dtype=torch.bfloat16)
-        # RoPE tables (llama.py:111-124)
-        inv_freq = 1.0 / (shape.rope_theta ** (torch.arange(0, d, 2, device=self.device, dtype=torch.float32) / d))
-        t = torch.arange(max_length + 8, device=self.device, dtype=torch.float32)
-        freqs = torch.outer(t, inv_freq)
-        emb = torch.cat([freqs, freqs], dim=-1)
-        self.cos, self.sin = emb.cos().to(torch.bfloat16), emb.sin().to(torch.bfloat16)
+        self.cos, self.sin = rope_tables(shape.rope_theta, d, max_length + 8, self.device)
         # static step buffers (CUDA-graph friendly)
         self.ids = torch.zeros((batch_size, 1), dtype=torch.long, device=self.device)
         self.pos = torch.zeros((batch_size,), dtype=torch.long, device=self.device)
