@@ -259,14 +259,15 @@ int mpig_plan(mpig_ctx *ctx, void *stream);
  * P + g tokens would have, centred with the prefill's mean key.  spilled_out int32 [B] (host, may be NULL) receives g_b.
  * Reads the device window lengths (synchronises `stream`), so it is correct after eager plan() calls and after replays of a
  * captured step alike.  Not capturable.  A decode step captured before a spill stays valid after it.  Dense layers are
- * untouched.  The spilled keys go into the store and tables of the request's slot, so a request with g_b > 0 must be alone on its
- * slot among requests with a non-empty window: a request that shares its context generates at most generation_buffer tokens --
- * unless the context is in shared spill mode (reserved[3]), where the requests of a slot spill into it in request order, n_old is
- * the slot's count plus the rows of the slot's earlier requests, and each spilled key is private to its request.
- * MPIG_EINVAL: keep < 0 or sink + keep >= window capacity; MPIG_ESTATE: n_old + g_b (shared spill: the slot's count plus all its
- * requests' rows) > max_length for some sparse layer, a spilling request shares its slot with another request whose window is not
- * empty (not in shared spill mode), the sparse layers of a slot disagree on its private key count (shared spill mode, after a
- * partial refill), or no hash_func set.  On these errors nothing is modified. */
+ * untouched.  The spilled keys go into the store and tables of the request's slot: the requests of a slot spill into it in
+ * request order, so n_old is the slot's count plus the rows of the slot's earlier requests.  The two modes differ in two ways
+ * only.  Without shared spill (reserved[3] = 0) a request with g_b > 0 must be alone on its slot among requests with a
+ * non-empty window: a request that shares its context generates at most generation_buffer tokens.  In shared spill mode
+ * several requests of a slot may spill, and each spilled key is private to its request.
+ * MPIG_EINVAL: keep < 0 or sink + keep >= window capacity; MPIG_ESTATE: the slot's count plus all its requests' rows >
+ * max_length for some sparse layer, a spilling request shares its slot with another request whose window is not empty (not in
+ * shared spill mode), the sparse layers of a slot disagree on its private key count (shared spill mode, after a partial
+ * refill), or no hash_func set.  On these errors nothing is modified. */
 int mpig_spill_window(mpig_ctx *ctx, int keep, int32_t *spilled_out, void *stream);
 /* Fused sparse-layer decode (attnserver.py:261-312): centre + append the new key/value to the
  * window, SimHash, probe, gather attention over window + sample with the LSE merge folded in -- one kernel launch.

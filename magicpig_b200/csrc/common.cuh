@@ -472,14 +472,11 @@ bool fused_applicable(const mpig_ctx *ctx);
 int fused_resident_clusters(int C, int threads);
 int fused_cluster_waves(const mpig_ctx *ctx);   // waves of clusters one fused launch takes (0 = not applicable / unknown)
 int launch_pack_nhd(mpig_ctx *ctx, const void *k, const void *v, uint8_t *rec, int Hkv, int n, int rows_cap, cudaStream_t s);
-// window spill, table side (tables.cu): merge the codes of the keys [n_old[b], n_old[b] + g[b]) of every request into the
-// tables of `layer`.  codes (Hkv, L, g[b]) int16 per request, request b's block starting at pre[b] * Hkv * L; g / pre / n_old
-// are device arrays [B].
+// window spill, table side (tables.cu): merge the codes of the keys [n_old[c], n_old[c] + g[c]) of every context slot c into
+// its tables of `layer`.  codes (Hkv, L, g[c]) int16 per slot, slot c's block starting at pre[c] * Hkv * L; g / pre / n_old
+// are device arrays [C].
 int launch_table_merge(mpig_ctx *ctx, int layer, const int16_t *codes, const int32_t *g, const int32_t *pre, const int32_t *n_old,
                        cudaStream_t s);
-// the same merge over n entries of slot-indexed arrays (entry i merges into slot i): shared spill mode merges once per slot
-int launch_table_merge_slots(mpig_ctx *ctx, int layer, const int16_t *codes, const int32_t *g, const int32_t *pre,
-                             const int32_t *n_old, cudaStream_t s);
 // shared spill mode: a request's place in the visibility map changes (store.cu).  src >= 0: dst sees exactly the private keys src
 // sees (a fork); src < 0: dst sees no private key (a bind).  Every slot's map is rewritten.
 int launch_vis_rebind(mpig_ctx *ctx, int src, int dst, cudaStream_t s);

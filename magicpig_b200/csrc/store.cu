@@ -56,38 +56,38 @@ __global__ void pack_records_nhd_kernel(const uint4 *__restrict__ k, const uint4
     }
 }
 
-// Window spill, store side (mpig_spill_window): one CTA per (kv-head, request) of one sparse layer, 8 warps.  With g = spill_g[b]:
-//   window rows [sink, sink + g) -> records n_old .. n_old + g - 1 of the store of the request's slot (slot_of[b], or b when
-//   slot_of is null) (bitwise), their key norms kn = bf16(||k||_2) widened to fp32 (fp32 sum of squares, one rounding: what fill()
-//   stores), and their key halves -> the staging for the key hash: a block (Hkv, g, d) bf16 at row spill_pre[b] * Hkv;
+// Window spill, store side (mpig_spill_window): one CTA per (kv-head, request) of one sparse layer, 8 warps.  The requests of a
+// slot c spill into it one after the other: request b, bound to c = req_slot[b], owns rows off = req_off[b] .. off + g - 1 of
+// the slot's g_c = slot_g[c] new rows.  With g = req_g[b]:
+//   window rows [sink, sink + g) -> records n_old[c] + off .. + g - 1 of the slot's store (bitwise), their key norms
+//   kn = bf16(||k||_2) widened to fp32 (fp32 sum of squares, one rounding: what fill() stores), and their key halves -> the
+//   slot's staging block for the key hash, (Hkv, g_c, d) bf16 at row slot_pre[c] * Hkv, at offset off of every kv-head's run
+//   (so the slot's new keys are hashed and merged together);
 //   window rows [sink + g, sink + g + keep) -> [sink, sink + keep).
-// Shared spill mode (blk != null, [3][B]): the requests of one slot stage into ONE block (Hkv, blk[b], d) at row spill_pre[b] * Hkv,
-// request b's rows at offset blk[B + b] of every kv-head's run, so that the slot's new keys are hashed and merged together; with
-// vis != null (one sparse layer's launch: the map is the same for every layer) the CTAs of kv-head 0 also make private keys
-// blk[2B + b] .. + g - 1 of the slot visible to b alone.
+// With vis != null (shared spill mode, one sparse layer's launch: the map is the same for every layer) the CTAs of kv-head 0
+// also make private keys slot_priv[c] + off .. + g - 1 of the slot visible to b alone.
 // The kept rows move down in place, so they are copied in chunks of ascending rows, each chunk read completely before any of
 // it is written (a row is only ever written after every row it lands on has been read).  One CTA owns the whole window of its
 // (request, kv-head): no ordering between CTAs is involved.
 __global__ void __launch_bounds__(256) spill_move_kernel(uint4 *win, uint4 *__restrict__ rec, float *__restrict__ kn_store,
-                                                         uint4 *__restrict__ stage, const int32_t *__restrict__ spill_g,
-                                                         const int32_t *__restrict__ spill_pre, const int32_t *__restrict__ n_old_b,
-                                                         const int32_t *__restrict__ slot_of, int Hkv, int M, int Wcap, int sink, int keep,
-                                                         const int32_t *__restrict__ blk, uint32_t *__restrict__ vis) {
+                                                         uint4 *__restrict__ stage, const int32_t *__restrict__ req_g,
+                                                         const int32_t *__restrict__ req_slot, const int32_t *__restrict__ req_off,
+                                                         const int32_t *__restrict__ slot_g, const int32_t *__restrict__ slot_pre,
+                                                         const int32_t *__restrict__ n_old, int Hkv, int M, int Wcap, int sink, int keep,
+                                                         const int32_t *__restrict__ slot_priv, uint32_t *__restrict__ vis) {
     constexpr int T = 256, UN = 4;
     const int gi = blockIdx.x, b = blockIdx.y, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int g = spill_g[b];
+    const int g = req_g[b];
     if (g == 0) return;
+    const int c = req_slot[b], off = req_off[b];
     const size_t bg = (size_t)b * Hkv + gi;
-    const int slot = slot_of ? slot_of[b] : b;
-    const size_t sg = (size_t)slot * Hkv + gi;   // store side: the request's slot
+    const size_t sg = (size_t)c * Hkv + gi;   // store side: the request's slot
     uint4 *w = win + bg * Wcap * 32;
-    uint4 *r = rec + (sg * M + n_old_b[b]) * 32;
-    float *kns = kn_store + sg * M + n_old_b[b];
-    const int B = gridDim.y;
-    const size_t st_rows = blk ? blk[b] : g, st_off = blk ? blk[B + b] : 0;
-    uint4 *st = stage + ((size_t)spill_pre[b] * Hkv + (size_t)gi * st_rows + st_off) * 16;
+    uint4 *r = rec + (sg * M + n_old[c] + off) * 32;
+    float *kns = kn_store + sg * M + n_old[c] + off;
+    uint4 *st = stage + ((size_t)slot_pre[c] * Hkv + (size_t)gi * slot_g[c] + off) * 16;
     if (vis && gi == 0)
-        for (int j = tid; j < g; j += T) vis[(size_t)slot * M + blk[2 * B + b] + j] = 1u << b;
+        for (int j = tid; j < g; j += T) vis[(size_t)c * M + slot_priv[c] + off + j] = 1u << b;
     for (int j = warp; j < g; j += T / 32) {
         const uint4 x = w[(size_t)(sink + j) * 32 + lane];
         r[(size_t)j * 32 + lane] = x;
@@ -252,32 +252,27 @@ int mpig_spill_window(mpig_ctx *ctx, int keep, int32_t *spilled_out, void *strea
     if (rc) return rc;
     rc = refresh_maps(ctx, s);   // each request's keys go to the slot it is bound to now
     if (rc) return rc;
-    // meta = g[B] | pre[B] (staging block of each request) | n_old[num_layers][B]; shared spill mode appends blk[3][B] (rows of
-    // the request's staging block, the request's offset in it, its first private offset) | g[C] | pre[C] | n_old[num_layers][C]
-    // per slot.  Exclusive requests stage in request order; in shared spill mode the requests of a slot stage in request order
-    // inside one block per slot, the blocks in slot order, so each slot's new keys are contiguous in the staging and the store.
-    const bool shared = ctx->shared_spill;
+    // The spill is planned per context slot: the requests of a slot spill into its store in request order, and the slot's new
+    // keys are staged as one block, the blocks in slot order, so that they are hashed and merged together.
+    // meta = per request g[B] | slot[B] | off[B] (the rows the slot's earlier requests spill) | per slot g[C] (the sum over its
+    // requests) | pre[C] (its staging block) | priv[C] (its first new private offset, shared spill mode) | n_old[num_layers][C]
     const int C = ctx->C;
-    const size_t o_blk = (size_t)(2 + nl) * B, o_sg = o_blk + 3 * (size_t)B, o_spre = o_sg + C, o_sn = o_spre + C;
-    std::vector<int32_t> meta(shared ? o_sn + (size_t)nl * C : o_blk, 0);
+    const size_t o_slot = B, o_off = 2 * (size_t)B, o_sg = 3 * (size_t)B, o_spre = o_sg + C, o_priv = o_spre + C, o_n = o_priv + C;
+    std::vector<int32_t> meta(o_n + (size_t)nl * C, 0);
     const std::vector<int> &slot = ctx->h_slot_of;
-    int tot = 0;
     for (int b = 0; b < B; ++b) {
         const int g = std::max(0, wl[b] - sink - keep);
         meta[b] = g;
-        if (!shared) {
-            meta[B + b] = tot;
-            tot += g;
-        } else {
-            meta[o_blk + B + b] = meta[o_sg + slot[b]];   // offset inside the slot's block
-            meta[o_sg + slot[b]] += g;
-        }
+        meta[o_slot + b] = slot[b];
+        meta[o_off + b] = meta[o_sg + slot[b]];
+        meta[o_sg + slot[b]] += g;
     }
-    if (shared) {
-        for (int c = 0; c < C; ++c) {
-            meta[o_spre + c] = tot;
-            tot += meta[o_sg + c];
-        }
+    int tot = 0;
+    for (int c = 0; c < C; ++c) {
+        meta[o_spre + c] = tot;
+        tot += meta[o_sg + c];
+    }
+    if (ctx->shared_spill) {
         // private keys have the same offsets in every sparse layer only while the layers agree on the slot's private count
         std::vector<int> priv(C, -1);
         for (int l = 0; l < nl; ++l) {
@@ -291,11 +286,7 @@ int mpig_spill_window(mpig_ctx *ctx, int keep, int32_t *spilled_out, void *strea
                 priv[c] = pc;
             }
         }
-        for (int b = 0; b < B; ++b) {
-            meta[B + b] = meta[o_spre + slot[b]];
-            meta[o_blk + b] = meta[o_sg + slot[b]];
-            meta[o_blk + 2 * B + b] = std::max(priv[slot[b]], 0) + meta[o_blk + B + b];
-        }
+        for (int c = 0; c < C; ++c) meta[o_priv + c] = std::max(priv[c], 0);
     } else {
         // a shared slot's store and tables are every bound request's context: spilling one request's generated tokens into them
         // would put those tokens into the others' samples
@@ -308,16 +299,13 @@ int mpig_spill_window(mpig_ctx *ctx, int keep, int32_t *spilled_out, void *strea
     }
     for (int l = 0; l < nl; ++l) {
         if (!ctx->layers[l].sparse) continue;
-        for (int b = 0; b < B; ++b) {
-            const int n_old = ctx->n_off[l][slot[b]];
-            const int add = shared ? meta[o_sg + slot[b]] : meta[b];   // shared spill: the capacity is the slot's
-            MPIG_REQUIRE(n_old + add <= M, MPIG_ESTATE,
-                         "mpig_spill_window: layer %d request %d: %d offloaded + %d spilled keys exceed max_length=%d", l, b,
-                         n_old, add, M);
-            meta[(size_t)(2 + l) * B + b] = n_old + (shared ? meta[o_blk + B + b] : 0);
+        for (int c = 0; c < C; ++c) {
+            const int n_old = ctx->n_off[l][c];
+            MPIG_REQUIRE(n_old + meta[o_sg + c] <= M, MPIG_ESTATE,
+                         "mpig_spill_window: layer %d context slot %d: %d offloaded + %d spilled keys exceed max_length=%d", l, c,
+                         n_old, meta[o_sg + c], M);
+            meta[o_n + (size_t)l * C + c] = n_old;
         }
-        if (shared)
-            for (int c = 0; c < C; ++c) meta[o_sn + (size_t)l * C + c] = ctx->n_off[l][c];
     }
     if (tot > 0) {
         // scratch for the worst case (every request spills all its non-sink rows), allocated once
@@ -343,24 +331,20 @@ int mpig_spill_window(mpig_ctx *ctx, int keep, int32_t *spilled_out, void *strea
         for (int l = 0; l < nl; ++l) {
             LayerStore &ls = ctx->layers[l];
             if (!ls.sparse) continue;
-            const int32_t *n_old = d_meta + (size_t)(2 + l) * B;
+            const int32_t *n_old = d_meta + o_n + (size_t)l * C;
             spill_move_kernel<<<dim3(Hkv, B), 256, 0, s>>>(reinterpret_cast<uint4 *>(ls.win), reinterpret_cast<uint4 *>(ls.kv), ls.kn,
-                                                          reinterpret_cast<uint4 *>(keys), d_meta, d_meta + B, n_old, ctx->slot_map(),
-                                                          Hkv, M, ctx->Wcap, sink, keep, shared ? d_meta + o_blk : nullptr,
-                                                          shared && !vis_done ? ctx->vis : nullptr);
+                                                          reinterpret_cast<uint4 *>(keys), d_meta, d_meta + o_slot, d_meta + o_off,
+                                                          d_meta + o_sg, d_meta + o_spre, n_old, Hkv, M, ctx->Wcap, sink, keep,
+                                                          d_meta + o_priv, ctx->shared_spill && !vis_done ? ctx->vis : nullptr);
             MPIG_LAUNCH_CHECK(ctx);
             vis_done = true;
-            // the key hash and the merge: per request, or per slot in shared spill mode
-            const int nb = shared ? C : B;
-            const int32_t *g_of = shared ? meta.data() + o_sg : meta.data(), *pre_of = shared ? meta.data() + o_spre : meta.data() + B;
-            for (int i = 0; i < nb; ++i) {
-                if (g_of[i] == 0) continue;
-                const int rc = mpig_hash_keys(ctx, keys + (size_t)pre_of[i] * Hkv * d, g_of[i], codes + (size_t)pre_of[i] * Hkv * L,
-                                              stream);
+            for (int c = 0; c < C; ++c) {
+                const int g = meta[o_sg + c], pre = meta[o_spre + c];
+                if (g == 0) continue;
+                const int rc = mpig_hash_keys(ctx, keys + (size_t)pre * Hkv * d, g, codes + (size_t)pre * Hkv * L, stream);
                 if (rc) return rc;
             }
-            const int rc = shared ? launch_table_merge_slots(ctx, l, codes, d_meta + o_sg, d_meta + o_spre, d_meta + o_sn + (size_t)l * C, s)
-                                  : launch_table_merge(ctx, l, codes, d_meta, d_meta + B, n_old, s);
+            const int rc = launch_table_merge(ctx, l, codes, d_meta + o_sg, d_meta + o_spre, n_old, s);
             if (rc) return rc;
         }
         for (int b = 0; b < B; ++b)
@@ -370,7 +354,7 @@ int mpig_spill_window(mpig_ctx *ctx, int keep, int32_t *spilled_out, void *strea
         MPIG_CUDA(cudaStreamSynchronize(s));
         for (int l = 0; l < nl; ++l)
             if (ctx->layers[l].sparse)
-                for (int b = 0; b < B; ++b) ctx->n_off[l][slot[b]] += meta[b];
+                for (int c = 0; c < C; ++c) ctx->n_off[l][c] += meta[o_sg + c];
         if (ctx->h_len_exact)
             for (int b = 0; b < B; ++b) ctx->h_win_len[b] = wl[b];
     }

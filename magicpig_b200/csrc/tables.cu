@@ -121,8 +121,9 @@ __global__ void __launch_bounds__(1024) build_segments_kernel(const int16_t *__r
 }
 
 // ---------------------------------------------------------------------------------------------
-// Table merge of a window spill (mpig_spill_window): add the keys [n_old, n_old + g) of a request, whose codes are given, to
-// its tables in place.  One CTA per (table, kv-head, request x key segment); segments the new keys do not touch return at once.
+// Table merge of a window spill (mpig_spill_window): add the keys [n_old, n_old + g) of a context slot, whose codes are given,
+// to its tables in place.  One CTA per (table, kv-head, slot x key segment), so no two CTAs write the same table row; segments
+// the new keys do not touch return at once.
 // With ex[c] = exclusive prefix of the histogram of the new codes over buckets and ro[c] = old offset relative to the segment:
 //   new offset of bucket c           = ro[c] + ex[c]
 //   old item at relative position p  -> p + ex[bucket(p)]          (old items of a bucket first ...)
@@ -131,24 +132,23 @@ __global__ void __launch_bounds__(1024) build_segments_kernel(const int16_t *__r
 // chunk read completely before any of it is written: a write lands only on positions already read.  No staging copy of the
 // segment is needed, so every K works in place (the old offsets are kept in shared memory when they fit beside the
 // histogram, K <= 14, and read from HBM otherwise).  A segment whose offsets are all equal has no old items, which covers a
-// segment beyond the old keys and tables that were never built (offsets still zero).  The tables are those of the request's slot
-// (slot_of[b], or b when slot_of is null; the host lets only a request that is alone on its slot spill).  grid (L, Hkv, B * S), 512 threads;
+// segment beyond the old keys and tables that were never built (offsets still zero).  grid (L, Hkv, C * S), 512 threads;
 // dynamic smem = (NB + 1 + 40 [+ NB + 1 when staged]) ints.
 // ---------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(512) table_merge_kernel(const int16_t *__restrict__ codes, int32_t *offsets, uint16_t *items,
                                                           const int32_t *__restrict__ spill_g, const int32_t *__restrict__ spill_pre,
-                                                          const int32_t *__restrict__ n_old_b, const int32_t *__restrict__ slot_of,
-                                                          int Hkv, int L, int NB, int M, int S, int seg_len, int staged) {
+                                                          const int32_t *__restrict__ spill_n_old, int Hkv, int L, int NB, int M, int S,
+                                                          int seg_len, int staged) {
     extern __shared__ int smem_i[];
     constexpr int T = 512, UN = 4;
     int *ex = smem_i;                // NB + 1: histogram of the new codes -> exclusive prefix -> placement cursors
     int *wsum = smem_i + NB + 1;     // 40
     int *oo_s = wsum + 40;           // NB + 1 old offsets (staged)
-    const int l = blockIdx.x, gi = blockIdx.y, b = blockIdx.z / S, seg = blockIdx.z % S, tid = threadIdx.x;
-    const int g = spill_g[b], n_old = n_old_b[b];
+    const int l = blockIdx.x, gi = blockIdx.y, slot = blockIdx.z / S, seg = blockIdx.z % S, tid = threadIdx.x;
+    const int g = spill_g[slot], n_old = spill_n_old[slot];
     const int seg_lo = seg * seg_len, seg_hi = min(seg_lo + seg_len, M);
     const int k0 = max(n_old, seg_lo), k1 = min(n_old + g, seg_hi);   // new keys of this segment
-    const size_t row = ((size_t)(slot_of ? slot_of[b] : b) * Hkv + gi) * L + l;
+    const size_t row = ((size_t)slot * Hkv + gi) * L + l;
     int32_t *off = offsets + (row * S + seg) * (size_t)(NB + 1);
     if (k0 >= k1) {
         // a segment beyond all keys gets the offsets a build writes there (every bucket empty at seg_lo), so that tables that
@@ -158,7 +158,7 @@ __global__ void __launch_bounds__(512) table_merge_kernel(const int16_t *__restr
         return;
     }
     uint16_t *it = items + row * (size_t)M + seg_lo;
-    const int16_t *cn = codes + (size_t)spill_pre[b] * Hkv * L + ((size_t)gi * L + l) * g - n_old;   // cn[key]
+    const int16_t *cn = codes + (size_t)spill_pre[slot] * Hkv * L + ((size_t)gi * L + l) * g - n_old;   // cn[key]
     const int base0 = off[0];
     const int32_t *oo = off;
     if (staged) {
@@ -571,27 +571,8 @@ int mpig::launch_table_merge(mpig_ctx *ctx, int layer, const int16_t *codes, con
     const int staged = base + (size_t)(NB + 1) * sizeof(int) <= 200 * 1024;   // K <= 14
     const size_t smem = base + (staged ? (size_t)(NB + 1) * sizeof(int) : 0);
     MPIG_FUNC_ATTR(table_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    table_merge_kernel<<<dim3(L, Hkv, ctx->cfg.batch_size * S), 512, smem, s>>>(
-        codes, ls.offsets, reinterpret_cast<uint16_t *>(ls.items), g, pre, n_old, ctx->slot_map(), Hkv, L, NB, ctx->cfg.max_length, S,
-        ctx->seg_len, staged);
-    MPIG_LAUNCH_CHECK(ctx);
-    return MPIG_OK;
-}
-
-// shared spill mode: entry c of g / pre / n_old ([C] each) merges the keys the requests of slot c spilled, contiguous in the
-// slot's store and in the staging, into slot c's tables -- one CTA per (table, kv-head, slot x segment), so no two CTAs write
-// the same table row
-int mpig::launch_table_merge_slots(mpig_ctx *ctx, int layer, const int16_t *codes, const int32_t *g, const int32_t *pre,
-                                   const int32_t *n_old, cudaStream_t s) {
-    const LayerStore &ls = ctx->layers[layer];
-    const int Hkv = ctx->cfg.num_key_value_heads, L = ctx->cfg.L, S = ctx->nseg, NB = ctx->NB;
-    const size_t base = (size_t)(NB + 1 + 40) * sizeof(int);
-    const int staged = base + (size_t)(NB + 1) * sizeof(int) <= 200 * 1024;
-    const size_t smem = base + (staged ? (size_t)(NB + 1) * sizeof(int) : 0);
-    MPIG_FUNC_ATTR(table_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
     table_merge_kernel<<<dim3(L, Hkv, ctx->C * S), 512, smem, s>>>(codes, ls.offsets, reinterpret_cast<uint16_t *>(ls.items), g, pre,
-                                                                   n_old, nullptr, Hkv, L, NB, ctx->cfg.max_length, S, ctx->seg_len,
-                                                                   staged);
+                                                                   n_old, Hkv, L, NB, ctx->cfg.max_length, S, ctx->seg_len, staged);
     MPIG_LAUNCH_CHECK(ctx);
     return MPIG_OK;
 }

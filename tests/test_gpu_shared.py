@@ -6,7 +6,8 @@ request, each filled with the same data, given the same per-request q / k / v:
     and bf16 outputs on four fused shapes, fused_kreg 0 / 1 and the host-buffer entry point; the three-launch path is within
     1e-5; a forked request is within 1e-3 of the oracle; dense layers are equal;
   * two documents on two slots, a refill through one request, bind, a step captured before fork / bind;
-  * spill of an exclusive request on a slot other than its index, refused spills of shared requests, refused calls;
+  * spill of an exclusive request on a slot other than its index, of two exclusive requests whose slots are in the reverse of
+    their request order, refused spills of shared requests, refused calls;
   * memory: one slot less is the per-slot bytes less; B = 8 on one C2-size context;
   * the drop-in class and the Llama runner.
 """
@@ -316,6 +317,19 @@ def test_graph_replays_new_bindings(cuda_lib):
     step()
 
 
+def twin_step(sh, tw, gen):
+    """One single-token step of a context with slots and its twin on the same random q / k / v: bitwise equal outputs and nnz."""
+    q = torch.randn((sh.B, sh.Hq, d), generator=gen).bfloat16().to(DEV)
+    k = torch.randn((sh.B, sh.Hkv, d), generator=gen).bfloat16().to(DEV)
+    v = torch.randn((sh.B, sh.Hkv, d), generator=gen).bfloat16().to(DEV)
+    outs = []
+    for c in (sh, tw):
+        c.plan()
+        outs.append(c.decode(1, q, k, v).clone())
+    assert torch.equal(outs[0], outs[1])
+    assert torch.equal(sh.last_probe()[0], tw.last_probe()[0])
+
+
 def test_spill_exclusive_and_refused(cuda_lib):
     K, L, n, Hq, Hkv = 8, 60, 1500, 8, 2
     hf = synth.make_hash_func(d, K, L, seed=17)
@@ -330,20 +344,8 @@ def test_spill_exclusive_and_refused(cuda_lib):
     for b, doc in ((0, short), (1, short), (2, long_)):
         doc.fill_store(tw, b); doc.fill_request(tw, b)
     gen = torch.Generator().manual_seed(3)
-
-    def step():
-        q = torch.randn((3, Hq, d), generator=gen).bfloat16().to(DEV)
-        k = torch.randn((3, Hkv, d), generator=gen).bfloat16().to(DEV)
-        v = torch.randn((3, Hkv, d), generator=gen).bfloat16().to(DEV)
-        outs = []
-        for c in (sh, tw):
-            c.plan()
-            outs.append(c.decode(1, q, k, v).clone())
-        assert torch.equal(outs[0], outs[1])
-        assert torch.equal(sh.last_probe()[0], tw.last_probe()[0])
-
     for _ in range(4):
-        step()
+        twin_step(sh, tw, gen)
     assert sh.spill_window().tolist() == [0, 0, 10] == tw.spill_window().tolist()
     # the slot's tables equal a device rebuild over the keys the slot now stores
     k_st = sh.read_cache(1, True, False, False)[0]
@@ -354,7 +356,7 @@ def test_spill_exclusive_and_refused(cuda_lib):
     ro, ri = slot_tables(ref, 1)
     assert_slot_tables_equal(o[1], i[1], ro[0], ri[0])
     for _ in range(3):
-        step()
+        twin_step(sh, tw, gen)
     # a request that would spill into a slot another non-empty request reads is refused, and nothing changes
     shr = make_ctx(2, 1, Hq, Hkv, n + 256, K, L, hf)
     ref2 = make_ctx(2, 1, Hq, Hkv, n + 256, K, L, hf)
@@ -376,6 +378,42 @@ def test_spill_exclusive_and_refused(cuda_lib):
         c.plan()
         outs.append(c.decode(1, q, kv, kv).clone())
     assert torch.equal(outs[0], outs[1])
+
+
+def test_spill_exclusive_slots_out_of_request_order(cuda_lib):
+    # B = 4, C = 3: request 0 alone on slot 2, request 3 alone on slot 0, requests 1 and 2 share slot 1 with short windows; the
+    # two spilling requests spill different row counts, and slot order differs from request order
+    K, L, n, Hq, Hkv = 8, 60, 1500, 8, 2
+    hf = synth.make_hash_func(d, K, L, seed=19)
+    short = Doc(Hkv, n, K, L, hf, 700, w=NS + 8)
+    docs = [Doc(Hkv, n, K, L, hf, 800, w=NS + NL + 6), short, short, Doc(Hkv, n, K, L, hf, 900, w=NS + NL + 13)]
+    sh = make_ctx(4, 3, Hq, Hkv, n + 256, K, L, hf)
+    tw = make_ctx(4, 0, Hq, Hkv, n + 256, K, L, hf)
+    sh.bind(0, 2)
+    sh.bind(2, 1)
+    for b in (0, 3, 1):
+        docs[b].fill_store(sh, b)
+    for b in range(4):
+        docs[b].fill_request(sh, b)
+        docs[b].fill_store(tw, b); docs[b].fill_request(tw, b)
+    gen = torch.Generator().manual_seed(5)
+    for _ in range(4):
+        twin_step(sh, tw, gen)
+    assert sh.spill_window().tolist() == [10, 0, 0, 17] == tw.spill_window().tolist()
+    # slot 2 holds request 0's keys, slot 0 request 3's, slot 1 the prompt alone: the records and norms of the twin's request,
+    # and tables equal to a rebuild over the stored keys
+    cache_sh, cache_tw = sh.read_cache(1), tw.read_cache(1)
+    o, i = slot_tables(sh, 1)
+    ref = Context(K, L, 2, Hq, Hkv, d, 1, n + 256, NS, NL, 8, dense_layers=[0], device=DEV)
+    ref.set_hash_func(hf.to(DEV))
+    for c, b, g in ((2, 0, 10), (0, 3, 17), (1, 1, 0)):
+        for a, t in zip(cache_sh, cache_tw):
+            assert torch.equal(a[c, :, : n + g], t[b, :, : n + g]), f"slot {c}: stored records differ"
+        ref.lsh_build(1, 0, sh.hash_keys(cache_sh[0][c, :, : n + g].contiguous()))
+        ro, ri = slot_tables(ref, 1)
+        assert_slot_tables_equal(o[c], i[c], ro[0], ri[0])
+    for _ in range(3):
+        twin_step(sh, tw, gen)
 
 
 def test_refusals(cuda_lib):
