@@ -69,12 +69,12 @@ def softmax_state(z: torch.Tensor, v: torch.Tensor, skip_rescale: bool = False, 
     keeps a weight too large by e^jump, jump = how far the running max rises there.  The tile is the one where that matters
     most (largest excess weight)."""
     if z.numel() == 0 or not bool(torch.isfinite(z).any()):
-        return torch.zeros(v.shape[-1], dtype=torch.float64), -math.inf
+        return torch.zeros(v.shape[-1], dtype=torch.float64, device=z.device), -math.inf
     v = v.double()
     m = z.max()
     e = torch.exp(z - m)
     if skip_rescale:
-        pad = torch.full((-len(z) % tile,), -math.inf, dtype=z.dtype)
+        pad = torch.full((-len(z) % tile,), -math.inf, dtype=z.dtype, device=z.device)
         run = torch.cummax(torch.cat([z, pad]).reshape(-1, tile).max(dim=1).values, 0).values
         if len(run) > 1:
             jumps = (run[1:] - run[:-1]).clamp(max=700.0)
