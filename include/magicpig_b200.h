@@ -139,7 +139,7 @@ int mpig_set_option(mpig_ctx *ctx, const char *key, int64_t value);
  * 0 = fused decode not applicable), "window_capacity" (sink + local + generation_buffer rows), "table_segments" (key segments S
  * of the tables, see mpig_lsh_table_ptrs), "query_tokens_max" (t_max of mpig_reserve_query_tokens, 1 without), "tokens_cluster_waves"
  * (waves of clusters the last mpig_decode_tokens launch with T > 1 took), "num_contexts" (context slots C, see reserved[1]), "dense_tail_rows" (R, see reserved[2]),
- * "shared_spill" (0 / 1, see reserved[3]). */
+ * "shared_spill" (0 / 1, see reserved[3]), "chunk_tokens_max" (t_max of mpig_reserve_chunk_tokens, 0 without). */
 int mpig_get_info(mpig_ctx *ctx, const char *key, int64_t *value);
 /* Capacity errors the DEVICE detected (the lengths saturate there): bit 0 = a sparse window is full (generation_buffer
  * exhausted: each further token overwrites the previous one's K/V), bit 1 = a dense cache reached its capacity (max_length, or base + R with reserved[2]), bit 2 = mpig_rewind
@@ -368,6 +368,39 @@ int mpig_plan_tree(mpig_ctx *ctx, int T, const int32_t *parents, void *stream);
  * (the accept may then be repeated).  At most one rewind or accept per plan (MPIG_ESTATE).  Row accesses stay inside the window and
  * dense capacities even after a plan that saturated.  mpig_clear forgets the pending step. */
 int mpig_accept(mpig_ctx *ctx, const int32_t *nodes, const int32_t *count, void *stream);
+
+/* ---- chunk steps: a prompt chunk appended to running requests (follow-up turns, a question per forked request) ------------------
+ *   mpig_reserve_chunk_tokens(t_max) once -> mpig_plan_chunk(T) -> per layer mpig_chunk_attend(T) -> [mpig_rewind(drop)]
+ *   -> mpig_spill_window() before the window fills.
+ * A chunk step appends the T new K/V rows of request b at base_b .. base_b + T - 1 of every layer (1 <= T <= t_max <= 1024), exactly
+ * as a T-token verification step does (sparse layers centre the keys with avg_k, dense layers store them raw), and query token t
+ * gets EXACT softmax attention (scale 1/sqrt(d); no sampling, no importance weights) over
+ *   sparse layer: every key of the slot's sampled store the request sees (shared spill mode, reserved[3]: the prompt keys and the
+ *                 private keys it spilled or inherited) plus window rows [0, base_b + t];
+ *   dense layer:  dense rows [0, base_b + t] (reserved[2] = R > 0: the slot's prompt rows below the request's dense base, then its
+ *                 tail).
+ * Store and window keys of a request carry the same -avg_k shift, to which softmax is invariant: the result is the attention a
+ * prefill of the whole conversation computes, up to rounding.  mpig_rewind(drop) afterwards keeps T - drop[b] tokens of request b
+ * (attention is causal: the kept tokens' outputs do not depend on the dropped ones); mpig_spill_window then folds the chunk into
+ * the store and the tables, and ordinary decode steps continue.  mpig_accept refuses a chunk step; mpig_decode_tokens and
+ * mpig_dense_decode_tokens refuse it too.  After mpig_chunk_attend, mpig_last_out_f32 returns B*T*Hq rows; mpig_last_probe and
+ * mpig_last_codes refuse until the next decode (a chunk step has no LSH sample).
+ *
+ * Allocates the chunk scratch (key-split states, merge tickets; the out_f32 copy grows to B*t_max*Hq rows).  Like
+ * mpig_reserve_query_tokens: not capturable (allocates, synchronises the device) and refused (MPIG_ESTATE) once a plan has been
+ * captured into a CUDA graph.  MPIG_EINVAL for t_max outside [1, 1024].  mpig_get_info("chunk_tokens_max") reports t_max. */
+int mpig_reserve_chunk_tokens(mpig_ctx *ctx, int t_max);
+/* mpig_plan_tokens for a chunk step: every window and dense length advances by T, with the same host-mirror checks (T must fit the
+ * window and the dense capacity, else MPIG_ESTATE and nothing changes) and the same device saturation bits.  Records the pending step
+ * as a chunk step of T tokens.  Capturable.  MPIG_EINVAL for T outside [1, reserved]. */
+int mpig_plan_chunk(mpig_ctx *ctx, int T, void *stream);
+/* Sparse or dense layer, a chunk step of T tokens: query bf16 (B, T, Hq, d), key / value bf16 (B, T, Hkv, d), out bf16 (B, T, Hq*d),
+ * rounded as the other attention outputs.  One append launch (the T-token verification step's), then the chunk attention kernel under
+ * programmatic dependent launch (csrc/attend_chunk.cu, mma.sync tensor-core tiles); no host synchronisation.  Capturable for a fixed
+ * T: a replay reads the lengths, bindings, store lengths and visibility maps of the replay.  MPIG_ESTATE when the pending step is not
+ * a chunk step of this T (or a dense layer has no dense KV); MPIG_EINVAL for T outside [1, reserved]. */
+int mpig_chunk_attend(mpig_ctx *ctx, int layer, int T, const void *query_bf16, const void *key_bf16, const void *value_bf16,
+                      void *out_bf16, void *stream);
 
 /* ---- dense layers (attnserver.py:116-120, 235-259), only with cfg.alloc_dense_kv -------------- */
 /* k, v bf16 (P, Hkv, d) -- the prefill cache in NHD layout as models/llama.py:282 passes it. */

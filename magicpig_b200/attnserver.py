@@ -68,7 +68,8 @@ class LSHSparseAttnServer:
                  max_query_tokens: int = 1,
                  num_contexts: Optional[int] = None,
                  dense_tail_rows: Optional[int] = None,
-                 shared_spill: bool = False) -> None:
+                 shared_spill: bool = False,
+                 max_chunk_tokens: int = 0) -> None:
         """Keywords up to `dtype` are the reference's (attnserver.py:9-20).  Extras:
         hash_func   inject the (d, K*L) bf16 projection (the reference draws it unseeded, :55);
         table_build "device" = counting sort on the GPU (mpig_lsh_build); "sorted" = the reference's
@@ -86,6 +87,7 @@ class LSHSparseAttnServer:
         shared_spill  requests that share a context may spill_window() into it (needs num_contexts < batch_size <= 32): each
                     spilled token is private to the request that spilled it and to requests later forked from it.  Size max_length
                     for the prompt plus every request's spilled tokens.
+        max_chunk_tokens  largest T of a chunk step (plan_chunk(T): T new prompt tokens per request, attended exactly); 0 = none.
         """
         self.K, self.L = K, L
         self.config = config
@@ -114,6 +116,8 @@ class LSHSparseAttnServer:
                            dense_layers=self.dense_layers, alloc_dense_kv=True, device=self.device,
                            max_query_tokens=max_query_tokens, num_contexts=num_contexts or 0,
                            dense_tail_rows=dense_tail_rows or 0, shared_spill=shared_spill)
+        if max_chunk_tokens > 0:
+            self.ctx.reserve_chunk_tokens(max_chunk_tokens)
         if hash_func is None:
             hash_func = torch.randn((self.head_dim, K * L), device=self.device, dtype=torch.bfloat16)  # attnserver.py:55
         self.hash_func = hash_func.to(device=self.device, dtype=torch.bfloat16).contiguous()
@@ -213,6 +217,13 @@ class LSHSparseAttnServer:
         T = int(num_tokens)
         self.ctx.plan(T, parents=self._stage_int32("parents", parents, (self.batch_size, T)))
 
+    def plan_chunk(self, num_tokens: int):
+        """Not in the reference.  A chunk step: num_tokens (<= max_chunk_tokens) new prompt tokens per request -- a follow-up turn, or
+        a forked request's question.  The decode calls of the step take q_len = num_tokens on sparse and dense layers alike, and token t
+        gets exact causal attention over the whole context (the request's store and window, or its dense rows) and the chunk's tokens up
+        to t.  rewind() afterwards keeps a ragged prefix per request; spill_window() folds the chunk into the store."""
+        self.ctx.plan_chunk(int(num_tokens))
+
     def accept(self, nodes, num_accepted):
         """Not in the reference.  Commits the root path nodes[b][0 .. num_accepted[b]) of the pending step (tree or chain): the
         path's K/V rows become the step's first rows in every layer and the lengths grow by num_accepted[b] only.  nodes: (T,) list
@@ -264,6 +275,8 @@ class LSHSparseAttnServer:
         """attnserver.py:228-312.  q (B,Hq,1,d), k/v (B,Hkv,1,d) -> (B, 1, Hq*d).  In a verification step of T tokens (plan(T)):
         q (B,Hq,T,d), k/v (B,Hkv,T,d) -> (B, T, Hq*d), token t attending causally to the tokens before it."""
         T = query_states.shape[2]
+        if self.ctx.pending_chunk:
+            return self._decode_tokens(query_states, key_states, value_states, layer_idx, T, chunk=True)
         if T > 1:
             return self._decode_tokens(query_states, key_states, value_states, layer_idx, T)
         q = query_states.to(torch.bfloat16).contiguous()
@@ -281,7 +294,7 @@ class LSHSparseAttnServer:
             self.ctx.decode(layer_idx, q, k, v, out)
         return out.reshape(self.batch_size, 1, self.num_attention_heads * self.head_dim).to(query_states.dtype)
 
-    def _decode_tokens(self, query_states, key_states, value_states, layer_idx: int, T: int):
+    def _decode_tokens(self, query_states, key_states, value_states, layer_idx: int, T: int, chunk: bool = False):
         # (B, H, T, d) -> the (B, T, H, d) layout of the T-token entry points
         q = query_states.to(torch.bfloat16).transpose(1, 2).contiguous()
         k = key_states.to(torch.bfloat16).transpose(1, 2).contiguous()
@@ -290,7 +303,9 @@ class LSHSparseAttnServer:
         if out is None:
             out = self._out[(layer_idx, T)] = torch.empty((self.batch_size, T, self.num_attention_heads * self.head_dim),
                                                           dtype=torch.bfloat16, device=self.device)
-        if layer_idx in self.dense_layers:
+        if chunk:
+            self.ctx.chunk_attend(layer_idx, T, q, k, v, out)
+        elif layer_idx in self.dense_layers:
             self.ctx.dense_decode_tokens(layer_idx, T, q, k, v, out)
         else:
             self.ctx.decode_tokens(layer_idx, T, q, k, v, out)

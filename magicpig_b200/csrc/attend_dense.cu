@@ -597,6 +597,7 @@ int launch_attend_dense(mpig_ctx *ctx, const LayerStore &ls, int T, const void *
     MPIG_CUDA(cudaLaunchKernelEx(&cfg, kernel, p, T, anc, sl));
     MPIG_LAUNCH_CHECK(ctx);
     ctx->last_tokens = T;
+    ctx->last_chunk = false;
     return MPIG_OK;
 }
 

@@ -116,10 +116,12 @@ struct PendingStep {
     int T = 0;            // node count of the last plan (0 = no plan since create / clear); decode_tokens must match it
     bool open = false;    // the step may still be rewound or accepted (at most once per plan)
     bool tree = false;    // the step came from mpig_plan_tree (mpig_rewind is refused)
-    void begin(int t, bool is_tree) {
+    bool chunk = false;   // the step came from mpig_plan_chunk (only mpig_chunk_attend decodes it; mpig_accept is refused)
+    void begin(int t, bool is_tree, bool is_chunk = false) {
         T = t;
         open = true;
         tree = is_tree;
+        chunk = is_chunk;
     }
     // forget = true (mpig_clear): no step to decode either
     void end(bool forget = false) {
@@ -127,6 +129,7 @@ struct PendingStep {
         if (forget) {
             T = 0;
             tree = false;
+            chunk = false;
         }
     }
 };
@@ -249,6 +252,7 @@ struct mpig_ctx {
     int tok_max = 1;                         // largest T a step may verify (1 until mpig_reserve_query_tokens)
     mpig::PendingStep pending;               // the step of the last plan (step.cu)
     int last_tokens = 1;                     // rows of the readers (mpig_last_probe / _codes / _out_f32) = B * last_tokens * Hq
+    bool last_chunk = false;                 // the last attention call was a chunk step: it has no probe or codes to read
     bool plan_captured = false;              // a plan has been captured into a CUDA graph (the scratch addresses are baked in)
     int last_tokens_waves = 0;               // cluster waves of the last mpig_decode_tokens launch
     // token trees (mpig_plan_tree / mpig_accept).  step_buf is allocated at create time for the largest step (8 nodes), so it never
@@ -259,6 +263,14 @@ struct mpig_ctx {
     void *accept_layers = nullptr;
     int n_accept_layers = 0;
     int reorder_cols = 0;                    // CTA columns of the reorder kernel's copy grid (the last entry's x0 + its columns)
+    // chunk steps (mpig_reserve_chunk_tokens / mpig_plan_chunk / mpig_chunk_attend, attend_chunk.cu).  store_n mirrors n_off on the
+    // device ([num_layers][C], written by the fills, the spill and mpig_clear) so that a captured chunk step reads the store length
+    // of the replay.  The split scratch is allocated by the reservation and never moves after a capture.
+    int chunk_max = 0;                       // largest T of a chunk step (0 until mpig_reserve_chunk_tokens)
+    int32_t *store_n = nullptr;              // [num_layers][C]
+    float *chunk_partials = nullptr;         // [chunk_part_tiles][CK_ROWS][PART_FLOATS] split states
+    int32_t *chunk_counters = nullptr;       // [B*Hkv][m-blocks of t_max] merge tickets (self-resetting)
+    int chunk_part_tiles = 0;
 };
 
 namespace mpig {
@@ -462,6 +474,14 @@ int launch_fused_tokens(mpig_ctx *ctx, int layer, int T, const void *q, const vo
 // (ancestor masks); q / out (B, T, Hq, d), rows already appended.  Shared dense mode (dense_tail_rows > 0) reads the slot stores
 // and the request tails.
 int launch_attend_dense(mpig_ctx *ctx, const LayerStore &ls, int T, const void *q, void *out, cudaStream_t s, bool pdl);
+// chunk step of T tokens on layer `layer` (attend_chunk.cu): append of the T rows, then exact causal attention over the request's
+// store + window (sparse) or dense rows (dense); q / out (B, T, Hq, d), k / v (B, T, Hkv, d)
+int launch_chunk_attend(mpig_ctx *ctx, int layer, int T, const void *q, const void *k, const void *v, void *out, cudaStream_t s);
+int chunk_partial_tiles(const mpig_ctx *ctx);
+size_t chunk_partial_bytes(const mpig_ctx *ctx);
+int chunk_counter_count(const mpig_ctx *ctx, int t_max);
+// store_n[layer] from the host mirror n_off[layer] (an asynchronous copy of pageable memory: the values are read at the call)
+int upload_store_n(mpig_ctx *ctx, int layer, cudaStream_t s);
 int launch_probe(mpig_ctx *ctx, int layer, const int32_t *query, int32_t *results, int32_t *nnz, cudaStream_t s, bool pdl);
 int launch_attend_mma(mpig_ctx *ctx, const AttendParams &p, cudaStream_t s, bool pdl);
 int launch_fused(mpig_ctx *ctx, int layer, const void *q, const void *k, const void *v, void *out, cudaStream_t s, bool pdl,

@@ -215,6 +215,8 @@ int mpig_create(const mpig_config *cfg, mpig_ctx **out) {
         TRY(dev_alloc(ctx, &ctx->vis, (size_t)ctx->C * M * sizeof(uint32_t)));
         TRY(dev_alloc(ctx, &ctx->private_lo, (size_t)cfg->num_layers * ctx->C * sizeof(int32_t)));
     }
+    // store_n [num_layers][C], allocated for C = batch_size so that a context's bytes per slot stay the store's and the tables'
+    TRY(dev_alloc(ctx, &ctx->store_n, (size_t)cfg->num_layers * cfg->batch_size * sizeof(int32_t)));
     {
         const cudaError_t e = cudaMemcpy(ctx->slot_of, ctx->h_slot_of.data(), (size_t)cfg->batch_size * sizeof(int32_t),
                                          cudaMemcpyHostToDevice);
@@ -283,6 +285,12 @@ int mpig_create(const mpig_config *cfg, mpig_ctx **out) {
 
 }  // extern "C"
 
+int mpig::upload_store_n(mpig_ctx *ctx, int layer, cudaStream_t s) {
+    MPIG_CUDA(cudaMemcpyAsync(ctx->store_n + (size_t)layer * ctx->C, ctx->n_off[layer].data(), ctx->C * sizeof(int32_t),
+                              cudaMemcpyHostToDevice, s));
+    return MPIG_OK;
+}
+
 int mpig::refresh_maps(mpig_ctx *ctx, cudaStream_t s) {
     if (ctx->h_map_exact) return MPIG_OK;
     const int B = ctx->cfg.batch_size;
@@ -322,6 +330,9 @@ void mpig_destroy(mpig_ctx *ctx) {
     cudaFree(ctx->dense_base);
     cudaFree(ctx->vis);
     cudaFree(ctx->private_lo);
+    cudaFree(ctx->store_n);
+    cudaFree(ctx->chunk_partials);
+    cudaFree(ctx->chunk_counters);
     cudaFree(ctx->codes);
     cudaFree(ctx->qnorm);
     cudaFree(ctx->results);
@@ -362,6 +373,7 @@ int mpig_clear(mpig_ctx *ctx, void *stream) {
         }
         for (auto &n : ctx->n_off[l]) n = 0;
     }
+    MPIG_CUDA(cudaMemsetAsync(ctx->store_n, 0, (size_t)ctx->cfg.num_layers * ctx->C * sizeof(int32_t), s));
     MPIG_CUDA(cudaMemsetAsync(ctx->win_len, 0, ctx->cfg.batch_size * sizeof(int32_t), s));
     MPIG_CUDA(cudaMemsetAsync(ctx->dense_len, 0, ctx->cfg.batch_size * sizeof(int32_t), s));
     if (ctx->dense_base) MPIG_CUDA(cudaMemsetAsync(ctx->dense_base, 0, ctx->cfg.batch_size * sizeof(int32_t), s));
@@ -386,6 +398,7 @@ int mpig_clear(mpig_ctx *ctx, void *stream) {
     ctx->h_len_exact = true;
     ctx->h_map_exact = !ctx->reorder_captured;
     ctx->last_tokens = 1;
+    ctx->last_chunk = false;
     ctx->pending.end(true);   // no plan to decode, rewind or accept since the clear
     return MPIG_OK;
 }
@@ -428,7 +441,7 @@ int mpig_set_option(mpig_ctx *ctx, const char *key, int64_t value) {
     else if (k == "out_f32") {
         ctx->want_out_f32 = (int)value;
         if (value && !ctx->out_f32) {
-            const size_t bytes = (size_t)ctx->H * ctx->tok_max * ctx->cfg.head_dim * sizeof(float);
+            const size_t bytes = (size_t)ctx->H * std::max(ctx->tok_max, ctx->chunk_max) * ctx->cfg.head_dim * sizeof(float);
             MPIG_CUDA(cudaMalloc(&ctx->out_f32, bytes));
             MPIG_CUDA(cudaMemset(ctx->out_f32, 0, bytes));
         }
@@ -463,6 +476,7 @@ int mpig_debug_read(mpig_ctx *ctx, unsigned long long *host_out, int nwarps) {
 int mpig_last_codes(mpig_ctx *ctx, int32_t *codes_out, void *stream) {
     mpig::DeviceGuard _dg(ctx);
     MPIG_REQUIRE(ctx && codes_out, MPIG_EINVAL, "mpig_last_codes: null argument");
+    MPIG_REQUIRE(!ctx->last_chunk, MPIG_ESTATE, "mpig_last_codes: the last call was a chunk step (no LSH sample)");
     MPIG_REQUIRE(!ctx->last_decode_fused || ctx->save_mask, MPIG_ESTATE,
                  "mpig_last_codes: the fused decode keeps the query codes in shared memory; set option save_mask before the decode");
     MPIG_CUDA(cudaMemcpyAsync(codes_out, ctx->codes, (size_t)ctx->H * ctx->last_tokens * ctx->cfg.L * sizeof(int32_t),
@@ -482,7 +496,8 @@ int mpig_reserve_query_tokens(mpig_ctx *ctx, int t_max) {
     // Everything is allocated first, so a failed allocation leaves the context as it was.
     const size_t H = (size_t)ctx->H * t_max, L = ctx->cfg.L, M = ctx->cfg.max_length, d = ctx->cfg.head_dim;
     const size_t sz[7] = {H * L * sizeof(int32_t), H * sizeof(float), H * M * sizeof(int32_t), H * sizeof(int32_t),
-                          H * 2 * (size_t)ctx->bitmap_words * sizeof(uint32_t), 2 * H * sizeof(float), H * d * sizeof(float)};
+                          H * 2 * (size_t)ctx->bitmap_words * sizeof(uint32_t), 2 * H * sizeof(float),
+                          (size_t)ctx->H * std::max(t_max, ctx->chunk_max) * d * sizeof(float)};   // out_f32 also serves chunk steps
     const int n = ctx->out_f32 ? 7 : 6;
     void *nb[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
     MPIG_CUDA(cudaDeviceSynchronize());   // scratch of a decode still in flight is about to be freed
@@ -505,6 +520,47 @@ int mpig_reserve_query_tokens(mpig_ctx *ctx, int t_max) {
         if (i < 6) ctx->bytes += sz[i] - sz[i] / H * old_rows;   // (out_f32, an option's buffer, is not counted)
     }
     ctx->tok_max = t_max;
+    return MPIG_OK;
+}
+
+int mpig_reserve_chunk_tokens(mpig_ctx *ctx, int t_max) {
+    mpig::DeviceGuard _dg(ctx);
+    MPIG_REQUIRE(ctx, MPIG_EINVAL, "mpig_reserve_chunk_tokens: null context");
+    MPIG_REQUIRE(t_max >= 1 && t_max <= 1024, MPIG_EINVAL, "mpig_reserve_chunk_tokens: t_max=%d outside [1, 1024]", t_max);
+    if (t_max <= ctx->chunk_max) return MPIG_OK;
+    MPIG_REQUIRE(!ctx->plan_captured, MPIG_ESTATE,
+                 "mpig_reserve_chunk_tokens: a step has been captured into a CUDA graph; reserve before capturing");
+    // split states (a fixed size: see chunk_partial_tiles), merge tickets per m-block of t_max tokens, and the out_f32 copy grown to
+    // B*t_max*Hq rows when the option has allocated it.  Everything is allocated first: a failed allocation changes nothing.
+    const size_t sz[3] = {ctx->chunk_partials ? 0 : chunk_partial_bytes(ctx), (size_t)chunk_counter_count(ctx, t_max) * sizeof(int32_t),
+                          ctx->out_f32 ? (size_t)ctx->H * std::max(t_max, ctx->tok_max) * ctx->cfg.head_dim * sizeof(float) : 0};
+    void *nb[3] = {nullptr, nullptr, nullptr};
+    MPIG_CUDA(cudaDeviceSynchronize());   // scratch of a step still in flight is about to be freed
+    for (int i = 0; i < 3; ++i) {
+        if (!sz[i]) continue;
+        cudaError_t e = cudaMalloc(&nb[i], sz[i]);
+        if (e == cudaSuccess) e = cudaMemset(nb[i], 0, sz[i]);
+        if (e != cudaSuccess) {
+            for (int j = 0; j <= i; ++j) cudaFree(nb[j]);
+            (void)cudaGetLastError();
+            set_error("mpig_reserve_chunk_tokens: cudaMalloc(%zu bytes) failed: %s", sz[i], cudaGetErrorString(e));
+            return MPIG_ENOMEM;
+        }
+    }
+    if (nb[0]) {
+        ctx->chunk_partials = (float *)nb[0];
+        ctx->chunk_part_tiles = chunk_partial_tiles(ctx);
+        ctx->bytes += sz[0];
+    }
+    if (ctx->chunk_counters) ctx->bytes -= (size_t)chunk_counter_count(ctx, ctx->chunk_max) * sizeof(int32_t);
+    cudaFree(ctx->chunk_counters);
+    ctx->chunk_counters = (int32_t *)nb[1];
+    ctx->bytes += sz[1];
+    if (nb[2]) {
+        cudaFree(ctx->out_f32);
+        ctx->out_f32 = (float *)nb[2];
+    }
+    ctx->chunk_max = t_max;
     return MPIG_OK;
 }
 
@@ -548,6 +604,7 @@ int mpig_get_info(mpig_ctx *ctx, const char *key, int64_t *value) {
     else if (k == "num_contexts") *value = ctx->C;
     else if (k == "dense_tail_rows") *value = ctx->dense_tail_rows;
     else if (k == "shared_spill") *value = ctx->shared_spill ? 1 : 0;
+    else if (k == "chunk_tokens_max") *value = ctx->chunk_max;
     else {
         set_error("mpig_get_info: unknown key '%s'", key);
         return MPIG_EINVAL;
@@ -643,6 +700,7 @@ int mpig_bind_request(mpig_ctx *ctx, int request, int slot, void *stream) {
 int mpig_last_probe(mpig_ctx *ctx, int32_t *nnz_out, int32_t *results_out, void *stream) {
     mpig::DeviceGuard _dg(ctx);  // run on the context's device whatever the caller's current device is
     MPIG_REQUIRE(ctx && nnz_out, MPIG_EINVAL, "mpig_last_probe: null argument");
+    MPIG_REQUIRE(!ctx->last_chunk, MPIG_ESTATE, "mpig_last_probe: the last call was a chunk step (no LSH sample)");
     const size_t rows = (size_t)ctx->H * ctx->last_tokens;
     MPIG_CUDA(cudaMemcpyAsync(nnz_out, ctx->nnz, rows * sizeof(int32_t), cudaMemcpyDeviceToDevice, as_stream(stream)));
     if (results_out)

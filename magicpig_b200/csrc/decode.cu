@@ -16,6 +16,7 @@ static int decode_sparse(mpig_ctx *ctx, int layer, const void *q, const void *k,
     if (!ev && fused_applicable(ctx)) return launch_fused(ctx, layer, q, k, v, out, s, true);
     ctx->last_decode_fused = 0;
     ctx->last_tokens = 1;
+    ctx->last_chunk = false;
     const LayerStore &ls = ctx->layers[layer];
     const AppendParams ap = append_params(ctx, ls, k, v, false);
     const bool pdl = (ev == nullptr);
@@ -188,6 +189,7 @@ static int dense_decode(mpig_ctx *ctx, int layer, int T, const void *q, const vo
     p.win_len = ctx->dense_len;
     p.Wcap = ctx->cfg.max_length;
     ctx->last_tokens = 1;
+    ctx->last_chunk = false;
     return launch_attend_mma(ctx, p, s, false);
 }
 
@@ -209,6 +211,8 @@ static int tokens_checks(mpig_ctx *ctx, int layer, int T, const void *q, const v
     MPIG_REQUIRE(T >= 1 && T <= ctx->tok_max, MPIG_EINVAL, "%s: T=%d outside [1, %d] (mpig_reserve_query_tokens sets the upper bound)",
                  who, T, ctx->tok_max);
     MPIG_REQUIRE(T == ctx->pending.T, MPIG_ESTATE, "%s: T=%d but the last plan was for %d token(s)", who, T, ctx->pending.T);
+    MPIG_REQUIRE(!ctx->pending.chunk, MPIG_ESTATE, "%s: the pending step is a chunk step (mpig_plan_chunk): decode it with mpig_chunk_attend",
+                 who);
     return MPIG_OK;
 }
 
@@ -227,6 +231,21 @@ int mpig_dense_decode_tokens(mpig_ctx *ctx, int layer, int T, const void *query_
     int rc = tokens_checks(ctx, layer, T, query_bf16, key_bf16, value_bf16, out_bf16, false, "mpig_dense_decode_tokens");
     if (rc) return rc;
     return dense_decode(ctx, layer, T, query_bf16, key_bf16, value_bf16, out_bf16, as_stream(stream), "mpig_dense_decode_tokens");
+}
+
+int mpig_chunk_attend(mpig_ctx *ctx, int layer, int T, const void *query_bf16, const void *key_bf16, const void *value_bf16,
+                      void *out_bf16, void *stream) {
+    mpig::DeviceGuard _dg(ctx);
+    int rc = check_layer(ctx, layer, false, "mpig_chunk_attend");
+    if (rc) return rc;
+    MPIG_REQUIRE(query_bf16 && key_bf16 && value_bf16 && out_bf16, MPIG_EINVAL, "mpig_chunk_attend: null argument");
+    MPIG_REQUIRE(T >= 1 && T <= ctx->chunk_max, MPIG_EINVAL,
+                 "mpig_chunk_attend: T=%d outside [1, %d] (mpig_reserve_chunk_tokens sets the upper bound)", T, ctx->chunk_max);
+    MPIG_REQUIRE(ctx->pending.chunk && T == ctx->pending.T, MPIG_ESTATE,
+                 "mpig_chunk_attend: the pending step is not a chunk step of %d token(s) (mpig_plan_chunk)", T);
+    const LayerStore &ls = ctx->layers[layer];
+    MPIG_REQUIRE(ls.sparse || ls.dense_kv, MPIG_ESTATE, "mpig_chunk_attend: dense layer %d has no dense KV (alloc_dense_kv = 0)", layer);
+    return launch_chunk_attend(ctx, layer, T, query_bf16, key_bf16, value_bf16, out_bf16, as_stream(stream));
 }
 
 }  // extern "C"

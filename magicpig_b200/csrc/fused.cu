@@ -1210,6 +1210,7 @@ int launch_fused(mpig_ctx *ctx, int layer, const void *q, const void *k, const v
     const int rc = fused_launch(ctx, layer, fp, p, pdl && (ctx->pdl_first || !fp.hash_in_kernel), s);
     if (rc) return rc;
     ctx->last_tokens = 1;
+    ctx->last_chunk = false;
     return MPIG_OK;
 }
 
@@ -1235,6 +1236,7 @@ int launch_fused_tokens(mpig_ctx *ctx, int layer, int T, const void *q, const vo
     rc = fused_launch(ctx, layer, fp, p, true, s);   // under PDL behind the append (or the SimHash kernel)
     if (rc) return rc;
     ctx->last_tokens = T;
+    ctx->last_chunk = false;
     ctx->last_tokens_waves = fp.cluster_waves;
     return MPIG_OK;
 }

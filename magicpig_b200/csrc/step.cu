@@ -33,21 +33,23 @@ __global__ void rewind_kernel(const int32_t *drop, int32_t *win_len, int32_t *de
 // The step's node records go to step_buf: the bases (lengths after the plan minus T), the parents and the ancestor masks (bit j of
 // mask t: node j is node t or one of its ancestors).  parents == null: a chain (node t's parent is t - 1).  A malformed tree
 // (parents[b][0] != -1 or parents[b][t] outside [0, t)) raises bit 3 and request b runs as a chain.  apply = 0: only that check
-// (an eager mpig_plan_tree that refuses changes nothing).
+// (an eager mpig_plan_tree that refuses changes nothing).  A chunk step longer than TREE_MAX (mpig_plan_chunk) writes the bases
+// only: its rows have no node records.
 __global__ void plan_kernel(int32_t *win_len, int32_t *dense_len, int32_t *err_flag, int B, int T, int wcap, int dcap,
                             int has_window, int has_dense, int32_t *step_buf, const int32_t *parents, int apply,
                             const int32_t *dense_base, int tail_rows) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b < B) {
+        const int TN = (T <= TREE_MAX) ? T : 0;   // nodes with records
         int par[TREE_MAX];
         bool ok = true;
-        for (int t = 0; t < T; ++t) {
+        for (int t = 0; t < TN; ++t) {
             par[t] = parents ? parents[b * T + t] : t - 1;
             ok &= (t == 0) ? (par[t] == -1) : (par[t] >= 0 && par[t] < t);
         }
         if (!ok) {
             atomicOr(err_flag, 8);
-            for (int t = 0; t < T; ++t) par[t] = t - 1;
+            for (int t = 0; t < TN; ++t) par[t] = t - 1;
         }
         if (!apply) return;
         int w = win_len[b] + T, dl = dense_len[b] + T;
@@ -66,7 +68,7 @@ __global__ void plan_kernel(int32_t *win_len, int32_t *dense_len, int32_t *err_f
         bases[2 * b] = w - T;
         bases[2 * b + 1] = dl - T;
         uint32_t m[TREE_MAX];
-        for (int t = 0; t < T; ++t) {
+        for (int t = 0; t < TN; ++t) {
             m[t] = (t > 0 ? m[par[t]] : 0u) | (1u << t);
             masks[t] = (int32_t)m[t];
             pout[t] = par[t];
@@ -248,7 +250,7 @@ static int plan_checks(mpig_ctx *ctx, int T, bool has_window, bool has_dense, co
 
 // mpig_plan / mpig_plan_tokens / mpig_plan_tree: the host-mirror checks (exact until a plan is captured into a CUDA graph: replays
 // advance only the device side), then every length advances by T on the device and the step's node records are written
-static int plan_step(mpig_ctx *ctx, int T, cudaStream_t s, const char *who, const int32_t *parents = nullptr) {
+static int plan_step(mpig_ctx *ctx, int T, cudaStream_t s, const char *who, const int32_t *parents = nullptr, bool chunk = false) {
     const int B = ctx->cfg.batch_size;
     int has_window = 0, has_dense = 0;
     for (const auto &ls : ctx->layers) {
@@ -273,7 +275,7 @@ static int plan_step(mpig_ctx *ctx, int T, cudaStream_t s, const char *who, cons
                                                has_window, has_dense, ctx->step_buf, parents, 1, ctx->dense_base_map(),
                                                ctx->dense_tail_rows);
     MPIG_LAUNCH_CHECK(ctx);
-    ctx->pending.begin(T, parents != nullptr);
+    ctx->pending.begin(T, parents != nullptr, chunk);
     return MPIG_OK;
 }
 
@@ -383,6 +385,14 @@ int mpig_plan_tokens(mpig_ctx *ctx, int T, void *stream) {
     return plan_step(ctx, T, as_stream(stream), "mpig_plan_tokens");
 }
 
+int mpig_plan_chunk(mpig_ctx *ctx, int T, void *stream) {
+    mpig::DeviceGuard _dg(ctx);
+    MPIG_REQUIRE(ctx, MPIG_EINVAL, "mpig_plan_chunk: null context");
+    MPIG_REQUIRE(T >= 1 && T <= ctx->chunk_max, MPIG_EINVAL,
+                 "mpig_plan_chunk: T=%d outside [1, %d] (mpig_reserve_chunk_tokens sets the upper bound)", T, ctx->chunk_max);
+    return plan_step(ctx, T, as_stream(stream), "mpig_plan_chunk", nullptr, true);
+}
+
 int mpig_rewind(mpig_ctx *ctx, const int32_t *drop, void *stream) {
     mpig::DeviceGuard _dg(ctx);
     MPIG_REQUIRE(ctx && drop, MPIG_EINVAL, "mpig_rewind: null argument");
@@ -447,6 +457,7 @@ int mpig_accept(mpig_ctx *ctx, const int32_t *nodes, const int32_t *count, void 
     MPIG_REQUIRE(ctx && nodes && count, MPIG_EINVAL, "mpig_accept: null argument");
     MPIG_REQUIRE(ctx->pending.T > 0 && ctx->pending.open, MPIG_ESTATE,
                  "mpig_accept: at most one rewind or accept per plan (no plan since the last one)");
+    MPIG_REQUIRE(!ctx->pending.chunk, MPIG_ESTATE, "mpig_accept: the pending step is a chunk step (mpig_plan_chunk); use mpig_rewind");
     const int B = ctx->cfg.batch_size, T = ctx->pending.T;
     cudaStream_t s = as_stream(stream);
     bool eager = true, refused = false;

@@ -189,6 +189,8 @@ int mpig_attn_fill(mpig_ctx *ctx, int layer, int request, const void *k_bf16, co
     rc = reset_private(ctx, layer, request, n, as_stream(stream));
     if (rc) return rc;
     ctx->n_off[layer][slot] = n;
+    rc = upload_store_n(ctx, layer, as_stream(stream));
+    if (rc) return rc;
     if (n == 0) return MPIG_OK;
     uint4 *rec = reinterpret_cast<uint4 *>(ls.kv + (size_t)slot * Hkv * M * ctx->rec_bytes);
     float *kns = ls.kn + (size_t)slot * Hkv * M;
@@ -219,6 +221,7 @@ int mpig_attention_wrapper(mpig_ctx *ctx, int layer, int K, int L, void *output_
     p.K = K;
     p.L = L;
     ctx->last_tokens = 1;
+    ctx->last_chunk = false;
     return launch_attend_mma(ctx, p, as_stream(stream), false);
 }
 
@@ -353,8 +356,11 @@ int mpig_spill_window(mpig_ctx *ctx, int keep, int32_t *spilled_out, void *strea
         // the pageable host buffers above must outlive the copies
         MPIG_CUDA(cudaStreamSynchronize(s));
         for (int l = 0; l < nl; ++l)
-            if (ctx->layers[l].sparse)
+            if (ctx->layers[l].sparse) {
                 for (int c = 0; c < C; ++c) ctx->n_off[l][c] += meta[o_sg + c];
+                rc = upload_store_n(ctx, l, s);
+                if (rc) return rc;
+            }
         if (ctx->h_len_exact)
             for (int b = 0; b < B; ++b) ctx->h_win_len[b] = wl[b];
     }

@@ -57,6 +57,24 @@ def rope_tables(theta: float, d: int, rows: int, device) -> tuple[torch.Tensor, 
     return emb.cos().to(torch.bfloat16), emb.sin().to(torch.bfloat16)
 
 
+def plan_turn_chunks(lengths, t_max: int, room: int):
+    """The chunk steps that feed a turn of lengths[b] tokens to request b: a list of (start, T, drop) with T <= min(t_max, room) tokens
+    from position `start` of the turn, drop[b] = the tokens of the step past request b's length (rewound after it).  room = the window
+    rows free after a spill (generation_buffer).  Pure host arithmetic."""
+    step = min(int(t_max), int(room))
+    if step < 1:
+        raise ValueError(f"no room for a chunk: t_max={t_max}, room={room}")
+    lengths = [int(n) for n in lengths]
+    if any(n < 0 for n in lengths):
+        raise ValueError(f"negative turn length in {lengths}")
+    total = max(lengths, default=0)
+    plan = []
+    for start in range(0, total, step):
+        T = min(step, total - start)
+        plan.append((start, T, [T - min(max(n - start, 0), T) for n in lengths]))
+    return plan
+
+
 class LlamaDecodeRunner:
     # The CUDA-core GEMV issues 24*rows + 16 instructions per KB of weights per warp; at the HBM rate an SM has ~23 clocks per
     # KB (4 issue slots each), so it streams at the memory rate for rows <= 2 and is ALU-bound beyond (measured at rows = 8:
@@ -67,7 +85,7 @@ class LlamaDecodeRunner:
                  seed: int = 0, generation_buffer: int = 256, dense_layers=(0, 16, 32, 48, 64), num_layers: int | None = None,
                  tp_rank: int = 0, tp_world: int = 1, tp_group=None, fused: bool = True, tp_mode: str = "ag",
                  tp_transport: str = "nccl", max_query_tokens: int = 1, num_contexts: int | None = None,
-                 dense_tail_rows: int | None = None, shared_spill: bool = False):
+                 dense_tail_rows: int | None = None, shared_spill: bool = False, max_chunk_tokens: int = 0):
         """tp_mode (only with tp_world > 1; see magicpig_b200/tp.py):
              "ag"        attention sharded by KV head, one all-gather of head outputs per layer, wo / MLP replicated (north-star)
              "megatron"  + wo row-split, gate/up column-split, down row-split, two all-reduces per layer (llama_dist.py:49-70)
@@ -79,7 +97,8 @@ class LlamaDecodeRunner:
            dense_tail_rows: R > 0 keeps the dense layers' prompt once per context, R rows per request after it; None = a full
            dense cache per request.
            shared_spill: requests forked from one prompt may spill their windows into the shared context (spill_window()), each
-           seeing only its own spilled tokens; needs num_contexts < batch_size <= 32."""
+           seeing only its own spilled tokens; needs num_contexts < batch_size <= 32.
+           max_chunk_tokens: largest chunk step extend() feeds at once (0 = extend() unavailable)."""
         assert tp_mode in ("ag", "megatron") and tp_transport in ("nccl", "peer")
         self.tp_mode, self.tp_transport = tp_mode, tp_transport
         self.shape = shape
@@ -117,7 +136,10 @@ class LlamaDecodeRunner:
                                           generation_buffer=generation_buffer, dense_layers=dense_layers, device=device,
                                           hash_func=hash_func, num_key_value_heads=self.Hkv_loc,
                                           num_attention_heads=self.Hq_loc, max_query_tokens=max_query_tokens,
-                                          num_contexts=num_contexts, dense_tail_rows=dense_tail_rows, shared_spill=shared_spill)
+                                          num_contexts=num_contexts, dense_tail_rows=dense_tail_rows, shared_spill=shared_spill,
+                                          max_chunk_tokens=max_chunk_tokens)
+        self.max_chunk_tokens = max_chunk_tokens
+        self.generation_buffer = generation_buffer
 
         def w(*shape_):
             return (torch.randn(shape_, generator=g, device=self.device, dtype=torch.float32) * 0.02).to(torch.bfloat16)
@@ -428,12 +450,64 @@ class LlamaDecodeRunner:
                 self.pos.add_(torch.as_tensor(count if not isinstance(count, int) else [count] * B, device=self.device).long())
         return self.logits_tok[:, :T]
 
+    def extend(self, ids: torch.Tensor, lengths=None):
+        """Feed a turn of new prompt tokens to every request (a follow-up turn after generating, or a forked request's question):
+        ids (B, T_total) device long, lengths (B,) the real tokens per request (default T_total; the rest of a row is padding).  The
+        turn goes in chunk steps of at most min(max_chunk_tokens, generation_buffer) tokens, each with exact causal attention over the
+        whole conversation, spill_window() before each (the window keeps its newest num_local_tokens rows), rewind() of the padding.
+        Token t of request b sits at RoPE position pos[b] + 1 + t.  Afterwards self.pos has advanced by lengths[b] and self.logits[b]
+        holds the logits after request b's last real token (unchanged where lengths[b] = 0), and every window has a free row (a last
+        chunk that filled it is spilled), so a captured step() continues the generation.  Before anything is planned, the turn is
+        checked against the dense capacity: pos[b] + 1 + lengths[b] <= max_length (with dense_tail_rows, also lengths[b] <= R; the
+        exact tail capacity, prompt base + R, is checked by each chunk's plan).  Eager-path math (library GEMMs over the B*T rows of
+        a chunk); synchronises, not capturable."""
+        assert self.tp_world == 1, "extend is built for a single GPU"
+        assert self.max_chunk_tokens > 0, "construct the runner with max_chunk_tokens > 0"
+        srv, B = self.server, self.B
+        ids = ids.to(self.device).long()
+        assert ids.dim() == 2 and ids.shape[0] == B, f"ids must be (B={B}, T_total), got {tuple(ids.shape)}"
+        n = [ids.shape[1]] * B if lengths is None else [int(x) for x in torch.as_tensor(lengths).reshape(-1).tolist()]
+        assert len(n) == B and all(0 <= x <= ids.shape[1] for x in n), f"lengths {n} outside [0, {ids.shape[1]}]"
+        # the dense layers hold every token of the conversation: pos[b] + 1 rows before the turn
+        rows = [p + 1 + x for p, x in zip(self.pos.tolist(), n)]
+        R = srv.ctx.dense_tail_rows
+        if srv.dense_layers and (max(rows) > srv.max_length or (R > 0 and max(n) > R)):
+            raise N.MagicPigError(f"extend: a turn of {n} tokens does not fit the dense caches ({rows} rows after it, max_length "
+                                  f"{srv.max_length}" + (f", dense_tail_rows {R})" if R > 0 else ")"))
+        plan = plan_turn_chunks(n, self.max_chunk_tokens, self.generation_buffer)
+        for start, T, drop in plan:
+            srv.spill_window()
+            srv.plan_chunk(T)
+            pos = self.pos[:, None] + 1 + torch.arange(T, device=self.device)   # (B, T)
+            h = self._forward_rows(F.embedding(ids[:, start:start + T], self.embed), T, pos)
+            last = [x - 1 - start for x in n]   # the row of request b's last real token in this chunk, if it is here
+            sel = [b for b in range(B) if 0 <= last[b] < T]
+            if sel:
+                rows = h[sel, [last[b] for b in sel]]   # (len(sel), hs)
+                x = F.rms_norm(rows, (self.shape.hidden_size,), self.norm, self.shape.rms_norm_eps)
+                self.logits[sel] = F.linear(x, self.lm_head).float()
+            kept = torch.tensor([T - x for x in drop], device=self.device, dtype=torch.long)
+            if any(drop):
+                srv.rewind(drop)
+            self.pos.add_(kept)
+        if plan and plan[-1][1] >= self.generation_buffer:
+            srv.spill_window()   # the last chunk may have filled a window: the next step() needs a free row
+        torch.cuda.synchronize(self.device)
+        return self.logits
+
     def _forward_tokens(self, T: int, pos: torch.Tensor):
         """The eager forward of the T rows of a verification step (after its plan): embeddings of self.ids_tok[:, :T] at RoPE
         positions pos (B, T) through every layer into self.logits_tok[:, :T] (B, T, vocab)."""
+        sh = self.shape
+        h = self._forward_rows(F.embedding(self.ids_tok[:, :T], self.embed), T, pos)
+        x = F.rms_norm(h, (sh.hidden_size,), self.norm, sh.rms_norm_eps)
+        self.logits_tok[:, :T].copy_(F.linear(x, self.lm_head).float())
+
+    def _forward_rows(self, h: torch.Tensor, T: int, pos: torch.Tensor) -> torch.Tensor:
+        """The layers over the T rows of a step (after its plan): h (B, T, hs) embeddings at RoPE positions pos (B, T) -> the final
+        residual stream (B, T, hs).  The attention server decodes the step the plan made (verification, tree or chunk step)."""
         sh, srv = self.shape, self.server
         B, d, Hq, Hkv, hs, it = self.B, self.d, self.Hq_loc, self.Hkv_loc, sh.hidden_size, self.it_loc
-        h = F.embedding(self.ids_tok[:, :T], self.embed)   # (B, T, hs)
         for li, lw in enumerate(self.layers):
             x = F.rms_norm(h, (hs,), lw["ln1"], sh.rms_norm_eps)
             qkv = F.linear(x, lw["wqkv"])   # (B, T, (Hq+2Hkv)d)
@@ -445,8 +519,7 @@ class LlamaDecodeRunner:
             x = F.rms_norm(h, (hs,), lw["ln2"], sh.rms_norm_eps)
             gu = F.linear(x, lw["w_gate_up"])
             h = h + F.linear(F.silu(gu[..., :it]) * gu[..., it:], lw["w_down"])
-        x = F.rms_norm(h, (hs,), self.norm, sh.rms_norm_eps)
-        self.logits_tok[:, :T].copy_(F.linear(x, self.lm_head).float())
+        return h
 
     def _rope_at(self, x: torch.Tensor, pos: torch.Tensor) -> torch.Tensor:
         # x (B, H, T, d), pos (B, T): token t of request b rotated by its own position

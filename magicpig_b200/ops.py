@@ -92,6 +92,8 @@ class Context:
         self.max_query_tokens = 1
         self.last_tokens = 1   # T of the last decode: the readers return B*T*Hq rows
         self.pending_tokens = 0   # T of the last plan (the shape accept() expects)
+        self.pending_chunk = False   # the last plan was plan_chunk(): the layers' calls of the step are chunk_attend()
+        self.max_chunk_tokens = 0
         if max_query_tokens > 1:
             self.reserve_query_tokens(max_query_tokens)
 
@@ -122,6 +124,7 @@ class Context:
         N.check(self.lib.mpig_clear(self._h, _stream()), "mpig_clear")
         self.last_tokens = 1
         self.pending_tokens = 0
+        self.pending_chunk = False
 
     @property
     def num_contexts(self) -> int:
@@ -306,6 +309,31 @@ class Context:
         else:
             N.check(self.lib.mpig_plan_tokens(self._h, int(tokens), _stream()), "mpig_plan_tokens")
         self.pending_tokens = int(tokens)
+        self.pending_chunk = False
+
+    def reserve_chunk_tokens(self, t_max: int):
+        """Allocate the scratch of chunk steps of up to t_max <= 1024 tokens (plan_chunk / chunk_attend).  Not capturable, and
+        refused once a step has been captured into a CUDA graph: reserve before capturing."""
+        N.check(self.lib.mpig_reserve_chunk_tokens(self._h, int(t_max)), "mpig_reserve_chunk_tokens")
+        self.max_chunk_tokens = max(self.max_chunk_tokens, int(t_max))
+
+    def plan_chunk(self, T: int):
+        """Advance every request's lengths by T for a chunk step: T new prompt tokens per request, which every layer then attends
+        with chunk_attend() (exact causal attention over the whole context).  rewind() afterwards makes the chunk ragged.
+        Capturable; eager calls raise, changing nothing, when T does not fit a window or a dense cache."""
+        N.check(self.lib.mpig_plan_chunk(self._h, int(T), _stream()), "mpig_plan_chunk")
+        self.pending_tokens = int(T)
+        self.pending_chunk = True
+
+    def chunk_attend(self, layer: int, T: int, query: torch.Tensor, key: torch.Tensor, value: torch.Tensor,
+                     out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Sparse or dense layer, chunk step of T tokens: query (B,T,Hq,d), key/value (B,T,Hkv,d) bf16 -> out (B, T, Hq*d).  Token
+        t attends exactly (softmax over every key, no sampling) to the request's context and the chunk's tokens up to t."""
+        q, k, v, out = self._decode_args(T, query, key, value, out, (self.B, T, self.Hq * self.d))
+        N.check(self.lib.mpig_chunk_attend(self._h, layer, int(T), _ptr(q), _ptr(k), _ptr(v), _ptr(out), _stream()),
+                "mpig_chunk_attend")
+        self.last_tokens = int(T)
+        return out
 
     def accept(self, nodes: torch.Tensor, count: torch.Tensor):
         """Commit the root path nodes[b][0 .. count[b]) of the pending step of request b: the path's rows move to the front of

@@ -7,8 +7,10 @@ shapes, two key segments) / gather-attention kernels, the fused single-launch de
 segments, one CTA per head with codes from the SimHash kernel, several selection passes), the three-launch decode, the dense
 kernel, the tensor-core key hash, the table build, the window spill, verification steps of T tokens, token trees with an accept,
 requests sharing one context slot, shared spill (several requests of one slot spill, a fork, single-token and T-token decodes), and
-the device-side reorder of requests (`reorder`: the in-place copy between requests, eager, refused and captured).  Results are also
-checked against each other so a tool run doubles as a test.
+the device-side reorder of requests (`reorder`: the in-place copy between requests, eager, refused and captured), and chunk steps
+(`chunk`: the chunk attention kernel on sparse and dense layers with one and several key splits, a partial m-block and a partial last
+tile, shared spill with private keys, the shared dense prefix, a rewind and a captured step).  Results are also checked against each
+other so a tool run doubles as a test.
 """
 import os
 import sys
@@ -498,8 +500,91 @@ def reorder_case(B, Hq, Hkv, n, K, L, R):
     print(f"reorder B={B} Hq={Hq} Hkv={Hkv} n={n} R={R}: ok")
 
 
+def chunk_case(B, Hq, Hkv, n, K, L, T, R):
+    """Chunk steps: B requests on one slot (shared spill, dense prefix with R tail rows) against a twin with one slot per request and
+    a full dense cache each.  Both get the same prompt, windows and 30 generated tokens on both layers, spill (private keys in the
+    shared slot), then a chunk of T on the sparse layer 1 and the dense layer 0 (T*G rows: a partial second m-block when T*G > 128;
+    n decides one key split or several), a rewind of part of it, a second chunk, and that second chunk captured into a graph and
+    replayed.  Shared and twin agree to summation order; the replay equals the eager call."""
+    M = n + 600
+    g = torch.Generator(device=dev).manual_seed(21)
+    hf = torch.randn((d, K * L), generator=g, device=dev).bfloat16()
+    key = torch.randn((Hkv, n, d), generator=g, device=dev).bfloat16()
+    val = torch.randn((Hkv, n, d), generator=g, device=dev).bfloat16()
+    dk = torch.randn((n, Hkv, d), generator=g, device=dev).bfloat16()
+    ctxs = []
+    for shared in (True, False):
+        ctx = Context(K, L, 2, Hq, Hkv, d, B, M, num_local_tokens=64, generation_buffer=T + 40, dense_layers=[0], alloc_dense_kv=True,
+                      device=dev, num_contexts=1 if shared else 0, dense_tail_rows=R if shared else 0, shared_spill=shared)
+        ctx.set_option("out_f32", 1)
+        ctx.set_hash_func(hf)
+        ctx.reserve_chunk_tokens(T)
+        for b in (range(1) if shared else range(B)):
+            ctx.attn_fill(1, b, key, val, key.norm(p=2, dim=-1).float())
+            ctx.lsh_build(1, b, ctx.hash_keys(key))
+            ctx.dense_fill(0, b, dk, dk, n)
+        for b in range(1, B if shared else 1):
+            ctx.fork(0, b)
+        g2 = torch.Generator(device=dev).manual_seed(22)
+        for b in range(B):
+            w = 68 + 5 * b
+            ctx.window_fill(1, b, torch.zeros((Hkv, d), dtype=torch.bfloat16, device=dev),
+                            torch.randn((Hkv, w, d), generator=g2, device=dev).bfloat16(),
+                            torch.randn((Hkv, w, d), generator=g2, device=dev).bfloat16())
+        ctxs.append(ctx)
+    for _ in range(30):
+        q = torch.randn((B * Hq, d), generator=g, device=dev).bfloat16()
+        kv = torch.randn((B * Hkv, d), generator=g, device=dev).bfloat16()
+        for c in ctxs:
+            c.plan()
+            c.decode(1, q, kv, kv)
+            c.dense_decode(0, q, kv, kv)
+    spilled = [c.spill_window().tolist() for c in ctxs]
+    assert spilled[0] == spilled[1] and min(spilled[0]) > 0, spilled
+
+    def chunk(c, T_, q, kv, outs=None):
+        res = []
+        for i, layer in enumerate((1, 0)):
+            c.chunk_attend(layer, T_, q, kv, kv, None if outs is None else outs[i])
+            res.append(c.last_out_f32())
+        return res
+
+    q = torch.randn((B, T, Hq, d), generator=g, device=dev).bfloat16()
+    kv = torch.randn((B, T, Hkv, d), generator=g, device=dev).bfloat16()
+    got = []
+    for c in ctxs:
+        c.plan_chunk(T)
+        got.append(chunk(c, T, q, kv))
+        c.rewind(torch.tensor([(3 * b) % (T + 1) for b in range(B)], dtype=torch.int32, device=dev))
+    for layer in range(2):
+        err = float((got[0][layer] - got[1][layer]).abs().max())
+        assert err <= 1e-5, f"chunk T={T} layer {1 - layer}: shared != twin ({err:.3g})"
+    T2 = max(1, T // 3)
+    q2, kv2 = q[:, :T2].contiguous(), kv[:, :T2].contiguous()
+    sh = ctxs[0]
+    sh.plan_chunk(T2)
+    eager = chunk(sh, T2, q2, kv2)
+    sh.rewind(torch.full((B,), T2, dtype=torch.int32, device=dev))
+    outs = [torch.empty((B, T2, Hq * d), dtype=torch.bfloat16, device=dev) for _ in range(2)]
+    st = torch.cuda.Stream()
+    st.wait_stream(torch.cuda.current_stream())
+    graph = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(graph, stream=st):
+        sh.plan_chunk(T2)
+        chunk(sh, T2, q2, kv2, outs)
+    graph.replay()
+    torch.cuda.synchronize()
+    err = float((sh.last_out_f32() - eager[1]).abs().max())
+    assert err <= 1e-5 and sh.error_flags() == 0, f"captured chunk != eager ({err:.3g})"
+    print(f"chunk B={B} Hq={Hq} Hkv={Hkv} n={n} T={T} R={R}: ok")
+
+
 if __name__ == "__main__":
-    which = sys.argv[1:] or ["stages", "dense", "decode", "hostpeer", "spill", "tokens", "tree", "shared", "shared_spill", "reorder"]
+    which = sys.argv[1:] or ["stages", "dense", "decode", "hostpeer", "spill", "tokens", "tree", "shared", "shared_spill", "reorder",
+                             "chunk"]
+    if "chunk" in which:
+        chunk_case(3, 8, 2, 600, 6, 24, 37, 200)      # one key split; T*G = 148: a partial second m-block, partial last tiles
+        chunk_case(3, 8, 2, 2100, 6, 24, 5, 200)      # several key splits merged by the last CTA
     if "reorder" in which:
         reorder_case(4, 4, 2, 700, 6, 24, 40)
     if "shared_spill" in which:

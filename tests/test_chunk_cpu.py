@@ -1,0 +1,104 @@
+"""Chunk steps on the host: the turn planner of LlamaDecodeRunner.extend() and the fp64 reference tests/test_gpu_chunk.py uses."""
+import math
+
+import pytest
+import torch
+
+from magicpig_b200.llama_runner import plan_turn_chunks
+
+
+def causal_ref(q, kctx, vctx, kc, vc):
+    """Exact softmax attention of one kv-group's chunk in fp64.  q (T, G, d) queries of the chunk's T tokens; kctx / vctx (n, d)
+    rows every token sees; kc / vc (T, d) the chunk's own rows, token t seeing rows [0, t].  Scale 1/sqrt(d).  -> (T, G, d) fp64."""
+    T, G, d = q.shape
+    K = torch.cat([kctx.double(), kc.double()], 0)
+    V = torch.cat([vctx.double(), vc.double()], 0)
+    n = kctx.shape[0]
+    s = torch.einsum("tgd,kd->tgk", q.double(), K) / d ** 0.5
+    j = torch.arange(T, device=q.device)
+    mask = torch.ones((T, n + T), dtype=torch.bool, device=q.device)
+    mask[:, n:] = j[None, :] <= j[:, None]
+    s = s.masked_fill(~mask[:, None, :], float("-inf"))
+    return torch.einsum("tgk,kd->tgd", torch.softmax(s, dim=-1), V)
+
+
+def test_plan_turn_chunks_ragged():
+    plan = plan_turn_chunks([300, 250, 0], t_max=256, room=128)
+    assert [(s, T) for s, T, _ in plan] == [(0, 128), (128, 128), (256, 44)]
+    assert plan[0][2] == [0, 0, 128] and plan[1][2] == [0, 6, 128] and plan[2][2] == [0, 44, 44]
+    # every request keeps exactly its length over the turn
+    for b, n in enumerate([300, 250, 0]):
+        assert sum(T - drop[b] for _, T, drop in plan) == n
+
+
+@pytest.mark.parametrize("t_max,room", [(1024, 192), (64, 1000), (1, 5)])
+def test_plan_turn_chunks_bounds(t_max, room):
+    lengths = [1, 777, 512]
+    plan = plan_turn_chunks(lengths, t_max, room)
+    assert all(1 <= T <= min(t_max, room) for _, T, _ in plan)
+    assert len(plan) == math.ceil(max(lengths) / min(t_max, room))
+    assert [s for s, _, _ in plan] == [i * min(t_max, room) for i in range(len(plan))]
+    for b, n in enumerate(lengths):
+        assert sum(T - drop[b] for _, T, drop in plan) == n
+        assert all(0 <= drop[b] <= T for _, T, drop in plan)
+
+
+def test_plan_turn_chunks_refuses():
+    assert plan_turn_chunks([0, 0], 8, 8) == []
+    with pytest.raises(ValueError):
+        plan_turn_chunks([3], 0, 8)
+    with pytest.raises(ValueError):
+        plan_turn_chunks([-1], 8, 8)
+
+
+def test_causal_ref_matches_naive_loop():
+    g = torch.Generator().manual_seed(3)
+    T, G, d, n = 5, 3, 16, 7
+    q, kc, vc = torch.randn((T, G, d), generator=g), torch.randn((T, d), generator=g), torch.randn((T, d), generator=g)
+    kx, vx = torch.randn((n, d), generator=g), torch.randn((n, d), generator=g)
+    out = causal_ref(q, kx, vx, kc, vc)
+    for t in range(T):
+        for j in range(G):
+            keys = [kx[i] for i in range(n)] + [kc[i] for i in range(t + 1)]
+            vals = [vx[i] for i in range(n)] + [vc[i] for i in range(t + 1)]
+            s = [float(q[t, j].double() @ k.double()) / math.sqrt(d) for k in keys]
+            m = max(s)
+            w = [math.exp(x - m) for x in s]
+            o = sum(wi * v.double() for wi, v in zip(w, vals)) / sum(w)
+            assert torch.allclose(out[t, j], o, atol=1e-12)
+
+
+def _chunk_kernel_emulation(q, K, V, split):
+    """The chunk kernel's arithmetic for one kv-group: 64-key tiles, online softmax in fp32 (log2 units), P = exp2(s - m) in fp32,
+    l summed from that P, and P entering P.V either rounded to bf16 (split = False) or as bf16 hi + bf16 lo (split = True)."""
+    bf = lambda x: x.bfloat16().float()   # noqa: E731
+    R, d = q.shape
+    m, l, acc = torch.full((R,), -math.inf), torch.zeros(R), torch.zeros(R, d)
+    c = 1.4426950408889634 / math.sqrt(d)
+    for k0 in range(0, K.shape[0], 64):
+        s = (q @ K[k0:k0 + 64].T) * c
+        mn = torch.maximum(m, s.max(1).values)
+        corr = torch.where(m == -math.inf, torch.zeros(R), torch.exp2(m - mn))
+        p = torch.exp2(s - mn[:, None])
+        l, acc = l * corr + p.sum(1), acc * corr[:, None]
+        ph = bf(p)
+        acc = acc + ph @ V[k0:k0 + 64]
+        if split:
+            acc = acc + bf(p - ph) @ V[k0:k0 + 64]
+        m = mn
+    return acc / l[:, None]
+
+
+def test_p_split_is_needed_for_the_1e3_bar():
+    """Why P enters P.V as bf16 hi + lo: with queries 4x the usual scale (logit std 4, a few keys take most of the probability) over
+    20 000 keys, plain bf16 P misses 1e-3 of fp64; the split stays ~1e-5.  (At unit scale both pass.)"""
+    g = torch.Generator().manual_seed(0)
+    n, d = 20000, 128
+    K = torch.randn((n, d), generator=g).bfloat16().float()
+    V = torch.randn((n, d), generator=g).bfloat16().float()
+    q = (torch.randn((128, d), generator=g) * 4).bfloat16().float()
+    ref = torch.softmax(q.double() @ K.double().T / math.sqrt(d), 1) @ V.double()
+    plain = (_chunk_kernel_emulation(q, K, V, False).double() - ref).abs().max().item()
+    split = (_chunk_kernel_emulation(q, K, V, True).double() - ref).abs().max().item()
+    assert plain > 1e-3, plain
+    assert split < 1e-4, split
