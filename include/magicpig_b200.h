@@ -139,7 +139,8 @@ int mpig_set_option(mpig_ctx *ctx, const char *key, int64_t value);
  * 0 = fused decode not applicable), "window_capacity" (sink + local + generation_buffer rows), "table_segments" (key segments S
  * of the tables, see mpig_lsh_table_ptrs), "query_tokens_max" (t_max of mpig_reserve_query_tokens, 1 without), "tokens_cluster_waves"
  * (waves of clusters the last mpig_decode_tokens launch with T > 1 took), "num_contexts" (context slots C, see reserved[1]), "dense_tail_rows" (R, see reserved[2]),
- * "shared_spill" (0 / 1, see reserved[3]), "chunk_tokens_max" (t_max of mpig_reserve_chunk_tokens, 0 without). */
+ * "shared_spill" (0 / 1, see reserved[3]), "chunk_tokens_max" (t_max of mpig_reserve_chunk_tokens, 0 without), "chunk_splits"
+ * (key splits of the last mpig_chunk_attend launch, 0 before any). */
 int mpig_get_info(mpig_ctx *ctx, const char *key, int64_t *value);
 /* Capacity errors the DEVICE detected (the lengths saturate there): bit 0 = a sparse window is full (generation_buffer
  * exhausted: each further token overwrites the previous one's K/V), bit 1 = a dense cache reached its capacity (max_length, or base + R with reserved[2]), bit 2 = mpig_rewind

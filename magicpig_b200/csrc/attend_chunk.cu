@@ -355,6 +355,7 @@ int launch_chunk_attend(mpig_ctx *ctx, int layer, int T, const void *q, const vo
     MPIG_LAUNCH_CHECK(ctx);
     ctx->last_tokens = T;
     ctx->last_chunk = true;
+    ctx->last_chunk_splits = splits;
     return MPIG_OK;
 }
 

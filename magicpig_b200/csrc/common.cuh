@@ -255,6 +255,7 @@ struct mpig_ctx {
     bool last_chunk = false;                 // the last attention call was a chunk step: it has no probe or codes to read
     bool plan_captured = false;              // a plan has been captured into a CUDA graph (the scratch addresses are baked in)
     int last_tokens_waves = 0;               // cluster waves of the last mpig_decode_tokens launch
+    int last_chunk_splits = 0;               // key splits of the last mpig_chunk_attend launch (0 before any)
     // token trees (mpig_plan_tree / mpig_accept).  step_buf is allocated at create time for the largest step (8 nodes), so it never
     // moves: int32 [B][T] ancestor masks (bit j of node t = node j is t or one of its ancestors) | int32 [B][T] parents | int32
     // [B][2] step bases (window, dense length before the plan, after saturation).  Every plan writes it (chains for plan_tokens).

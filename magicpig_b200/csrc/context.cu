@@ -605,6 +605,7 @@ int mpig_get_info(mpig_ctx *ctx, const char *key, int64_t *value) {
     else if (k == "dense_tail_rows") *value = ctx->dense_tail_rows;
     else if (k == "shared_spill") *value = ctx->shared_spill ? 1 : 0;
     else if (k == "chunk_tokens_max") *value = ctx->chunk_max;
+    else if (k == "chunk_splits") *value = ctx->last_chunk_splits;
     else {
         set_error("mpig_get_info: unknown key '%s'", key);
         return MPIG_EINVAL;
