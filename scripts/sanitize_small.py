@@ -7,10 +7,11 @@ shapes, two key segments) / gather-attention kernels, the fused single-launch de
 segments, one CTA per head with codes from the SimHash kernel, several selection passes), the three-launch decode, the dense
 kernel, the tensor-core key hash, the table build, the window spill, verification steps of T tokens, token trees with an accept,
 requests sharing one context slot, shared spill (several requests of one slot spill, a fork, single-token and T-token decodes), and
-the device-side reorder of requests (`reorder`: the in-place copy between requests, eager, refused and captured), and chunk steps
+the device-side reorder of requests (`reorder`: the in-place copy between requests, eager, refused and captured), chunk steps
 (`chunk`: the chunk attention kernel on sparse and dense layers with one and several key splits, a partial m-block and a partial last
-tile, shared spill with private keys, the shared dense prefix, a rewind and a captured step).  Results are also checked against each
-other so a tool run doubles as a test.
+tile, shared spill with private keys, the shared dense prefix, a rewind and a captured step), and BASELINE's C4 and C5 per-rank
+geometry (`configs`: K11 L300 over 4 segments in clusters of 4, Hq 8 / Hkv 1 over 8 segments in clusters of 8).  Results are
+also checked against each other so a tool run doubles as a test.
 """
 import os
 import sys
@@ -25,7 +26,7 @@ dev = "cuda:0"
 d = 128
 
 
-def decode_case(B, Hq, Hkv, n, K, L, selcap=2048, seed=0):
+def decode_case(B, Hq, Hkv, n, K, L, selcap=2048, seed=0, tol=1e-5):
     M = n + 160
     g = torch.Generator(device=dev).manual_seed(seed)
     hf = torch.randn((d, K * L), generator=g, device=dev).bfloat16()
@@ -63,7 +64,7 @@ def decode_case(B, Hq, Hkv, n, K, L, selcap=2048, seed=0):
     assert torch.equal(a[3], b_[3]), "masks differ"
     for h in range(B * Hq):
         assert torch.equal(a[2][h, : a[1][h]], b_[2][h, : b_[1][h]])
-    assert float((a[0] - b_[0]).abs().max()) <= 1e-5 * float(a[0].abs().max())
+    assert float((a[0] - b_[0]).abs().max()) <= tol * float(a[0].abs().max())
     print(f"decode B={B} Hq={Hq} Hkv={Hkv} n={n} K={K} L={L} selcap={selcap}: nnz/head {float(a[1].float().mean()):.1f} ok")
 
 
@@ -581,7 +582,13 @@ def chunk_case(B, Hq, Hkv, n, K, L, T, R):
 
 if __name__ == "__main__":
     which = sys.argv[1:] or ["stages", "dense", "decode", "hostpeer", "spill", "tokens", "tree", "shared", "shared_spill", "reorder",
-                             "chunk"]
+                             "chunk", "configs"]
+    if "configs" in which:   # BASELINE's C4 and C5 per-rank geometry at small n, each against its decode_impl = 0 twin
+        # the i.i.d. keys sampled here have weights near 1e-2, where 1 - (1-p)^(L-1) (Lp + 1 - p) cancels in fp32 and amplifies
+        # last-bit differences: the variants differ by up to 4e-4 of a head's largest element at K11 L300 (2e-5 at K10 L150), so
+        # they are held to the 1e-3 bar; against fp64 both stay within 2 % of it (tests/test_gpu_config_numerics.py)
+        decode_case(1, 32, 8, 3900, 11, 300, tol=1e-3)  # L = 300 over 4 segments: two tag passes, clusters of 4
+        decode_case(1, 8, 1, 7900, 10, 150, tol=1e-3)   # one kv-group of 8 heads over 8 segments: clusters of 8
     if "chunk" in which:
         chunk_case(3, 8, 2, 600, 6, 24, 37, 200)      # one key split; T*G = 148: a partial second m-block, partial last tiles
         chunk_case(3, 8, 2, 2100, 6, 24, 5, 200)      # several key splits merged by the last CTA

@@ -78,17 +78,20 @@ def _unit(rnd, *shape):
 
 
 def make_batch(regime, B, C=1, n=N_C2, T=1, lens=LENS, place="key", seed=0, dev=DEV, Hq=HQ, Hkv=HKV, K=KK, L=LL,
-               parents=None):
+               parents=None, dominant=None, base=None):
     """Sparse-layer inputs of one regime for B requests bound to C slots (request b on slot b % C).  Per slot: key / value
     (Hkv, n, d) centred store, kn, avg (Hkv, d), kcodes (fp64), the group directions u.  Per request: its window win_k / win_v
     (Hkv, w_b, d) centred, w_b = lens[b % len(lens)] - T filled rows; q (B, T, Hq, d), k_new / v_new (B, T, Hkv, d) as the model
-    produces them (uncentred).  R4: place = "key" (the last stored key dominates) or "win" (every request's last window row)."""
+    produces them (uncentred).  R4: place = "key" (stored key `dominant`, default the last, dominates) or "win" (every request's
+    last window row).  base: an earlier case of the same regime, C, n and heads whose hash functions and stores (copied, without
+    their R4 dominant key: generate it with place = "win") to reuse instead of drawing new ones; the seed draws the rest."""
     g = torch.Generator(device=dev).manual_seed(seed)
     rnd = lambda *s: torch.randn(s, generator=g, device=dev, dtype=torch.float64)   # noqa: E731
     G = Hq // Hkv
-    hf = synth.make_hash_func(d, K, L, seed=seed + 1).to(dev)
-    slots = []
-    for _ in range(C):
+    hf = synth.make_hash_func(d, K, L, seed=seed + 1).to(dev) if base is None else base["hf"]
+    slots = [] if base is None else [dict(st, key=st["key"].clone(), kn=st["kn"].clone(), kcodes=st["kcodes"].clone())
+                                     for st in base["slots"]]
+    for _ in range(C if base is None else 0):
         u = _unit(rnd, Hkv)
         mu = torch.zeros((Hkv, 1, d), dtype=torch.float64, device=dev)
         if regime == "R1":   # |mu| ~ 4 |noise|, partly along the queries
@@ -120,7 +123,7 @@ def make_batch(regime, B, C=1, n=N_C2, T=1, lens=LENS, place="key", seed=0, dev=
     c = dict(B=B, C=C, Hq=Hq, Hkv=Hkv, G=G, K=K, L=L, n=n, hf=hf, slots=slots, slot_of=slot_of, regime=regime, place=place,
              q=q.bfloat16(), win_k=win_k, win_v=win_v, k_new=(rnd(B, T, Hkv, d) + MU.reshape(B, 1, Hkv, d)).bfloat16(),
              v_new=torch.randn((B, T, Hkv, d), generator=g, device=dev).bfloat16(), vis=None)
-    _tune(c, regime, place, parents)
+    _tune(c, regime, place, parents, c["n"] - 1 if dominant is None else dominant)
     return c
 
 
@@ -193,7 +196,8 @@ def restate_batch(c, codes, variant=None, parents=None, heads=None, sets=None):
                 for h in hs:
                     qh, idx = c["q"][b, t, h], sets[b][t][h]
                     zs = sample_scores(qh, st["key"][g, idx], st["kn"][g, idx], K, L)
-                    zw = (wk.double() @ qh.double()) / RD
+                    qw = c["q"][b, t, g * G] if variant == "window_of_head_0" else qh
+                    zw = (wk.double() @ qw.double()) / RD
                     if variant == "skip_rescale":
                         o[b, t, h], _ = softmax_state(torch.cat([zw, zs]), torch.cat([wv, st["value"][g, idx]]), True)
                         continue
@@ -236,7 +240,7 @@ def _each_head(c):
     return [(b, t, h) for b in range(B) for t in range(T) for h in range(Hq)]
 
 
-def _tune(c, regime, place, parents):
+def _tune(c, regime, place, parents, pos):
     G, Hkv = c["G"], c["Hkv"]
     if regime == "R2":
         # sink rows (and the new tokens) along the group direction, strong enough that the window holds >= 90 % of the mass
@@ -253,13 +257,12 @@ def _tune(c, regime, place, parents):
             c["win_k"][b][:, :NS] = sink[:, None]
             c["k_new"][b] = (c["k_new"][b].double() * 0.25 + (sink.double() + st["avg"].double())[None]).bfloat16()
     if regime == "R4" and place == "key":
-        # the last stored key of every slot along the group direction (last key segment, last tile of its CTA's sample),
-        # scaled so that it takes about half the mass of the median query that samples it
-        pos = c["n"] - 1
+        # stored key pos of every slot (by default the last: last key segment, last tile of its CTA's sample) along the group
+        # direction, scaled so that it takes about half the mass of the median query that samples it
         for st in c["slots"]:
             st["key"][:, pos] = (RD * st["u"]).bfloat16()
             st["kn"][:, pos] = st["key"][:, pos].norm(p=2, dim=-1).float()
-            st["kcodes"][:, :, pos:] = key_codes(st["key"][:, pos:], c["hf"], c["K"], c["L"])
+            st["kcodes"][:, :, pos:pos + 1] = key_codes(st["key"][:, pos:pos + 1], c["hf"], c["K"], c["L"])
         sets = batch_sets(c, query_codes(c["q"], c["hf"], c["K"], c["L"])[0])
         deltas = [[] for _ in c["slots"]]
         for b, t, h in _each_head(c):
@@ -274,7 +277,7 @@ def _tune(c, regime, place, parents):
             delta = max(sorted(ds)[len(ds) // 2], 2.0 ** -6)
             st["key"][:, pos] = (RD * st["u"] * delta).bfloat16()
             st["kn"][:, pos] = st["key"][:, pos].norm(p=2, dim=-1).float()
-            st["kcodes"][:, :, pos:] = key_codes(st["key"][:, pos:], c["hf"], c["K"], c["L"])
+            st["kcodes"][:, :, pos:pos + 1] = key_codes(st["key"][:, pos:pos + 1], c["hf"], c["K"], c["L"])
         c["dominant"] = pos
     if regime == "R4" and place == "win":
         # every request's last filled window row (in the window's last tile) dominates, about half the median query's mass
@@ -296,7 +299,7 @@ def perturbations(c):
     names = [SELF_CHECK[c["regime"]]]
     if c["B"] > 1 and len({w.shape[1] for w in c["win_k"]}) > 1:
         names.append("window_of_request_0")
-    if c["C"] == 2 and (c["regime"] == "R1" or c["place"] == "key" and c["regime"] == "R4"):   # the store carries mass
+    if c["C"] >= 2 and (c["regime"] == "R1" or c["place"] == "key" and c["regime"] == "R4"):   # the store carries mass
         names.append("wrong_document")
     if c["regime"] == "R1":   # the sampled half carries nearly all the mass of every head
         names.append("drop_sampled")
