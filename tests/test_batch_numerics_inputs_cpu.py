@@ -8,9 +8,9 @@ own, `window_of_request_0` and `wrong_document` -- must move the fp64 output by 
 import pytest
 import torch
 
-from tests.test_gpu_batch_numerics import (LENS, TREE, check_dense_inputs, check_inputs, key_codes, make_batch,
-                                           make_dense_slots, perturbations, query_codes)
 from magicpig_b200 import synth
+from tests.support.fp64 import key_codes, query_codes
+from tests.support.sparse_cases import LENS, TREE, check_dense_inputs, check_inputs, make_batch, make_dense_slots, perturbations
 
 SMALL = dict(n=3000, dev="cpu", Hq=8, Hkv=2, K=8, L=60)
 

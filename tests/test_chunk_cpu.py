@@ -1,25 +1,13 @@
-"""Chunk steps on the host: the turn planner of LlamaDecodeRunner.extend() and the fp64 reference tests/test_gpu_chunk.py uses."""
+"""Chunk steps on the host: the turn planner of LlamaDecodeRunner.extend() and the fp64 reference tests/test_gpu_chunk.py uses
+(support.fp64.causal_ref)."""
 import math
 
 import pytest
 import torch
 
 from magicpig_b200.llama_runner import plan_turn_chunks
-
-
-def causal_ref(q, kctx, vctx, kc, vc):
-    """Exact softmax attention of one kv-group's chunk in fp64.  q (T, G, d) queries of the chunk's T tokens; kctx / vctx (n, d)
-    rows every token sees; kc / vc (T, d) the chunk's own rows, token t seeing rows [0, t].  Scale 1/sqrt(d).  -> (T, G, d) fp64."""
-    T, G, d = q.shape
-    K = torch.cat([kctx.double(), kc.double()], 0)
-    V = torch.cat([vctx.double(), vc.double()], 0)
-    n = kctx.shape[0]
-    s = torch.einsum("tgd,kd->tgk", q.double(), K) / d ** 0.5
-    j = torch.arange(T, device=q.device)
-    mask = torch.ones((T, n + T), dtype=torch.bool, device=q.device)
-    mask[:, n:] = j[None, :] <= j[:, None]
-    s = s.masked_fill(~mask[:, None, :], float("-inf"))
-    return torch.einsum("tgk,kd->tgd", torch.softmax(s, dim=-1), V)
+from tests.support.chunk_cases import Case
+from tests.support.fp64 import BAR, causal_ref, rel_rows
 
 
 def test_plan_turn_chunks_ragged():
@@ -133,7 +121,6 @@ def test_split_merge_stays_inside_the_bar(regime, place):
     """The kernel's arithmetic over 98 000 keys cut into 16 splits and merged (a 64-token chunk of one kv-group of four heads,
     the generator of tests/test_gpu_chunk_numerics.py on the host) stays >= 10x inside the per-row relative bar of that file
     in every one of its regimes: the bar's basis."""
-    from tests.test_gpu_chunk_numerics import BAR, Case, rel_rows
     c = Case(regime, 1, 32, Hq=4, Hkv=1, n=97932, p=64, place=place or "split_start", seed=3, dev="cpu",
              check_layers=("sparse",))
     sp = c.splits("sparse")

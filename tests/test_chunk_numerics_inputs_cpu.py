@@ -8,7 +8,8 @@ library calls.  The host split formula is checked against the counts the GPU fil
 import pytest
 import torch
 
-from tests.test_gpu_chunk_numerics import BAR, Case, host_splits, split_per
+from tests.support.chunk_cases import Case, host_splits, split_per
+from tests.support.fp64 import BAR, causal_ref, centred
 
 SMALL = dict(n=3000, p=3000, Hq=8, Hkv=2, dev="cpu")
 
@@ -66,8 +67,6 @@ def test_host_split_formula():
 
 def test_restatement_matches_causal_ref():
     """The combined-axis restatement equals causal_ref (store + window before the chunk, the chunk causal)."""
-    from tests.test_chunk_cpu import causal_ref
-    from tests.test_gpu_chunk_numerics import centred
     c = Case("R1", 1, 9, Hq=4, Hkv=1, n=300, p=200, seed=19, sms=132, dev="cpu")
     o = c.restate("sparse")
     ctx_k = torch.cat([c.store_k[0][0], c.win_k[0][0]])

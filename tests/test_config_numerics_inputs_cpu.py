@@ -8,8 +8,9 @@ every head.
 """
 import pytest
 
-from tests.test_gpu_batch_numerics import LENS, make_batch, perturbations, query_codes
-from tests.test_gpu_config_numerics import REG_CHUNKS, chunk_streams, check_config_inputs, pass_sets, seg_bounds
+from tests.support.config_cases import REG_CHUNKS, check_config_inputs, chunk_streams, pass_sets, seg_bounds
+from tests.support.fp64 import query_codes
+from tests.support.sparse_cases import LENS, make_batch, perturbations
 
 SMALL = dict(n=20000, dev="cpu", Hq=8, Hkv=1, K=11, L=300)
 SEGS = seg_bounds(4, 20480)

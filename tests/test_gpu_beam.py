@@ -16,25 +16,18 @@ import torch
 
 from magicpig_b200 import _native as N
 from magicpig_b200.ops import Context
-from tests.test_gpu_parity import assert_1e3_f32, oracle_decode
-from tests.test_gpu_shared import Doc
+from tests.support.fp64 import assert_1e3_f32, oracle_decode
+from tests.support.library import DEV, NL, NS, Doc, d, two_layer_context
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-d, NS, NL, GEN = 128, 4, 64, 64
+GEN = 64
 Hq, Hkv, K, L, M, N_KEYS, P_DENSE = 8, 2, 8, 60, 4096, 2000, 300
 B, C = 4, 2
 
 
 def make_ctx(hf, C=C, R=0, spill=False, impl=1, kreg=0):
-    ctx = Context(K, L, 2, Hq, Hkv, d, B, M, NS, NL, GEN, dense_layers=[0], alloc_dense_kv=True, device=DEV, max_query_tokens=4,
-                  num_contexts=C, dense_tail_rows=R, shared_spill=spill)
-    ctx.set_option("decode_impl", impl)
-    ctx.set_option("fused_kreg", kreg)
-    ctx.set_option("out_f32", 1)
-    ctx.set_option("save_mask", 1)
-    ctx.set_hash_func(hf.to(DEV))
-    return ctx
+    return two_layer_context(K, L, Hq, Hkv, B, M, GEN, hf, dict(decode_impl=impl, fused_kreg=kreg, out_f32=1, save_mask=1),
+                             alloc_dense_kv=True, max_query_tokens=4, num_contexts=C, dense_tail_rows=R, shared_spill=spill)
 
 
 def fill(ctx, docs, wins):

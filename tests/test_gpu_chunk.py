@@ -21,17 +21,11 @@ import torch.nn.functional as F
 
 from magicpig_b200 import _native as N
 from magicpig_b200 import synth
-from tests.test_chunk_cpu import causal_ref
-from tests.test_gpu_tokens import bf16_half_up
+from tests.support.fp64 import assert_rounded_half_up, causal_ref, centred, rel_rows
+from tests.support.library import DEV, NL, NS, assert_tables_equal, d, lsh_tables, two_layer_context
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-d, NS, NL, K_, L_ = 128, 4, 64, 6, 16
-
-
-def centred(k, avg):
-    """bf16(k - avg) with an fp32 subtraction, as the append kernel centres a sparse layer's keys."""
-    return (k.float() - avg.float()).bfloat16()
+K_, L_ = 6, 16
 
 
 class Setup:
@@ -41,13 +35,10 @@ class Setup:
                  one_prompt=False):
         """one_prompt: every slot is filled with the same prompt (drawn as for one slot), so that C = B gives the exclusive-slot twin
         of a context with C = 1."""
-        from magicpig_b200.ops import Context
         self.B, self.Hq, self.Hkv, self.G = B, Hq, Hkv, Hq // Hkv
-        self.ctx = ctx = Context(K_, L_, 2, Hq, Hkv, d, B, M, NS, NL, gen, dense_layers=[0], alloc_dense_kv=True, device=DEV,
-                                 num_contexts=C, dense_tail_rows=tail, shared_spill=shared_spill)
-        ctx.set_hash_func(synth.make_hash_func(d, K_, L_, seed=seed).to(DEV))
+        self.ctx = ctx = two_layer_context(K_, L_, Hq, Hkv, B, M, gen, synth.make_hash_func(d, K_, L_, seed=seed), dict(out_f32=1),
+                                           alloc_dense_kv=True, num_contexts=C, dense_tail_rows=tail, shared_spill=shared_spill)
         ctx.reserve_chunk_tokens(t_max)
-        ctx.set_option("out_f32", 1)
         self.g = g = torch.Generator(device=DEV).manual_seed(seed + 1)
         rnd = lambda *s: torch.randn(s, generator=g, device=DEV).bfloat16()   # noqa: E731
         nslots = C or B
@@ -95,8 +86,7 @@ class Setup:
 
 def check(f32, ref, what):
     """Per row (token, q-head): max|out_f32 - fp64| <= 1e-3 max|fp64|."""
-    a, o = f32.double().reshape(-1, d), ref.double().reshape(-1, d)
-    err = float(((a - o).abs().amax(-1) / o.abs().amax(-1).clamp_min(1e-30)).max())
+    err = rel_rows(f32, ref)
     assert err <= 1e-3, f"{what}: max|out_f32 - fp64| / max|fp64| = {err:.3g}"
 
 
@@ -119,8 +109,8 @@ def test_chunk_sparse_and_dense_vs_fp64(cuda_lib, B, T):
     out1, f1 = s.chunk(1, T, q, k, v)
     q0, k0, v0 = s.qkv(T)
     out0, f0 = s.chunk(0, T, q0, k0, v0)
-    for out, f in ((out1, f1), (out0, f0)):   # the bf16 output is the fp32 output rounded half-up
-        assert torch.equal(out.reshape(-1, d).cpu().view(torch.int16).int() & 0xFFFF, bf16_half_up(f).reshape(-1, d))
+    for out, f, layer in ((out1, f1, "sparse"), (out0, f0, "dense")):
+        assert_rounded_half_up(out, f, f"{layer} chunk")
     for b in range(B):
         for h in range(s.Hkv):
             check(f1[b, :, h * s.G:(h + 1) * s.G], sparse_ref(s, b, h, q, k, v), f"sparse b={b} h={h}")
@@ -201,37 +191,6 @@ def test_chunk_shared_spill_sees_own_keys(cuda_lib):
             check(f1[b, :, h * s.G:(h + 1) * s.G], sparse_ref(s, b, h, q, k, v, store), f"shared spill b={b} h={h}")
 
 
-def _tables(ctx, layer):
-    """The raw tables of `layer`: offsets int32 (C*Hkv*L, S, NB+1) and items as int64 (C*Hkv*L, M)."""
-    import ctypes
-    off, it = ctypes.c_void_p(), ctypes.c_void_p()
-    N.check(ctx.lib.mpig_lsh_table_ptrs(ctx._h, layer, ctypes.byref(off), ctypes.byref(it)), "mpig_lsh_table_ptrs")
-    S, R = ctx.get_info("table_segments"), ctx.C * ctx.Hkv * ctx.L
-    torch.cuda.synchronize()
-
-    class _A:
-        def __init__(self, ptr, shape, ts):
-            self.__cuda_array_interface__ = {"shape": shape, "typestr": ts, "data": (ptr, False), "version": 2}
-    o = torch.as_tensor(_A(off.value, (R, S, ctx.NB + 1), "<i4"), device=DEV).clone()
-    i = torch.as_tensor(_A(it.value, (R, ctx.M), "<i2"), device=DEV).clone()
-    return o, (i.int() & 0xFFFF).long()
-
-
-def assert_tables_equal(ctx_a, ctx_b, layer):
-    """Identical offsets, and per (row, segment, bucket) the same items (the merge's order inside a bucket is not fixed)."""
-    (oa, ia), (ob, ib) = _tables(ctx_a, layer), _tables(ctx_b, layer)
-    assert torch.equal(oa, ob), "offsets differ"
-    o = oa.long()
-    S, NB = o.shape[1], o.shape[2] - 1
-    pos = torch.arange(ia.shape[1], device=DEV)[None].expand(o.shape[0], -1).contiguous()
-    for s in range(S):
-        bucket = torch.searchsorted(o[:, s, :NB].contiguous(), pos, right=True) - 1
-        valid = (pos >= o[:, s, :1]) & (pos < o[:, s, NB:])
-        ka = torch.where(valid, (bucket << 16) | ia, -1).sort(dim=1).values
-        kb = torch.where(valid, (bucket << 16) | ib, -1).sort(dim=1).values
-        assert torch.equal(ka, kb), f"segment {s}: bucket contents differ"
-
-
 @pytest.mark.parametrize("shared", [False, True])
 def test_chunk_then_spill_equals_single_token_steps(cuda_lib, shared):
     kw = dict(C=1, shared_spill=True) if shared else {}
@@ -248,7 +207,7 @@ def test_chunk_then_spill_equals_single_token_steps(cuda_lib, shared):
     assert a.ctx.spill_window().tolist() == b_.ctx.spill_window().tolist() == [T] * B
     for x, y in zip(a.ctx.read_cache(1), b_.ctx.read_cache(1)):
         assert torch.equal(x, y)
-    assert_tables_equal(a.ctx, b_.ctx, 1)
+    assert_tables_equal(lsh_tables(a.ctx, 1), lsh_tables(b_.ctx, 1))
     # the windows, dense rows and lengths: the next step's outputs are bitwise equal
     qx, kx, vx = a.qkv(1)
     for s in (a, b_):

@@ -30,16 +30,13 @@ import pytest
 import torch
 
 from magicpig_b200 import synth
-from tests.test_gpu_batch_numerics import (GEN, LENS, NL, NS, TREE, batch_ctx, batch_sets, check_codes_lists, check_inputs,
-                                           check_outputs, d, make_batch, pick, query_codes, restate_batch, seed_of,
-                                           skip_unless_132_sms, step)
-from tests.test_gpu_numerics import BAR
-from tests.test_gpu_parity import SIMHASH_EPS
+from tests.support.config_cases import REG_CHUNKS, check_config_inputs, chunk_streams, seg_bounds
+from tests.support.fp64 import SIMHASH_EPS
+from tests.support.library import DEV, NL, NS, assert_tables_equal, d, lsh_tables, skip_unless_132_sms, two_layer_context
+from tests.support.sparse_cases import (GEN, LENS, TREE, batch_ctx, check_codes_lists, check_outputs, make_batch, seed_of,
+                                        step)
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-TPP = 253        # tables per tag pass of the fused kernel (one-byte tags)
-REG_CHUNKS = 256   # 32-candidate chunks a CTA keeps in registers per pass (8 per warp x 32 warps, 16 x 16 at 512 threads)
 
 SHAPES = {
     "C4": dict(B=1, Hq=32, Hkv=8, K=11, L=300, n=199932, M=200448),
@@ -60,11 +57,6 @@ TOKEN_WAVES = {("C4", 4): 3, ("C4", 8): 5, ("C5", 4): 2}
 
 def slot_count(shape):
     return SHAPES[shape]["B"]   # C3: one document per request; the others: B = 1
-
-
-def seg_bounds(nseg, M):
-    """(number of key segments, keys per segment) of tables over max_length M cut into nseg segments (mpig_create's rule)."""
-    return nseg, (((M + nseg - 1) // nseg) + 63) & ~63
 
 
 def segments(shape):
@@ -105,102 +97,6 @@ def make_case(label, shape, regime, place="key", dominant=None, T=1, parents=Non
     return make_batch(regime, s["B"], C=slot_count(shape), n=s["n"], T=T, lens=lens, place=place, seed=seed_of(label),
                       Hq=s["Hq"], Hkv=s["Hkv"], K=s["K"], L=s["L"], parents=parents, dominant=dominant,
                       base=base_case(shape, regime))
-
-
-# ------------------------------------------------------------------------------------------------
-# self-checks beyond those of test_gpu_batch_numerics.check_inputs
-# ------------------------------------------------------------------------------------------------
-def pass_sets(c, codes, tpp=TPP):
-    """Index lists of the keys that collide in >= 2 tables of ONE pass of tpp tables (the counts of the passes never combined),
-    and per head the number of keys that collide exactly once in every pass and twice or more overall (`cross` keys)."""
-    B, T, Hq = codes.shape[:3]
-    G, L = c["G"], c["L"]
-    sets, cross = [], torch.zeros((B, T, Hq), dtype=torch.int64)
-    for b in range(B):
-        kc = c["slots"][c["slot_of"][b]]["kcodes"]
-        rows = []
-        for t in range(T):
-            heads = []
-            for g in range(c["Hkv"]):
-                qc = codes[b, t, g * G:(g + 1) * G].to(kc.device, torch.int16)
-                any_pass = torch.zeros((G, kc.shape[-1]), dtype=torch.bool, device=kc.device)
-                total = torch.zeros((G, kc.shape[-1]), dtype=torch.int64, device=kc.device)
-                for p0 in range(0, L, tpp):
-                    cnt = torch.zeros((G, kc.shape[-1]), dtype=torch.int64, device=kc.device)
-                    for l0 in range(p0, min(L, p0 + tpp), 25):
-                        l1 = min(l0 + 25, p0 + tpp, L)
-                        cnt += (kc[g, None, l0:l1] == qc[:, l0:l1, None]).sum(dim=1)
-                    any_pass |= cnt > 1
-                    total += cnt
-                for j in range(G):
-                    heads.append(torch.nonzero(any_pass[j]).flatten())
-                    cross[b, t, g * G + j] = int(((total[j] > 1) & ~any_pass[j]).sum())
-            rows.append(heads)
-        sets.append(rows)
-    return sets, cross
-
-
-def chunk_streams(c, codes, segs, tpp=TPP):
-    """The largest number of 32-candidate chunks one CTA streams in one tag pass: per head, key segment and pass, the sum over
-    the pass's tables of ceil(keys of the segment in the query's bucket / 32)."""
-    B, T, Hq = codes.shape[:3]
-    G, L, NB = c["G"], c["L"], 1 << c["K"]
-    nseg, seg_len = segs
-    worst = 0
-    for b in range(B):
-        kc = c["slots"][c["slot_of"][b]]["kcodes"]
-        n = kc.shape[-1]
-        seg = torch.arange(n, device=kc.device) // seg_len
-        for g in range(c["Hkv"]):
-            idx = (torch.arange(L, device=kc.device)[:, None] * nseg + seg[None]) * NB + kc[g].long()
-            cnt = torch.bincount(idx.flatten(), minlength=L * nseg * NB).reshape(L, nseg, NB)
-            for t in range(T):
-                qc = codes[b, t, g * G:(g + 1) * G].to(kc.device).long()                          # (G, L)
-                per = cnt[torch.arange(L, device=kc.device)[None, :, None], torch.arange(nseg, device=kc.device)[None, None, :],
-                          qc[:, :, None]]                                                             # (G, L, nseg)
-                ch = (per + 31) // 32
-                for p0 in range(0, L, tpp):
-                    worst = max(worst, int(ch[:, p0:p0 + tpp].sum(dim=1).max()))
-    return worst
-
-
-def _moved(c, o, alt):
-    """Per checked head, max|alt - o| / max|o|."""
-    a, b = pick(alt, c, None), pick(o, c, None)
-    return (a - b).abs().amax(-1) / b.abs().amax(-1).clamp_min(1e-30)
-
-
-def check_config_inputs(c, segs, label):
-    """check_inputs of test_gpu_batch_numerics (the regime's property, its own perturbation, window_of_request_0, wrong_document,
-    drop_sampled), then this file's: cross_pass and wrong_weights (K11 L300), drop_segment_s, window_of_head_0 (one kv-head).
-    Prints how far each moves the output; returns the fp64 query codes."""
-    moved = check_inputs(c)
-    codes = query_codes(c["q"], c["hf"], c["K"], c["L"])[0]
-    sets = batch_sets(c, codes)
-    o, _ = restate_batch(c, codes, sets=sets)
-    extra = {}
-    if c["L"] > TPP:
-        psets, cross = pass_sets(c, codes)
-        assert int(cross.min()) > 0, f"{label}: some head has no key hit once in each tag pass ({int(cross.min())})"
-        extra["cross_pass"] = float(_moved(c, o, restate_batch(c, codes, sets=psets)[0]).max())
-        extra["wrong_weights"] = float(_moved(c, o, restate_batch(dict(c, K=10, L=150), codes, sets=sets)[0]).max())
-    nseg, seg_len = segs
-    need = {"window_of_head_0"}
-    if c["regime"] == "R1":   # the sampled half carries the mass, spread over the whole store
-        need |= {"cross_pass", "wrong_weights"} | {f"drop_segment_{s}" for s in range(nseg)}
-    elif c.get("dominant") is not None:   # one stored key carries the mass (R2, R4 "win": the window does)
-        need.add(f"drop_segment_{c['dominant'] // seg_len}")
-    for s in range(nseg):
-        cut = [[[x[(x < s * seg_len) | (x >= (s + 1) * seg_len)] for x in row] for row in rows] for rows in sets]
-        extra[f"drop_segment_{s}"] = float(_moved(c, o, restate_batch(c, codes, sets=cut)[0]).max())
-    if c["G"] == c["Hq"]:
-        extra["window_of_head_0"] = float(_moved(c, o, restate_batch(c, codes, "window_of_head_0", sets=sets)[0]).max())
-    moved.update(extra)
-    print(f"{label}: perturbations move the output by " + ", ".join(f"{k} {v:.2e}" for k, v in moved.items()))
-    for name, v in extra.items():
-        if name in need:
-            assert v >= 10 * BAR, f"{label}: inputs are insensitive: '{name}' moves the output by {v:.2e} only"
-    return codes
 
 
 # ------------------------------------------------------------------------------------------------
@@ -287,12 +183,11 @@ def config_case(label, shape, regime, place="key", dominant=None, T=1, parents=N
 def test_config_geometry(cuda_lib, shape):
     """table_segments, fused_applicable, fused_cluster_waves and last_decode_fused of a single-token step, and
     tokens_cluster_waves of T-token steps, on a 132-SM H100."""
-    from magicpig_b200.ops import Context
     skip_unless_132_sms()
     s = SHAPES[shape]
     B, Hq, Hkv, K, L = s["B"], s["Hq"], s["Hkv"], s["K"], s["L"]
     for T in [1] + sorted(t for (sh, t) in TOKEN_WAVES if sh == shape):
-        ctx = Context(K, L, 2, Hq, Hkv, d, B, s["M"], NS, NL, GEN, dense_layers=[0], device=DEV, max_query_tokens=T)
+        ctx = two_layer_context(K, L, Hq, Hkv, B, s["M"], GEN, max_query_tokens=T)
         got = [ctx.get_info("table_segments"), ctx.get_info("fused_applicable"), ctx.get_info("fused_cluster_waves")]
         g = torch.Generator(device=DEV).manual_seed(1)
         ctx.set_hash_func(synth.make_hash_func(d, K, L, seed=1).to(DEV))
@@ -364,8 +259,6 @@ def test_c4_overflows_register_window(cuda_lib):
 def test_c4_spill(cuda_lib):
     """A full 324-row window at C4 spills 256 keys into segment 3: the tables equal a device rebuild over the stored keys, and a
     decode over the store as it now is matches fp64."""
-    from magicpig_b200.ops import Context
-    from tests.test_gpu_spill import assert_tables_equal
     s = SHAPES["C4"]
     nseg, seg_len = segments("C4")
     c = make_case("C4 spill", "C4", "R1", lens=(NS + NL + GEN,))
@@ -384,11 +277,10 @@ def test_c4_spill(cuda_lib):
     k_st, v_st, kn_st = ctx.read_cache(1)
     assert torch.equal(k_st[0, :, n:n + g].contiguous().view(torch.int16),
                        c["win_k"][0][:, NS:NS + g].contiguous().view(torch.int16)), "spilled keys"
-    other = Context(c["K"], c["L"], 2, c["Hq"], c["Hkv"], d, 1, s["M"], NS, NL, 8, dense_layers=[0], device=DEV)
-    other.set_hash_func(c["hf"].contiguous())
+    other = two_layer_context(c["K"], c["L"], c["Hq"], c["Hkv"], 1, s["M"], 8, c["hf"])
     new_codes = other.hash_keys(k_st[0, :, n:n + g].contiguous())
     other.lsh_build(1, 0, torch.cat([st["kcodes"], new_codes], dim=-1).contiguous())
-    assert_tables_equal(ctx, other, 1, [0])
+    assert_tables_equal(lsh_tables(ctx, 1), lsh_tables(other, 1), [0])
     del other
     torch.cuda.empty_cache()
     # the store as it now is: the prompt, the spilled keys (the library's codes of them), the window's sinks and newest rows

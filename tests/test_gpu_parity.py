@@ -23,6 +23,8 @@ import torch
 
 import oracle
 from magicpig_b200 import synth
+from tests.support.fp64 import SIMHASH_EPS, assert_1e3_before_rounding, assert_1e3_f32, bf16_from_u16, oracle_decode
+from tests.support.library import _Cfg
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -31,36 +33,6 @@ GOLD = os.path.join(os.path.dirname(__file__), "golden")
 
 def rel_err(a: torch.Tensor, b: torch.Tensor) -> float:
     return float((a.double() - b.double()).abs().max() / b.double().abs().max().clamp_min(1e-12))
-
-
-def assert_1e3_before_rounding(out_bf16: torch.Tensor, o_exact: torch.Tensor, tol: float = 1e-3):
-    """out is the bf16 the ABI prescribes; o_exact the same quantity before that rounding.  Error budget per element:
-    half a bf16 ulp of o_exact (<= |o| * 2^-8, round-to-nearest) + tol * max|o| for the arithmetic."""
-    o = o_exact.double()
-    diff = (out_bf16.double() - o).abs()
-    bound = o.abs() * 2.0 ** -8 + tol * o.abs().max()
-    worst = float((diff - bound).max())
-    assert worst <= 0.0, f"arithmetic error beyond {tol:g} relative before the bf16 rounding (excess {worst:.3e})"
-
-
-def assert_1e3_f32(out_f32: torch.Tensor, o_exact: torch.Tensor, tol: float = 1e-3):
-    """The product path's fp32 output (option "out_f32": the value BEFORE the ABI's bf16 rounding) against the oracle's
-    un-rounded result, per head: max|diff| <= tol * max|o|  (BASELINE.json: "within 1e-3 relative on the attention output")."""
-    o = o_exact.double()
-    diff = (out_f32.double() - o).abs().amax(dim=-1)
-    scale = o.abs().amax(dim=-1).clamp_min(1e-30)
-    worst = float((diff / scale).max())
-    assert worst <= tol, f"fp32 output differs from the oracle by {worst:.3e} relative (bar {tol:g})"
-
-
-# SimHash parity: exact bf16 products, fp32 accumulation in a different order than the oracle's fp64 -- a code may differ from
-# the oracle's only where one of its K projections is within accumulation noise of zero.  eps is relative to the projection's
-# own scale (its standard deviation: |norm_q| = 1 and N(0,1) hash entries give 1.0 for queries; keys are not normalised).
-SIMHASH_EPS = 2e-5
-
-
-def bf16_from_u16(a: np.ndarray) -> torch.Tensor:
-    return torch.from_numpy(a.view(np.int16).copy()).view(torch.bfloat16)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -371,45 +343,6 @@ def test_golden_c1_chain(cuda_lib):
 # ------------------------------------------------------------------------------------------------
 # fused decode: SimHash -> probe -> attention over window + sample, vs the oracle chain + merge
 # ------------------------------------------------------------------------------------------------
-def oracle_decode(t, q, k_new, v_new, win_k, win_v, G):
-    """Reference semantics of attnserver.py:261-312 on the CPU oracle, for one layer.
-    Returns (o, nnz, codes, o_exact): o follows the reference's data flow (the CPU operator rounds its output to bf16 before
-    merge_state); o_exact is the same quantity with NO intermediate rounding -- the oracle's fp32 probabilities times V in
-    fp64, merged with the window state in fp64 -- i.e. what the 1e-3 bar is measured against."""
-    B, Hq, Hkv, d, K, L, n, M = t["B"], t["Hq"], t["Hkv"], t["d"], t["K"], t["L"], t["n"], t["M"]
-    H = B * Hq
-    codes, _ = oracle.simhash(q.reshape(H, d), t["hash_func"], K, L)
-    sc, si = t["kcodes"].sort()
-    res, nz = [], []
-    for b in range(B):
-        T = oracle.Tables(Hkv, L, K, M)
-        T.fill(sc[b].contiguous(), si[b].int().contiguous())
-        r, n_, _ = oracle.batch_retrieve(T, codes[b * Hq:(b + 1) * Hq].contiguous(), G)
-        res.append(r), nz.append(n_)
-    res, nz = torch.cat(res), torch.cat(nz)
-    kp = torch.zeros((B * Hkv, M, d), dtype=torch.bfloat16); vp = torch.zeros((B * Hkv, M, d), dtype=torch.bfloat16); knp = torch.zeros((B * Hkv, M))
-    kp[:, :n], vp[:, :n], knp[:, :n] = t["key"].reshape(-1, n, d), t["value"].reshape(-1, n, d), t["key_norm"].reshape(-1, n)
-    qn = q.reshape(H, d).float().norm(p=2, dim=-1)
-    o_s, mve, score = oracle.attention_wrapper(kp, vp, knp, K, L, q.reshape(H, d), qn, res, nz, want_score=True)
-    # window = stored window rows + the new (centred) key/value (attnserver.py:275-296)
-    kc = (k_new.reshape(B * Hkv, 1, d) - t["avg_k"].reshape(B * Hkv, 1, d))
-    wk = torch.cat([win_k.reshape(B * Hkv, -1, d), kc], dim=1)
-    wv = torch.cat([win_v.reshape(B * Hkv, -1, d), v_new.reshape(B * Hkv, 1, d)], dim=1)
-    o_w, lse_w = oracle.window_attention(wk, wv, q.reshape(H, d), G)
-    o, lse = oracle.merge_state(o_w, lse_w, o_s.float(), mve[1])
-    # un-rounded: sum_j p_j V_j in fp64, LSE merge in fp64
-    o_s64 = torch.zeros((H, d), dtype=torch.float64)
-    for h in range(H):
-        sel = res[h, : nz[h]].long()
-        if len(sel):
-            o_s64[h] = score[h, : nz[h]].double() @ vp[h // G][sel].double()
-    lw, ls = lse_w.double(), mve[1].double()
-    m = torch.maximum(lw, ls)
-    a, b_ = torch.exp2(lw - m), torch.exp2(ls - m)          # ls = -inf (nnz = 0) -> b_ = 0
-    o_exact = (a[:, None] * o_w.double() + b_[:, None] * o_s64) / (a + b_)[:, None]
-    return o, nz, codes, o_exact
-
-
 @pytest.mark.parametrize("impl", [1, 0])
 @pytest.mark.parametrize("B,Hq,Hkv,n,K,L,dist", [(1, 32, 8, 4096, 10, 150, "clustered"), (2, 8, 2, 1500, 8, 60, "gauss"), (1, 4, 4, 300, 6, 24, "gauss"),
                                                  (1, 8, 1, 70000, 8, 40, "clustered"), (4, 32, 8, 2000, 8, 60, "gauss"),
@@ -621,13 +554,6 @@ def test_dense_decode_checks_out(cuda_lib):
 # ------------------------------------------------------------------------------------------------
 # the drop-in class on a small Llama-shaped config
 # ------------------------------------------------------------------------------------------------
-class _Cfg:
-    num_hidden_layers = 3
-    num_key_value_heads = 2
-    num_attention_heads = 8
-    hidden_size = 8 * 128
-
-
 @pytest.mark.parametrize("table_build,key_hash", [("device", "tcgen05"), ("sorted", "torch"), ("sorted", "tcgen05")])
 def test_attnserver_dropin(cuda_lib, table_build, key_hash):
     from magicpig_b200.attnserver import LSHSparseAttnServer

@@ -11,100 +11,23 @@ request, each filled with the same data, given the same per-request q / k / v:
   * memory: one slot less is the per-slot bytes less; B = 8 on one C2-size context;
   * the drop-in class and the Llama runner.
 """
-import ctypes
-
 import pytest
 import torch
 
 from magicpig_b200 import _native as N
 from magicpig_b200 import synth
 from magicpig_b200.ops import Context
-from tests.test_gpu_parity import _Cfg, assert_1e3_f32, oracle_decode
+from tests.support.fp64 import assert_1e3_f32, oracle_decode
+from tests.support.library import (DEV, NL, NS, Doc, _Cfg, assert_lists_equal, assert_tables_equal, d, lsh_tables,
+                                   two_layer_context)
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-d, NS, NL, GEN = 128, 4, 64, 32
-
-
-class _DevArray:
-    def __init__(self, ptr, shape, typestr):
-        self.__cuda_array_interface__ = {"shape": tuple(shape), "typestr": typestr, "data": (ptr, False), "version": 2}
-
-
-def slot_tables(ctx, layer):
-    """Copies of the raw tables of `layer`: offsets int32 (C, Hkv, L, S, NB+1), items (C, Hkv, L, M) as int32."""
-    off, it = ctypes.c_void_p(), ctypes.c_void_p()
-    N.check(ctx.lib.mpig_lsh_table_ptrs(ctx._h, layer, ctypes.byref(off), ctypes.byref(it)), "mpig_lsh_table_ptrs")
-    S = ctx.get_info("table_segments")
-    torch.cuda.synchronize()
-    o = torch.as_tensor(_DevArray(off.value, (ctx.C, ctx.Hkv, ctx.L, S, ctx.NB + 1), "<i4"), device=DEV).clone()
-    i = torch.as_tensor(_DevArray(it.value, (ctx.C, ctx.Hkv, ctx.L, ctx.M), "<i2"), device=DEV).clone()
-    return o, i.int() & 0xFFFF
-
-
-def assert_lists_equal(nnz_a, res_a, nnz_b, res_b):
-    """Equal nnz and, per row, equal index lists (the first nnz entries)."""
-    assert torch.equal(nnz_a, nnz_b), "nnz differ"
-    valid = torch.arange(res_a.shape[1], device=DEV)[None] < nnz_a[:, None]
-    assert torch.equal(torch.where(valid, res_a, -1), torch.where(valid, res_b, -1)), "index lists differ"
-
-
-def assert_slot_tables_equal(oa, ia, ob, ib):
-    """Identical offsets; per (row, segment, bucket) the same items as a set (a merge and a build may order a bucket differently)."""
-    assert torch.equal(oa, ob), "offsets differ"
-    o = oa.reshape(-1, oa.shape[-2], oa.shape[-1]).long()
-    xa, xb = ia.reshape(o.shape[0], -1).long(), ib.reshape(o.shape[0], -1).long()
-    S, NB = o.shape[1], o.shape[2] - 1
-    p = torch.arange(xa.shape[1], device=DEV)[None].expand(o.shape[0], -1).contiguous()
-    for s in range(S):
-        bucket = torch.searchsorted(o[:, s, :NB].contiguous(), p, right=True) - 1
-        valid = (p >= o[:, s, :1]) & (p < o[:, s, NB:])
-        ka = torch.where(valid, (bucket << 16) | xa, -1).sort(dim=1).values
-        kb = torch.where(valid, (bucket << 16) | xb, -1).sort(dim=1).values
-        assert torch.equal(ka, kb), f"segment {s}: bucket contents differ"
-
-
-class Doc:
-    """One context: offloaded keys of one request, its window and its dense-layer prefix (CPU tensors)."""
-
-    def __init__(self, Hkv, n, K, L, hf, seed, w=NS + NL, P_dense=300, on_gpu=False):
-        self.n, self.w = n, w
-        if on_gpu:
-            g = torch.Generator(device=DEV).manual_seed(seed)
-            self.key = torch.randn((Hkv, n, d), generator=g, device=DEV).bfloat16()
-            self.value = torch.randn((Hkv, n, d), generator=g, device=DEV).bfloat16()
-            self.kn = self.key.float().norm(p=2, dim=-1)
-            self.avg = torch.zeros((Hkv, d), dtype=torch.bfloat16)
-            self.kcodes = None
-        else:
-            key, value, kn, avg = synth.make_kv(1, Hkv, n, d, seed=seed, dist="gauss")
-            self.key, self.value, self.kn, self.avg = key[0], value[0], kn[0], avg[0].reshape(Hkv, d)
-            self.kcodes = synth.hash_keys(key, hf, K, L)[0]
-        g = torch.Generator().manual_seed(seed + 1)
-        self.wk = torch.randn((Hkv, w, d), generator=g).bfloat16()
-        self.wv = torch.randn((Hkv, w, d), generator=g).bfloat16()
-        self.dk = torch.randn((P_dense, Hkv, d), generator=g).bfloat16()
-        self.dv = torch.randn((P_dense, Hkv, d), generator=g).bfloat16()
-
-    def fill_store(self, ctx, b):
-        kd = self.key.to(DEV).contiguous()
-        ctx.attn_fill(1, b, kd, self.value.to(DEV).contiguous(), self.kn.to(DEV).contiguous())
-        ctx.lsh_build(1, b, ctx.hash_keys(kd) if self.kcodes is None else self.kcodes.to(DEV).contiguous())
-
-    def fill_request(self, ctx, b):
-        ctx.window_fill(1, b, self.avg.to(DEV).contiguous(), self.wk.to(DEV).contiguous(), self.wv.to(DEV).contiguous())
-        ctx.dense_fill(0, b, self.dk.to(DEV), self.dv.to(DEV), self.dk.shape[0])
+GEN = 32
 
 
 def make_ctx(B, C, Hq, Hkv, M, K, L, hf, impl=1, kreg=0, t_max=1, gen=GEN):
-    ctx = Context(K, L, 2, Hq, Hkv, d, B, M, NS, NL, gen, dense_layers=[0], alloc_dense_kv=True, device=DEV,
-                  max_query_tokens=t_max, num_contexts=C)
-    ctx.set_option("decode_impl", impl)
-    ctx.set_option("fused_kreg", kreg)
-    ctx.set_option("out_f32", 1)
-    ctx.set_option("save_mask", 1)
-    ctx.set_hash_func(hf.to(DEV))
-    return ctx
+    return two_layer_context(K, L, Hq, Hkv, B, M, gen, hf, dict(decode_impl=impl, fused_kreg=kreg, out_f32=1, save_mask=1),
+                             alloc_dense_kv=True, max_query_tokens=t_max, num_contexts=C)
 
 
 class Pair:
@@ -352,9 +275,9 @@ def test_spill_exclusive_and_refused(cuda_lib):
     ref = Context(K, L, 2, Hq, Hkv, d, 1, n + 256, NS, NL, 8, dense_layers=[0], device=DEV)
     ref.set_hash_func(hf.to(DEV))
     ref.lsh_build(1, 0, sh.hash_keys(k_st[1, :, : n + 10].contiguous()))
-    o, i = slot_tables(sh, 1)
-    ro, ri = slot_tables(ref, 1)
-    assert_slot_tables_equal(o[1], i[1], ro[0], ri[0])
+    o, i = lsh_tables(sh, 1)
+    ro, ri = lsh_tables(ref, 1)
+    assert_tables_equal((o[1], i[1]), (ro[0], ri[0]))
     for _ in range(3):
         twin_step(sh, tw, gen)
     # a request that would spill into a slot another non-empty request reads is refused, and nothing changes
@@ -365,10 +288,10 @@ def test_spill_exclusive_and_refused(cuda_lib):
     for c in (shr, ref2):
         c.plan()
         c.decode(1, *(torch.ones((2, h, d), dtype=torch.bfloat16, device=DEV) for h in (Hq, Hkv, Hkv)))
-    before = slot_tables(shr, 1), shr.read_cache(1)
+    before = lsh_tables(shr, 1), shr.read_cache(1)
     with pytest.raises(N.MagicPigError, match="shares"):
         shr.spill_window()
-    after = slot_tables(shr, 1), shr.read_cache(1)
+    after = lsh_tables(shr, 1), shr.read_cache(1)
     assert all(torch.equal(a, b) for a, b in zip(before[0], after[0]))
     assert all(torch.equal(a, b) for a, b in zip(before[1], after[1]))
     q = torch.randn((2, Hq, d), generator=gen).bfloat16().to(DEV)
@@ -403,15 +326,15 @@ def test_spill_exclusive_slots_out_of_request_order(cuda_lib):
     # slot 2 holds request 0's keys, slot 0 request 3's, slot 1 the prompt alone: the records and norms of the twin's request,
     # and tables equal to a rebuild over the stored keys
     cache_sh, cache_tw = sh.read_cache(1), tw.read_cache(1)
-    o, i = slot_tables(sh, 1)
+    o, i = lsh_tables(sh, 1)
     ref = Context(K, L, 2, Hq, Hkv, d, 1, n + 256, NS, NL, 8, dense_layers=[0], device=DEV)
     ref.set_hash_func(hf.to(DEV))
     for c, b, g in ((2, 0, 10), (0, 3, 17), (1, 1, 0)):
         for a, t in zip(cache_sh, cache_tw):
             assert torch.equal(a[c, :, : n + g], t[b, :, : n + g]), f"slot {c}: stored records differ"
         ref.lsh_build(1, 0, sh.hash_keys(cache_sh[0][c, :, : n + g].contiguous()))
-        ro, ri = slot_tables(ref, 1)
-        assert_slot_tables_equal(o[c], i[c], ro[0], ri[0])
+        ro, ri = lsh_tables(ref, 1)
+        assert_tables_equal((o[c], i[c]), (ro[0], ri[0]))
     for _ in range(3):
         twin_step(sh, tw, gen)
 

@@ -12,22 +12,16 @@ import torch
 from magicpig_b200 import _native as N
 from magicpig_b200 import synth
 from magicpig_b200.ops import Context
-from tests.test_gpu_parity import _Cfg
-from tests.test_gpu_shared import NL, NS, Doc, assert_lists_equal
+from tests.support.library import DEV, NL, NS, Doc, _Cfg, assert_lists_equal, d, two_layer_context
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-d, GEN = 128, 32
+GEN = 32
 TOL = 1e-5
 
 
 def make_ctx(B, C, Hq, Hkv, M, K, L, hf, R=0, t_max=1, gen=GEN):
-    ctx = Context(K, L, 2, Hq, Hkv, d, B, M, NS, NL, gen, dense_layers=[0], alloc_dense_kv=True, device=DEV,
-                  max_query_tokens=t_max, num_contexts=C, dense_tail_rows=R)
-    ctx.set_option("out_f32", 1)
-    ctx.set_option("save_mask", 1)
-    ctx.set_hash_func(hf.to(DEV))
-    return ctx
+    return two_layer_context(K, L, Hq, Hkv, B, M, gen, hf, dict(out_f32=1, save_mask=1), alloc_dense_kv=True,
+                             max_query_tokens=t_max, num_contexts=C, dense_tail_rows=R)
 
 
 def dense_ref(q, rows_k, rows_v, G):

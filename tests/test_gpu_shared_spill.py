@@ -16,25 +16,18 @@ import torch
 from magicpig_b200 import _native as N
 from magicpig_b200 import synth
 from magicpig_b200.ops import Context
-from tests.test_gpu_shared import Doc, assert_slot_tables_equal, slot_tables
-from tests.test_gpu_parity import _Cfg, assert_1e3_f32, oracle_decode
+from tests.support.fp64 import assert_1e3_f32, oracle_decode
+from tests.support.library import DEV, NL, NS, Doc, _Cfg, assert_tables_equal, d, lsh_tables, two_layer_context
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-d, NS, NL, GEN = 128, 4, 64, 32
+GEN = 32
 Hq, Hkv, K, L, M = 8, 2, 8, 60, 4096
 
 
 def make_ctx(B, C, hf, shared, impl=1, kreg=0, selcap=2048, save_mask=1):
-    ctx = Context(K, L, 2, Hq, Hkv, d, B, M, NS, NL, GEN, dense_layers=[0], device=DEV, max_query_tokens=4, num_contexts=C,
-                  shared_spill=shared)
-    ctx.set_option("decode_impl", impl)
-    ctx.set_option("fused_kreg", kreg)
-    ctx.set_option("fused_selcap", selcap)
-    ctx.set_option("out_f32", 1)
-    ctx.set_option("save_mask", save_mask)
-    ctx.set_hash_func(hf.to(DEV))
-    return ctx
+    return two_layer_context(K, L, Hq, Hkv, B, M, GEN, hf, dict(decode_impl=impl, fused_kreg=kreg, fused_selcap=selcap, out_f32=1,
+                                                                save_mask=save_mask),
+                             max_query_tokens=4, num_contexts=C, shared_spill=shared)
 
 
 class Model:
@@ -265,9 +258,9 @@ def test_tables_fork_and_bind(cuda_lib):
     k_st = sh.read_cache(1, True, False, False)[0]
     ref = make_ctx(B, 2, hf, False)   # the same batch shape: the same key segments
     ref.lsh_build(1, 0, sh.hash_keys(k_st[0, :, : n + model.count[0]].contiguous()))
-    o, i = slot_tables(sh, 1)
-    ro, ri = slot_tables(ref, 1)
-    assert_slot_tables_equal(o[0], i[0], ro[0], ri[0])
+    o, i = lsh_tables(sh, 1)
+    ro, ri = lsh_tables(ref, 1)
+    assert_tables_equal((o[0], i[0]), (ro[0], ri[0]))
     for _ in range(3):
         run.single()
     run.spill(NL - 10)
@@ -367,10 +360,10 @@ def test_refusals(cuda_lib):
         for b in range(2):
             c.window_fill(1, b, doc.avg.to(DEV).contiguous(), doc.wk.contiguous().to(DEV), doc.wv.contiguous().to(DEV))
     a, b_ = ctxs
-    before = slot_tables(a, 1), a.read_cache(1)
+    before = lsh_tables(a, 1), a.read_cache(1)
     with pytest.raises(N.MagicPigError, match="max_length"):
         a.spill_window()   # 2 x 15 keys into 20 free rows
-    after = slot_tables(a, 1), a.read_cache(1)
+    after = lsh_tables(a, 1), a.read_cache(1)
     assert all(torch.equal(x, y) for x, y in zip(before[0], after[0]))
     assert all(torch.equal(x, y) for x, y in zip(before[1], after[1]))
     g = torch.Generator().manual_seed(3)
@@ -488,10 +481,10 @@ def test_partial_refill_refused(cuda_lib):
         doc.fill_store(c, 0)   # refills layer 1 only: layer 2 keeps its 22 private keys
     step()
     a = ctxs[0]
-    before = [slot_tables(a, layer) for layer in (1, 2)], [a.read_cache(layer) for layer in (1, 2)]
+    before = [lsh_tables(a, layer) for layer in (1, 2)], [a.read_cache(layer) for layer in (1, 2)]
     with pytest.raises(N.MagicPigError, match="private keys"):
         a.spill_window()
-    after = [slot_tables(a, layer) for layer in (1, 2)], [a.read_cache(layer) for layer in (1, 2)]
+    after = [lsh_tables(a, layer) for layer in (1, 2)], [a.read_cache(layer) for layer in (1, 2)]
     for x, y in zip(before, after):
         for tx, ty in zip(x, y):
             assert all(torch.equal(p, q_) for p, q_ in zip(tx, ty))

@@ -8,145 +8,19 @@ and the hash tables, so a generation can run past generation_buffer.
   * the drop-in class generates 3 x generation_buffer + 5 tokens;
   * a refused spill changes nothing.
 """
-import ctypes
-
 import pytest
 import torch
 
 from magicpig_b200 import _native as N
 from magicpig_b200 import synth
-from tests.test_gpu_parity import _Cfg, assert_1e3_f32, oracle_decode
+from tests.support.fp64 import assert_1e3_f32, oracle_decode
+from tests.support.library import DEV, NL, NS, Run, _Cfg, assert_tables_equal, d, lsh_tables
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-d, NS, NL = 128, 4, 64
-
-
-class _DevArray:
-    def __init__(self, ptr, shape, typestr):
-        self.__cuda_array_interface__ = {"shape": tuple(shape), "typestr": typestr, "data": (ptr, False), "version": 2}
-
-
-def tables(ctx, layer):
-    """Copies of the raw tables of `layer`: offsets int32 (B, Hkv, L, S, NB+1), items (B, Hkv, L, M) as int32 in [0, 65536)."""
-    off, it = ctypes.c_void_p(), ctypes.c_void_p()
-    N.check(ctx.lib.mpig_lsh_table_ptrs(ctx._h, layer, ctypes.byref(off), ctypes.byref(it)), "mpig_lsh_table_ptrs")
-    S = ctx.get_info("table_segments")
-    torch.cuda.synchronize()
-    o = torch.as_tensor(_DevArray(off.value, (ctx.B, ctx.Hkv, ctx.L, S, ctx.NB + 1), "<i4"), device=DEV).clone()
-    i = torch.as_tensor(_DevArray(it.value, (ctx.B, ctx.Hkv, ctx.L, ctx.M), "<i2"), device=DEV).clone()
-    return o, i.int() & 0xFFFF
-
-
-def assert_tables_equal(ctx_a, ctx_b, layer, requests):
-    """Identical offsets; per (row, segment, bucket) the same items.  Every position of a segment's item range gets the key
-    (bucket << 16 | item); sorting these per row must give the same sequence on both sides."""
-    oa, ia = tables(ctx_a, layer)
-    ob, ib = tables(ctx_b, layer)
-    for b in requests:
-        assert torch.equal(oa[b], ob[b]), f"request {b}: offsets differ"
-        o = oa[b].reshape(-1, oa.shape[3], oa.shape[4]).long()           # (R, S, NB+1)
-        xa, xb = ia[b].reshape(o.shape[0], -1).long(), ib[b].reshape(o.shape[0], -1).long()
-        S, NB = o.shape[1], o.shape[2] - 1
-        pos = torch.arange(xa.shape[1], device=DEV)
-        for s in range(S):
-            lo, hi = o[:, s, :1], o[:, s, NB:]
-            p = pos[None].expand(o.shape[0], -1).contiguous()
-            bucket = torch.searchsorted(o[:, s, :NB].contiguous(), p, right=True) - 1
-            valid = (p >= lo) & (p < hi)
-            ka = torch.where(valid, (bucket << 16) | xa, -1).sort(dim=1).values
-            kb = torch.where(valid, (bucket << 16) | xb, -1).sort(dim=1).values
-            assert torch.equal(ka, kb), f"request {b} segment {s}: bucket contents differ"
-
-
-class Run:
-    """One context with a sparse layer 1 (layer 0 dense) filled from seeded keys, and the window history on the host."""
-
-    def __init__(self, B, Hq, Hkv, n, K, L, M, gen, seed, route="build", on_gpu=False, w0=NS + NL, impl=1):
-        from magicpig_b200.ops import Context
-        self.B, self.Hq, self.Hkv, self.n, self.K, self.L, self.M, self.G = B, Hq, Hkv, n, K, L, M, Hq // Hkv
-        self.hf = synth.make_hash_func(d, K, L, seed=seed)
-        self.g = torch.Generator().manual_seed(seed + 1)
-        if on_gpu:   # full-size keys are drawn on the device
-            gg = torch.Generator(device=DEV).manual_seed(seed + 2)
-            self.key = torch.randn((B, Hkv, n, d), generator=gg, device=DEV).bfloat16()
-            self.value = torch.randn((B, Hkv, n, d), generator=gg, device=DEV).bfloat16()
-            self.kn = self.key.norm(p=2, dim=-1).float()
-            self.avg = torch.zeros((B, Hkv, 1, d), dtype=torch.bfloat16)
-        else:
-            self.key, self.value, self.kn, self.avg = synth.make_kv(B, Hkv, n, d, seed=seed + 2, dist="gauss")
-        self.wk = torch.randn((B, Hkv, w0, d), generator=self.g).bfloat16()
-        self.wv = torch.randn((B, Hkv, w0, d), generator=self.g).bfloat16()
-        self.ctx = Context(K, L, 2, Hq, Hkv, d, B, M, NS, NL, gen, dense_layers=[0], device=DEV)
-        self.ctx.set_option("decode_impl", impl)
-        self.ctx.set_option("out_f32", 1)
-        self.ctx.set_hash_func(self.hf.to(DEV))
-        for b in range(B):
-            kb = self.key[b].to(DEV).contiguous()
-            self.ctx.attn_fill(1, b, kb, self.value[b].to(DEV).contiguous(), self.kn[b].to(DEV).contiguous())
-            codes = self.ctx.hash_keys(kb)
-            if route == "sorted":
-                sc, si = codes.sort()
-                self.ctx.lsh_fill(1, b, sc.contiguous(), si.int().contiguous())
-            else:
-                self.ctx.lsh_build(1, b, codes)
-            self.ctx.window_fill(1, b, self.avg[b].reshape(Hkv, d).to(DEV), self.wk[b].to(DEV), self.wv[b].to(DEV))
-        self.n_off = n   # offloaded keys per request
-
-    def token(self, q=None):
-        """One eager decode step (plan + layer-1 decode); the window history gains the centred key."""
-        B, Hq, Hkv = self.B, self.Hq, self.Hkv
-        if q is None:
-            q = torch.randn((B, Hq, 1, d), generator=self.g).bfloat16()
-        k_new = torch.randn((B, Hkv, 1, d), generator=self.g).bfloat16()
-        v_new = torch.randn((B, Hkv, 1, d), generator=self.g).bfloat16()
-        self.ctx.plan()
-        out = self.ctx.decode(1, q.to(DEV), k_new.to(DEV), v_new.to(DEV))
-        return q, k_new, v_new, out
-
-    def push(self, k_new, v_new):
-        self.wk = torch.cat([self.wk, k_new - self.avg], dim=2)
-        self.wv = torch.cat([self.wv, v_new], dim=2)
-
-    def spill(self, keep=NL):
-        """Spill through the context and apply the same semantics to the host history; returns the spilled rows."""
-        got = self.ctx.spill_window(keep)
-        w = self.wk.shape[2]
-        g = max(0, w - NS - keep)
-        assert got.tolist() == [g] * self.B
-        rows = (self.wk[:, :, NS:NS + g], self.wv[:, :, NS:NS + g])
-        if g:
-            self.wk = torch.cat([self.wk[:, :, :NS], self.wk[:, :, NS + g:]], dim=2)
-            self.wv = torch.cat([self.wv[:, :, :NS], self.wv[:, :, NS + g:]], dim=2)
-        self.n_off += g
-        return g, rows
-
-    def rebuild(self):
-        """A second context whose layer-1 tables are built by mpig_lsh_build over the keys the first one now stores."""
-        from magicpig_b200.ops import Context
-        k_st, _, _ = self.ctx.read_cache(1, True, False, False)
-        other = Context(self.K, self.L, 2, self.Hq, self.Hkv, d, self.B, self.M, NS, NL, 8, dense_layers=[0], device=DEV)
-        other.set_hash_func(self.hf.to(DEV))
-        for b in range(self.B):
-            other.lsh_build(1, b, self.ctx.hash_keys(k_st[b, :, : self.n_off].contiguous()))
-        return other
-
-    def check_decode(self, q, k_new, v_new, out_f32):
-        """Oracle on exactly the stored state (keys, norms, codes of the stored keys), n = all offloaded keys."""
-        n = self.n_off
-        k_st, v_st, kn_st = (x.cpu() for x in self.ctx.read_cache(1))
-        k_dev = k_st[:, :, :n].contiguous()
-        kcodes = torch.stack([self.ctx.hash_keys(k_dev[b].to(DEV)).cpu() for b in range(self.B)])
-        t = dict(B=self.B, Hq=self.Hq, Hkv=self.Hkv, d=d, K=self.K, L=self.L, n=n, M=self.M, hash_func=self.hf, kcodes=kcodes,
-                 key=k_dev, value=v_st[:, :, :n].contiguous(), key_norm=kn_st[:, :, :n].contiguous(), avg_k=self.avg)
-        _, nz_ref, _, o_exact = oracle_decode(t, q, k_new, v_new, self.wk, self.wv, self.G)
-        nnz, _ = self.ctx.last_probe()
-        assert torch.equal(nnz.cpu(), nz_ref)
-        assert_1e3_f32(out_f32, o_exact)
 
 
 def _segment_len(ctx):
-    o, _ = tables(ctx, 1)
+    o, _ = lsh_tables(ctx, 1)
     assert o.shape[3] >= 2, "shape must have two key segments"
     return int(o[0, 0, 0, 1, 0])
 
@@ -168,7 +42,7 @@ def test_tables_equal_rebuild(cuda_lib, route, B, Hq, Hkv, n, K, L, M, gen, step
     if straddle:
         seg_len = _segment_len(r.ctx)
         assert any(n_old < s * seg_len < n_old + g for s in range(1, M // seg_len + 1)), "spill should straddle a segment"
-    assert_tables_equal(r.ctx, r.rebuild(), 1, range(B))
+    assert_tables_equal(lsh_tables(r.ctx, 1), lsh_tables(r.rebuild(), 1), range(B))
     # store: spilled records are the window rows bit for bit, norms within one bf16 ulp of torch's norm of them
     k_st, v_st, kn_st = (x.cpu() for x in r.ctx.read_cache(1))
     assert torch.equal(k_st[:, :, n_old:n_old + g].view(torch.int16), sk.contiguous().view(torch.int16))
@@ -185,7 +59,7 @@ def test_tables_equal_rebuild(cuda_lib, route, B, Hq, Hkv, n, K, L, M, gen, step
         r.push(k, v)
     g2, _ = r.spill()
     assert g2 == 12
-    assert_tables_equal(r.ctx, r.rebuild(), 1, range(B))
+    assert_tables_equal(lsh_tables(r.ctx, 1), lsh_tables(r.rebuild(), 1), range(B))
 
 
 def test_tables_equal_rebuild_c2(cuda_lib):
@@ -199,7 +73,7 @@ def test_tables_equal_rebuild_c2(cuda_lib):
     assert r.wk.shape[2] == 324
     g, _ = r.spill()
     assert g == 256
-    assert_tables_equal(r.ctx, r.rebuild(), 1, [0])
+    assert_tables_equal(lsh_tables(r.ctx, 1), lsh_tables(r.rebuild(), 1), [0])
 
 
 def test_decode_after_spill(cuda_lib):
@@ -333,7 +207,7 @@ def test_long_generation_dropin(cuda_lib):
     srv.clear()
 
 def _snapshot(ctx):
-    o, i = tables(ctx, 1)
+    o, i = lsh_tables(ctx, 1)
     k, v, kn = ctx.read_cache(1)
     return [o, i, k.view(torch.int16), v.view(torch.int16), kn]
 

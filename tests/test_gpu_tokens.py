@@ -7,79 +7,15 @@ A step of T tokens must equal T single-token steps on the same inputs:
   * a rewind leaves the state of a twin that decoded only the accepted tokens; a captured plan -> layers -> rewind replays with
     changing drops; multi-token steps run into a spill; every refusal leaves the state unchanged.
 """
-import numpy as np
 import pytest
 import torch
 
 from magicpig_b200 import _native as N
 from magicpig_b200 import synth
-from tests.test_gpu_parity import _Cfg, assert_1e3_f32, oracle_decode
-from tests.test_gpu_spill import Run, assert_tables_equal
+from tests.support.fp64 import assert_1e3_f32, assert_rounded_half_up, oracle_decode, rel_max
+from tests.support.library import DEV, NL, NS, Run, Twins, _Cfg, assert_tables_equal, d, lsh_tables
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-d, NS, NL = 128, 4, 64
-
-
-def bf16_half_up(x: torch.Tensor) -> torch.Tensor:
-    """The ABI's fp32 -> bf16 rounding (add 2^15, truncate), as bit patterns."""
-    u = x.float().cpu().numpy().view(np.uint32).astype(np.uint64)
-    return torch.from_numpy((((u + 0x8000) >> 16) & 0xFFFF).astype(np.int32))
-
-
-def rel_max(a, b):
-    return float((a.double() - b.double()).abs().max() / b.double().abs().max().clamp_min(1e-30))
-
-
-class Twins:
-    """Two identically filled contexts (sparse layer 1, dense layer 0): `tok` runs T-token steps, `seq` single-token steps.
-    Request b's window starts with NS + NL - 5*b rows."""
-
-    def __init__(self, B, Hq, Hkv, n, K, L, T, seed, gen=32, P_dense=300, on_gpu=False):
-        from magicpig_b200.ops import Context
-        self.B, self.Hq, self.Hkv, self.n, self.K, self.L, self.G = B, Hq, Hkv, n, K, L, Hq // Hkv
-        self.M = max(n, P_dense) + 256
-        self.hf = synth.make_hash_func(d, K, L, seed=seed)
-        self.g = torch.Generator().manual_seed(seed + 1)
-        if on_gpu:
-            gg = torch.Generator(device=DEV).manual_seed(seed + 2)
-            self.key = torch.randn((B, Hkv, n, d), generator=gg, device=DEV).bfloat16()
-            self.value = torch.randn((B, Hkv, n, d), generator=gg, device=DEV).bfloat16()
-            self.kn = self.key.norm(p=2, dim=-1).float()
-            self.avg = torch.zeros((B, Hkv, 1, d), dtype=torch.bfloat16)
-            self.kcodes = None
-        else:
-            qd = synth.make_query(B, Hq, d, seed=seed + 3).reshape(B, Hkv, self.G, d)[:, :, 0].float()
-            # K10 L150 samples few keys of i.i.d. Gaussian data: keys clustered around query directions, as test_fused_decode
-            dist = "clustered" if K >= 10 else "gauss"
-            self.key, self.value, self.kn, self.avg = synth.make_kv(B, Hkv, n, d, seed=seed + 2, dist=dist, q_dirs=qd)
-            self.kcodes = synth.hash_keys(self.key, self.hf, K, L)
-        self.win = [(torch.randn((Hkv, NS + NL - 5 * b, d), generator=self.g).bfloat16(),
-                     torch.randn((Hkv, NS + NL - 5 * b, d), generator=self.g).bfloat16()) for b in range(B)]
-        self.dk = torch.randn((B, P_dense, Hkv, d), generator=self.g).bfloat16()
-        self.dv = torch.randn((B, P_dense, Hkv, d), generator=self.g).bfloat16()
-        self.ctxs = []
-        for tmax in (T, 1):
-            ctx = Context(K, L, 2, Hq, Hkv, d, B, self.M, NS, NL, gen, dense_layers=[0], alloc_dense_kv=True, device=DEV,
-                          max_query_tokens=tmax)
-            ctx.set_option("save_mask", 1)
-            ctx.set_option("out_f32", 1)
-            ctx.set_hash_func(self.hf.to(DEV))
-            for b in range(B):
-                kb = self.key[b].to(DEV).contiguous()
-                ctx.attn_fill(1, b, kb, self.value[b].to(DEV).contiguous(), self.kn[b].to(DEV).contiguous())
-                ctx.lsh_build(1, b, self.kcodes[b].to(DEV) if self.kcodes is not None else ctx.hash_keys(kb))
-                ctx.window_fill(1, b, self.avg[b].reshape(Hkv, d).to(DEV), self.win[b][0].to(DEV), self.win[b][1].to(DEV))
-                ctx.dense_fill(0, b, self.dk[b].to(DEV), self.dv[b].to(DEV), P_dense)
-            self.ctxs.append(ctx)
-        self.tok, self.seq = self.ctxs
-
-    def inputs(self, T):
-        B, Hq, Hkv = self.B, self.Hq, self.Hkv
-        q = torch.randn((B, T, Hq, d), generator=self.g).bfloat16()
-        k = torch.randn((B, T, Hkv, d), generator=self.g).bfloat16()
-        v = torch.randn((B, T, Hkv, d), generator=self.g).bfloat16()
-        return q, k, v
 
 
 def run_sparse_step(tw, T, q, k, v):
@@ -114,8 +50,7 @@ def assert_same_as_sequential(a, s):
                 n_ = int(a["nnz"][b, t, h])
                 assert torch.equal(a["res"][b, t, h, :n_], s["res"][b, t, h, :n_]), (b, t, h)
     assert rel_max(a["o32"], s["o32"]) <= 1e-5
-    # the bf16 output is the fp32 output rounded once
-    assert torch.equal(a["out"].view(torch.int16).int() & 0xFFFF, bf16_half_up(a["o32"]).reshape(a["out"].shape))
+    assert_rounded_half_up(a["out"], a["o32"], "T-token step")
 
 
 @pytest.mark.parametrize("T", [2, 3, 8])
@@ -176,7 +111,7 @@ def test_dense_tokens(cuda_lib, B, Hq, Hkv, P, T):
         tw.seq.dense_decode(0, q[:, t].contiguous().to(DEV), k[:, t].contiguous().to(DEV), v[:, t].contiguous().to(DEV))
         seq.append(tw.seq.last_out_f32().cpu().reshape(B, Hq, d))
     assert rel_max(o32, torch.stack(seq, dim=1)) <= 1e-5
-    assert torch.equal(out.view(torch.int16).int() & 0xFFFF, bf16_half_up(o32).reshape(out.shape))
+    assert_rounded_half_up(out, o32, "dense T-token step")
     # fp64 causal restatement
     kk = torch.cat([tw.dk, k], dim=1).double()   # (B, P+T, Hkv, d)
     vv = torch.cat([tw.dv, v], dim=1).double()
@@ -327,7 +262,7 @@ def test_tokens_then_spill(cuda_lib):
         used += 4 - drop
     g, _ = r.spill()
     assert g == used
-    assert_tables_equal(r.ctx, r.rebuild(), 1, range(B))
+    assert_tables_equal(lsh_tables(r.ctx, 1), lsh_tables(r.rebuild(), 1), range(B))
     q, k, v, o32, nnz = step(0)
     for t in range(4):
         qt, kt, vt = q[:, t][:, :, None], k[:, t][:, :, None], v[:, t][:, :, None]

@@ -14,9 +14,8 @@ import torch
 
 from magicpig_b200 import _native as N
 from magicpig_b200 import synth
-from tests.test_gpu_parity import _Cfg, assert_1e3_f32, oracle_decode
-from tests.test_gpu_spill import Run, assert_tables_equal
-from tests.test_gpu_tokens import Twins, bf16_half_up, rel_max
+from tests.support.fp64 import assert_1e3_f32, assert_rounded_half_up, oracle_decode, rel_max
+from tests.support.library import Run, Twins, _Cfg, assert_tables_equal, lsh_tables
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -133,7 +132,7 @@ def test_sparse_tree_matches_paths(cuda_lib, B, Hq, Hkv, n, K, L, T, kreg):
     out, a = tree_step(tw.tok, pars, q, k, v)[1]
     s = path_chains(tw.seq, pars, q, k, v)[1]
     assert_sparse_equal(a, s)
-    assert torch.equal(out.view(torch.int16).int() & 0xFFFF, bf16_half_up(a["o32"]).reshape(out.shape))
+    assert_rounded_half_up(out, a["o32"], "tree step")
     if n > 5000 or K >= 10:
         return   # (as in test_sparse_tokens_match_sequential: the chains themselves are checked against the oracle there)
     for b in range(B):
@@ -161,7 +160,7 @@ def test_dense_tree(cuda_lib, B, Hq, Hkv, P, T):
     out, a = tree_step(tw.tok, pars, q, k, v, layers=(0,))[0]
     s = path_chains(tw.seq, pars, q, k, v, layers=(0,))[0]
     assert rel_max(a["o32"], s["o32"]) <= 1e-5
-    assert torch.equal(out.view(torch.int16).int() & 0xFFFF, bf16_half_up(a["o32"]).reshape(out.shape))
+    assert_rounded_half_up(out, a["o32"], "tree step")
     for b in range(B):
         for t in range(T):
             vis = root_path(pars[b], t)
@@ -337,7 +336,7 @@ def test_tree_steps_then_spill(cuda_lib):
     k_st, v_st, _ = (x.cpu() for x in r.ctx.read_cache(1))
     assert torch.equal(k_st[:, :, n_old:n_old + g], rk)
     assert torch.equal(v_st[:, :, n_old:n_old + g], rv)
-    assert_tables_equal(r.ctx, r.rebuild(), 1, range(B))
+    assert_tables_equal(lsh_tables(r.ctx, 1), lsh_tables(r.rebuild(), 1), range(B))
     assert r.ctx.error_flags() == 0
 
 

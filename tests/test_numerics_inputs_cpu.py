@@ -10,8 +10,8 @@ import math
 import pytest
 import torch
 
-from tests.test_gpu_numerics import (BAR, TREE, check_case, check_dense, make_case, make_dense, merge2,
-                                     restate, softmax_state)
+from tests.support.fp64 import BAR, merge2, restate, softmax_state
+from tests.support.sparse_cases import TREE, check_case, check_dense, cpu_codes, make_case, make_dense
 
 REGIMES = [("R1", "last"), ("R2", "last"), ("R3", "last"), ("R4", "first"), ("R4", "last"), ("R5", "last")]
 
@@ -52,6 +52,6 @@ def test_restatement_pieces():
     assert not torch.allclose(merge2(oa, la, ob, lb, natural=True), o, rtol=0, atol=1e-9)
     # clamp: a key exactly along q with a norm rounded down gets the weight of cos = 1, not NaN
     c = make_case("R5", 1, 4, 1, 400, 6, 20, seed=1)
-    out, _, _ = restate(c)
+    out, _, _ = restate(c, cpu_codes(c))
     assert torch.isfinite(out).all()
     assert BAR == 1e-3

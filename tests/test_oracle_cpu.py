@@ -17,14 +17,11 @@ import torch
 import oracle
 from oracle import ref_loader
 from magicpig_b200 import synth, _native
+from tests.support.fp64 import bf16_from_u16
 from tests.golden.make_golden import (LIVE_PROBE_CASES, checksum, live_attention_inputs, live_probe_inputs, reference_attention,
                                       reference_probe)
 
 GOLD = os.path.join(os.path.dirname(__file__), "golden")
-
-
-def bf16_from_u16(a: np.ndarray) -> torch.Tensor:
-    return torch.from_numpy(a.view(np.int16).copy()).view(torch.bfloat16)
 
 
 def load_small():

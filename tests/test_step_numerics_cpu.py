@@ -13,9 +13,10 @@ import pytest
 import torch
 
 from magicpig_b200.llama_runner import rope_tables
-from tests.test_gpu_step_numerics import (Fp64Llama, U, assert_rule, bf16_rne, gamma, gemv_ref, hull_ok, neighbours,
-                                          prompt_kv, rmsnorm_ref, rope_cands, rule_ok, run_reference, run_rel_err,
-                                          ss_roundings_add_rmsnorm, ss_roundings_prologue, swiglu_cands)
+from tests.support.fp64 import bf16_rne
+from tests.support.step_rule import (Fp64Llama, U, assert_rule, gamma, gemv_ref, hull_ok, neighbours, prompt_kv, rmsnorm_ref,
+                                     rope_cands, rule_ok, run_reference, run_rel_err, ss_roundings_add_rmsnorm,
+                                     ss_roundings_prologue, swiglu_cands)
 
 F32 = np.float32
 
