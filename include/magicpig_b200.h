@@ -96,7 +96,7 @@ typedef struct mpig_config {
      *   mpig_fork_request, so its result equals that of an exclusive slot holding those keys (codes, nnz and index sets equal after
      *   renumbering, fp32 outputs up to summation order).  The capacity is shared (prompt + all private keys of a slot <=
      *   max_length).  A fill of a slot (mpig_attn_fill, mpig_lsh_build / mpig_lsh_fill) and mpig_clear drop its private keys;
-     *   private keys nobody sees any more keep their rows until then.  mpig_lsh_collision_counts stays unfiltered.
+     *   private keys nobody sees any more keep their rows until then, or until mpig_compact_context reclaims them.  mpig_lsh_collision_counts stays unfiltered.
      *   mpig_get_info("shared_spill") reports the flag. */
     int32_t reserved[8];
 } mpig_config;
@@ -270,6 +270,24 @@ int mpig_plan(mpig_ctx *ctx, void *stream);
  * shared spill mode), the sparse layers of a slot disagree on its private key count (shared spill mode, after a partial
  * refill), or no hash_func set.  On these errors nothing is modified. */
 int mpig_spill_window(mpig_ctx *ctx, int keep, int32_t *spilled_out, void *stream);
+/* Shared spill mode (reserved[3]): reclaim the dead private keys of context slot `slot` (-1: every slot).  A private key is
+ * dead when no request sees it any more (vis[slot][p] == 0: its owner was forked over, reordered over, rebound or retired).
+ * Every live private key keeps its time order and moves to the lowest free offset: live key j (ascending offsets) becomes
+ * store index private_lo + j of every sparse layer, its record and key norm with it, vis[slot][j] takes its word (the words
+ * past the live count become 0), the slot's key count drops by the number reclaimed, and the slot's tables become what a
+ * build over the compacted keys would make (the live keys are rehashed with the spill's kernel, so their codes are the same).
+ * Every request then samples exactly what it sampled before, up to that renumbering.  Windows, lengths, avg_k, dense layers
+ * and the pending step are untouched; no array moves, so a step captured before the call stays valid after it.  reclaimed_out
+ * int32 [C] (host, may be NULL) receives the keys removed per slot.  Without shared spill there are no private keys: zeros and
+ * nothing launched.  Synchronises `stream`; not capturable.  Allocates scratch for the live keys of one layer (live x Hkv x
+ * (2 d + 2 L) bytes) for the call.
+ * MPIG_EINVAL: slot outside [-1, C); MPIG_ESTATE: the sparse layers of a slot disagree on its private key count (after a partial
+ * refill), or no hash_func set; MPIG_ENOMEM: the scratch allocation failed.  On these errors nothing is modified. */
+int mpig_compact_context(mpig_ctx *ctx, int slot, int32_t *reclaimed_out, void *stream);
+/* Diagnostic accessor (the tests and scripts/compact_bench.py read the map through it; decoding never needs it).  Shared spill
+ * mode: copy the visibility map (uint32 [C][max_length], bit b of word [c][p] = request b sees private key p of slot c) to the
+ * device buffer vis_out.  MPIG_ESTATE without shared spill. */
+int mpig_read_visibility(mpig_ctx *ctx, uint32_t *vis_out, void *stream);
 /* Fused sparse-layer decode (attnserver.py:261-312): centre + append the new key/value to the
  * window, SimHash, probe, gather attention over window + sample with the LSE merge folded in -- one kernel launch.
  * query bf16 (B, Hq, d); key/value bf16 (B, Hkv, d); out bf16 (B, Hq*d).

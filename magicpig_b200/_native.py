@@ -71,6 +71,8 @@ _SIGNATURES = {
     "mpig_window_fill": (_i, [_vp, _i, _i, _vp, _vp, _vp, _i, _vp]),
     "mpig_plan": (_i, [_vp, _vp]),
     "mpig_spill_window": (_i, [_vp, _i, ctypes.POINTER(ctypes.c_int32), _vp]),
+    "mpig_compact_context": (_i, [_vp, _i, ctypes.POINTER(ctypes.c_int32), _vp]),
+    "mpig_read_visibility": (_i, [_vp, _vp, _vp]),
     "mpig_decode": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp]),
     "mpig_decode_timed": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp]),
     "mpig_timing_collect": (_i, [_vp, ctypes.POINTER(ctypes.c_float), _i, ctypes.POINTER(_i)]),

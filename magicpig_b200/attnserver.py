@@ -86,7 +86,8 @@ class LSHSparseAttnServer:
                     rows it adds after its prompt (needs num_contexts < batch_size); None = a full dense cache per request.
         shared_spill  requests that share a context may spill_window() into it (needs num_contexts < batch_size <= 32): each
                     spilled token is private to the request that spilled it and to requests later forked from it.  Size max_length
-                    for the prompt plus every request's spilled tokens.
+                    for the prompt plus every request's spilled tokens, or call compact() after spills to free the
+                    tokens no request sees any more and size it for the live ones.
         max_chunk_tokens  largest T of a chunk step (plan_chunk(T): T new prompt tokens per request, attended exactly); 0 = none.
         """
         self.K, self.L = K, L
@@ -270,6 +271,17 @@ class LSHSparseAttnServer:
         may spill only with shared_spill=True; their spilled tokens then go to the shared context but each request samples only
         its own (and those inherited through fork())."""
         return self.ctx.spill_window(keep)
+
+    def compact(self, context: Optional[int] = None) -> torch.Tensor:
+        """Not in the reference.  With shared_spill=True, frees the spilled tokens of a context (None: every context) that no
+        request sees any more: those of a request that fork() overwrote, that a beam step's reorder dropped, that bind() moved
+        away, or that was retired.  Every request keeps sampling exactly the tokens it sampled before.  Call it between tokens
+        when spill_window() would exceed max_length (so max_length needs to hold the prompt plus the live spilled tokens only),
+        for example after each spill of a beam search or after re-forking questions from one prompt.  To retire a finished
+        request, bind() it to its own context first: its spilled tokens then die.  It synchronises, so it is never part of a
+        captured step, but a step captured before it stays valid.  Returns the tokens freed per context, int32
+        (num_contexts,) on the host (zeros without shared_spill)."""
+        return self.ctx.compact(context)
 
     def decode(self, query_states: torch.Tensor, key_states: torch.Tensor, value_states: torch.Tensor, layer_idx: int):
         """attnserver.py:228-312.  q (B,Hq,1,d), k/v (B,Hkv,1,d) -> (B, 1, Hq*d).  In a verification step of T tokens (plan(T)):

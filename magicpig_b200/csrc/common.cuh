@@ -498,6 +498,9 @@ int launch_pack_nhd(mpig_ctx *ctx, const void *k, const void *v, uint8_t *rec, i
 // are device arrays [C].
 int launch_table_merge(mpig_ctx *ctx, int layer, const int16_t *codes, const int32_t *g, const int32_t *pre, const int32_t *n_old,
                        cudaStream_t s);
+// a compaction (store.cu): drop the keys >= lo[c] from slot c's tables of `layer`, whose keys were [0, hi[c]) (tables.cu);
+// lo / hi are device arrays [C], and lo[c] == hi[c] leaves slot c untouched
+int launch_table_truncate(mpig_ctx *ctx, int layer, const int32_t *lo, const int32_t *hi, cudaStream_t s);
 // shared spill mode: a request's place in the visibility map changes (store.cu).  src >= 0: dst sees exactly the private keys src
 // sees (a fork); src < 0: dst sees no private key (a bind).  Every slot's map is rewritten.
 int launch_vis_rebind(mpig_ctx *ctx, int src, int dst, cudaStream_t s);

@@ -5,8 +5,11 @@
 //   get_key_cache / get_value_cache / get_key_norm :1213-1234 -> unpack_records_kernel
 //   attention_wrapper                    :629-745   -> mpig_attention_wrapper (launches attend_mma_kernel, attend_mma.cu)
 // and the dense layers' prefill copy (attnserver.py:116-120) -> pack_records_nhd_kernel; mpig_spill_window (no reference
-// equivalent: generated window rows -> store + tables) -> spill_move_kernel, mpig_hash_keys, table_merge_kernel (tables.cu).
+// equivalent: generated window rows -> store + tables) -> spill_move_kernel, mpig_hash_keys, table_merge_kernel (tables.cu);
+// mpig_compact_context (dead private keys out of a shared context) -> compact_live_kernel, compact_move_kernel,
+// compact_stage_kernel, mpig_hash_keys, table_truncate_kernel and table_merge_kernel (tables.cu).
 #include "attend_common.cuh"
+#include "probe_common.cuh"
 
 namespace mpig {
 
@@ -158,6 +161,120 @@ int reset_private(mpig_ctx *ctx, int layer, int request, int n, cudaStream_t s) 
     return MPIG_OK;
 }
 
+// ---------------------------------------------------------------------------------------------
+// Compaction (mpig_compact_context, shared spill mode): the slot's private keys that no request sees any more are dropped, the
+// live ones keep their time order and move down to the offsets 0 .. live - 1.
+// ---------------------------------------------------------------------------------------------
+// Live list: one CTA per slot.  The ascending offsets p in [0, priv[c]) with vis[c][p] != 0 -> list[list_pre[c] ...], their
+// count -> live[c].
+__global__ void __launch_bounds__(1024) compact_live_kernel(const uint32_t *__restrict__ vis, int M, const int32_t *__restrict__ priv,
+                                                            const int32_t *__restrict__ list_pre, int32_t *__restrict__ list,
+                                                            int32_t *__restrict__ live) {
+    __shared__ int wsum[40];
+    const int c = blockIdx.x, n = priv[c];
+    int32_t *out = list + list_pre[c];
+    int base = 0;
+    for (int p0 = 0; p0 < n; p0 += 1024) {
+        const int p = p0 + (int)threadIdx.x;
+        const int f = p < n && vis[(size_t)c * M + p] != 0u;
+        int tot;
+        const int ex = block_exclusive_scan(f, wsum, &tot);
+        if (f) out[base + ex] = p;
+        base += tot;
+    }
+    if (threadIdx.x == 0) live[c] = base;
+}
+
+struct CompactLayer {
+    uint4 *kv;
+    float *kn;
+    const int32_t *plo;   // [C] the layer's private starts
+};
+
+// Record move, in place: one CTA per (kv-head, slot, sparse layer).  Live key j of a slot with work[c] moves from store index
+// plo + list[j] to plo + j, record and key norm.  Sources ascend and every destination is at or below its source, so the rows
+// are moved in ascending chunks, each chunk read completely before any of it is written: a write lands only on a row already
+// read.  The CTA (0, c, 0) then moves the slot's vis words the same way and zeroes the words past the live count.
+__global__ void __launch_bounds__(1024) compact_move_kernel(const CompactLayer *__restrict__ layers, const int32_t *__restrict__ list,
+                                                            const int32_t *__restrict__ list_pre, const int32_t *__restrict__ live,
+                                                            const int32_t *__restrict__ work, const int32_t *__restrict__ priv,
+                                                            uint32_t *vis, int Hkv, int M) {
+    constexpr int T = 1024, UN = 4, ROWS = T * UN / 32;   // 128 records (64 KB) per chunk
+    const int gi = blockIdx.x, c = blockIdx.y, tid = threadIdx.x;
+    if (!work[c]) return;
+    const CompactLayer ly = layers[blockIdx.z];
+    const int n = live[c], plo = ly.plo[c];
+    const int32_t *src = list + list_pre[c];
+    const size_t sg = (size_t)c * Hkv + gi;
+    uint4 *r = ly.kv + (sg * M + plo) * 32;
+    float *kns = ly.kn + sg * M + plo;
+    for (int j0 = 0; j0 < n; j0 += ROWS) {
+        uint4 v[UN];
+        float kv_n = 0.f;
+#pragma unroll
+        for (int u = 0; u < UN; ++u) {
+            const int j = j0 + u * (T / 32) + (tid >> 5);
+            if (j < n) v[u] = r[(size_t)src[j] * 32 + (tid & 31)];
+        }
+        if (tid < ROWS && j0 + tid < n) kv_n = kns[src[j0 + tid]];
+        __syncthreads();
+#pragma unroll
+        for (int u = 0; u < UN; ++u) {
+            const int j = j0 + u * (T / 32) + (tid >> 5);
+            if (j < n) r[(size_t)j * 32 + (tid & 31)] = v[u];
+        }
+        if (tid < ROWS && j0 + tid < n) kns[j0 + tid] = kv_n;
+        __syncthreads();
+    }
+    if (gi != 0 || blockIdx.z != 0) return;
+    uint32_t *vs = vis + (size_t)c * M;
+    for (int j0 = 0; j0 < n; j0 += T) {
+        const int j = j0 + tid;
+        const uint32_t w = j < n ? vs[src[j]] : 0u;
+        __syncthreads();
+        if (j < n) vs[j] = w;
+        __syncthreads();
+    }
+    for (int j = n + tid; j < priv[c]; j += T) vs[j] = 0u;
+}
+
+// The key halves of a slot's compacted live records [plo, plo + live) of one sparse layer -> its staging block for the key
+// hash, (Hkv, live, d) bf16 at row spre[c] * Hkv, the layout the spill stages in.  grid (x, C).
+__global__ void compact_stage_kernel(const uint4 *__restrict__ rec, const int32_t *__restrict__ plo, const int32_t *__restrict__ live,
+                                     const int32_t *__restrict__ work, const int32_t *__restrict__ spre, uint4 *__restrict__ stage,
+                                     int Hkv, int M) {
+    const int c = blockIdx.y;
+    if (!work[c]) return;
+    const int n = live[c], p = plo[c];
+    const size_t total = (size_t)Hkv * n * 16;
+    uint4 *st = stage + (size_t)spre[c] * Hkv * 16;
+    for (size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (size_t)gridDim.x * blockDim.x) {
+        const size_t row = t >> 4;   // gi * n + j
+        const int gi = (int)(row / n), j = (int)(row % n);
+        st[t] = rec[(((size_t)c * Hkv + gi) * M + p + j) * 32 + (t & 15)];
+    }
+}
+
+// shared spill mode: private keys have the same offsets in every sparse layer only while the layers agree on a slot's private
+// count.  priv[c] = that count for every slot with want[c] (0 for the others); MPIG_ESTATE when two sparse layers disagree.
+static int private_counts(const mpig_ctx *ctx, const std::vector<char> &want, std::vector<int> &priv, const char *who) {
+    const int C = ctx->C;
+    priv.assign(C, -1);
+    for (int l = 0; l < ctx->cfg.num_layers; ++l) {
+        if (!ctx->layers[l].sparse) continue;
+        for (int c = 0; c < C; ++c) {
+            if (!want[c]) continue;
+            const int pc = ctx->n_off[l][c] - ctx->h_private_lo[l][c];
+            MPIG_REQUIRE(priv[c] < 0 || priv[c] == pc, MPIG_ESTATE,
+                         "%s: context slot %d holds %d private keys in layer %d but %d in an earlier sparse layer "
+                         "(a partial refill?); refill every sparse layer of the slot", who, c, pc, l, priv[c]);
+            priv[c] = pc;
+        }
+    }
+    for (int c = 0; c < C; ++c) priv[c] = std::max(priv[c], 0);
+    return MPIG_OK;
+}
+
 int launch_pack_nhd(mpig_ctx *ctx, const void *k, const void *v, uint8_t *rec, int Hkv, int n, int rows_cap, cudaStream_t s) {
     const size_t total = (size_t)Hkv * n * 32;
     const int blocks = (int)std::min<size_t>((total + 255) / 256, (size_t)ctx->num_sms * 16);
@@ -276,20 +393,12 @@ int mpig_spill_window(mpig_ctx *ctx, int keep, int32_t *spilled_out, void *strea
         tot += meta[o_sg + c];
     }
     if (ctx->shared_spill) {
-        // private keys have the same offsets in every sparse layer only while the layers agree on the slot's private count
-        std::vector<int> priv(C, -1);
-        for (int l = 0; l < nl; ++l) {
-            if (!ctx->layers[l].sparse) continue;
-            for (int c = 0; c < C; ++c) {
-                if (meta[o_sg + c] == 0) continue;
-                const int pc = ctx->n_off[l][c] - ctx->h_private_lo[l][c];
-                MPIG_REQUIRE(priv[c] < 0 || priv[c] == pc, MPIG_ESTATE,
-                             "mpig_spill_window: context slot %d holds %d private keys in layer %d but %d in an earlier sparse layer "
-                             "(a partial refill?); refill every sparse layer of the slot", c, pc, l, priv[c]);
-                priv[c] = pc;
-            }
-        }
-        for (int c = 0; c < C; ++c) meta[o_priv + c] = std::max(priv[c], 0);
+        std::vector<char> want(C);
+        for (int c = 0; c < C; ++c) want[c] = meta[o_sg + c] > 0;
+        std::vector<int> priv;
+        rc = private_counts(ctx, want, priv, "mpig_spill_window");
+        if (rc) return rc;
+        for (int c = 0; c < C; ++c) meta[o_priv + c] = priv[c];
     } else {
         // a shared slot's store and tables are every bound request's context: spilling one request's generated tokens into them
         // would put those tokens into the others' samples
@@ -366,6 +475,150 @@ int mpig_spill_window(mpig_ctx *ctx, int keep, int32_t *spilled_out, void *strea
     }
     if (spilled_out)
         for (int b = 0; b < B; ++b) spilled_out[b] = meta[b];
+    return MPIG_OK;
+}
+
+int mpig_read_visibility(mpig_ctx *ctx, uint32_t *vis_out, void *stream) {
+    mpig::DeviceGuard _dg(ctx);  // run on the context's device whatever the caller's current device is
+    MPIG_REQUIRE(ctx && vis_out, MPIG_EINVAL, "mpig_read_visibility: null argument");
+    MPIG_REQUIRE(ctx->shared_spill, MPIG_ESTATE, "mpig_read_visibility: the context has no shared spill (reserved[3])");
+    MPIG_CUDA(cudaMemcpyAsync(vis_out, ctx->vis, (size_t)ctx->C * ctx->cfg.max_length * sizeof(uint32_t), cudaMemcpyDeviceToDevice,
+                              as_stream(stream)));
+    return MPIG_OK;
+}
+
+// scratch of one compaction, freed on every return
+struct CompactScratch {
+    std::vector<void *> bufs;
+    ~CompactScratch() {
+        for (void *p : bufs) (void)cudaFree(p);
+    }
+    int alloc(size_t bytes, void **p) {
+        cudaError_t e = cudaMalloc(p, std::max<size_t>(bytes, 16));
+        if (e != cudaSuccess) {
+            (void)cudaGetLastError();
+            set_error("mpig_compact_context: cudaMalloc(%zu bytes) failed: %s", bytes, cudaGetErrorString(e));
+            return MPIG_ENOMEM;
+        }
+        bufs.push_back(*p);
+        return MPIG_OK;
+    }
+};
+
+int mpig_compact_context(mpig_ctx *ctx, int slot, int32_t *reclaimed_out, void *stream) {
+    mpig::DeviceGuard _dg(ctx);  // run on the context's device whatever the caller's current device is
+    MPIG_REQUIRE(ctx, MPIG_EINVAL, "mpig_compact_context: null context");
+    const int C = ctx->C, M = ctx->cfg.max_length, nl = ctx->cfg.num_layers;
+    const int Hkv = ctx->cfg.num_key_value_heads, L = ctx->cfg.L, d = ctx->cfg.head_dim;
+    MPIG_REQUIRE(slot >= -1 && slot < C, MPIG_EINVAL, "mpig_compact_context: slot %d outside [-1, %d)", slot, C);
+    if (reclaimed_out)
+        for (int c = 0; c < C; ++c) reclaimed_out[c] = 0;
+    if (!ctx->shared_spill) return MPIG_OK;   // no private keys
+    MPIG_REQUIRE(ctx->hash_func_set, MPIG_ESTATE, "mpig_compact_context before mpig_set_hash_func: the live keys cannot be rehashed");
+    cudaStream_t s = as_stream(stream);
+    std::vector<char> want(C, 0);
+    for (int c = 0; c < C; ++c) want[c] = slot < 0 || c == slot;
+    std::vector<int> priv;
+    int rc = private_counts(ctx, want, priv, "mpig_compact_context");
+    if (rc) return rc;
+    std::vector<int> sparse;
+    for (int l = 0; l < nl; ++l)
+        if (ctx->layers[l].sparse) sparse.push_back(l);
+    const int nsl = (int)sparse.size();
+    // meta = list_pre[C] | priv[C] | live[C] | work[C] | spre[C] | g[C] (live where work, else 0: the keys merged back) |
+    // lo[nsl][C] | hi[nsl][C], then the layer table
+    const size_t o_priv = C, o_live = 2 * (size_t)C, o_work = 3 * (size_t)C, o_spre = 4 * (size_t)C, o_g = 5 * (size_t)C,
+                 o_lo = 6 * (size_t)C, o_hi = o_lo + (size_t)nsl * C;
+    std::vector<int32_t> meta(o_hi + (size_t)nsl * C, 0);
+    int tot_priv = 0;
+    for (int c = 0; c < C; ++c) {
+        meta[c] = tot_priv;
+        meta[o_priv + c] = priv[c];
+        tot_priv += priv[c];
+    }
+    if (tot_priv == 0) return MPIG_OK;
+    const size_t meta_bytes = (meta.size() * sizeof(int32_t) + 255) & ~(size_t)255;
+    const size_t table_bytes = (nsl * sizeof(CompactLayer) + 255) & ~(size_t)255;
+    CompactScratch scratch;
+    uint8_t *small = nullptr;
+    rc = scratch.alloc(meta_bytes + table_bytes + (size_t)tot_priv * sizeof(int32_t), (void **)&small);
+    if (rc) return rc;
+    int32_t *d_meta = reinterpret_cast<int32_t *>(small);
+    CompactLayer *d_layers = reinterpret_cast<CompactLayer *>(small + meta_bytes);
+    int32_t *d_list = reinterpret_cast<int32_t *>(small + meta_bytes + table_bytes);
+    // 1. the live lists and counts (nothing is written to the context before the scratch below is allocated)
+    MPIG_CUDA(cudaMemcpyAsync(d_meta, meta.data(), 2 * C * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    compact_live_kernel<<<C, 1024, 0, s>>>(ctx->vis, M, d_meta + o_priv, d_meta, d_list, d_meta + o_live);
+    MPIG_LAUNCH_CHECK(ctx);
+    MPIG_CUDA(cudaMemcpyAsync(meta.data() + o_live, d_meta + o_live, C * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    MPIG_CUDA(cudaStreamSynchronize(s));
+    int tot_live = 0, nwork = 0;
+    for (int c = 0; c < C; ++c) {
+        const int live = meta[o_live + c];
+        meta[o_work + c] = want[c] && live < priv[c];
+        meta[o_spre + c] = tot_live;
+        if (!meta[o_work + c]) continue;
+        ++nwork;
+        meta[o_g + c] = live;
+        tot_live += live;
+    }
+    if (nwork == 0) return MPIG_OK;
+    std::vector<CompactLayer> table(nsl);
+    for (int i = 0; i < nsl; ++i) {
+        const int l = sparse[i];
+        LayerStore &ls = ctx->layers[l];
+        table[i] = {reinterpret_cast<uint4 *>(ls.kv), ls.kn, ctx->private_lo + (size_t)l * C};
+        for (int c = 0; c < C; ++c) {
+            const int lo = ctx->h_private_lo[l][c];
+            meta[o_lo + (size_t)i * C + c] = lo;
+            meta[o_hi + (size_t)i * C + c] = meta[o_work + c] ? ctx->n_off[l][c] : lo;   // lo == hi: the truncate leaves c alone
+        }
+    }
+    // 2. hash scratch sized to the live keys of one layer: their key halves (Hkv, live, d) bf16 and codes (Hkv, L, live) int16
+    const size_t key_bytes = ((size_t)tot_live * Hkv * d * sizeof(__nv_bfloat16) + 255) & ~(size_t)255;
+    uint8_t *big = nullptr;
+    rc = scratch.alloc(key_bytes + (size_t)tot_live * Hkv * L * sizeof(int16_t), (void **)&big);
+    if (rc) return rc;
+    __nv_bfloat16 *keys = reinterpret_cast<__nv_bfloat16 *>(big);
+    int16_t *codes = reinterpret_cast<int16_t *>(big + key_bytes);
+    MPIG_CUDA(cudaMemcpyAsync(d_meta, meta.data(), meta.size() * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    MPIG_CUDA(cudaMemcpyAsync(d_layers, table.data(), nsl * sizeof(CompactLayer), cudaMemcpyHostToDevice, s));
+    // 3. records, norms and the visibility map, every sparse layer in one launch
+    compact_move_kernel<<<dim3(Hkv, C, nsl), 1024, 0, s>>>(d_layers, d_list, d_meta, d_meta + o_live, d_meta + o_work, d_meta + o_priv,
+                                                           ctx->vis, Hkv, M);
+    MPIG_LAUNCH_CHECK(ctx);
+    // 4. per sparse layer: stage and hash the live keys, drop every private item from the tables, merge the live keys back
+    for (int i = 0; i < nsl; ++i) {
+        const int l = sparse[i];
+        const int32_t *lo = d_meta + o_lo + (size_t)i * C;
+        if (tot_live > 0) {
+            const int blocks = (int)std::min<size_t>(((size_t)tot_live * Hkv * 16 + 255) / 256, (size_t)ctx->num_sms * 4);
+            compact_stage_kernel<<<dim3(std::max(blocks / nwork, 1), C), 256, 0, s>>>(reinterpret_cast<const uint4 *>(ctx->layers[l].kv),
+                                                                                    lo, d_meta + o_live, d_meta + o_work,
+                                                                                    d_meta + o_spre, reinterpret_cast<uint4 *>(keys), Hkv, M);
+            MPIG_LAUNCH_CHECK(ctx);
+            for (int c = 0; c < C; ++c) {
+                const int g = meta[o_live + c], pre = meta[o_spre + c];
+                if (!meta[o_work + c] || g == 0) continue;
+                rc = mpig_hash_keys(ctx, keys + (size_t)pre * Hkv * d, g, codes + (size_t)pre * Hkv * L, stream);
+                if (rc) return rc;
+            }
+        }
+        rc = launch_table_truncate(ctx, l, lo, d_meta + o_hi + (size_t)i * C, s);
+        if (rc) return rc;
+        rc = launch_table_merge(ctx, l, codes, d_meta + o_g, d_meta + o_spre, lo, s);
+        if (rc) return rc;
+    }
+    MPIG_CUDA(cudaStreamSynchronize(s));
+    for (int l : sparse) {
+        for (int c = 0; c < C; ++c)
+            if (meta[o_work + c]) ctx->n_off[l][c] = ctx->h_private_lo[l][c] + meta[o_live + c];
+        rc = upload_store_n(ctx, l, s);
+        if (rc) return rc;
+    }
+    MPIG_CUDA(cudaStreamSynchronize(s));
+    if (reclaimed_out)
+        for (int c = 0; c < C; ++c) reclaimed_out[c] = meta[o_work + c] ? priv[c] - meta[o_live + c] : 0;
     return MPIG_OK;
 }
 

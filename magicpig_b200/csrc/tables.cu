@@ -5,7 +5,8 @@
 //   sort()+LSH::fill     attnserver.py:186-193 -> build_segments_kernel<false> (counting sort on device)
 //   LSH::batch_retrieve  :210-241, LSH::retrieve :243-288 -> probe_kernel
 //   LSH::get_mask        :308-314  -> expand_mask_kernel
-// and, with no reference equivalent, the table side of a window spill (mpig_spill_window, store.cu) -> table_merge_kernel
+// and, with no reference equivalent, the table side of a window spill (mpig_spill_window, store.cu) -> table_merge_kernel, and
+// of a compaction (mpig_compact_context, store.cu) -> table_truncate_kernel then table_merge_kernel
 //
 // Table format (per context slot c, kv-head g, table l; row = (c*Hkv+g)*L + l): segmented compact CSR.  Request b reads the tables
 // of slot slot_of[b] (b itself when the map is null).
@@ -224,6 +225,92 @@ __global__ void __launch_bounds__(512) table_merge_kernel(const int16_t *__restr
     __syncthreads();
     // every thread reads and rewrites only its own entries of `off` (base0 was read before the first barrier)
     for (int c = tid; c <= NB; c += T) off[c] = seg_lo + (oo[c] - base0) + (c ? ex[c - 1] : 0);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Table truncate of a compaction (mpig_compact_context, store.cu), the mirror of table_merge_kernel: drop from every bucket of a
+// context slot's tables the items of keys >= lo[c], in place.  One CTA per (table, kv-head, slot x key segment); segments
+// holding no key of [lo[c], hi[c]) return at once, so lo[c] == hi[c] leaves a slot untouched.  No assumption is made on where
+// the dropped items sit inside a bucket: the segment's items are partitioned stably, kept ones moving down in ascending chunks
+// (a kept item at position p lands at or below p, so a write never reaches a position a later chunk still has to read, and the
+// block scan between the reads and the writes of a chunk orders them inside it).  With kc[c] = kept items of bucket c:
+//   new offset of bucket c = seg_lo + sum of kc over the buckets before c
+// A segment at or past lo keeps nothing: every bucket ends empty at seg_lo, what a build writes there.
+// grid (L, Hkv, C * S), 512 threads; dynamic smem = (NB + 1 + 40 [+ NB + 1 when staged]) ints.
+// ---------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(512) table_truncate_kernel(int32_t *offsets, uint16_t *items, const int32_t *__restrict__ lo_,
+                                                             const int32_t *__restrict__ hi_, int Hkv, int L, int NB, int M, int S,
+                                                             int seg_len, int staged) {
+    extern __shared__ int smem_i[];
+    constexpr int T = 512, UN = 8;
+    int *kc = smem_i;                // NB + 1: kept items per bucket -> exclusive prefix
+    int *wsum = smem_i + NB + 1;     // 40
+    int *oo_s = wsum + 40;           // NB + 1 old offsets (staged)
+    const int l = blockIdx.x, gi = blockIdx.y, slot = blockIdx.z / S, seg = blockIdx.z % S, tid = threadIdx.x;
+    const int lo = lo_[slot], hi = hi_[slot];
+    const int seg_lo = seg * seg_len, seg_hi = min(seg_lo + seg_len, M);
+    if (max(lo, seg_lo) >= min(hi, seg_hi)) return;
+    const size_t row = ((size_t)slot * Hkv + gi) * L + l;
+    int32_t *off = offsets + (row * S + seg) * (size_t)(NB + 1);
+    uint16_t *it = items + row * (size_t)M + seg_lo;
+    const int lim = lo - seg_lo;   // items (key - seg_lo) below lim are kept
+    const int base0 = off[0];
+    const int32_t *oo = off;
+    if (staged) {
+        for (int c = tid; c <= NB; c += T) oo_s[c] = off[c];
+        oo = oo_s;
+    }
+    for (int c = tid; c <= NB; c += T) kc[c] = 0;
+    __syncthreads();
+    const int cnt = oo[NB] - base0;
+    for (int p = tid; p < cnt; p += T) {
+        if ((int)it[p] >= lim) continue;
+        int a = 0, z = NB;   // last bucket whose start is <= p: the bucket holding p
+        while (z - a > 1) {
+            const int mid = (a + z) >> 1;
+            if (oo[mid] - base0 <= p) a = mid; else z = mid;
+        }
+        atomicAdd(&kc[a], 1);
+    }
+    __syncthreads();
+    {   // exclusive scan of kc[0..NB) in place; kc[NB] = kept items
+        const int per = (NB + T - 1) / T;
+        const int c0 = min(tid * per, NB), c1 = min(c0 + per, NB);
+        int local = 0;
+        for (int c = c0; c < c1; ++c) local += kc[c];
+        int total;
+        int run = block_exclusive_scan(local, wsum, &total);
+        for (int c = c0; c < c1; ++c) {
+            const int h = kc[c];
+            kc[c] = run;
+            run += h;
+        }
+        if (tid == 0) kc[NB] = total;
+    }
+    __syncthreads();
+    // stable partition: thread t of a chunk owns positions p0 + t*UN .. + UN - 1
+    int out = 0;
+    for (int p0 = 0; p0 < cnt; p0 += T * UN) {
+        uint16_t v[UN];
+        int keep = 0;
+#pragma unroll
+        for (int u = 0; u < UN; ++u) {
+            const int p = p0 + tid * UN + u;
+            v[u] = p < cnt ? it[p] : (uint16_t)0xffffu;
+            keep += (p < cnt && (int)v[u] < lim);
+        }
+        int total;
+        int dst = out + block_exclusive_scan(keep, wsum, &total);   // its barriers order every read above before any write below
+#pragma unroll
+        for (int u = 0; u < UN; ++u) {
+            const int p = p0 + tid * UN + u;
+            if (p < cnt && (int)v[u] < lim) it[dst++] = v[u];
+        }
+        out += total;
+    }
+    __syncthreads();
+    // every thread rewrites only its own entries of `off` (base0 and, unstaged, oo were read before the barriers above)
+    for (int c = tid; c <= NB; c += T) off[c] = seg_lo + kc[c];
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -573,6 +660,19 @@ int mpig::launch_table_merge(mpig_ctx *ctx, int layer, const int16_t *codes, con
     MPIG_FUNC_ATTR(table_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
     table_merge_kernel<<<dim3(L, Hkv, ctx->C * S), 512, smem, s>>>(codes, ls.offsets, reinterpret_cast<uint16_t *>(ls.items), g, pre,
                                                                    n_old, Hkv, L, NB, ctx->cfg.max_length, S, ctx->seg_len, staged);
+    MPIG_LAUNCH_CHECK(ctx);
+    return MPIG_OK;
+}
+
+int mpig::launch_table_truncate(mpig_ctx *ctx, int layer, const int32_t *lo, const int32_t *hi, cudaStream_t s) {
+    const LayerStore &ls = ctx->layers[layer];
+    const int Hkv = ctx->cfg.num_key_value_heads, L = ctx->cfg.L, S = ctx->nseg, NB = ctx->NB;
+    const size_t base = (size_t)(NB + 1 + 40) * sizeof(int);
+    const int staged = base + (size_t)(NB + 1) * sizeof(int) <= 200 * 1024;   // K <= 14
+    const size_t smem = base + (staged ? (size_t)(NB + 1) * sizeof(int) : 0);
+    MPIG_FUNC_ATTR(table_truncate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    table_truncate_kernel<<<dim3(L, Hkv, ctx->C * S), 512, smem, s>>>(ls.offsets, reinterpret_cast<uint16_t *>(ls.items), lo, hi, Hkv,
+                                                                      L, NB, ctx->cfg.max_length, S, ctx->seg_len, staged);
     MPIG_LAUNCH_CHECK(ctx);
     return MPIG_OK;
 }

@@ -50,8 +50,8 @@ class Context:
         filled or forked with.  0 = one full dense cache per request.
         shared_spill: requests that share a slot may spill_window() into it (needs 0 < C < batch_size <= 32).  Each spilled key is
         private: it is seen by the request that spilled it and by requests later forked from it, so every request decodes as if
-        it had the slot to itself.  Private keys nobody sees any more keep their place in the slot until it is refilled: size
-        max_length for the prompt plus every request's spilled tokens."""
+        it had the slot to itself.  Private keys nobody sees any more keep their place in the slot until it is refilled or
+        compact() reclaims them: size max_length for the prompt plus the spilled tokens still seen and one spill."""
         self.lib = N.load()
         self.device = torch.device(device)
         if self.device.type != "cuda":
@@ -399,6 +399,23 @@ class Context:
         out = (ctypes.c_int32 * self.B)()
         N.check(self.lib.mpig_spill_window(self._h, keep, out, _stream()), "mpig_spill_window")
         return torch.tensor(list(out), dtype=torch.int32)
+
+    def compact(self, slot: Optional[int] = None) -> torch.Tensor:
+        """shared_spill only: drop the spilled keys that no request sees any more (their owner was forked over, reordered over,
+        rebound or retired) from the store and the tables of context slot `slot` (None: every slot), in place.  Every request
+        samples exactly what it sampled before; the live keys keep their time order at the lowest offsets.  Returns the keys
+        reclaimed per slot, int32 (C,) on the host (zeros without shared_spill).  Synchronises; not capturable, but a decode step
+        captured before the call stays valid after it."""
+        out = (ctypes.c_int32 * self.C)()
+        N.check(self.lib.mpig_compact_context(self._h, -1 if slot is None else int(slot), out, _stream()), "mpig_compact_context")
+        return torch.tensor(list(out), dtype=torch.int32)
+
+    def visibility(self) -> torch.Tensor:
+        """Diagnostic accessor, shared_spill only: a copy of the visibility map, int32 (C, max_length) on the device; bit b of
+        [c, p] = request b sees the spilled key at private offset p of slot c."""
+        out = torch.empty((self.C, self.M), dtype=torch.int32, device=self.device)
+        N.check(self.lib.mpig_read_visibility(self._h, _ptr(out), _stream()), "mpig_read_visibility")
+        return out
 
     def decode(self, layer: int, query: torch.Tensor, key: torch.Tensor, value: torch.Tensor,
                out: Optional[torch.Tensor] = None) -> torch.Tensor:

@@ -7,7 +7,8 @@ shapes, two key segments) / gather-attention kernels, the fused single-launch de
 segments, one CTA per head with codes from the SimHash kernel, several selection passes), the three-launch decode, the dense
 kernel, the tensor-core key hash, the table build, the window spill, verification steps of T tokens, token trees with an accept,
 requests sharing one context slot, shared spill (several requests of one slot spill, a fork, single-token and T-token decodes), and
-the device-side reorder of requests (`reorder`: the in-place copy between requests, eager, refused and captured), chunk steps
+the device-side reorder of requests (`reorder`: the in-place copy between requests, eager, refused and captured), the compaction
+of a shared context (`compact`: eager and between replays of a captured step, against a twin), chunk steps
 (`chunk`: the chunk attention kernel on sparse and dense layers with one and several key splits, a partial m-block and a partial last
 tile, shared spill with private keys, the shared dense prefix, a rewind and a captured step), and BASELINE's C4 and C5 per-rank
 geometry (`configs`: K11 L300 over 4 segments in clusters of 4, Hq 8 / Hkv 1 over 8 segments in clusters of 8).  Results are
@@ -427,6 +428,78 @@ def shared_spill_case(B, Hq, Hkv, n, K, L, T):
     print(f"shared spill B={B} Hq={Hq} Hkv={Hkv} n={n} T={T}: ok")
 
 
+def compact_case(B, C, Hq, Hkv, n, K, L):
+    """mpig_compact_context on C slots against a twin with one slot per request: request B-1-i is fed request i's inputs
+    (i < C, request b starts on slot b % C), so a fork i -> B-1-i kills the private keys it left in its slot and leaves its twin
+    right.  With C = 2 both slots then hold dead keys and one compact() reclaims both (their live keys staged, hashed and merged
+    side by side).  compact() (the live list, the in-place record / vis move, the key staging, the table truncate and merge)
+    runs eagerly and between two replays of a step captured before it; every decode matches the twin in nnz and within 1e-5 in
+    fp32."""
+    M = n + 400
+    g = torch.Generator(device=dev).manual_seed(21)
+    hf = torch.randn((d, K * L), generator=g, device=dev).bfloat16()
+    key = torch.randn((Hkv, n, d), generator=g, device=dev).bfloat16()
+    val = torch.randn((Hkv, n, d), generator=g, device=dev).bfloat16()
+    ctxs = []
+    mirror = {B - 1 - i: i for i in range(C)}
+    for nc, shared in ((C, True), (0, False)):
+        ctx = Context(K, L, 1, Hq, Hkv, d, B, M, num_local_tokens=64, generation_buffer=24, device=dev, num_contexts=nc,
+                      shared_spill=shared)
+        ctx.set_option("out_f32", 1)
+        ctx.set_hash_func(hf)
+        for b in (range(C) if shared else range(B)):
+            ctx.attn_fill(0, b, key, val, key.norm(p=2, dim=-1).float())
+            ctx.lsh_build(0, b, ctx.hash_keys(key))
+        g2 = torch.Generator(device=dev).manual_seed(22)
+        wins = [(torch.randn((Hkv, 68 + 4 * b, d), generator=g2, device=dev).bfloat16(),
+                 torch.randn((Hkv, 68 + 4 * b, d), generator=g2, device=dev).bfloat16()) for b in range(B)]
+        for b in range(B):   # request B - 1 - i starts as a copy of request i
+            ctx.window_fill(0, b, torch.zeros((Hkv, d), dtype=torch.bfloat16, device=dev), *wins[mirror.get(b, b)])
+        ctxs.append(ctx)
+    sh, tw = ctxs
+    q = torch.zeros((B * Hq, d), dtype=torch.bfloat16, device=dev)
+    kv = torch.zeros((B * Hkv, d), dtype=torch.bfloat16, device=dev)
+    out = torch.zeros((B, Hq * d), dtype=torch.bfloat16, device=dev)
+    for c in ctxs:
+        c.plan()
+        c.decode(0, q, kv, kv)
+    s = torch.cuda.Stream()
+    s.wait_stream(torch.cuda.current_stream())
+    graph = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(graph, stream=s):
+        sh.plan()
+        sh.decode(0, q, kv, kv, out)
+
+    def step(replay):
+        q.copy_(torch.randn((B * Hq, d), generator=g, device=dev).bfloat16())
+        kv.copy_(torch.randn((B * Hkv, d), generator=g, device=dev).bfloat16())
+        for dst, src in mirror.items():
+            q.view(B, Hq, d)[dst], kv.view(B, Hkv, d)[dst] = q.view(B, Hq, d)[src], kv.view(B, Hkv, d)[src]
+        if replay:
+            graph.replay()
+        else:
+            sh.plan()
+            sh.decode(0, q, kv, kv, out)
+        tw.plan()
+        tw.decode(0, q, kv, kv)
+        torch.cuda.synchronize()
+        o_s, o_t = sh.last_out_f32(), tw.last_out_f32()
+        assert torch.equal(sh.last_probe()[0], tw.last_probe()[0]) and float((o_s - o_t).abs().max()) <= 1e-5 * float(o_t.abs().max()), \
+            "compacted shared context != twin"
+
+    for rnd in range(2):
+        for c in ctxs:
+            assert c.spill_window(48).sum() > 0
+        step(False)
+        for dst, src in mirror.items():
+            sh.fork(src, dst)   # the twin of dst already holds what the twin of src holds
+        reclaimed = sh.compact()
+        assert bool((reclaimed > 0).all()), reclaimed
+        step(rnd == 1)
+        step(rnd == 1)
+    print(f"compact B={B} C={C} Hq={Hq} Hkv={Hkv} n={n}: ok")
+
+
 def reorder_case(B, Hq, Hkv, n, K, L, R):
     """mpig_reorder_requests: the in-place copy of windows, avg_k and dense tails between requests of one slot (shared dense mode,
     shared spill: the visibility rewrite of the same launch) and the slot-map staging, against a twin that forks request by request;
@@ -582,7 +655,7 @@ def chunk_case(B, Hq, Hkv, n, K, L, T, R):
 
 if __name__ == "__main__":
     which = sys.argv[1:] or ["stages", "dense", "decode", "hostpeer", "spill", "tokens", "tree", "shared", "shared_spill", "reorder",
-                             "chunk", "configs"]
+                             "chunk", "configs", "compact"]
     if "configs" in which:   # BASELINE's C4 and C5 per-rank geometry at small n, each against its decode_impl = 0 twin
         # the i.i.d. keys sampled here have weights near 1e-2, where 1 - (1-p)^(L-1) (Lp + 1 - p) cancels in fp32 and amplifies
         # last-bit differences: the variants differ by up to 4e-4 of a head's largest element at K11 L300 (2e-5 at K10 L150), so
@@ -592,6 +665,9 @@ if __name__ == "__main__":
     if "chunk" in which:
         chunk_case(3, 8, 2, 600, 6, 24, 37, 200)      # one key split; T*G = 148: a partial second m-block, partial last tiles
         chunk_case(3, 8, 2, 2100, 6, 24, 5, 200)      # several key splits merged by the last CTA
+    if "compact" in which:
+        compact_case(3, 1, 4, 2, 700, 6, 24)
+        compact_case(4, 2, 4, 2, 700, 6, 24)             # both slots reclaimed in one call
     if "reorder" in which:
         reorder_case(4, 4, 2, 700, 6, 24, 40)
     if "shared_spill" in which:
