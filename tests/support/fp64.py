@@ -213,7 +213,7 @@ def _window(c, b, t, g, variant=None, parents=None):
     """Request b's window rows for token t of group g: its filled rows, the step's visible rows and the token, centred."""
     wb = 0 if variant == "window_of_request_0" else b
     new = c["k_new"][b, :, g] if variant == "uncentred" else c["k_new"][b, :, g] - avg_of(c, b)[g]
-    vis = visible(parents, b, t)
+    vis = visible(None if variant == "tree_as_chain" else parents, b, t)
     wk = torch.cat([c["win_k"][wb][g], new[vis], new[t:t + 1]])
     wv = torch.cat([c["win_v"][wb][g], c["v_new"][b, vis, g], c["v_new"][b, t:t + 1, g]])
     if variant == "drop_newest":
@@ -227,7 +227,8 @@ def restate(c, codes, variant=None, parents=None, heads=None, sets=None):
     applied, the window rows plus bf16(k_new - avg) attended under the causal / ancestor mask of the step, and the two halves
     merged by their base-2 LSEs.  Returns (o (B, T, Hq, d), lse_s (B, T, Hq) the sampled half's base-2 LSE, share (B, T, Hq)
     the window's share of the merged mass).  variant: a named perturbation (uncentred, drop_newest, ln_merge, skip_rescale,
-    drop_sampled, window_of_request_0, window_of_head_0, wrong_document) or None.  heads: bool (B, Hq), the heads to restate
+    drop_sampled, window_of_request_0, window_of_head_0, wrong_document, tree_as_chain: the ancestor mask read as a chain) or
+    None.  heads: bool (B, Hq), the heads to restate
     (None: all)."""
     B, T, Hq = c["q"].shape[:3]
     G, K, L = c["G"], c["K"], c["L"]

@@ -6,7 +6,9 @@ window lists):
   * make_batch: test_gpu_batch_numerics.py's and test_gpu_config_numerics.py's batches of B requests on C slots at the measured
     shapes, ragged windows, tuned on fp64 query codes, on any device.
 They draw different inputs on purpose and keep their own tuning.  Dense cases: make_dense (one prompt per request, or one for
-all) and make_dense_slots (shared prefix, ragged tails).
+all) and make_dense_slots (shared prefix, ragged tails).  next_case / next_dense turn an R2 case and the nodes its step commits
+(an accepted path, a rewind) into the case of the next step; check_after / check_dense_after self-check such a sequence against
+wrong commits (ACCEPT_VARIANTS).
 """
 import math
 import zlib
@@ -15,13 +17,23 @@ import torch
 
 import oracle
 from magicpig_b200 import synth
-from tests.support.fp64 import (BAR, SIMHASH_EPS, assert_rounded_half_up, avg_of, head_mask, key_codes, lsh_weight, query_codes,
-                                rel_rows, restate, sample_sets, softmax_state, unit, visible)
+from tests.support.fp64 import (BAR, SIMHASH_EPS, assert_rounded_half_up, avg_of, centred, head_mask, key_codes, lsh_weight,
+                                query_codes, rel_rows, restate, sample_sets, softmax_state, unit, visible)
 from tests.support.library import DEV, NL, NS, d, two_layer_context
 
 RD = math.sqrt(d)
 SELF_CHECK = {"R1": "uncentred", "R2": "drop_newest", "R3": "ln_merge", "R4": "skip_rescale"}
 TREE = [-1, 0, 0, 1, 1, 2, 3, 3]
+# the tree line's trees (node t's parent), and its accept cases: (label, the step's tree -- None: a T = 8 chain --, the nodes
+# committed in order: an accepted root path, or the 5 a rewind(3) keeps)
+LINE_TREES = {"binary_depth3": [-1, 0, 0, 1, 1, 2, 2], "star_1+7": [-1] + [0] * 7}
+COMB = [-1, 0, 0, 2, 3, 4, 5, 6]
+ACCEPTS = [("binary_depth3 [0,2,5]", LINE_TREES["binary_depth3"], [0, 2, 5]),
+           ("star_1+7 [0,7]", LINE_TREES["star_1+7"], [0, 7]),
+           ("comb [0,2,3,4,5,6,7]", COMB, [0, 2, 3, 4, 5, 6, 7]),
+           ("star_1+7 count 0", LINE_TREES["star_1+7"], []),
+           ("T8 rewind 3", None, [0, 1, 2, 3, 4])]
+ACCEPT_IDS = ["binary", "star", "comb", "star-none", "rewind"]
 # the measured lines: Llama-3.1-8B heads, K10 L150, one 98 K-token context (C2)
 HQ, HKV, KK, LL = 32, 8, 10, 150
 N_C2, M_C2, M_LONG = 97932, 98304, 131072
@@ -225,21 +237,22 @@ def check_case(c, parents=None):
 
 
 # ---- dense layers, one prompt per request ----------------------------------------------------------------------------------
-def make_dense(regime, B, Hq, Hkv, P, T, seed, place="last", one_prompt=False):
-    """Dense-layer inputs: prompt rows dk/dv (B, P, Hkv, d), q (B, T, Hq, d), step rows k/v (B, T, Hkv, d).
-    R2: the first NS prompt rows and the step's keys lie along the group direction and hold >= 90 % of the mass;
-    R4: queries x 16 and one dominant row at the first / last prompt row (place="new": the step's last key).
+def make_dense(regime, B, Hq, Hkv, P, T, seed, place="last", one_prompt=False, dev="cpu"):
+    """Dense-layer inputs: prompt rows dk/dv (B, P, Hkv, d), q (B, T, Hq, d), step rows k/v (B, T, Hkv, d), the group
+    directions u (B, Hkv, d), drawn on dev.
+    R2: the first NS prompt rows and the step's keys lie along the group direction (sigma sqrt(d) u) and hold >= 90 % of the
+    mass; R4: queries x 16 and one dominant row at the first / last prompt row (place="new": the step's last key).
     one_prompt: every request has the same prompt (and query direction), as the requests bound to one context slot."""
-    g = torch.Generator().manual_seed(seed)
-    rnd = lambda *s: torch.randn(s, generator=g, dtype=torch.float64)   # noqa: E731
+    g = torch.Generator(device=dev).manual_seed(seed)
+    rnd = lambda *s: torch.randn(s, generator=g, device=dev, dtype=torch.float64)   # noqa: E731
     G = Hq // Hkv
     u = unit(rnd, 1 if one_prompt else B, Hkv).expand(B, Hkv, d)
-    q = 0.5 * torch.randn((B, T, Hq, d), generator=g, dtype=torch.float64) + RD * u.repeat_interleave(G, 1)[:, None]
-    dk = torch.randn((1 if one_prompt else B, P, Hkv, d), generator=g, dtype=torch.float64).expand(B, P, Hkv, d).clone()
-    dv = torch.randn((1 if one_prompt else B, P, Hkv, d), generator=g).bfloat16().expand(B, P, Hkv, d).clone()
-    k = torch.randn((B, T, Hkv, d), generator=g, dtype=torch.float64)
-    v = torch.randn((B, T, Hkv, d), generator=g).bfloat16()
-    c = dict(B=B, Hq=Hq, Hkv=Hkv, G=G, P=P, regime=regime, place=place)
+    q = 0.5 * rnd(B, T, Hq, d) + RD * u.repeat_interleave(G, 1)[:, None]
+    dk = rnd(1 if one_prompt else B, P, Hkv, d).expand(B, P, Hkv, d).clone()
+    dv = torch.randn((1 if one_prompt else B, P, Hkv, d), generator=g, device=dev).bfloat16().expand(B, P, Hkv, d).clone()
+    k = rnd(B, T, Hkv, d)
+    v = torch.randn((B, T, Hkv, d), generator=g, device=dev).bfloat16()
+    c = dict(B=B, Hq=Hq, Hkv=Hkv, G=G, P=P, regime=regime, place=place, u=u)
     if regime == "R2":
         qq = q.bfloat16().double()
         a = torch.einsum("bthd,bhd->bth", qq, u.repeat_interleave(G, 1)).min()
@@ -248,6 +261,7 @@ def make_dense(regime, B, Hq, Hkv, P, T, seed, place="last", one_prompt=False):
         ns = min(NS, P)
         dk[:, :ns] = sigma * RD * u[:, None]
         k = 0.25 * k + sigma * RD * u[:, None]
+        c["sigma"] = sigma
     else:
         q = q * 16.0
         qq = q.bfloat16().double()
@@ -266,12 +280,13 @@ def make_dense(regime, B, Hq, Hkv, P, T, seed, place="last", one_prompt=False):
 
 
 def restate_dense(c, parents=None, variant=None):
-    """fp64 output (B, T, Hq, d) of a dense step: prompt rows + the visible step rows (causal or ancestors) + the token."""
+    """fp64 output (B, T, Hq, d) of a dense step: prompt rows + the visible step rows (causal or ancestors) + the token.
+    variant: drop_newest, skip_rescale, tree_as_chain (the ancestor mask read as a chain) or None."""
     B, T, Hq, G = c["B"], c["q"].shape[1], c["Hq"], c["G"]
-    o = torch.zeros((B, T, Hq, d), dtype=torch.float64)
+    o = torch.zeros((B, T, Hq, d), dtype=torch.float64, device=c["q"].device)
     for b in range(B):
         for t in range(T):
-            rows = visible(parents, b, t) + [t]
+            rows = visible(None if variant == "tree_as_chain" else parents, b, t) + [t]
             kk = torch.cat([c["dk"][b], c["k"][b, rows]])
             vv = torch.cat([c["dv"][b], c["v"][b, rows]])
             if variant == "drop_newest":
@@ -287,12 +302,124 @@ def restate_dense(c, parents=None, variant=None):
     return o
 
 
-def check_dense(c, parents=None):
+def dense_moves(c, parents=None, extra=()):
+    """The dense generator's self-check: the regime's perturbation (R2 drop_newest, R4 skip_rescale) and the opt-in ones of
+    extra must each move the fp64 output by >= 10x the bar.  Returns (output, {perturbation: how far it moves the output})."""
     o = restate_dense(c, parents)
-    variant = "drop_newest" if c["regime"] == "R2" else "skip_rescale"
-    moved = rel_rows(restate_dense(c, parents, variant), o)
-    assert moved >= 10 * BAR, f"dense {c['regime']}: '{variant}' moves the output by {moved:.2e} only"
-    return o
+    moved = {}
+    for variant in ("drop_newest" if c["regime"] == "R2" else "skip_rescale",) + tuple(extra):
+        moved[variant] = rel_rows(restate_dense(c, parents, variant), o)
+        assert moved[variant] >= 10 * BAR, f"dense {c['regime']}: '{variant}' moves the output by {moved[variant]:.2e} only"
+    return o, moved
+
+
+def check_dense(c, parents=None):
+    return dense_moves(c, parents)[0]
+
+
+# ------------------------------------------------------------------------------------------------
+# the steps after an accept or a rewind
+# ------------------------------------------------------------------------------------------------
+ACCEPT_VARIANTS = ("node_order", "path_dropped", "step_kept")
+
+
+def committed_as(variant, keep, T):
+    """What a wrong accept or rewind of a T-node step commits instead of keep (per request, the nodes in order): node_order --
+    nodes 0 .. count - 1 (the path's length, not its nodes); path_dropped -- nothing; step_kept -- every node (the accept or
+    rewind ignored)."""
+    return {"node_order": [list(range(len(k))) for k in keep], "path_dropped": [[] for _ in keep],
+            "step_kept": [list(range(T)) for _ in keep]}[variant]
+
+
+def next_case(c, keep, T, seed):
+    """The sparse case of the step after c's.  Request b's step committed c's nodes keep[b], in that order (an accepted root path,
+    the first T' - r nodes after rewind(r), or none), so its window gains their rows -- keys centred as the append centres them.
+    Then a step of T new tokens drawn as make_batch draws R2's: queries along the slot's group direction, keys on its sink rows,
+    so that the window, committed rows included, holds the mass.  The draws depend on the seed only, not on keep."""
+    assert c["regime"] == "R2", "next_case draws R2 steps"
+    dev = c["q"].device
+    g = torch.Generator(device=dev).manual_seed(seed)
+    rnd = lambda *s: torch.randn(s, generator=g, device=dev, dtype=torch.float64)   # noqa: E731
+    B, Hq, Hkv, G = c["B"], c["Hq"], c["Hkv"], c["G"]
+    win_k, win_v = [], []
+    for b in range(B):
+        rows = torch.tensor(keep[b], dtype=torch.long, device=dev)
+        win_k.append(torch.cat([c["win_k"][b], centred(c["k_new"][b, rows], avg_of(c, b)).transpose(0, 1)], dim=1))
+        win_v.append(torch.cat([c["win_v"][b], c["v_new"][b, rows].transpose(0, 1)], dim=1))
+    U = torch.stack([c["slots"][s]["u"] for s in c["slot_of"]])
+    sink = torch.stack([c["win_k"][b][:, 0].double() + avg_of(c, b).double() for b in range(B)])   # (B, Hkv, d) uncentred
+    q = rnd(B, T, Hq, d) + RD * U.repeat_interleave(G, 1)[:, None]
+    k_new = 0.25 * rnd(B, T, Hkv, d) + sink[:, None]
+    v_new = torch.randn((B, T, Hkv, d), generator=g, device=dev).bfloat16()
+    return dict(c, q=q.bfloat16(), k_new=k_new.bfloat16(), v_new=v_new, win_k=win_k, win_v=win_v)
+
+
+def next_dense(c, keep, T, seed):
+    """The dense case of the step after c's: c's nodes keep[b] (as many for every request) follow request b's prompt rows, in
+    that order, then a step of T new tokens drawn as make_dense draws R2's.  The draws depend on the seed only."""
+    assert c["regime"] == "R2", "next_dense draws R2 steps"
+    assert len({len(k) for k in keep}) == 1, "every request commits as many rows"
+    dev = c["q"].device
+    g = torch.Generator(device=dev).manual_seed(seed)
+    rnd = lambda *s: torch.randn(s, generator=g, device=dev, dtype=torch.float64)   # noqa: E731
+    B, Hq, Hkv, G, u = c["B"], c["Hq"], c["Hkv"], c["G"], c["u"]
+    idx = [torch.tensor(k, dtype=torch.long, device=dev) for k in keep]
+    dk = torch.cat([c["dk"], torch.stack([c["k"][b, idx[b]] for b in range(B)])], dim=1)
+    dv = torch.cat([c["dv"], torch.stack([c["v"][b, idx[b]] for b in range(B)])], dim=1)
+    q = 0.5 * rnd(B, T, Hq, d) + RD * u.repeat_interleave(G, 1)[:, None]
+    k = 0.25 * rnd(B, T, Hkv, d) + c["sigma"] * RD * u[:, None]
+    v = torch.randn((B, T, Hkv, d), generator=g, device=dev).bfloat16()
+    return dict(c, P=dk.shape[1], q=q.bfloat16(), dk=dk, dv=dv, k=k.bfloat16(), v=v)
+
+
+def after_steps(c, keep, steps, seed, nxt=next_case):
+    """The cases of the steps after c's when c's step commits keep and each following step, of steps[i] tokens, commits all of
+    its tokens."""
+    out, cur = [], c
+    for i, T in enumerate(steps):
+        cur = nxt(cur, keep, T, seed + i)
+        out.append(cur)
+        keep = [list(range(T))] * c["B"]
+    return out
+
+
+def _accept_moves(c, keep, steps, seed, nxt, restate_fn, moved):
+    """Every accept variant that commits other rows than keep must move the restated output of every following step by >= 10x
+    the bar; moved[variant] = its smallest move."""
+    refs = [restate_fn(x) for x in after_steps(c, keep, steps, seed, nxt)]
+    for variant in ACCEPT_VARIANTS:
+        alt = committed_as(variant, keep, c["q"].shape[1])
+        if alt == keep:
+            continue
+        moved[variant] = min(rel_rows(restate_fn(x), o) for x, o in zip(after_steps(c, alt, steps, seed, nxt), refs))
+        assert moved[variant] >= 10 * BAR, f"inputs are insensitive: '{variant}' moves a following step by {moved[variant]:.2e} only"
+    return moved
+
+
+def check_after(c, keep, steps, seed):
+    """The sparse steps after c's (after_steps), each self-checked by check_inputs, and the accept variants (_accept_moves).
+    Returns (cases, {perturbation: smallest move over the steps})."""
+    cases = after_steps(c, keep, steps, seed)
+    moved = {}
+    for x in cases:
+        for k, v in check_inputs(x).items():
+            moved[k] = min(v, moved.get(k, v))
+
+    def restate_fn(x):   # (the draws, hence the codes, are the same whichever rows were committed)
+        codes = query_codes(x["q"], x["hf"], x["K"], x["L"])[0]
+        return restate(x, codes)[0]
+    return cases, _accept_moves(c, keep, steps, seed, next_case, restate_fn, moved)
+
+
+def check_dense_after(c, keep, steps, seed):
+    """The dense steps after c's (after_steps with next_dense), each self-checked by dense_moves, and the accept variants.
+    Returns (cases, {perturbation: smallest move over the steps})."""
+    cases = after_steps(c, keep, steps, seed, next_dense)
+    moved = {}
+    for x in cases:
+        for k, v in dense_moves(x)[1].items():
+            moved[k] = min(v, moved.get(k, v))
+    return cases, _accept_moves(c, keep, steps, seed, next_dense, restate_dense, moved)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -421,9 +548,10 @@ def perturbations(c):
     return names
 
 
-def check_inputs(c, parents=None, heads=None):
+def check_inputs(c, parents=None, heads=None, extra=()):
     """The generator's self-checks on fp64 query codes, before any library call: the regime's property holds and every named
-    perturbation moves the restated output by >= 10x the bar.  Returns {perturbation: how far it moves the output}."""
+    perturbation (those of the case, then the opt-in ones of extra, e.g. tree_as_chain) moves the restated output by >= 10x the
+    bar.  Returns {perturbation: how far it moves the output}."""
     codes = query_codes(c["q"], c["hf"], c["K"], c["L"])[0]
     sets = sample_sets(c, codes)
     o, _, share = restate(c, codes, parents=parents, heads=heads, sets=sets)
@@ -440,7 +568,7 @@ def check_inputs(c, parents=None, heads=None):
                 span.append(float(z.max() - z.min()))
         assert min(span) >= 40.0, f"R4: scores span {min(span):.1f} nats only"
     moved = {}
-    for name in perturbations(c):
+    for name in perturbations(c) + list(extra):
         a = pick(restate(c, codes, name, parents, heads, sets=None if name == "wrong_document" else sets)[0], c, heads)
         b = pick(o, c, heads)
         per_head = (a - b).abs().amax(-1) / b.abs().amax(-1).clamp_min(1e-30)
@@ -565,6 +693,35 @@ def step(ctx, c, parents=None, lists=True):
              fused=ctx.get_info("last_decode_fused"))
     if lists:
         r.update(res=res.reshape(B, T, Hq, -1), codes=ctx.last_codes().reshape(B, T, Hq, -1))
+    return r
+
+
+def twin_lists(r, rt, label):
+    """Codes and lists of a save_mask = 0 step r from the same step rt of a save_mask = 1 twin filled identically, which must
+    have run the fused kernel and sampled the same counts."""
+    assert rt["fused"] == 1, f"{label}: the twin did not run the fused kernel"
+    assert torch.equal(r["nnz"], rt["nnz"]), f"{label}: save_mask = 0 sampled other counts than its twin"
+    r.update(res=rt["res"], codes=rt["codes"])
+    return r
+
+
+def twin_step(make_ctx, c, label, parents=None, fused=True, hook=None):
+    """One step of case c on the context make_ctx(save_mask) returns.  Fused steps run as the measured lines run them, with
+    save_mask = 0 (the CTAs list their selection in the carved extra row buffers), and take their codes and lists from a
+    save_mask = 1 twin (twin_lists); the three-launch path always writes its lists.  hook(ctx, r) sees the context before it is
+    released, which happens before the twin is made."""
+    save_mask = 0 if fused else 1
+    ctx = make_ctx(save_mask)
+    r = step(ctx, c, parents, lists=bool(save_mask))
+    assert r["fused"] == int(fused), f"{label}: last_decode_fused = {r['fused']}"
+    if hook is not None:
+        hook(ctx, r)
+    del ctx
+    if fused:
+        tw = make_ctx(1)
+        rt = step(tw, c, parents)
+        del tw
+        twin_lists(r, rt, label)
     return r
 
 

@@ -33,7 +33,7 @@ from tests.support.fp64 import BAR, SIMHASH_EPS, assert_rounded_half_up, avg_of,
 from tests.support.library import DEV, NL, NS, d, skip_unless_132_sms, two_layer_context
 from tests.support.sparse_cases import (GEN, HKV, HQ, KK, LENS, LL, M_C2, M_LONG, N_C2, TREE, batch_ctx, check_codes_lists,
                                         check_dense_inputs, check_inputs, check_outputs, make_batch, make_dense_slots, seed_of,
-                                        step)
+                                        step, twin_step)
 
 LONG_GEN = 4104                       # generation_buffer of the long-generation line's "no spill" arm: windows of up to 4 172 rows
 LONG_LENS = (4000, 4172, 4100, 4050)
@@ -91,20 +91,11 @@ def sparse_case(label, regime, B, C=1, lens=LENS, place="key", T=1, parents=None
     """Generate, self-check, run one step and check it.  Fused steps run as the measured lines run them, with save_mask = 0
     (the CTAs list their selection in the carved extra row buffers); their codes and lists come from a save_mask = 1 twin
     filled identically, which must sample the same counts.  The three-launch path always writes its lists."""
-    save_mask = 0 if fused else 1
     c = make_batch(regime, B, C=C, n=n, T=T, lens=lens, place=place, seed=seed_of(label, regime, place, kreg), parents=parents)
     moved = check_inputs(c, parents, heads)
     print(f"{label}: perturbations move the output by " + ", ".join(f"{k} {v:.2e}" for k, v in moved.items()))
-    ctx = batch_ctx(c, C=0 if B == 1 else C, M=M, gen=gen, kreg=kreg, save_mask=save_mask, t_max=T)
-    r = step(ctx, c, parents, lists=bool(save_mask))
-    assert r["fused"] == int(fused), f"{label}: last_decode_fused = {r['fused']}"
-    if not save_mask:
-        tw = batch_ctx(c, C=0 if B == 1 else C, M=M, gen=gen, kreg=kreg, save_mask=1, t_max=T)
-        rt = step(tw, c, parents)
-        assert rt["fused"] == 1, f"{label}: the twin did not run the fused kernel"
-        assert torch.equal(r["nnz"], rt["nnz"]), f"{label}: save_mask = 0 sampled other counts than its twin"
-        r.update(res=rt["res"], codes=rt["codes"])
-        del tw
+    r = twin_step(lambda save_mask: batch_ctx(c, C=0 if B == 1 else C, M=M, gen=gen, kreg=kreg, save_mask=save_mask, t_max=T),
+                  c, label, parents, fused)
     sets = check_codes_lists(c, r)
     return check_outputs(c, r, sets, label, parents, heads)
 

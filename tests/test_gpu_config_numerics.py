@@ -34,7 +34,7 @@ from tests.support.config_cases import REG_CHUNKS, check_config_inputs, chunk_st
 from tests.support.fp64 import SIMHASH_EPS
 from tests.support.library import DEV, NL, NS, assert_tables_equal, d, lsh_tables, skip_unless_132_sms, two_layer_context
 from tests.support.sparse_cases import (GEN, LENS, TREE, batch_ctx, check_codes_lists, check_outputs, make_batch, seed_of,
-                                        step)
+                                        step, twin_step)
 
 pytestmark = pytest.mark.gpu
 
@@ -141,23 +141,13 @@ def run_path(c, shape, label, kreg=0, impl=1, parents=None, ctx_hook=None):
     with save_mask = 0 and take codes and lists from a save_mask = 1 twin, which must sample the same counts."""
     s = SHAPES[shape]
     T = c["q"].shape[1]
-    fused = impl == 1 and (T > 1 or is_fused(shape))
-    save_mask = 0 if fused else 1
-    ctx = batch_ctx(c, C=0, M=s["M"], kreg=kreg, save_mask=save_mask, t_max=T)
-    if impl == 0:
-        ctx.set_option("decode_impl", 0)
-    r = step(ctx, c, parents, lists=bool(save_mask))
-    assert r["fused"] == int(fused), f"{label}: last_decode_fused = {r['fused']}"
-    if ctx_hook is not None:
-        ctx_hook(ctx, r)
-    del ctx
-    if not save_mask:
-        tw = batch_ctx(c, C=0, M=s["M"], kreg=kreg, save_mask=1, t_max=T)
-        rt = step(tw, c, parents)
-        del tw
-        assert rt["fused"] == 1, f"{label}: the twin did not run the fused kernel"
-        assert torch.equal(r["nnz"], rt["nnz"]), f"{label}: save_mask = 0 sampled other counts than its twin"
-        r.update(res=rt["res"], codes=rt["codes"])
+
+    def make_ctx(save_mask):
+        ctx = batch_ctx(c, C=0, M=s["M"], kreg=kreg, save_mask=save_mask, t_max=T)
+        if impl == 0:
+            ctx.set_option("decode_impl", 0)
+        return ctx
+    r = twin_step(make_ctx, c, label, parents, impl == 1 and (T > 1 or is_fused(shape)), ctx_hook)
     sets = check_codes_lists(c, r)
     worst = check_outputs(c, r, sets, label, parents)
     torch.cuda.empty_cache()
