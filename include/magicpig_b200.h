@@ -77,28 +77,32 @@ typedef struct mpig_config {
     int32_t num_dense_layers;     /* entries used in dense_layers[] */
     int32_t dense_layers[16];     /* attnserver.py:18; tables/offload store are NOT allocated for these */
     int32_t alloc_dense_kv;       /* 1: also own the dense layers' full KV cache + dense decode kernel */
-    /* reserved[0]: 2 = plan the probing / fused clusters for two 512-thread CTAs per SM (experiment switch; otherwise one).
-     * reserved[1]: number of context slots C in [0, batch_size]; 0 means C = batch_size (every request owns its slot).  The
-     *   sampled store and the L hash tables of every sparse layer exist once per SLOT; the window, avg_k, the dense layers' KV,
-     *   the lengths and the per-step scratch stay per REQUEST.  Request b is bound to slot b mod C at creation and after
-     *   mpig_clear; mpig_fork_request / mpig_bind_request change the binding.  Requests bound to one slot decode over one copy of
-     *   the context (parallel sampling, several questions about one document).
-     * reserved[2]: dense tail rows R; 0 (default) = every request owns a full dense KV cache [Hkv][max_length].  R > 0 (only
-     *   with 0 < C < batch_size, alloc_dense_kv = 1 and R <= max_length; otherwise MPIG_EINVAL) shares the dense layers' prompt
-     *   too: per dense layer a slot store [C][Hkv][max_length] and a tail [B][Hkv][R] per request.  mpig_dense_fill writes the
-     *   rows of the slot the request is bound to and makes seq_len the request's base; mpig_fork_request copies only src's rows
-     *   past its base; a request's dense capacity is min(max_length, base + R) (the plans refuse past it, a captured plan
-     *   saturates and raises mpig_error_flags bit 1); a rebound request must be dense-filled before its dense outputs mean
-     *   anything; dense_impl = 0 is MPIG_EUNSUPPORTED.  mpig_get_info("dense_tail_rows") reports R.
-     * reserved[3]: 1 = shared spill (only with 0 < C < batch_size <= 32; otherwise MPIG_EINVAL).  mpig_spill_window accepts
-     *   requests that share a slot: their rows go into the slot's store and tables in request order, and every spilled key is
-     *   PRIVATE: request b samples the slot's prompt keys plus the private keys it spilled itself or inherited through
-     *   mpig_fork_request, so its result equals that of an exclusive slot holding those keys (codes, nnz and index sets equal after
-     *   renumbering, fp32 outputs up to summation order).  The capacity is shared (prompt + all private keys of a slot <=
-     *   max_length).  A fill of a slot (mpig_attn_fill, mpig_lsh_build / mpig_lsh_fill) and mpig_clear drop its private keys;
-     *   private keys nobody sees any more keep their rows until then, or until mpig_compact_context reclaims them.  mpig_lsh_collision_counts stays unfiltered.
-     *   mpig_get_info("shared_spill") reports the flag. */
-    int32_t reserved[8];
+    int32_t ctas_per_sm;          /* probing / fused clusters planned for: 0 or 1 = one 1024-thread CTA per SM, 2 = two 512-thread
+                                   * CTAs per SM (experiment switch); anything else is MPIG_EINVAL */
+    /* number of context slots C in [0, batch_size]; 0 means C = batch_size (every request owns its slot).  The sampled store
+     * and the L hash tables of every sparse layer exist once per SLOT; the window, avg_k, the dense layers' KV, the lengths and
+     * the per-step scratch stay per REQUEST.  Request b is bound to slot b mod C at creation and after mpig_clear;
+     * mpig_fork_request / mpig_bind_request change the binding.  Requests bound to one slot decode over one copy of the context
+     * (parallel sampling, several questions about one document). */
+    int32_t num_contexts;
+    /* dense tail rows R; 0 (default) = every request owns a full dense KV cache [Hkv][max_length].  R > 0 (only with
+     * 0 < C < batch_size, alloc_dense_kv = 1 and R <= max_length; otherwise MPIG_EINVAL) shares the dense layers' prompt too:
+     * per dense layer a slot store [C][Hkv][max_length] and a tail [B][Hkv][R] per request.  mpig_dense_fill writes the rows of
+     * the slot the request is bound to and makes seq_len the request's base; mpig_fork_request copies only src's rows past its
+     * base; a request's dense capacity is min(max_length, base + R) (the plans refuse past it, a captured plan saturates and
+     * raises mpig_error_flags bit 1); a rebound request must be dense-filled before its dense outputs mean anything;
+     * dense_impl = 0 is MPIG_EUNSUPPORTED.  mpig_get_info("dense_tail_rows") reports R. */
+    int32_t dense_tail_rows;
+    /* 1 = shared spill (only with 0 < C < batch_size <= 32; otherwise MPIG_EINVAL).  mpig_spill_window accepts requests that
+     * share a slot: their rows go into the slot's store and tables in request order, and every spilled key is PRIVATE:
+     * request b samples the slot's prompt keys plus the private keys it spilled itself or inherited through mpig_fork_request,
+     * so its result equals that of an exclusive slot holding those keys (codes, nnz and index sets equal after renumbering,
+     * fp32 outputs up to summation order).  The capacity is shared (prompt + all private keys of a slot <= max_length).  A fill
+     * of a slot (mpig_attn_fill, mpig_lsh_build / mpig_lsh_fill) and mpig_clear drop its private keys; private keys nobody
+     * sees any more keep their rows until then, or until mpig_compact_context reclaims them.  mpig_lsh_collision_counts stays
+     * unfiltered.  mpig_get_info("shared_spill") reports the flag. */
+    int32_t shared_spill;
+    int32_t reserved[4];          /* must be zero (MPIG_EINVAL otherwise) */
 } mpig_config;
 
 /* ---- lifetime ------------------------------------------------------------------------------- */
@@ -125,11 +129,8 @@ size_t mpig_device_bytes(const mpig_ctx *ctx);
  *                     this is where the parity tests apply the 1e-3 bar
  *   "attend_tma"      stand-alone gather kernel: 1 = per-row cp.async.bulk copies (default), 0 = per-row 16-B cp.async copies
  *   "attend_ctas" / "attend_warps"   grid / CTA shape of the stand-alone gather kernel (0 = automatic)
- *   "attend_impl"     only 1 (tensor-core tile math) exists; anything else returns MPIG_EUNSUPPORTED
  *   "dense_impl"      1 = GQA-shared dense kernel (default), 0 = the gather kernel in range mode
  *   "keyhash_impl"    1 = persistent warp-specialised wgmma pipeline (default), 0 = one tile per CTA
- *   "keyhash_stages"  B-tile ring depth of that pipeline (2..4, default 2; capped at what fits in shared memory beside
- *                     the two key tiles, which is 2 on sm_90a)
  *   "pdl_first"       1 = launch the first kernel of mpig_decode with programmatic stream serialization too (default)
  *   "attend_skip" / "attend_debug" / "fused_debug" / "keyhash_skip"   timing-only elimination switches and clock stamps
  *                     (results are WRONG while a skip bit is set; used by scripts/kernel_bench.py and scripts/keyhash_bench.py) */
@@ -138,12 +139,12 @@ int mpig_set_option(mpig_ctx *ctx, const char *key, int64_t value);
  * "fused_cluster_waves" (waves of thread-block clusters one fused launch takes on this device; 1 = all resident at once,
  * 0 = fused decode not applicable), "window_capacity" (sink + local + generation_buffer rows), "table_segments" (key segments S
  * of the tables, see mpig_lsh_table_ptrs), "query_tokens_max" (t_max of mpig_reserve_query_tokens, 1 without), "tokens_cluster_waves"
- * (waves of clusters the last mpig_decode_tokens launch with T > 1 took), "num_contexts" (context slots C, see reserved[1]), "dense_tail_rows" (R, see reserved[2]),
- * "shared_spill" (0 / 1, see reserved[3]), "chunk_tokens_max" (t_max of mpig_reserve_chunk_tokens, 0 without), "chunk_splits"
+ * (waves of clusters the last mpig_decode_tokens launch with T > 1 took), "num_contexts" (context slots C, see mpig_config), "dense_tail_rows" (R),
+ * "shared_spill" (0 / 1), "chunk_tokens_max" (t_max of mpig_reserve_chunk_tokens, 0 without), "chunk_splits"
  * (key splits of the last mpig_chunk_attend launch, 0 before any). */
 int mpig_get_info(mpig_ctx *ctx, const char *key, int64_t *value);
 /* Capacity errors the DEVICE detected (the lengths saturate there): bit 0 = a sparse window is full (generation_buffer
- * exhausted: each further token overwrites the previous one's K/V), bit 1 = a dense cache reached its capacity (max_length, or base + R with reserved[2]), bit 2 = mpig_rewind
+ * exhausted: each further token overwrites the previous one's K/V), bit 1 = a dense cache reached its capacity (max_length, or base + R with dense_tail_rows = R), bit 2 = mpig_rewind
  * met a drop outside [0, T] (that request was left untouched), bit 3 = mpig_plan_tree met a malformed tree (that request ran as a
  * chain) or mpig_accept met a path that is not a root path of the step (that request was left untouched), bit 4 =
  * mpig_reorder_requests met a map that breaks its rule (every request was left untouched).  mpig_plan
@@ -159,7 +160,7 @@ int mpig_clear(mpig_ctx *ctx, void *stream);
 /* hash_func: bf16 (d, K*L) row-major, column l*K+i = bit i of table l (attnserver.py:55,268-270). */
 int mpig_set_hash_func(mpig_ctx *ctx, const void *hash_func_bf16, void *stream);
 
-/* ---- context slots (no reference equivalent; see mpig_config.reserved[1]) ------------------------------------------------------
+/* ---- context slots (no reference equivalent; see mpig_config.num_contexts) -------------------------------------------------
  * Fork and bind return MPIG_ESTATE when C = batch_size (the bindings are then fixed: request b reads slot b), are not capturable
  * (mpig_reorder_requests is the capturable form of a batch of forks), and
  * end the pending step: mpig_rewind / mpig_accept are refused (MPIG_ESTATE) until the next plan.  A step captured before either
@@ -168,7 +169,7 @@ int mpig_set_hash_func(mpig_ctx *ctx, const void *hash_func_bf16, void *stream);
  * Bind `dst` to the slot of `src` and make dst's per-request state a copy of src's: for every sparse layer window rows
  * [0, win_len[src]) of every kv-head and avg_k, for every dense layer KV rows [0, dense_len[src]) of every kv-head, and both
  * lengths (device and host mirror).  Reads the device lengths and synchronises `stream` (correct after replays of a captured
- * plan); copy-engine calls only, plus in shared spill mode (reserved[3]) one kernel: dst then sees exactly the private keys src
+ * plan); copy-engine calls only, plus in shared spill mode (shared_spill) one kernel: dst then sees exactly the private keys src
  * sees, and no longer its own.  MPIG_EINVAL: src == dst or either outside [0, batch_size). */
 int mpig_fork_request(mpig_ctx *ctx, int src, int dst, void *stream);
 /* Bind `request` to `slot` (in [0, C)); its window and lengths are left alone: fill the slot (mpig_attn_fill + mpig_lsh_build /
@@ -178,8 +179,8 @@ int mpig_bind_request(mpig_ctx *ctx, int request, int slot, void *stream);
 /* Request b continues request src_of[b]'s sequence (device int32 [B]; src_of[b] == b leaves b as it is).  The device-side,
  * capturable form of mpig_fork_request(src_of[b], b) for every b with src_of[b] != b, all at once (beam search: each step, each new
  * beam continues some old beam).  For every moved request b, with s = src_of[b]: window rows [0, win_len[s]) of every sparse layer
- * and kv-head and avg_k; dense rows [0, dense_len[s]) (reserved[2] = R > 0: tail rows [0, min(dense_len[s] - dense_base[s], R))
- * and the base); both lengths; the slot binding; in shared spill mode (reserved[3]) b then sees exactly the private keys s sees.
+ * and kv-head and avg_k; dense rows [0, dense_len[s]) (dense_tail_rows = R > 0: tail rows [0, min(dense_len[s] - dense_base[s], R))
+ * and the base); both lengths; the slot binding; in shared spill mode (shared_spill) b then sees exactly the private keys s sees.
  * Every later decode output equals the output after those forks, bitwise.  One kernel launch plus one device-to-device copy of
  * the slot map (the decode kernels read the map before they wait on their predecessor, so no kernel writes it).
  * The map's rule: 0 <= src_of[b] < B and src_of[src_of[b]] == src_of[b] for every b -- a request that is a source keeps its own
@@ -237,7 +238,7 @@ int mpig_attention_wrapper(mpig_ctx *ctx, int layer, int K, int L, void *output_
                            const int32_t *nnz, void *stream);
 /* get_key_cache / get_value_cache / get_key_norm (sparse_attention.cc:1213-1234), copied out
  * of the interleaved HBM layout: k, v bf16 (C, Hkv, M, d) and/or kn fp32 (C, Hkv, M), one entry per context slot (C = B unless
- * reserved[1] says otherwise; request b's store is entry slot-of-b); NULL skips. */
+ * num_contexts says otherwise; request b's store is entry slot-of-b); NULL skips. */
 int mpig_attn_read_cache(mpig_ctx *ctx, int layer, void *k_bf16, void *v_bf16, float *kn, void *stream);
 
 /* ---- the GPU-side glue of LSHSparseAttnServer.decode ------------------------------------------ */
@@ -262,7 +263,7 @@ int mpig_plan(mpig_ctx *ctx, void *stream);
  * captured step alike.  Not capturable.  A decode step captured before a spill stays valid after it.  Dense layers are
  * untouched.  The spilled keys go into the store and tables of the request's slot: the requests of a slot spill into it in
  * request order, so n_old is the slot's count plus the rows of the slot's earlier requests.  The two modes differ in two ways
- * only.  Without shared spill (reserved[3] = 0) a request with g_b > 0 must be alone on its slot among requests with a
+ * only.  Without shared spill (shared_spill = 0) a request with g_b > 0 must be alone on its slot among requests with a
  * non-empty window: a request that shares its context generates at most generation_buffer tokens.  In shared spill mode
  * several requests of a slot may spill, and each spilled key is private to its request.
  * MPIG_EINVAL: keep < 0 or sink + keep >= window capacity; MPIG_ESTATE: the slot's count plus all its requests' rows >
@@ -270,7 +271,7 @@ int mpig_plan(mpig_ctx *ctx, void *stream);
  * shared spill mode), the sparse layers of a slot disagree on its private key count (shared spill mode, after a partial
  * refill), or no hash_func set.  On these errors nothing is modified. */
 int mpig_spill_window(mpig_ctx *ctx, int keep, int32_t *spilled_out, void *stream);
-/* Shared spill mode (reserved[3]): reclaim the dead private keys of context slot `slot` (-1: every slot).  A private key is
+/* Shared spill mode (shared_spill = 1): reclaim the dead private keys of context slot `slot` (-1: every slot).  A private key is
  * dead when no request sees it any more (vis[slot][p] == 0: its owner was forked over, reordered over, rebound or retired).
  * Every live private key keeps its time order and moves to the lowest free offset: live key j (ascending offsets) becomes
  * store index private_lo + j of every sparse layer, its record and key norm with it, vis[slot][j] takes its word (the words
@@ -394,9 +395,9 @@ int mpig_accept(mpig_ctx *ctx, const int32_t *nodes, const int32_t *count, void 
  * A chunk step appends the T new K/V rows of request b at base_b .. base_b + T - 1 of every layer (1 <= T <= t_max <= 1024), exactly
  * as a T-token verification step does (sparse layers centre the keys with avg_k, dense layers store them raw), and query token t
  * gets EXACT softmax attention (scale 1/sqrt(d); no sampling, no importance weights) over
- *   sparse layer: every key of the slot's sampled store the request sees (shared spill mode, reserved[3]: the prompt keys and the
+ *   sparse layer: every key of the slot's sampled store the request sees (shared spill mode: the prompt keys and the
  *                 private keys it spilled or inherited) plus window rows [0, base_b + t];
- *   dense layer:  dense rows [0, base_b + t] (reserved[2] = R > 0: the slot's prompt rows below the request's dense base, then its
+ *   dense layer:  dense rows [0, base_b + t] (dense_tail_rows = R > 0: the slot's prompt rows below the request's dense base, then its
  *                 tail).
  * Store and window keys of a request carry the same -avg_k shift, to which softmax is invariant: the result is the attention a
  * prefill of the whole conversation computes, up to rounding.  mpig_rewind(drop) afterwards keeps T - drop[b] tokens of request b

@@ -35,7 +35,11 @@ class MpigConfig(ctypes.Structure):
         ("num_dense_layers", ctypes.c_int32),
         ("dense_layers", ctypes.c_int32 * 16),
         ("alloc_dense_kv", ctypes.c_int32),
-        ("reserved", ctypes.c_int32 * 8),
+        ("ctas_per_sm", ctypes.c_int32),
+        ("num_contexts", ctypes.c_int32),
+        ("dense_tail_rows", ctypes.c_int32),
+        ("shared_spill", ctypes.c_int32),
+        ("reserved", ctypes.c_int32 * 4),
     ]
 
 

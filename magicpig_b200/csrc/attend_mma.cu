@@ -431,7 +431,6 @@ int launch_attend_mma(mpig_ctx *ctx, const AttendParams &p_in, cudaStream_t s, b
     AttendParams p = p_in;
     const int warps = ctx->attend.warps;
     MPIG_REQUIRE(warps >= 1 && warps <= 12, MPIG_EINVAL, "attend(mma): warps=%d outside [1,12]", warps);
-    p.stages = 1;
     p.dbg = ctx->attend_debug ? ctx->dbg_buf : nullptr;
     p.skip = ctx->attend_skip;
     if (p.dbg) MPIG_CUDA(cudaMemsetAsync(p.dbg, 0, (size_t)ctx->max_partial_warps * 16 * sizeof(unsigned long long), s));

@@ -1,6 +1,6 @@
 // common.cuh -- context layout, error plumbing and PTX wrappers shared by the sm_90a kernels.
 //
-// HBM layout owned by a context (all per SPARSE layer unless noted; B requests, C context slots (mpig_config.reserved[1], 0 = B),
+// HBM layout owned by a context (all per SPARSE layer unless noted; B requests, C context slots (mpig_config.num_contexts, 0 = B),
 // Hkv kv-heads, M = max_length rows of capacity, d = head_dim, REC = 2*d bf16 = 512 B at d = 128).  The sampled store and the
 // tables are per SLOT; request b reads slot slot_of[b] (slot group slot_of[b]*Hkv + h/G), its window and lengths are its own:
 //
@@ -14,7 +14,7 @@
 //   avg_k   [B][Hkv][d]      bf16 mean offloaded key (attnserver.py:142-148)
 //   dense   [B][Hkv][M]      REC-byte records (dense layers, only with alloc_dense_kv)
 //
-// Shared dense mode (mpig_config.reserved[2] = R tail rows > 0, only with C < B): per dense layer the prompt rows live once per
+// Shared dense mode (mpig_config.dense_tail_rows = R > 0, only with C < B): per dense layer the prompt rows live once per
 // slot and the rows a request adds after its prompt in a tail of its own.  Row r of request b is row r of slot slot_of[b]'s store
 // when r < dense_base[b], else row r - dense_base[b] of b's tail:
 //   dense   [C][Hkv][M]      REC-byte records (the slot store)
@@ -106,7 +106,6 @@ constexpr int REORDER_ROWS = 64;   // rows one CTA of the reorder kernel copies 
 struct AttendTuning {
     int ctas = 0;    // 0 = one per SM * occupancy
     int warps = 12;
-    int stages = 1;
     int tma = 1;     // 1 = per-row cp.async.bulk (TMA engine), 0 = per-row 32 x 16 B cp.async (LSU path)
 };
 
@@ -144,7 +143,7 @@ struct mpig_ctx {
     int seg_len = 0;   // keys per segment: ceil(M / nseg) rounded up to 64 -- equal segments, so a probing cluster's CTAs own equal ranges
     int NB = 0, Wcap = 0, G = 0, H = 0 /* B*Hq */, BG = 0 /* B*Hkv */, rec_bytes = 0, num_sms = 0;
     int bitmap_words = 0;  // ceil(M/32)
-    int cta_per_sm = 1;    // probing / fused CTAs per SM the geometry is planned for (mpig_config.reserved[0] == 2 -> 2)
+    int cta_per_sm = 1;    // probing / fused CTAs per SM the geometry is planned for (mpig_config.ctas_per_sm == 2 -> 2)
     int max_cluster = 8;   // largest probing / fused cluster whose B*Hq copies are all resident at once (mpig_create)
     std::vector<mpig::LayerStore> layers;
     std::vector<std::vector<int>> n_off;  // [layer][slot] offloaded key count (host bookkeeping)
@@ -179,7 +178,7 @@ struct mpig_ctx {
     int dense_cap(int b) const {
         return dense_tail_rows > 0 ? std::min(cfg.max_length, h_dense_base[b] + dense_tail_rows) : cfg.max_length;
     }
-    // shared spill mode (mpig_config.reserved[3] = 1, DESIGN.md section 3.12): requests that share a slot spill into it, and each
+    // shared spill mode (mpig_config.shared_spill = 1, DESIGN.md section 3.12): requests that share a slot spill into it, and each
     // spilled key is private.  Keys [private_lo[layer][slot], ...) of a slot's store are private; the private key at offset p is
     // seen by request b iff bit b of vis[slot][p] is set.  Both arrays are allocated at create time and never move (a captured
     // step reads the current ones).  Kernels write them (fills, spill, fork, bind) as well as mpig_clear's memsets, so the decode
@@ -212,7 +211,6 @@ struct mpig_ctx {
     int save_mask = 0;
     int max_partial_warps = 0;
     mpig::AttendTuning attend;
-    int last_probe_layer = -1;
     unsigned long long *dbg_buf = nullptr;   // attend stage timestamps when option "attend_debug" is set
     int attend_debug = 0;
     int attend_skip = 0;
@@ -220,7 +218,6 @@ struct mpig_ctx {
     bool hash_func_set = false;  // mpig_set_hash_func has been called (hashing with the zero projection is refused)
     int pdl_first = 1;     // launch the first kernel of a decode (simhash) with programmatic stream serialization as well
     int keyhash_skip = 0;  // debug/timing only: 1 = no stores, 2 = no sign pack, 4 = no MMAs (results are wrong)
-    int keyhash_stages = 2;  // B-tile ring depth of the pipelined key-hash kernel (2..4)
     int keyhash_impl = 1;  // 1 = persistent warp-specialised pipeline (keyhash.cu), 0 = one tile per CTA
     std::vector<cudaEvent_t> timing_events;  // 4 per timed decode call
     int timing_calls = 0;
@@ -421,7 +418,7 @@ struct AttendParams {
     float *mve;               // [2][H] or null: row0 = m*log2e, row1 = LSE2
     float *partials;          // [nwarps][2][PART_FLOATS]
     int32_t *counters;        // [H]
-    int H, G, Hq, M, Wcap, K, L, stages;
+    int H, G, Hq, M, Wcap, K, L;
     unsigned long long *dbg;  // optional per-warp stage timestamps (16 x u64 per warp), null in production
     int skip;                 // measurement aid (option "attend_skip"): 1 = no row fetch, 2 = no tile math, 4 = no merges
 };

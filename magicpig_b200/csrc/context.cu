@@ -11,6 +11,15 @@
 
 #include "common.cuh"
 
+// The layout of ABI version 1, byte for byte: a caller built against any header of that version keeps working.
+static_assert(offsetof(mpig_config, alloc_dense_kv) == 120, "mpig_config layout");
+static_assert(offsetof(mpig_config, ctas_per_sm) == 124, "mpig_config layout");
+static_assert(offsetof(mpig_config, num_contexts) == 128, "mpig_config layout");
+static_assert(offsetof(mpig_config, dense_tail_rows) == 132, "mpig_config layout");
+static_assert(offsetof(mpig_config, shared_spill) == 136, "mpig_config layout");
+static_assert(offsetof(mpig_config, reserved) == 140, "mpig_config layout");
+static_assert(sizeof(mpig_config) == 156, "mpig_config layout");
+
 namespace mpig {
 
 int func_attr_once(const void *fn, cudaFuncAttribute attr, int value) {
@@ -93,24 +102,27 @@ int mpig_create(const mpig_config *cfg, mpig_ctx **out) {
     MPIG_REQUIRE(cfg->num_dense_layers >= 0 && cfg->num_dense_layers <= 16, MPIG_EINVAL, "mpig_create: num_dense_layers");
     MPIG_REQUIRE(cfg->num_sink_tokens >= 0 && cfg->num_local_tokens >= 0 && cfg->generation_buffer >= 0, MPIG_EINVAL,
                  "mpig_create: negative window size");
-    MPIG_REQUIRE(cfg->reserved[1] >= 0 && cfg->reserved[1] <= cfg->batch_size, MPIG_EINVAL,
-                 "mpig_create: num_contexts (reserved[1]) = %d outside [0, batch_size = %d]", cfg->reserved[1], cfg->batch_size);
-    if (cfg->reserved[2] != 0) {   // shared dense mode: R tail rows per request, the prompt rows once per slot
-        MPIG_REQUIRE(cfg->reserved[2] >= 1 && cfg->reserved[2] <= cfg->max_length, MPIG_EINVAL,
-                     "mpig_create: dense_tail_rows (reserved[2]) = %d outside [1, max_length = %d]", cfg->reserved[2], cfg->max_length);
-        MPIG_REQUIRE(cfg->reserved[1] > 0 && cfg->reserved[1] < cfg->batch_size, MPIG_EINVAL,
-                     "mpig_create: dense_tail_rows (reserved[2]) = %d needs fewer context slots than requests (num_contexts = "
-                     "reserved[1] = %d, batch_size = %d)", cfg->reserved[2], cfg->reserved[1], cfg->batch_size);
+    MPIG_REQUIRE(cfg->ctas_per_sm >= 0 && cfg->ctas_per_sm <= 2, MPIG_EINVAL,
+                 "mpig_create: ctas_per_sm = %d is not 0, 1 or 2", cfg->ctas_per_sm);
+    MPIG_REQUIRE(cfg->num_contexts >= 0 && cfg->num_contexts <= cfg->batch_size, MPIG_EINVAL,
+                 "mpig_create: num_contexts = %d outside [0, batch_size = %d]", cfg->num_contexts, cfg->batch_size);
+    if (cfg->dense_tail_rows != 0) {   // shared dense mode: R tail rows per request, the prompt rows once per slot
+        MPIG_REQUIRE(cfg->dense_tail_rows >= 1 && cfg->dense_tail_rows <= cfg->max_length, MPIG_EINVAL,
+                     "mpig_create: dense_tail_rows = %d outside [1, max_length = %d]", cfg->dense_tail_rows, cfg->max_length);
+        MPIG_REQUIRE(cfg->num_contexts > 0 && cfg->num_contexts < cfg->batch_size, MPIG_EINVAL,
+                     "mpig_create: dense_tail_rows = %d needs fewer context slots than requests (num_contexts = %d, batch_size = %d)",
+                     cfg->dense_tail_rows, cfg->num_contexts, cfg->batch_size);
         MPIG_REQUIRE(cfg->alloc_dense_kv, MPIG_EINVAL,
-                     "mpig_create: dense_tail_rows (reserved[2]) = %d needs alloc_dense_kv = 1 (the context owns the dense KV)",
-                     cfg->reserved[2]);
+                     "mpig_create: dense_tail_rows = %d needs alloc_dense_kv = 1 (the context owns the dense KV)", cfg->dense_tail_rows);
     }
-    if (cfg->reserved[3] != 0) {   // shared spill: requests that share a slot spill into it, each seeing only its own spilled keys
-        MPIG_REQUIRE(cfg->reserved[3] == 1, MPIG_EINVAL, "mpig_create: shared_spill (reserved[3]) = %d is not 0 or 1", cfg->reserved[3]);
-        MPIG_REQUIRE(cfg->reserved[1] > 0 && cfg->reserved[1] < cfg->batch_size && cfg->batch_size <= 32, MPIG_EINVAL,
-                     "mpig_create: shared_spill (reserved[3]) needs fewer context slots than requests and at most 32 requests (one "
-                     "visibility bit each): num_contexts = reserved[1] = %d, batch_size = %d", cfg->reserved[1], cfg->batch_size);
+    if (cfg->shared_spill != 0) {   // shared spill: requests that share a slot spill into it, each seeing only its own spilled keys
+        MPIG_REQUIRE(cfg->shared_spill == 1, MPIG_EINVAL, "mpig_create: shared_spill = %d is not 0 or 1", cfg->shared_spill);
+        MPIG_REQUIRE(cfg->num_contexts > 0 && cfg->num_contexts < cfg->batch_size && cfg->batch_size <= 32, MPIG_EINVAL,
+                     "mpig_create: shared_spill needs fewer context slots than requests and at most 32 requests (one "
+                     "visibility bit each): num_contexts = %d, batch_size = %d", cfg->num_contexts, cfg->batch_size);
     }
+    for (int i = 0; i < 4; ++i)
+        MPIG_REQUIRE(cfg->reserved[i] == 0, MPIG_EINVAL, "mpig_create: reserved[%d] = %d must be zero", i, cfg->reserved[i]);
     struct RestoreDevice {
         int prev = -1;
         RestoreDevice() { if (cudaGetDevice(&prev) != cudaSuccess) prev = -1; }
@@ -132,9 +144,9 @@ int mpig_create(const mpig_config *cfg, mpig_ctx **out) {
     // segment each stream all of its candidates and keep a sub-range: the same bucket bytes and sweep instructions r times over)
     {
         int c_target = 1;
-        // `occ` CTAs of the probing / fused kernels share an SM (reserved[0]; default 1: one 1024-thread CTA per SM; 2: clusters
+        // `occ` CTAs of the probing / fused kernels share an SM (ctas_per_sm; default 1: one 1024-thread CTA per SM; 2: clusters
         // twice as large made of 512-thread CTAs, two per SM, whose latency phases overlap each other)
-        const int occ = (cfg->reserved[0] == 2) ? 2 : 1;
+        const int occ = (cfg->ctas_per_sm == 2) ? 2 : 1;
         // ... and only while all B*Hq clusters stay resident at once: a cluster occupies SMs of ONE GPC and the H100's GPCs have
         // unequal SM counts, so fewer clusters of 4 fit than #SMs / 4 (a second wave of clusters doubles the launch)
         const long long heads = (long long)cfg->batch_size * cfg->num_attention_heads;
@@ -157,17 +169,17 @@ int mpig_create(const mpig_config *cfg, mpig_ctx **out) {
     ctx->BG = cfg->batch_size * cfg->num_key_value_heads;
     ctx->rec_bytes = 2 * cfg->head_dim * 2;
     ctx->num_sms = prop.multiProcessorCount;
-    ctx->cta_per_sm = (cfg->reserved[0] == 2) ? 2 : 1;
+    ctx->cta_per_sm = (cfg->ctas_per_sm == 2) ? 2 : 1;
     ctx->max_cluster = ctx_max_cluster;
     ctx->bitmap_words = (cfg->max_length + 31) / 32;
     ctx->layers.resize(cfg->num_layers);
-    ctx->C = cfg->reserved[1] > 0 ? cfg->reserved[1] : cfg->batch_size;
+    ctx->C = cfg->num_contexts > 0 ? cfg->num_contexts : cfg->batch_size;
     ctx->n_off.assign(cfg->num_layers, std::vector<int>(ctx->C, 0));
     ctx->h_slot_of.resize(cfg->batch_size);
     for (int b = 0; b < cfg->batch_size; ++b) ctx->h_slot_of[b] = b % ctx->C;
-    ctx->dense_tail_rows = cfg->reserved[2];
+    ctx->dense_tail_rows = cfg->dense_tail_rows;
     ctx->h_dense_base.assign(cfg->batch_size, 0);
-    ctx->shared_spill = cfg->reserved[3] == 1;
+    ctx->shared_spill = cfg->shared_spill == 1;
     ctx->h_private_lo.assign(cfg->num_layers, std::vector<int>(ctx->C, 0));
 
     const size_t M = (size_t)cfg->max_length, BG = (size_t)ctx->BG, L = (size_t)cfg->L, d = (size_t)cfg->head_dim;
@@ -423,10 +435,6 @@ int mpig_set_option(mpig_ctx *ctx, const char *key, int64_t value) {
     if (k == "save_mask") ctx->save_mask = (int)value;
     else if (k == "attend_ctas") ctx->attend.ctas = (int)value;
     else if (k == "attend_warps") ctx->attend.warps = (int)value;
-    else if (k == "attend_stages") ctx->attend.stages = (int)value;
-    else if (k == "attend_impl") {
-        MPIG_REQUIRE(value == 1, MPIG_EUNSUPPORTED, "attend_impl=%lld: the CUDA-core tile math was removed; only 1 (tensor-core) exists", (long long)value);
-    }
     else if (k == "decode_impl") ctx->decode_impl = (int)value;
     else if (k == "fused_selcap") ctx->fused_selcap = value < 16 ? 16 : (value > 8192 ? 8192 : ((int)value + 15) & ~15);
     else if (k == "fused_kreg") ctx->fused_kreg = value ? 1 : 0;
@@ -451,7 +459,6 @@ int mpig_set_option(mpig_ctx *ctx, const char *key, int64_t value) {
     else if (k == "keyhash_impl") ctx->keyhash_impl = (int)value;
     else if (k == "pdl_first") ctx->pdl_first = (int)value;
     else if (k == "keyhash_skip") ctx->keyhash_skip = (int)value;
-    else if (k == "keyhash_stages") ctx->keyhash_stages = value < 2 ? 2 : (value > 4 ? 4 : (int)value);
     else if (k == "attend_skip") ctx->attend_skip = (int)value;
     else if (k == "attend_debug") {
         ctx->attend_debug = (int)value;

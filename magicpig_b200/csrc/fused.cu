@@ -1188,7 +1188,6 @@ int launch_fused(mpig_ctx *ctx, int layer, const void *q, const void *k, const v
                  const mpig_peer *peer, int peer_rank, int peer_world, volatile uint32_t *host_flags, uint32_t host_epoch) {
     const FusedPlan &fp = fused_plan(ctx);
     MPIG_REQUIRE(fp.ok, MPIG_EUNSUPPORTED, "fused decode: shape not supported (L=%d, H=%d, segments=%d)", ctx->cfg.L, ctx->H, ctx->nseg);
-    ctx->last_probe_layer = layer;
     if (!fp.hash_in_kernel) {
         int rc = launch_simhash(ctx, q, ctx->codes, ctx->qnorm, nullptr, s, pdl && ctx->pdl_first);
         if (rc) return rc;
@@ -1220,7 +1219,6 @@ int launch_fused_tokens(mpig_ctx *ctx, int layer, int T, const void *q, const vo
     MPIG_REQUIRE(fp.ok, MPIG_EUNSUPPORTED, "mpig_decode_tokens: shape not supported by the fused decode (L=%d, H=%d, T=%d, segments=%d)",
                  ctx->cfg.L, ctx->H, T, ctx->nseg);
     MPIG_REQUIRE(ctx->hash_func_set, MPIG_ESTATE, "SimHash before mpig_set_hash_func: the projection has not been set");
-    ctx->last_probe_layer = layer;
     int rc = MPIG_OK;
     if (ctx->Wcap > 0) {   // the T new rows (centred keys) go to the window first: the attention reads them from HBM
         rc = launch_append_tokens(ctx, append_params(ctx, ctx->layers[layer], k, v, false), T, s);

@@ -295,10 +295,9 @@ extern "C" int mpig_hash_keys(mpig_ctx *ctx, const void *keys_bf16, int n, int16
     const int m_tiles = (int)((rows + KH_M - 1) / KH_M);
     const int n_tiles = (L + T - 1) / T;
     if (ctx->keyhash_impl == 1) {
-        // B stages: as many as fit beside the two A slots, at most keyhash_stages
+        // B stages: as many as fit beside the two A slots (2 on sm_90a)
         const size_t fixed = 1024 + 128;
         int nb = (int)((227 * 1024 - 2 * (size_t)KH_A_BYTES - fixed) / KH_B_BYTES);
-        if (nb > ctx->keyhash_stages) nb = ctx->keyhash_stages;
         if (nb > KHP_MAX_STAGES) nb = KHP_MAX_STAGES;
         const size_t smem = 2 * (size_t)KH_A_BYTES + (size_t)nb * KH_B_BYTES + fixed;
         MPIG_FUNC_ATTR(keyhash_pipe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);

@@ -407,7 +407,7 @@ int mpig_spill_window(mpig_ctx *ctx, int keep, int32_t *spilled_out, void *strea
                 MPIG_REQUIRE(o == b || slot[o] != slot[b] || wl[o] == 0, MPIG_ESTATE,
                              "mpig_spill_window: request %d would spill %d rows into context slot %d, which request %d (window of %d rows) "
                              "shares; a shared request generates at most generation_buffer tokens unless the context was created "
-                             "with shared spill (reserved[3])", b, meta[b], slot[b], o, wl[o]);
+                             "with shared spill (mpig_config.shared_spill)", b, meta[b], slot[b], o, wl[o]);
     }
     for (int l = 0; l < nl; ++l) {
         if (!ctx->layers[l].sparse) continue;
@@ -481,7 +481,7 @@ int mpig_spill_window(mpig_ctx *ctx, int keep, int32_t *spilled_out, void *strea
 int mpig_read_visibility(mpig_ctx *ctx, uint32_t *vis_out, void *stream) {
     mpig::DeviceGuard _dg(ctx);  // run on the context's device whatever the caller's current device is
     MPIG_REQUIRE(ctx && vis_out, MPIG_EINVAL, "mpig_read_visibility: null argument");
-    MPIG_REQUIRE(ctx->shared_spill, MPIG_ESTATE, "mpig_read_visibility: the context has no shared spill (reserved[3])");
+    MPIG_REQUIRE(ctx->shared_spill, MPIG_ESTATE, "mpig_read_visibility: the context has no shared spill (mpig_config.shared_spill)");
     MPIG_CUDA(cudaMemcpyAsync(vis_out, ctx->vis, (size_t)ctx->C * ctx->cfg.max_length * sizeof(uint32_t), cudaMemcpyDeviceToDevice,
                               as_stream(stream)));
     return MPIG_OK;

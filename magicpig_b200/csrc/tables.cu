@@ -622,7 +622,6 @@ static int launch_probe_t(mpig_ctx *ctx, int layer, const int32_t *query, int32_
 }
 
 int launch_probe(mpig_ctx *ctx, int layer, const int32_t *query, int32_t *results, int32_t *nnz, cudaStream_t s, bool pdl) {
-    ctx->last_probe_layer = layer;
     // table ids 0..L-1 must stay clear of the two reserved tag values
     if (ctx->cfg.L <= 254) return launch_probe_t<uint8_t>(ctx, layer, query, results, nnz, s, pdl);
     return launch_probe_t<uint16_t>(ctx, layer, query, results, nnz, s, pdl);

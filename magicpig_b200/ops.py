@@ -78,10 +78,10 @@ class Context:
         for i, l in enumerate(self.dense_layers):
             cfg.dense_layers[i] = l
         cfg.alloc_dense_kv = 1 if alloc_dense_kv else 0
-        cfg.reserved[0] = int(os.environ.get("MPIG_CTA_PER_SM", "1"))   # experiment switch: 2 = clusters of 512-thread CTAs, two per SM
-        cfg.reserved[1] = int(num_contexts)
-        cfg.reserved[2] = int(dense_tail_rows)
-        cfg.reserved[3] = 1 if shared_spill else 0
+        cfg.ctas_per_sm = int(os.environ.get("MPIG_CTA_PER_SM", "1"))   # experiment switch: 2 = clusters of 512-thread CTAs, two per SM
+        cfg.num_contexts = int(num_contexts)
+        cfg.dense_tail_rows = int(dense_tail_rows)
+        cfg.shared_spill = 1 if shared_spill else 0
         h = ctypes.c_void_p()
         with torch.cuda.device(self.device):
             N.check(self.lib.mpig_create(ctypes.byref(cfg), ctypes.byref(h)), "mpig_create")

@@ -24,7 +24,7 @@ ap.add_argument("--L", type=int, default=150)
 ap.add_argument("--layers", type=int, default=6)
 ap.add_argument("--reps", type=int, default=10)
 ap.add_argument("--fracs", default="")
-ap.add_argument("--variants", default="impl=1,tma=1,warps=12;impl=1,tma=0,warps=12;impl=0,tma=1,warps=12;impl=1,tma=1,warps=8;impl=1,tma=0,warps=8;impl=1,tma=1,warps=6;impl=1,tma=0,warps=6")
+ap.add_argument("--variants", default="tma=1,warps=12;tma=0,warps=12;tma=1,warps=8;tma=0,warps=8;tma=1,warps=6;tma=0,warps=6")
 args = ap.parse_args()
 
 dev = "cuda:0"
@@ -114,10 +114,8 @@ print(f"probe    {us:7.2f} us/launch   {pb / us / 1e3:7.1f} GB/s algorithmic")
 ab = tot * 520 + H * 520
 for var in args.variants.split(";"):
     kv = dict(x.split("=") for x in var.split(","))
-    ctx.set_option("attend_impl", int(kv.get("impl", 1)))
     ctx.set_option("attend_tma", int(kv.get("tma", 1)))
     ctx.set_option("attend_warps", int(kv.get("warps", 12)))
-    ctx.set_option("attend_stages", int(kv.get("stages", 1)))
     ctx.set_option("attend_ctas", int(kv.get("ctas", 0)))
     try:
         us = timeit(lambda l: ctx.attention_wrapper(l, K, L, out, mve, q[l], qn[l], res[l], nnz[l]), args.reps)
@@ -127,7 +125,7 @@ for var in args.variants.split(";"):
 
 # how does attend scale with the amount of work?  (separates fixed latency from throughput)
 if args.fracs:
-    ctx.set_option("attend_impl", 1); ctx.set_option("attend_tma", 1); ctx.set_option("attend_warps", 12)
+    ctx.set_option("attend_tma", 1); ctx.set_option("attend_warps", 12)
     for f in [float(x) for x in args.fracs.split(",")]:
         nnz_f = [(x.float() * f).int() for x in nnz]
         tot_f = sum(int(x.sum()) for x in nnz_f) / nl
@@ -147,9 +145,8 @@ kn_ = torch.randn((nl, B * Hkv, d), generator=g, device=dev).bfloat16()
 vn_ = torch.randn((nl, B * Hkv, d), generator=g, device=dev).bfloat16()
 out2 = torch.zeros((B, Hq * d), dtype=torch.bfloat16, device=dev)
 ctx.plan()
-for var in ["impl=1,tma=1,warps=12", "impl=1,tma=0,warps=12"]:
+for var in ["tma=1,warps=12", "tma=0,warps=12"]:
     kv = dict(x.split("=") for x in var.split(","))
-    ctx.set_option("attend_impl", int(kv.get("impl", 1)))
     ctx.set_option("attend_tma", int(kv.get("tma", 1)))
     ctx.set_option("attend_warps", int(kv.get("warps", 12)))
     us = timeit(lambda l: ctx.decode(l, q[l], kn_[l], vn_[l], out2), args.reps)

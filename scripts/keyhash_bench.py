@@ -37,10 +37,6 @@ for impl in (1, 0):
     ms = timeit(lambda: ctx.hash_keys(keys, out=out))
     print(f"mpig_hash_keys impl={impl} (wgmma): {ms * 1e3:8.1f} us   {flop / ms / 1e9:7.1f} TFLOP/s   out {out.numel() * 2 / 1e6:.0f} MB -> {out.numel() * 2 / ms / 1e6:.0f} GB/s")
 ctx.set_option("keyhash_impl", 1)
-ctx.set_option("keyhash_stages", 3)
-ms = timeit(lambda: ctx.hash_keys(keys, out=out))
-print(f"  3 B stages: {ms * 1e3:8.1f} us")
-ctx.set_option("keyhash_stages", 2)
 for sk in (1, 2, 3, 4, 7):
     ctx.set_option("keyhash_skip", sk)
     ms = timeit(lambda: ctx.hash_keys(keys, out=out))

@@ -1,4 +1,4 @@
-"""Batched decode over ONE shared context (context slots, mpig_config.reserved[1]) -> one JSON line.
+"""Batched decode over ONE shared context (context slots, mpig_config.num_contexts) -> one JSON line.
 
 Llama-3.1-8B with random weights, a synthetic P-token context filled once (request 0) and forked to the other requests, K10
 L150, one context slot (num_contexts = 1), B in {1, 2, 4, 8}, distinct token ids per request.  For every B: the captured step()

@@ -1,4 +1,4 @@
-"""Batched decode over one context with a shared dense prefix (dense_tail_rows, mpig_config.reserved[2]) -> one JSON line.
+"""Batched decode over one context with a shared dense prefix (mpig_config.dense_tail_rows) -> one JSON line.
 
 Llama-3.1-8B with random weights, a synthetic P-token context filled once (request 0) and forked, K10 L150, one context slot,
 R = generation_buffer + t_max dense tail rows.  For every B: the captured step() time (CUDA events, median over blocks of

@@ -2,7 +2,7 @@
 for B requests forked from one P-token prompt in one context slot, with dense_tail_rows R, replayed for N generated tokens per
 request in two arms:
 
-  a  shared spill (mpig_config.reserved[3]), generation_buffer = 256 (--gen-buf): spill_window() between replays whenever the
+  a  shared spill (mpig_config.shared_spill), generation_buffer = 256 (--gen-buf): spill_window() between replays whenever the
      window is full; each request's spilled tokens go into the shared store and tables, private to it
   b  generation_buffer = N + 8, no spill: every sparse layer attends the whole generation densely
 

@@ -11,6 +11,8 @@ request, each filled with the same data, given the same per-request q / k / v:
   * memory: one slot less is the per-slot bytes less; B = 8 on one C2-size context;
   * the drop-in class and the Llama runner.
 """
+import ctypes
+
 import pytest
 import torch
 
@@ -337,6 +339,31 @@ def test_spill_exclusive_slots_out_of_request_order(cuda_lib):
         assert_tables_equal((o[c], i[c]), (ro[0], ri[0]))
     for _ in range(3):
         twin_step(sh, tw, gen)
+
+
+def test_config_and_option_refusals(cuda_lib, monkeypatch):
+    """mpig_create refuses ctas_per_sm outside {0, 1, 2} and a non-zero reserved field; option keys that select nothing are
+    unknown keys."""
+    hf = synth.make_hash_func(d, 6, 24, seed=1)
+    for v in ("3", "-1"):
+        monkeypatch.setenv("MPIG_CTA_PER_SM", v)
+        with pytest.raises(N.MagicPigError, match="ctas_per_sm"):
+            make_ctx(3, 1, 4, 4, 400, 6, 24, hf)
+    monkeypatch.delenv("MPIG_CTA_PER_SM")
+    ctx = make_ctx(3, 1, 4, 4, 400, 6, 24, hf)
+    for key in ("attend_stages", "keyhash_stages", "attend_impl"):
+        with pytest.raises(N.MagicPigError, match="unknown key"):
+            ctx.set_option(key, 1)
+    cfg = N.MpigConfig(abi_version=N.MPIG_ABI_VERSION, device=torch.device(DEV).index or 0, K=6, L=24, num_layers=1,
+                       num_attention_heads=4, num_key_value_heads=4, head_dim=d, batch_size=3, max_length=400)
+    h = ctypes.c_void_p()
+    assert cuda_lib.mpig_create(ctypes.byref(cfg), ctypes.byref(h)) == N.MPIG_OK
+    cuda_lib.mpig_destroy(h)
+    for i in range(4):
+        cfg.reserved[i] = 1
+        assert cuda_lib.mpig_create(ctypes.byref(cfg), ctypes.byref(h)) == -1   # MPIG_EINVAL
+        assert f"reserved[{i}]".encode() in cuda_lib.mpig_last_error()
+        cfg.reserved[i] = 0
 
 
 def test_refusals(cuda_lib):
