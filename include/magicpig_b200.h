@@ -422,6 +422,16 @@ int mpig_plan_chunk(mpig_ctx *ctx, int T, void *stream);
 int mpig_chunk_attend(mpig_ctx *ctx, int layer, int T, const void *query_bf16, const void *key_bf16, const void *value_bf16,
                       void *out_bf16, void *stream);
 
+/* ---- prefill attention ---------------------------------------------------------------------------------------------------
+ * Exact causal attention of a prompt chunk over its keys (flashinfer single_prefill_with_kv_cache, causal, NHD;
+ * models/llama.py:250-257).  q bf16 (q_len, Hq, d), k/v bf16 (kv_len, Hkv, d) with the context's per-rank head counts;
+ * query i sees keys [0, kv_len - q_len + i].  out bf16 (q_len, Hq, d); out_f32 (q_len, Hq, d) or NULL.  Reads and writes
+ * no context state (any layer, any pending step); no host synchronisation; capturable.  csrc/attend_prefill.cu: wgmma
+ * tensor-core tiles fed by TMA.  MPIG_EINVAL: q_len < 1, kv_len < q_len, a null input or output, or a base pointer that is not
+ * 16-byte aligned; MPIG_EUNSUPPORTED: head_dim != 128 or Hq / Hkv outside [1, 8]. */
+int mpig_prefill_attend(mpig_ctx *ctx, const void *q_bf16, const void *k_bf16, const void *v_bf16, int q_len, int kv_len,
+                        void *out_bf16, float *out_f32, void *stream);
+
 /* ---- dense layers (attnserver.py:116-120, 235-259), only with cfg.alloc_dense_kv -------------- */
 /* k, v bf16 (P, Hkv, d) -- the prefill cache in NHD layout as models/llama.py:282 passes it. */
 int mpig_dense_fill(mpig_ctx *ctx, int layer, int request, const void *k_bf16, const void *v_bf16,

@@ -94,6 +94,7 @@ _SIGNATURES = {
     "mpig_reserve_chunk_tokens": (_i, [_vp, _i]),
     "mpig_plan_chunk": (_i, [_vp, _i, _vp]),
     "mpig_chunk_attend": (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "mpig_prefill_attend": (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp]),
     "mpig_fork_request": (_i, [_vp, _i, _i, _vp]),
     "mpig_bind_request": (_i, [_vp, _i, _i, _vp]),
     "mpig_reorder_requests": (_i, [_vp, _vp, _vp]),

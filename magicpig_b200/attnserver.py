@@ -47,6 +47,32 @@ def beam_sources(parents: torch.Tensor):
     return src_of.to(torch.int32), request_of.to(torch.int32)
 
 
+PREFILL_DTYPES = (torch.bfloat16, torch.float16, torch.float32)
+
+
+def check_prefill_args(q, k, v, num_attention_heads: int, num_key_value_heads: int, head_dim: int, causal: bool = True,
+                       kv_layout: str = "NHD"):
+    """The refusals of LSHSparseAttnServer.prefill_attention, before anything runs: ValueError unless causal, kv_layout "NHD",
+    q (q_len, Hq, d) and k / v (kv_len, Hkv, d) with the server's per-rank head counts, 1 <= q_len <= kv_len, k and v of one shape,
+    and floating dtypes (bf16, fp16 or fp32).  Shape and dtype checks only: the tensors may live anywhere."""
+    if not causal:
+        raise ValueError("prefill_attention computes causal attention only (causal=False is not supported)")
+    if kv_layout != "NHD":
+        raise ValueError(f"prefill_attention takes the NHD layout only, got kv_layout={kv_layout!r}")
+    Hq, Hkv, d = num_attention_heads, num_key_value_heads, head_dim
+    if q.dim() != 3 or tuple(q.shape[1:]) != (Hq, d):
+        raise ValueError(f"q must be (q_len, {Hq}, {d}), got {tuple(q.shape)}")
+    if k.dim() != 3 or tuple(k.shape[1:]) != (Hkv, d):
+        raise ValueError(f"k must be (kv_len, {Hkv}, {d}), got {tuple(k.shape)}")
+    if tuple(v.shape) != tuple(k.shape):
+        raise ValueError(f"v must have k's shape {tuple(k.shape)}, got {tuple(v.shape)}")
+    if not 1 <= q.shape[0] <= k.shape[0]:
+        raise ValueError(f"need 1 <= q_len <= kv_len, got q_len={q.shape[0]}, kv_len={k.shape[0]}")
+    for name, t in (("q", q), ("k", k), ("v", v)):
+        if t.dtype not in PREFILL_DTYPES:
+            raise ValueError(f"{name} must be bf16, fp16 or fp32, got {t.dtype}")
+
+
 class LSHSparseAttnServer:
     def __init__(self,
                  config,
@@ -322,6 +348,20 @@ class LSHSparseAttnServer:
         else:
             self.ctx.decode_tokens(layer_idx, T, q, k, v, out)
         return out.to(query_states.dtype)
+
+    def prefill_attention(self, q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, causal: bool = True,
+                          allow_fp16_qk_reduction: bool = False, kv_layout: str = "NHD") -> torch.Tensor:
+        """Not in the reference's server: the prefill attention the reference calls FlashInfer for (llama.py:250-257,
+        flashinfer.prefill.single_prefill_with_kv_cache), with the same keywords, so that call becomes
+        self.attention_server.prefill_attention(...).  q (q_len, Hq, d), k / v (kv_len, Hkv, d) NHD -> (q_len, Hq, d) in q's dtype:
+        exact causal softmax attention, query i seeing keys [0, kv_len - q_len + i] (the chunk's queries are the last q_len
+        positions), scale 1/sqrt(d).  Inputs are rounded to bf16 for the tensor cores; the product, the softmax and P.V accumulate
+        in fp32, so allow_fp16_qk_reduction is accepted and has no effect.  causal=False or another kv_layout raises ValueError.
+        Uses no server state (any layer, before or after fill); capturable."""
+        check_prefill_args(q, k, v, self.num_attention_heads, self.num_key_value_heads, self.head_dim, causal, kv_layout)
+        out = self.ctx.prefill_attend(q.to(torch.bfloat16).contiguous(), k.to(torch.bfloat16).contiguous(),
+                                      v.to(torch.bfloat16).contiguous())
+        return out.to(q.dtype)
 
     def clear(self):
         """attnserver.py:314-331."""

@@ -19,9 +19,7 @@
 // tiles; a producer warp keeps two A slots and a ring of B stages filled by TMA (a_full/a_empty, b_full/b_empty), so the
 // next tables' B tile is in shared memory while the consumer warpgroups run the MMAs and the sign-pack epilogue of the
 // current one.  keyhash_kernel is one tile per CTA.
-#include <cuda.h>
-
-#include "common.cuh"
+#include "gmma_common.cuh"
 
 namespace mpig {
 
@@ -30,28 +28,6 @@ constexpr int KH_D = 128;        // head_dim
 constexpr int KH_N = 256;        // accumulator columns per tile: T = KH_N / K whole tables
 constexpr uint32_t KH_A_BYTES = 2u * KH_M * 128u;   // two 64-dim atoms of 128 rows x 128 B
 constexpr uint32_t KH_B_BYTES = 2u * KH_N * 128u;   // two 64-dim atoms of 256 rows x 128 B
-
-__device__ __forceinline__ void tma_load_2d(void *smem_dst, const CUtensorMap *map, int c0, int c1, uint64_t *bar) {
-    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(
-                     smem_u32(smem_dst)),
-                 "l"(map), "r"(c0), "r"(c1), "r"(smem_u32(bar))
-                 : "memory");
-}
-__device__ __forceinline__ void expect_tx(uint64_t *bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (8-row x 128-byte atoms, 1024 B apart)
-__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t saddr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr >> 4) & 0x3FFF);   // start address
-    d |= (uint64_t)1 << 16;                    // leading byte offset (unused for swizzled K-major)
-    d |= (uint64_t)(1024 >> 4) << 32;          // stride byte offset: next 8-row group
-    d |= (uint64_t)1 << 62;                    // SWIZZLE_128B
-    return d;
-}
 
 // D(64 x 256, fp32) (+)= A(64 x 16, smem) * B(16 x 256, smem), both bf16 K-major; scale_d = 0 overwrites D
 __device__ __forceinline__ void wgmma_m64n256k16(float (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
@@ -248,19 +224,10 @@ __global__ void __launch_bounds__(KHP_THREADS, 1)
     }
 }
 
-typedef CUresult (*PFN_encodeTiled)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
-                                    const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                    CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
 static int make_map_2d(CUtensorMap *map, const void *base, uint64_t rows, uint32_t box_rows) {
-    static PFN_encodeTiled encode = nullptr;
-    if (!encode) {
-        void *fn = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        MPIG_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q));
-        MPIG_REQUIRE(fn && q == cudaDriverEntryPointSuccess, MPIG_ECUDA, "cuTensorMapEncodeTiled entry point not available");
-        encode = (PFN_encodeTiled)fn;
-    }
+    PFN_encodeTiled encode;
+    int rc = tensor_map_encoder(&encode);
+    if (rc) return rc;
     const cuuint64_t dims[2] = {(cuuint64_t)KH_D, (cuuint64_t)rows};   // innermost first
     const cuuint64_t strides[1] = {(cuuint64_t)KH_D * 2};              // bytes between rows
     const cuuint32_t box[2] = {64, box_rows};                          // 64 bf16 = 128 B = one swizzle atom wide

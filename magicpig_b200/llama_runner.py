@@ -8,9 +8,11 @@ residual -> RMSNorm -> gated MLP -> residual), random-init weights of the named 
 library GEMMs (cuBLAS through torch).  Only the attention server is product code; everything in
 this file is harness.
 
-Context is synthetic: instead of a 98K-token prefill the per-layer K/V caches are filled with seeded
-random tensors through the server's own `fill()` / `build_table()` (the reference's prefill-time
+Context is synthetic by default: instead of a 98K-token prefill the per-layer K/V caches are filled with
+seeded random tensors through the server's own `fill()` / `build_table()` (the reference's prefill-time
 API), so tables, key norms, centring and the sink/local window are all produced by the real path.
+`prefill()` is the real thing for one request: the forward of a prompt's token ids, with prefill
+attention on the server's tensor-core kernel (`prefill_attention`), into the same fill()/build_table().
 """
 from __future__ import annotations
 
@@ -73,6 +75,20 @@ def plan_turn_chunks(lengths, t_max: int, room: int):
         T = min(step, total - start)
         plan.append((start, T, [T - min(max(n - start, 0), T) for n in lengths]))
     return plan
+
+
+def plan_prefill_chunks(P: int, chunk_size: int, num_sink: int, num_local: int, max_length: int):
+    """The (start, end) row ranges of the prompt chunks of a P-token prefill (llama.py:310-313: chunks of chunk_size, the last one
+    ending at P).  Refuses (ValueError) a prompt the sparse layers cannot hold, P <= num_sink + num_local (nothing left to sample) or
+    P > max_length, and chunk_size < 1.  Pure host arithmetic."""
+    P, chunk_size = int(P), int(chunk_size)
+    if chunk_size < 1:
+        raise ValueError(f"chunk_size must be >= 1, got {chunk_size}")
+    if P <= num_sink + num_local:
+        raise ValueError(f"a prompt of {P} tokens does not reach past the sink + local window ({num_sink} + {num_local})")
+    if P > max_length:
+        raise ValueError(f"a prompt of {P} tokens exceeds max_length {max_length}")
+    return [(start, min(start + chunk_size, P)) for start in range(0, P, chunk_size)]
 
 
 class LlamaDecodeRunner:
@@ -219,6 +235,61 @@ class LlamaDecodeRunner:
             srv.fork(0, range(1, self.B))
         self.pos.fill_(P - 1)
         torch.cuda.synchronize(self.device)
+
+    def prefill(self, ids: torch.Tensor, request: int = 0, chunk_size: int = 8192):
+        """The reference's LLM.prefill (llama.py:304-325) for one request: ids (P,) or (1, P) token ids.  Layer by layer, chunk by
+        chunk: RMSNorm, the q/k/v projection, RoPE at positions 0 .. P-1, the chunk's K/V into one (P, Hkv, d) cache, the server's
+        prefill_attention over cache[:end], wo and the residual; then the MLP of every chunk; then fill() and build_table() of the
+        layer.  Afterwards self.pos[request] = P - 1 and self.logits[request] holds the logits after the last prompt token: the state
+        synthetic_prefill leaves, so a captured step() continues the generation.  With fewer contexts than requests the prompt goes
+        into request 0 and every other request is forked from it (as synthetic_prefill(shared=True)).  Prompts of P <= num_sink +
+        num_local or P > max_length are refused before anything is written.  Eager library GEMMs; synchronises, not capturable."""
+        assert self.tp_world == 1, "prefill is built for a single GPU"
+        sh, srv = self.shape, self.server
+        ids = ids.to(self.device).long().reshape(-1)
+        P = ids.numel()
+        chunks = plan_prefill_chunks(P, chunk_size, srv.num_sink_tokens, srv.num_local_tokens, srv.max_length)
+        fork = srv.ctx.num_contexts < self.B
+        if fork and request != 0:
+            raise ValueError(f"with {srv.ctx.num_contexts} contexts for {self.B} requests the prompt goes into request 0 (got {request})")
+        if not 0 <= request < self.B:
+            raise ValueError(f"request {request} outside [0, {self.B})")
+        d, Hq, Hkv, hs, it = self.d, self.Hq_loc, self.Hkv_loc, sh.hidden_size, self.it_loc
+        srv.alloc_buffer(P)
+        k_cache = torch.empty((P, Hkv, d), dtype=torch.bfloat16, device=self.device)
+        v_cache = torch.empty_like(k_cache)
+        h = F.embedding(ids, self.embed)   # (P, hs)
+        cos, sin = self.cos[:P, None, :], self.sin[:P, None, :]
+
+        def rope(x, a, b):   # x (n, H, d) at positions a .. b-1, rotate-half (models/utils.py:36-44)
+            x1, x2 = x[..., : d // 2], x[..., d // 2:]
+            return x * cos[a:b] + torch.cat([-x2, x1], dim=-1) * sin[a:b]
+
+        for li, lw in enumerate(self.layers):
+            for a, b in chunks:
+                x = F.rms_norm(h[a:b], (hs,), lw["ln1"], sh.rms_norm_eps)
+                qkv = F.linear(x, lw["wqkv"])   # (n, (Hq+2Hkv)d)
+                n = b - a
+                q = rope(qkv[:, : Hq * d].reshape(n, Hq, d), a, b)
+                k_cache[a:b] = rope(qkv[:, Hq * d:(Hq + Hkv) * d].reshape(n, Hkv, d), a, b)
+                v_cache[a:b] = qkv[:, (Hq + Hkv) * d:].reshape(n, Hkv, d)
+                o = srv.prefill_attention(q, k_cache[:b], v_cache[:b], causal=True, kv_layout="NHD")
+                h[a:b] += F.linear(o.reshape(n, Hq * d), lw["wo"])
+            for a, b in chunks:
+                x = F.rms_norm(h[a:b], (hs,), lw["ln2"], sh.rms_norm_eps)
+                gu = F.linear(x, lw["w_gate_up"])
+                h[a:b] += F.linear(F.silu(gu[:, :it]) * gu[:, it:], lw["w_down"])
+            srv.fill(li, request, k_cache, v_cache, P)
+            srv.build_table(li, request, P)
+        x = F.rms_norm(h[P - 1:], (hs,), self.norm, sh.rms_norm_eps)
+        self.logits[request] = F.linear(x, self.lm_head).float()[0]
+        self.pos[request] = P - 1
+        if fork:
+            srv.fork(0, range(1, self.B))
+            self.pos.fill_(P - 1)
+            self.logits[1:] = self.logits[0]
+        torch.cuda.synchronize(self.device)
+        return self.logits[request]
 
     def fork(self, src: int, dst: int):
         """Request dst continues from request src: the server's fork (shared context, copied window and dense KV) and src's

@@ -335,6 +335,25 @@ class Context:
         self.last_tokens = int(T)
         return out
 
+    def prefill_attend(self, q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, out: Optional[torch.Tensor] = None,
+                       out_f32: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Exact causal attention of a prompt chunk over its keys: q (q_len, Hq, d), k / v (kv_len, Hkv, d) bf16 NHD -> out (q_len, Hq, d)
+        bf16; query i sees keys [0, kv_len - q_len + i].  out_f32 (q_len, Hq, d) fp32, when given, receives the same values before the
+        bf16 rounding.  Uses no context state (any layer, any pending step); capturable."""
+        q_len, kv_len = q.shape[0], k.shape[0]
+        self._chk(q, torch.bfloat16, (q_len, self.Hq, self.d), "q")
+        self._chk(k, torch.bfloat16, (kv_len, self.Hkv, self.d), "k")
+        self._chk(v, torch.bfloat16, (kv_len, self.Hkv, self.d), "v")
+        if out is None:
+            out = torch.empty((q_len, self.Hq, self.d), dtype=torch.bfloat16, device=self.device)
+        else:
+            self._chk(out, torch.bfloat16, (q_len, self.Hq, self.d), "out")
+        if out_f32 is not None:
+            self._chk(out_f32, torch.float32, (q_len, self.Hq, self.d), "out_f32")
+        N.check(self.lib.mpig_prefill_attend(self._h, _ptr(q), _ptr(k), _ptr(v), int(q_len), int(kv_len), _ptr(out), _ptr(out_f32),
+                                             _stream()), "mpig_prefill_attend")
+        return out
+
     def accept(self, nodes: torch.Tensor, count: torch.Tensor):
         """Commit the root path nodes[b][0 .. count[b]) of the pending step of request b: the path's rows move to the front of
         the step in every sparse window and dense cache, and both lengths become base + count[b].  nodes: int32 (B, T), count: int32

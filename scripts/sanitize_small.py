@@ -10,7 +10,8 @@ requests sharing one context slot, shared spill (several requests of one slot sp
 the device-side reorder of requests (`reorder`: the in-place copy between requests, eager, refused and captured), the compaction
 of a shared context (`compact`: eager and between replays of a captured step, against a twin), chunk steps
 (`chunk`: the chunk attention kernel on sparse and dense layers with one and several key splits, a partial m-block and a partial last
-tile, shared spill with private keys, the shared dense prefix, a rewind and a captured step), and BASELINE's C4 and C5 per-rank
+tile, shared spill with private keys, the shared dense prefix, a rewind and a captured step), prefill attention (`prefill`: G = 7,
+partial m-blocks and a partial last key tile, eager and captured), and BASELINE's C4 and C5 per-rank
 geometry (`configs`: K11 L300 over 4 segments in clusters of 4, Hq 8 / Hkv 1 over 8 segments in clusters of 8).  Results are
 also checked against each other so a tool run doubles as a test.
 """
@@ -653,9 +654,34 @@ def chunk_case(B, Hq, Hkv, n, K, L, T, R):
     print(f"chunk B={B} Hq={Hq} Hkv={Hkv} n={n} T={T} R={R}: ok")
 
 
+def prefill_case(Hq, Hkv, q_len, kv_len):
+    """mpig_prefill_attend at G = Hq / Hkv: the last m-block and the last key tile partial; eager against a torch fp32 restatement
+    and a captured launch against the eager one."""
+    g = torch.Generator(device=dev).manual_seed(5)
+    ctx = Context(6, 24, 1, Hq, Hkv, d, 1, 512, device=dev)
+    q = torch.randn((q_len, Hq, d), generator=g, device=dev).bfloat16()
+    k = torch.randn((kv_len, Hkv, d), generator=g, device=dev).bfloat16()
+    v = torch.randn((kv_len, Hkv, d), generator=g, device=dev).bfloat16()
+    f32 = torch.empty((q_len, Hq, d), dtype=torch.float32, device=dev)
+    eager = ctx.prefill_attend(q, k, v, out_f32=f32)
+    G, off = Hq // Hkv, kv_len - q_len
+    s = torch.einsum("thd,khd->htk", q.float(), k.float().repeat_interleave(G, 1)) / d ** 0.5
+    vis = torch.arange(kv_len, device=dev)[None] <= off + torch.arange(q_len, device=dev)[:, None]
+    ref = torch.einsum("htk,khd->thd", torch.softmax(s.masked_fill(~vis[None], float("-inf")), -1), v.float().repeat_interleave(G, 1))
+    err = float((f32 - ref).abs().max() / ref.abs().max())
+    assert err <= 1e-3, f"prefill ({q_len}, {kv_len}) G={G}: {err:.3g} from the fp32 restatement"
+    out = torch.zeros_like(eager)
+    graph = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(graph):
+        ctx.prefill_attend(q, k, v, out)
+    graph.replay()
+    torch.cuda.synchronize()
+    assert torch.equal(out.view(torch.int16), eager.view(torch.int16)), "captured prefill != eager"
+    print(f"prefill Hq={Hq} Hkv={Hkv} q_len={q_len} kv_len={kv_len}: ok")
+
 if __name__ == "__main__":
     which = sys.argv[1:] or ["stages", "dense", "decode", "hostpeer", "spill", "tokens", "tree", "shared", "shared_spill", "reorder",
-                             "chunk", "configs", "compact"]
+                             "chunk", "configs", "compact", "prefill"]
     if "configs" in which:   # BASELINE's C4 and C5 per-rank geometry at small n, each against its decode_impl = 0 twin
         # the i.i.d. keys sampled here have weights near 1e-2, where 1 - (1-p)^(L-1) (Lp + 1 - p) cancels in fp32 and amplifies
         # last-bit differences: the variants differ by up to 4e-4 of a head's largest element at K11 L300 (2e-5 at K10 L150), so
@@ -665,6 +691,9 @@ if __name__ == "__main__":
     if "chunk" in which:
         chunk_case(3, 8, 2, 600, 6, 24, 37, 200)      # one key split; T*G = 148: a partial second m-block, partial last tiles
         chunk_case(3, 8, 2, 2100, 6, 24, 5, 200)      # several key splits merged by the last CTA
+    if "prefill" in which:
+        prefill_case(7, 1, 37, 300)      # 18 tokens per m-block: a partial third m-block; a partial third key tile
+        prefill_case(28, 4, 5, 129)      # one m-block of 5 tokens over two key tiles, the second holding one key
     if "compact" in which:
         compact_case(3, 1, 4, 2, 700, 6, 24)
         compact_case(4, 2, 4, 2, 700, 6, 24)             # both slots reclaimed in one call
