@@ -46,6 +46,35 @@ int mpig_aux_norm_qkv_rope(const void *wqkv, const void *h_in, const void *delta
  * Returns the previous mask. */
 int mpig_aux_set_pdl(int mask);
 
+/* One token for each of B rows of fp32 logits (B, V), row stride ld >= V: temperature / top-p sampling as the reference's
+ * caller does it (models/utils.py:57-100, topp_temperature_decode; argmax when the temperature is small).  Contract, row b,
+ * logits l_i, T = temperature[b], p = top_p[b] (device fp32 (B,) each, so a captured call picks up new values):
+ *   - T <= 0 (or NaN): greedy, the smallest i with l_i == max l (torch.argmax's first occurrence).
+ *   - T > 0: w_i = exp2f((l_i - m) * (1.44269504f / T)) in fp32, m = max l, -inf logits weigh 0; W_i = floor(w_i * 2^40) as a
+ *     u64, S = sum W_i.  Token i is kept iff the W of the tokens before it in the order (W descending, lower index first on
+ *     ties) sum to <= floor(p * S), computed exactly (p >= 1 keeps all, p <= 0 only the first).  r = the first 64 bits of
+ *     Philox4x32-10 (curand_Philox4x32_10, counter (*offset lo, *offset hi, b, 0), key (seed lo, seed hi)); target =
+ *     umulhi64(r, S_keep); the token is the kept index, in index order, at which the running kept sum first exceeds target.
+ *     Bitwise deterministic: everything after the fp32 weights is integer.
+ *   - a row with a NaN or +inf logit, or with no finite logit, gets token 0 and sets bit b % 32 of status[b / 32] (status may be
+ *     NULL; never cleared here).
+ * offset: device u64, read and never written (the caller advances it, e.g. in the same graph).  Optional bookkeeping:
+ *   ids_out (int64, may be NULL): ids_out[b * ids_stride] = token.
+ *   tokens_out (int32 (B, max_new), may be NULL; needs count and done, int32 (B,)): unless done[b], append the token at
+ *   count[b] and increment it; done[b] = 1 when the token is one of the n_eos <= 8 ids eos_ids (a HOST array) or count[b]
+ *   reaches max_new.
+ *   debug (int64 (B, 5), may be NULL): S, floor(p * S), S_keep, kept count, target (greedy rows: 0, 0, 0, 1, 0; invalid rows:
+ *   zeros).  debug_w (fp32 (B, V), may be NULL): the weights w_i of the rows with T > 0.
+ * One cluster of C <= 8 CTAs per row, C = ceil(V / 4096) (V up to 409 600).  Refused with MPIG_EINVAL: B < 1, V < 1, V beyond
+ * that, ld < V, null or misaligned logits, null temperature / top_p / offset, n_eos > 8, tokens_out without count / done.
+ * Capturable. */
+int mpig_aux_sample(const float *logits, int B, int V, int64_t ld, const float *temperature, const float *top_p, uint64_t seed,
+                    const uint64_t *offset, int64_t *ids_out, int64_t ids_stride, int32_t *tokens_out, int32_t *count,
+                    int32_t *done, int max_new, const int32_t *eos_ids, int n_eos, int32_t *status, int64_t *debug,
+                    float *debug_w, void *stream);
+/* Clusters of mpig_aux_sample's kernel at vocabulary size V that the current device keeps resident at once. */
+int mpig_aux_sample_occupancy(int V, int *clusters);
+
 #ifdef __cplusplus
 }
 #endif

@@ -126,6 +126,9 @@ _AUX_SIGNATURES = {
     "mpig_aux_norm_gemv": (_i, [_vp, _vp, _vp, _vp, ctypes.c_float, _vp, _vp, _i, _i, _i, _i, _vp]),
     "mpig_aux_set_pdl": (_i, [_i]),
     "mpig_aux_norm_qkv_rope": (_i, [_vp, _vp, _vp, _vp, ctypes.c_float, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
+    "mpig_aux_sample": (_i, [_vp, _i, _i, ctypes.c_int64, _vp, _vp, ctypes.c_uint64, _vp, _vp, ctypes.c_int64, _vp, _vp, _vp, _i,
+                             _vp, _i, _vp, _vp, _vp, _vp]),
+    "mpig_aux_sample_occupancy": (_i, [_i, ctypes.POINTER(_i)]),
 }
 
 

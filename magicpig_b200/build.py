@@ -13,7 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libmagicpig_b200.so")
-SOURCES = ["context.cu", "tables.cu", "store.cu", "fused.cu", "attend_mma.cu", "attend_dense.cu", "attend_chunk.cu", "attend_prefill.cu", "simhash.cu", "step.cu", "decode.cu", "peer.cu", "aux_ops.cu", "aux_gemv.cu", "keyhash.cu"]
+SOURCES = ["context.cu", "tables.cu", "store.cu", "fused.cu", "attend_mma.cu", "attend_dense.cu", "attend_chunk.cu", "attend_prefill.cu", "simhash.cu", "step.cu", "decode.cu", "peer.cu", "aux_ops.cu", "aux_gemv.cu", "aux_sample.cu", "keyhash.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
          "-ccbin", "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"]

@@ -1,0 +1,459 @@
+// aux_sample.cu -- temperature / top-p sampling of a batch's fp32 logits on the device (see include/magicpig_b200_aux.h).
+//
+// Stands in for the reference caller's topp_temperature_decode (models/utils.py:57-100) and its argmax for temperature < 0.1
+// (models/llama.py:340-343).  One launch samples one token for each of B rows.  Contract for row b, logits l_i (i < V),
+// T = temperature[b], p = top_p[b]:
+//   * invalid row: any l_i NaN or +inf, or no finite l_i  ->  token 0 and bit (b % 32) of status[b / 32] is set.
+//   * greedy, T <= 0 (or NaN): the smallest i with l_i == max l (torch.argmax's first occurrence).
+//   * weights, T > 0: w_i = exp2f((l_i - m) * k) in fp32 with m = max l and k = 1.44269504f / T (fp32 division), both
+//     products rounded to nearest; -inf logits get w_i = 0.  w_i <= 1 and w_i == 1 at the max.  Fixed point:
+//     W_i = floor(w_i * 2^40) (exact: a power-of-two scale, then truncation), S = sum W_i < V * 2^41.  From here on integer.
+//   * nucleus: order the tokens by W descending, ties by lower index first; token i is kept iff the sum of the W of the tokens
+//     ordered before it is <= floor(p * S), computed exactly from p's 24-bit significand times S in 128 bits.  p >= 1 keeps
+//     every token, p <= 0 (or NaN) only the first in that order.  This is the reference's `cumsum > top_p` shifted by one, with
+//     the order of tied probabilities made definite.
+//   * draw: r = x | y << 32 of curand_Philox4x32_10(counter (offset lo, offset hi, b, 0), key (seed lo, seed hi)) = (x, y, ..),
+//     target = umulhi64(r, S_keep) with S_keep the kept mass; the token is the kept index, in INDEX order, at which the running
+//     kept sum first exceeds target.  The kernel reads *offset and never writes it.
+// Every stage after the fp32 weights is integer arithmetic, so the result is bitwise deterministic and independent of how the
+// row is split across CTAs.
+//
+// Layout: one cluster of C <= 8 CTAs per row; CTA `rank` stages the contiguous slice [rank * slice, +slice) of the row in shared
+// memory (fp32 logits, then in place the 32-bit keys below), so HBM is read once and every later pass runs from SMEM.  Cluster
+// reductions go through distributed shared memory: each CTA publishes its partial in its own SMEM, cluster.sync(), and every CTA
+// combines the C partials in rank order, so all CTAs hold the same integers.  Exchange slots alternate between two buffers, so one
+// cluster barrier per exchange suffices.
+//   A  max with its first index, and the invalid flag
+//   B  S
+//   R  up to 4 radix passes of 256-bin (count, u64 mass) histograms that select the nucleus threshold value W*
+//   E  per CTA: mass and count above W*, and ties at W* -> tie ranks in CTA order (= index order) and the kept mass per CTA
+// The CTA holding target then scans its slice in index order (one warp per contiguous segment).
+//
+// Radix key: key(W) = bits of (float)W.  (float)W is exact (W < 2^24, or W = w * 2^40 with w's 24-bit significand), and positive
+// floats order like their bits, so the 32-bit key orders the W and determines W; 4 passes of 8 bits decide it.
+#include <cooperative_groups.h>
+#include <curand_philox4x32_x.h>
+
+#include "../../include/magicpig_b200_aux.h"
+#include "common.cuh"
+
+namespace cg = cooperative_groups;
+
+namespace mpig {
+
+constexpr int SMP_THREADS = 512;
+constexpr int SMP_WARPS = SMP_THREADS / 32;
+constexpr int SMP_MAX_C = 8;                     // portable cluster size
+constexpr int SMP_SLICE_ALIGN = 256;             // slice length granule (elements)
+constexpr int SMP_ROWS_PER_CTA_HINT = 4096;      // C = ceil(V / this), at most SMP_MAX_C
+constexpr int SMP_SMEM_CAP = 200 * 1024;         // dynamic shared memory of one slice (bytes)
+constexpr int SMP_MAX_EOS = 8;
+
+struct SampleParams {
+    const float *logits;
+    long long ld;
+    int V, C, slice;
+    const float *temperature, *top_p;
+    unsigned long long seed;
+    const unsigned long long *offset;
+    long long *ids_out;
+    long long ids_stride;
+    int *tokens_out, *count, *done;
+    int max_new, n_eos;
+    int eos[SMP_MAX_EOS];
+    int *status;
+    long long *dbg;   // (B, 5): S, floor(p S), S_keep, kept count, target
+    float *dbg_w;     // (B, V): w_i
+};
+
+__device__ __forceinline__ unsigned long long key_weight(unsigned key) { return __float2ull_rz(__uint_as_float(key)); }
+
+__device__ __forceinline__ unsigned long long warp_sum_u64(unsigned long long v) {
+#pragma unroll
+    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+__device__ __forceinline__ unsigned long long warp_incl_scan_u64(unsigned long long v, int lane) {
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const unsigned long long t = __shfl_up_sync(0xffffffffu, v, o);
+        if (lane >= o) v += t;
+    }
+    return v;
+}
+
+// sum over the CTA, returned to every thread (two barriers; scratch has SMP_WARPS entries)
+__device__ __forceinline__ unsigned long long block_sum_u64(unsigned long long v, unsigned long long *scratch) {
+    v = warp_sum_u64(v);
+    __syncthreads();   // scratch may still be read by a previous call
+    if ((threadIdx.x & 31) == 0) scratch[threadIdx.x >> 5] = v;
+    __syncthreads();
+    unsigned long long t = 0;
+#pragma unroll
+    for (int w = 0; w < SMP_WARPS; ++w) t += scratch[w];
+    return t;
+}
+
+// exact floor(p * S) for 0 < p < 1: p = m24 * 2^(e - 24) with m24 its 24-bit significand
+__device__ __forceinline__ unsigned long long nucleus_threshold(float p, unsigned long long S) {
+    if (p >= 1.f) return S;
+    if (!(p > 0.f)) return 0;
+    int e = 0;
+    const float mant = frexpf(p, &e);   // p = mant * 2^e, mant in [0.5, 1), e <= 0
+    const unsigned long long m24 = (unsigned long long)(mant * 16777216.f);
+    const unsigned long long lo = m24 * S, hi = __umul64hi(m24, S);
+    const int sh = 24 - e;   // >= 24
+    if (sh >= 128) return 0;
+    if (sh >= 64) return hi >> (sh - 64);
+    return (lo >> sh) | (hi << (64 - sh));
+}
+
+__device__ void sample_commit(const SampleParams &p, int b, int token) {
+    if (p.ids_out) p.ids_out[(size_t)b * p.ids_stride] = token;
+    if (p.tokens_out && !p.done[b]) {
+        int c = p.count[b];
+        if (c < p.max_new) {
+            p.tokens_out[(size_t)b * p.max_new + c] = token;
+            p.count[b] = ++c;
+        }
+        bool eos = false;
+        for (int k = 0; k < p.n_eos; ++k) eos |= token == p.eos[k];
+        if (eos || c >= p.max_new) p.done[b] = 1;
+    }
+}
+
+__global__ void __launch_bounds__(SMP_THREADS) sample_kernel(const __grid_constant__ SampleParams p) {
+    extern __shared__ __align__(16) unsigned sbuf[];   // the slice: fp32 logits, then their keys
+    // radix histograms (exchanged), alternating buffers.  The mass of a bin is kept as three u32 parts (bits 0-15, 16-31, 32-):
+    // a 64-bit shared atomic add is a compare-and-swap loop on sm_90, the 32-bit one a native atomic.  A part gains < 2^16 per
+    // add and a slice holds < 2^16 elements, so no part overflows.
+    __shared__ unsigned hmass[2][3][256];
+    __shared__ unsigned hcount[2][256];
+    __shared__ unsigned long long mmass[256];          // merged histogram of the current pass (local)
+    __shared__ unsigned mcount[256];
+    __shared__ unsigned long long scratch[SMP_WARPS], wscan[SMP_WARPS];
+    __shared__ unsigned long long xb_s, xe_mass;       // exchanges B, E
+    __shared__ unsigned xe_count, xe_ties;
+    __shared__ float xa_max, red_max[SMP_WARPS];       // exchange A
+    __shared__ int xa_idx, xa_bad, red_idx[SMP_WARPS];
+    __shared__ int sel_bin, sel_warp;
+    __shared__ unsigned long long sel_excl, sel_prefix, sel_tie_base;
+
+    cg::cluster_group cl = cg::this_cluster();
+    const int C = p.C, rank = (int)cl.block_rank(), b = blockIdx.x / C;
+    const int lo = rank * p.slice, n = max(0, min(p.slice, p.V - lo));
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    float *slf = reinterpret_cast<float *>(sbuf);
+    const float *src = p.logits + (size_t)b * p.ld + lo;
+
+    // ---- A: stage the slice; max with its first index; invalid flag ----
+    float mx = -INFINITY;
+    int mi = INT_MAX, bad = 0;
+    for (int i = tid; i < n; i += SMP_THREADS) {
+        const float v = __ldg(src + i);
+        slf[i] = v;
+        if (!(v < INFINITY)) bad = 1;   // NaN or +inf
+        else if (v > mx || mi == INT_MAX) { mx = v; mi = lo + i; }   // indices rise within a thread: first occurrence
+    }
+#pragma unroll
+    for (int o = 16; o; o >>= 1) {
+        const float om = __shfl_xor_sync(0xffffffffu, mx, o);
+        const int oi = __shfl_xor_sync(0xffffffffu, mi, o);
+        if (om > mx || (om == mx && oi < mi)) { mx = om; mi = oi; }
+    }
+    if (lane == 0) { red_max[warp] = mx; red_idx[warp] = mi; }
+    bad = __syncthreads_or(bad);
+    if (tid == 0) {
+        for (int w = 1; w < SMP_WARPS; ++w)
+            if (red_max[w] > mx || (red_max[w] == mx && red_idx[w] < mi)) { mx = red_max[w]; mi = red_idx[w]; }
+        xa_max = mx; xa_idx = mi; xa_bad = bad;
+    }
+    cl.sync();
+    {   // every warp combines the C partials (lane r reads rank r); rank order, same rule -> the same result everywhere
+        float om = -INFINITY;
+        int oi = INT_MAX, ob = 0;
+        if (lane < C) {
+            om = *cl.map_shared_rank(&xa_max, lane);
+            oi = *cl.map_shared_rank(&xa_idx, lane);
+            ob = *cl.map_shared_rank(&xa_bad, lane);
+        }
+#pragma unroll
+        for (int o = 16; o; o >>= 1) {
+            const float tm = __shfl_xor_sync(0xffffffffu, om, o);
+            const int ti = __shfl_xor_sync(0xffffffffu, oi, o);
+            if (tm > om || (tm == om && ti < oi)) { om = tm; oi = ti; }
+        }
+        mx = om; mi = oi;
+        bad = __any_sync(0xffffffffu, ob) || !(mx > -INFINITY);
+    }
+    const float T = p.temperature[b], top_p = p.top_p[b];
+    if (bad || !(T > 0.f)) {
+        if (rank == 0 && tid == 0) {
+            const int token = bad ? 0 : mi;
+            if (bad && p.status) atomicOr(p.status + (b >> 5), 1 << (b & 31));
+            sample_commit(p, b, token);
+            if (p.dbg) {
+                long long *d = p.dbg + (size_t)b * 5;
+                d[0] = d[1] = d[2] = d[4] = 0;
+                d[3] = bad ? 0 : 1;
+            }
+        }
+        cl.sync();   // no CTA leaves while a peer may still read its exchange slot
+        return;
+    }
+
+    // ---- B: weights, their keys in place of the logits, S ----
+    const float k = 1.44269504f / T;
+    unsigned long long s_loc = 0;
+    for (int i = tid; i < n; i += SMP_THREADS) {
+        const float w = exp2f((slf[i] - mx) * k);
+        const unsigned long long W = __float2ull_rz(w * 0x1p40f);
+        sbuf[i] = __float_as_uint(__ull2float_rn(W));
+        s_loc += W;
+        if (p.dbg_w) p.dbg_w[(size_t)b * p.V + lo + i] = w;
+    }
+    s_loc = block_sum_u64(s_loc, scratch);
+    if (tid == 0) xb_s = s_loc;
+    cl.sync();
+    unsigned long long S = lane < C ? *cl.map_shared_rank(&xb_s, lane) : 0ull;
+    S = warp_sum_u64(S);
+    const unsigned long long thr = nucleus_threshold(top_p, S);
+
+    // ---- R: the threshold key v* = the smallest present key whose strictly-greater mass is <= thr ----
+    unsigned vstar = 0;              // p >= 1: every token is kept (W* = 0: every zero-weight tie kept too)
+    unsigned long long above = 0;    // mass of the keys above the decided prefix
+    if (top_p < 1.f) {
+        for (int pass = 0; pass < 4; ++pass) {
+            const int shift = 24 - 8 * pass;
+            unsigned (*hm)[256] = hmass[pass & 1];
+            unsigned *hc = hcount[pass & 1];
+            if (tid < 256) { hm[0][tid] = 0; hm[1][tid] = 0; hm[2][tid] = 0; hc[tid] = 0; }
+            __syncthreads();
+            for (int i0 = 0; i0 < n; i0 += SMP_THREADS) {
+                const int i = i0 + tid;
+                const unsigned key = i < n ? sbuf[i] : 0u;
+                const bool ok = i < n && (pass == 0 || (key >> (shift + 8)) == (vstar >> (shift + 8)));
+                const unsigned bin = ok ? (key >> shift) & 255u : 256u;
+                const unsigned long long W = ok ? key_weight(key) : 0ull;
+                const unsigned grp = __match_any_sync(0xffffffffu, bin);
+                if (grp == 0xffffffffu) {   // the whole warp in one bin (flat or tied rows): one atomic pair
+                    const unsigned long long m = warp_sum_u64(W);
+                    if (lane == 0 && ok) {   // m < 2^46: its parts are < 2^16, < 2^16 and < 2^14
+                        atomicAdd(&hc[bin], 32u);
+                        atomicAdd(&hm[0][bin], (unsigned)(m & 0xFFFFu));
+                        atomicAdd(&hm[1][bin], (unsigned)((m >> 16) & 0xFFFFu));
+                        atomicAdd(&hm[2][bin], (unsigned)(m >> 32));
+                    }
+                } else if (ok) {
+                    atomicAdd(&hc[bin], 1u);
+                    atomicAdd(&hm[0][bin], (unsigned)(W & 0xFFFFu));
+                    atomicAdd(&hm[1][bin], (unsigned)((W >> 16) & 0xFFFFu));
+                    atomicAdd(&hm[2][bin], (unsigned)(W >> 32));
+                }
+            }
+            cl.sync();
+            unsigned long long mass = 0;
+            unsigned cnt = 0;
+            if (tid < 256) {
+                for (int r = 0; r < C; ++r) {
+                    const unsigned(*pm)[256] = cl.map_shared_rank(hm, r);
+                    mass += (unsigned long long)pm[0][tid] + ((unsigned long long)pm[1][tid] << 16) + ((unsigned long long)pm[2][tid] << 32);
+                    cnt += cl.map_shared_rank(hc, r)[tid];
+                }
+                mmass[tid] = mass;
+                mcount[tid] = cnt;
+            }
+            if (tid == 0) sel_bin = 256;
+            __syncthreads();
+            // suffix sums over the bins in descending order: thread t < 256 takes bin 255 - t
+            if (tid < 256) {
+                const int bin = 255 - tid;
+                const unsigned long long m = mmass[bin];
+                const unsigned long long incl = warp_incl_scan_u64(m, lane);
+                if (lane == 31) wscan[warp] = incl;
+                __syncwarp();
+                asm volatile("bar.sync 1, 256;" ::: "memory");
+                unsigned long long base = 0;
+                for (int w = 0; w < warp; ++w) base += wscan[w];
+                const unsigned long long excl = base + incl - m;   // mass of the bins above `bin`
+                if (mcount[bin] > 0 && above + excl <= thr) atomicMin(&sel_bin, bin);
+                asm volatile("bar.sync 1, 256;" ::: "memory");
+                if (bin == sel_bin) sel_excl = excl;
+            }
+            __syncthreads();
+            above += sel_excl;
+            vstar |= (unsigned)sel_bin << shift;
+        }
+    }
+    const unsigned long long Wstar = key_weight(vstar);
+
+    // ---- E: per CTA mass / count above v* and ties at v*; kept mass per CTA; target ----
+    unsigned long long gmass = 0;
+    unsigned gcount = 0, ties = 0;
+    for (int i = tid; i < n; i += SMP_THREADS) {
+        const unsigned key = sbuf[i];
+        if (key > vstar) { gmass += key_weight(key); ++gcount; }
+        else if (key == vstar) ++ties;
+    }
+    gmass = block_sum_u64(gmass, scratch);
+    gcount = (unsigned)block_sum_u64(gcount, scratch);
+    ties = (unsigned)block_sum_u64(ties, scratch);
+    if (tid == 0) { xe_mass = gmass; xe_count = gcount; xe_ties = ties; }
+    cl.sync();
+    // lane r < C: rank r's numbers (every warp computes the same)
+    unsigned long long r_mass = 0;
+    unsigned r_count = 0, r_ties = 0;
+    if (lane < C) {
+        r_mass = *cl.map_shared_rank(&xe_mass, lane);
+        r_count = *cl.map_shared_rank(&xe_count, lane);
+        r_ties = *cl.map_shared_rank(&xe_ties, lane);
+    }
+    const unsigned long long ties_total = warp_sum_u64(r_ties);
+    const unsigned long long ties_before = warp_incl_scan_u64(r_ties, lane) - r_ties;
+    const unsigned long long keep_ties = Wstar > 0 ? min(ties_total, (thr - above) / Wstar + 1) : ties_total;
+    const unsigned long long r_keep_ties = keep_ties > ties_before ? min(keep_ties - ties_before, (unsigned long long)r_ties) : 0ull;
+    const unsigned long long r_kept = r_mass + r_keep_ties * Wstar;
+    const unsigned long long S_keep = warp_sum_u64(r_kept);
+    const unsigned long long kept_count = warp_sum_u64(r_count + r_keep_ties);
+    const unsigned long long r_prefix = warp_incl_scan_u64(r_kept, lane) - r_kept;
+    const unsigned long long off = *p.offset;
+    const uint4 rnd = curand_Philox4x32_10(make_uint4((unsigned)off, (unsigned)(off >> 32), (unsigned)b, 0u),
+                                           make_uint2((unsigned)p.seed, (unsigned)(p.seed >> 32)));
+    const unsigned long long r64 = (unsigned long long)rnd.x | ((unsigned long long)rnd.y << 32);
+    const unsigned long long target = __umul64hi(r64, S_keep);
+    const unsigned holder = __ballot_sync(0xffffffffu, lane < C && r_prefix <= target && target < r_prefix + r_kept);
+    const int sel_rank = __ffs(holder) - 1;
+    if (rank == 0 && tid == 0 && p.dbg) {
+        long long *d = p.dbg + (size_t)b * 5;
+        d[0] = (long long)S; d[1] = (long long)thr; d[2] = (long long)S_keep; d[3] = (long long)kept_count; d[4] = (long long)target;
+    }
+
+    if (rank == sel_rank) {
+        const unsigned long long my_keep_ties = __shfl_sync(0xffffffffu, r_keep_ties, sel_rank);
+        const unsigned long long tl = target - __shfl_sync(0xffffffffu, r_prefix, sel_rank);   // target inside this slice
+        // one warp per contiguous segment, in index order
+        const int seg = (((n + SMP_WARPS - 1) / SMP_WARPS) + 31) & ~31;
+        const int s0 = warp * seg, s1 = min(n, s0 + seg);
+        unsigned long long wm = 0;
+        unsigned wt = 0;
+        for (int i = s0 + lane; i < s1; i += 32) {
+            const unsigned key = sbuf[i];
+            if (key > vstar) wm += key_weight(key);
+            else if (key == vstar) ++wt;
+        }
+        wm = warp_sum_u64(wm);
+        wt = (unsigned)warp_sum_u64(wt);
+        if (lane == 0) { scratch[warp] = wm; wscan[warp] = wt; }
+        __syncthreads();
+        if (tid == 0) {
+            unsigned long long tb = 0, pre = 0;
+            sel_warp = -1;
+            for (int w = 0; w < SMP_WARPS; ++w) {
+                const unsigned long long kt = my_keep_ties > tb ? min(my_keep_ties - tb, wscan[w]) : 0ull;
+                const unsigned long long kw = scratch[w] + kt * Wstar;
+                if (sel_warp < 0 && tl < pre + kw) { sel_warp = w; sel_prefix = pre; sel_tie_base = tb; }
+                pre += kw;
+                tb += wscan[w];
+            }
+        }
+        __syncthreads();
+        if (warp == sel_warp) {
+            unsigned long long run = sel_prefix, tie_rank = sel_tie_base;
+            for (int i0 = s0; i0 < s1; i0 += 32) {
+                const int i = i0 + lane;
+                const unsigned key = i < s1 ? sbuf[i] : 0u;
+                const bool tie = i < s1 && key == vstar;
+                const unsigned tmask = __ballot_sync(0xffffffffu, tie);
+                const unsigned long long my_rank = tie_rank + __popc(tmask & ((1u << lane) - 1u));
+                unsigned long long kw = 0;
+                if (i < s1 && key > vstar) kw = key_weight(key);
+                else if (tie && my_rank < my_keep_ties) kw = Wstar;
+                const unsigned long long incl = warp_incl_scan_u64(kw, lane);
+                const unsigned hit = __ballot_sync(0xffffffffu, kw > 0 && run + incl > tl);
+                if (hit) {
+                    if (lane == __ffs(hit) - 1) sample_commit(p, b, lo + i);
+                    break;
+                }
+                run += __shfl_sync(0xffffffffu, incl, 31);
+                tie_rank += __popc(tmask);
+            }
+        }
+    }
+    cl.sync();   // no CTA leaves while a peer may still read its exchange slots
+}
+
+}  // namespace mpig
+
+using namespace mpig;
+
+extern "C" {
+
+int mpig_aux_sample(const float *logits, int B, int V, int64_t ld, const float *temperature, const float *top_p, uint64_t seed,
+                    const uint64_t *offset, int64_t *ids_out, int64_t ids_stride, int32_t *tokens_out, int32_t *count,
+                    int32_t *done, int max_new, const int32_t *eos_ids, int n_eos, int32_t *status, int64_t *debug,
+                    float *debug_w, void *stream) {
+    MPIG_REQUIRE(B >= 1 && V >= 1, MPIG_EINVAL, "mpig_aux_sample: B=%d and V=%d must be >= 1", B, V);
+    const int C = std::min(SMP_MAX_C, (V + SMP_ROWS_PER_CTA_HINT - 1) / SMP_ROWS_PER_CTA_HINT);
+    const int slice = ((V + C - 1) / C + SMP_SLICE_ALIGN - 1) / SMP_SLICE_ALIGN * SMP_SLICE_ALIGN;
+    MPIG_REQUIRE((size_t)slice * 4 <= (size_t)SMP_SMEM_CAP, MPIG_EINVAL,
+                 "mpig_aux_sample: V=%d exceeds what %d CTAs' shared memory holds (%d)", V, SMP_MAX_C, SMP_MAX_C * (SMP_SMEM_CAP / 4));
+    MPIG_REQUIRE(ld >= V, MPIG_EINVAL, "mpig_aux_sample: ld=%lld < V=%d", (long long)ld, V);
+    MPIG_REQUIRE(logits && ((uintptr_t)logits & 3) == 0, MPIG_EINVAL, "mpig_aux_sample: logits null or misaligned");
+    MPIG_REQUIRE(temperature && top_p && offset, MPIG_EINVAL, "mpig_aux_sample: temperature, top_p and offset are required");
+    MPIG_REQUIRE(((uintptr_t)temperature & 3) == 0 && ((uintptr_t)top_p & 3) == 0 && ((uintptr_t)offset & 7) == 0, MPIG_EINVAL,
+                 "mpig_aux_sample: misaligned temperature, top_p or offset");
+    MPIG_REQUIRE(n_eos >= 0 && n_eos <= SMP_MAX_EOS && (n_eos == 0 || eos_ids), MPIG_EINVAL,
+                 "mpig_aux_sample: n_eos=%d outside [0, %d] (or eos_ids null)", n_eos, SMP_MAX_EOS);
+    MPIG_REQUIRE(!tokens_out || (count && done && max_new >= 1), MPIG_EINVAL,
+                 "mpig_aux_sample: tokens_out needs count, done and max_new >= 1");
+    MPIG_REQUIRE(!ids_out || ids_stride >= 1, MPIG_EINVAL, "mpig_aux_sample: ids_stride=%lld < 1", (long long)ids_stride);
+    MPIG_REQUIRE((long long)B * C <= INT_MAX, MPIG_EINVAL, "mpig_aux_sample: B=%d too large", B);
+
+    SampleParams prm = {};
+    prm.logits = logits; prm.ld = ld; prm.V = V; prm.C = C; prm.slice = slice;
+    prm.temperature = temperature; prm.top_p = top_p; prm.seed = seed; prm.offset = (const unsigned long long *)offset;
+    prm.ids_out = (long long *)ids_out; prm.ids_stride = ids_stride;
+    prm.tokens_out = tokens_out; prm.count = count; prm.done = done; prm.max_new = max_new;
+    prm.n_eos = n_eos;
+    for (int i = 0; i < n_eos; ++i) prm.eos[i] = eos_ids[i];
+    prm.status = status; prm.dbg = (long long *)debug; prm.dbg_w = debug_w;
+
+    MPIG_FUNC_ATTR(sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMP_SMEM_CAP);
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(B * C);
+    cfg.blockDim = dim3(SMP_THREADS);
+    cfg.dynamicSmemBytes = (size_t)slice * 4;
+    cfg.stream = as_stream(stream);
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = C;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    MPIG_CUDA(cudaLaunchKernelEx(&cfg, sample_kernel, prm));
+    return MPIG_OK;
+}
+
+int mpig_aux_sample_occupancy(int V, int *clusters) {
+    MPIG_REQUIRE(V >= 1 && clusters, MPIG_EINVAL, "mpig_aux_sample_occupancy: bad arguments");
+    const int C = std::min(SMP_MAX_C, (V + SMP_ROWS_PER_CTA_HINT - 1) / SMP_ROWS_PER_CTA_HINT);
+    const int slice = ((V + C - 1) / C + SMP_SLICE_ALIGN - 1) / SMP_SLICE_ALIGN * SMP_SLICE_ALIGN;
+    MPIG_REQUIRE((size_t)slice * 4 <= (size_t)SMP_SMEM_CAP, MPIG_EINVAL, "mpig_aux_sample_occupancy: V=%d too large", V);
+    MPIG_FUNC_ATTR(sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMP_SMEM_CAP);
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(C);
+    cfg.blockDim = dim3(SMP_THREADS);
+    cfg.dynamicSmemBytes = (size_t)slice * 4;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = C;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    MPIG_CUDA(cudaOccupancyMaxActiveClusters(clusters, (const void *)sample_kernel, &cfg));
+    return MPIG_OK;
+}
+
+}  // extern "C"

@@ -25,7 +25,7 @@ import torch
 import torch.nn.functional as F
 
 from . import _native as N
-from . import tp
+from . import ops, tp
 from .attnserver import LSHSparseAttnServer, beam_sources
 
 
@@ -40,6 +40,7 @@ class LlamaShape:
     vocab_size: int = 128256
     rope_theta: float = 500000.0
     rms_norm_eps: float = 1e-5
+    eos_token_ids: tuple = (128001, 128008, 128009)   # generate() stops a request at these ids (Llama-3.1's end-of-text ids)
 
     @property
     def head_dim(self):
@@ -89,6 +90,57 @@ def plan_prefill_chunks(P: int, chunk_size: int, num_sink: int, num_local: int, 
     if P > max_length:
         raise ValueError(f"a prompt of {P} tokens exceeds max_length {max_length}")
     return [(start, min(start + chunk_size, P)) for start in range(0, P, chunk_size)]
+
+
+GREEDY_TEMPERATURE = 0.1   # llama.py:340-343: below this temperature the reference takes the argmax
+
+
+def per_request(value, B: int, name: str) -> list:
+    """A scalar or a length-B sequence of floats -> B floats (ValueError otherwise)."""
+    if isinstance(value, torch.Tensor):
+        value = value.tolist()
+    if isinstance(value, (int, float)):
+        return [float(value)] * B
+    vals = [float(v) for v in value]
+    if len(vals) != B:
+        raise ValueError(f"{name}: expected a scalar or {B} values, got {len(vals)}")
+    return vals
+
+
+def generate_prompts(prompt, B: int, num_contexts: int):
+    """generate()'s prompt argument -> (list of 1-D prompts, shared): one tensor is every request's prompt; a list holds one prompt
+    per request and needs one context per request.  Pure host checks (ValueError)."""
+    if isinstance(prompt, torch.Tensor):
+        p = prompt.reshape(-1) if prompt.dim() == 2 and prompt.shape[0] == 1 else prompt
+        if p.dim() != 1:
+            raise ValueError(f"prompt: expected (P,) token ids, got shape {tuple(prompt.shape)}")
+        return [p] * B, True
+    prompts = [torch.as_tensor(p).reshape(-1) for p in prompt]
+    if len(prompts) != B:
+        raise ValueError(f"prompt: expected one tensor or {B} prompts, got {len(prompts)}")
+    if num_contexts < B:
+        raise ValueError(f"B different prompts need one context per request ({num_contexts} contexts for {B} requests)")
+    return prompts, False
+
+
+def check_generate_args(lengths, max_new_tokens: int, check_every: int, eos, max_length: int, num_sink: int, num_local: int,
+                        chunk_size: int, generation_buffer: int, can_spill: bool):
+    """generate()'s refusals before anything is written (ValueError): max_new_tokens and check_every >= 1, at most 8 EOS ids,
+    every prompt one the prefill takes with P + max_new_tokens <= max_length, and no spill needed where the server cannot spill
+    (requests sharing a context without shared_spill).  Pure host arithmetic."""
+    if int(max_new_tokens) < 1:
+        raise ValueError(f"max_new_tokens must be >= 1, got {max_new_tokens}")
+    if int(check_every) < 1:
+        raise ValueError(f"check_every must be >= 1, got {check_every}")
+    if len(eos) > ops.MAX_EOS_IDS:
+        raise ValueError(f"at most {ops.MAX_EOS_IDS} EOS ids, got {len(eos)}")
+    for P in lengths:
+        plan_prefill_chunks(P, chunk_size, num_sink, num_local, max_length)
+        if P + int(max_new_tokens) > max_length:
+            raise ValueError(f"a prompt of {P} tokens + {max_new_tokens} new tokens exceeds max_length {max_length}")
+    if int(max_new_tokens) - 1 > generation_buffer and not can_spill:
+        raise ValueError(f"{max_new_tokens} new tokens need window spills, which requests sharing a context cannot do without "
+                         "shared_spill")
 
 
 class LlamaDecodeRunner:
@@ -206,6 +258,17 @@ class LlamaDecodeRunner:
         self.n_collectives = 0
         self.graph = None
         self.aux_launches_per_step = 0
+        # sampling state (sample(), capture(sample=True), generate()): per-request parameters and the Philox counter on the device,
+        # and the record of generated tokens the sampler appends to (int32 (B, max_length), allocated on first use)
+        self.temperature = torch.zeros((batch_size,), dtype=torch.float32, device=self.device)
+        self.top_p = torch.ones((batch_size,), dtype=torch.float32, device=self.device)
+        self.sample_offset = torch.zeros((1,), dtype=torch.int64, device=self.device)
+        self.sample_seed = 0
+        self.sample_status = torch.zeros(((batch_size + 31) // 32,), dtype=torch.int32, device=self.device)
+        self.gen_tokens = self.gen_count = self.gen_done = None
+        self.eos_token_ids = tuple(shape.eos_token_ids)
+        self._gen_graph = None
+        self._gen_graph_key = None
 
     # ------------------------------------------------------------------------------------------
     def synthetic_prefill(self, P: int, seed: int = 100, dist: str = "gauss", shared: bool = False):
@@ -326,6 +389,107 @@ class LlamaDecodeRunner:
         self.ids[req, 0] = tokens
         scores[req] = new_scores
         return parents, tokens, request_of
+
+    # ------------------------------------------------------------------------------------------
+    def set_sampling(self, temperature=None, top_p=None, seed: int | None = None, offset: int | None = None):
+        """Per-request sampling parameters for sample(): temperature / top_p scalars or length-B sequences (a temperature below 0.1
+        is greedy, as in the reference's LLM.generate), the Philox seed (a host value a captured graph keeps) and the device
+        counter offset.  Not capturable (host -> device copies)."""
+        for name, val, buf in (("temperature", temperature, self.temperature), ("top_p", top_p, self.top_p)):
+            if val is None:
+                continue
+            v = per_request(val, self.B, name)
+            if name == "temperature":
+                v = [0.0 if t < GREEDY_TEMPERATURE else t for t in v]   # llama.py:340-343: argmax below 0.1
+            buf.copy_(torch.tensor(v, dtype=torch.float32))
+        if seed is not None:
+            self.sample_seed = int(seed)
+        if offset is not None:
+            self.sample_offset.fill_(int(offset))
+
+    def _gen_record(self):
+        if self.gen_tokens is None:
+            M = self.server.max_length
+            self.gen_tokens = torch.zeros((self.B, M), dtype=torch.int32, device=self.device)
+            self.gen_count = torch.zeros((self.B,), dtype=torch.int32, device=self.device)
+            self.gen_done = torch.zeros((self.B,), dtype=torch.int32, device=self.device)
+        return self.gen_tokens, self.gen_count, self.gen_done
+
+    def sample(self, temperature=None, top_p=None):
+        """The next token of every request from self.logits into self.ids[:, 0], on the device (one mpig_aux_sample launch: the
+        rule is stated in include/magicpig_b200_aux.h), then self.sample_offset += 1.  The token is also appended to the request's
+        record (gen_tokens / gen_count) unless gen_done is set; gen_done is set at an id of self.eos_token_ids.  temperature /
+        top_p: None keeps the device values (set_sampling()); given, they are written first (not capturable then).  Capturable
+        with None; capture(sample=True) puts step() and this into one graph."""
+        assert self.tp_world == 1, "sampling is built for a single GPU"
+        if temperature is not None or top_p is not None:
+            self.set_sampling(temperature, top_p)
+        tokens, count, done = self._gen_record()
+        ops.sample(self.logits, self.temperature, self.top_p, self.sample_seed, self.sample_offset, ids_out=self.ids,
+                   tokens_out=tokens, count=count, done=done, eos_token_ids=self.eos_token_ids, status=self.sample_status)
+        self.sample_offset.add_(1)
+        return self.ids
+
+    def generate(self, prompt, max_new_tokens: int, temperature=0.6, top_p=0.9, eos_token_ids=None, seed: int = 0,
+                 chunk_size: int = 8192, check_every: int = 16):
+        """The reference's LLM.generate (llama.py:328-360) for the batch.  prompt: one (P,) tensor of token ids for every request
+        (prefilled once and forked when the batch has fewer contexts than requests, prefilled into each request otherwise), or a
+        list of B prompts, one per request (needs one context per request; lengths may differ).  temperature / top_p: scalars or
+        per-request sequences; temperature < 0.1 is greedy (the first argmax), as in the reference.  eos_token_ids (at most 8; None
+        = the shape's) end a request, which keeps its EOS token.  Every request gets at most max_new_tokens tokens.
+        Order: the sampling graph (step() then sample()) is captured once per runner and seed on a short synthetic context, which is
+        then cleared; the prompts are prefilled; the prefill's logits are sampled eagerly; then the graph is replayed, with
+        spill_window() whenever the windows are full, and the requests' done flags are read every check_every replays.
+        Refused before anything is written: P + max_new_tokens > max_length, prompts the prefill refuses, a generation that needs
+        spills the server cannot do.  Returns B host lists of ints.  Single GPU; the runner's state stays as the generation
+        leaves it."""
+        assert self.tp_world == 1, "generate is built for a single GPU"
+        srv, B = self.server, self.B
+        prompts, shared = generate_prompts(prompt, B, srv.ctx.num_contexts)
+        eos = tuple(int(e) for e in (self.shape.eos_token_ids if eos_token_ids is None else eos_token_ids))
+        check_generate_args([int(p.numel()) for p in prompts], max_new_tokens, check_every, eos, srv.max_length,
+                            srv.num_sink_tokens, srv.num_local_tokens, chunk_size, self.generation_buffer,
+                            can_spill=srv.ctx.num_contexts == B or srv.ctx.shared_spill)
+        temps = per_request(temperature, B, "temperature")
+        tops = per_request(top_p, B, "top_p")
+        self.eos_token_ids = eos
+        key = (int(seed), eos)
+        if self._gen_graph is None or self._gen_graph_key != key:
+            # the capture's warm-up steps advance the state: capture on a short synthetic context, then clear it
+            self.sample_seed = int(seed)
+            self._gen_graph = None
+            srv.clear()
+            self.synthetic_prefill(srv.num_sink_tokens + srv.num_local_tokens + 64, shared=srv.ctx.num_contexts < B)
+            prev = self.graph
+            self.capture(sample=True)
+            self._gen_graph, self.graph = self.graph, prev
+            self._gen_graph_key = key
+        srv.clear()
+        if shared and srv.ctx.num_contexts < B:
+            self.prefill(prompts[0], chunk_size=chunk_size)
+        else:
+            for b, p in enumerate(prompts):
+                self.prefill(p, request=b, chunk_size=chunk_size)
+        tokens, count, done = self._gen_record()
+        count.zero_()
+        done.zero_()
+        self.sample_status.zero_()
+        self.set_sampling(temps, tops, seed=seed, offset=0)
+        self.sample()   # the first token, from the prefill's logits
+        used = 0        # generated rows in the windows
+        for i in range(max_new_tokens - 1):
+            if i % check_every == 0 and bool(done.all()):
+                break
+            if used == self.generation_buffer:
+                srv.spill_window()
+                used = 0
+            self._gen_graph.replay()
+            used += 1
+        n = count.tolist()
+        if int(self.sample_status.any()):
+            raise N.MagicPigError("generate: a request's logits held NaN / +inf or no finite value (its token was set to 0)")
+        rows = tokens[:, :max(n)].tolist() if max(n) else [[] for _ in range(B)]
+        return [rows[b][:n[b]] for b in range(B)]
 
     # ------------------------------------------------------------------------------------------
     def _rope(self, x: torch.Tensor, pos: torch.Tensor) -> torch.Tensor:
@@ -599,14 +763,18 @@ class LlamaDecodeRunner:
         x1, x2 = x[..., : self.d // 2], x[..., self.d // 2:]
         return x * cos + torch.cat([-x2, x1], dim=-1) * sin
 
-    def capture(self, warm: int = 3, beam_scores: torch.Tensor | None = None):
+    def capture(self, warm: int = 3, beam_scores: torch.Tensor | None = None, sample: bool = False):
         """Capture step() into a CUDA graph (launch-bound otherwise: ~600 small kernels per token).  With beam_scores (a device
         fp32 (B,) tensor that stays in place) the graph is step() followed by beam_step(beam_scores); the warm-up steps run it too,
-        so reset the beams' state (clear and prefill) before the first replay."""
+        so reset the beams' state (clear and prefill) before the first replay.  With sample=True the graph is step() followed by
+        sample(): each replay writes the next token into self.ids, appends it to the record and advances the Philox offset, with
+        the parameters on the device at replay time and the seed at capture time; the warm-up steps sample too."""
         def body():
             self.step()
             if beam_scores is not None:
                 self.beam_step(beam_scores)
+            if sample:
+                self.sample()
 
         s = torch.cuda.Stream(device=self.device)
         s.wait_stream(torch.cuda.current_stream(self.device))

@@ -499,6 +499,99 @@ class Context:
         return out
 
 
+MAX_EOS_IDS = 8
+
+
+def _sample_chk(t, dtype, shape, name, device):
+    if not isinstance(t, torch.Tensor):
+        raise N.MagicPigError(f"{name}: expected a tensor, got {type(t).__name__}")
+    if t.device != device:
+        raise N.MagicPigError(f"{name}: expected a tensor on {device}, got {t.device}")
+    if t.dtype != dtype:
+        raise N.MagicPigError(f"{name}: expected dtype {dtype}, got {t.dtype}")
+    if shape is not None and tuple(t.shape) != tuple(shape):
+        raise N.MagicPigError(f"{name}: expected shape {tuple(shape)}, got {tuple(t.shape)}")
+    return t
+
+
+def check_sample_args(logits, temperature, top_p, offset, ids_out=None, tokens_out=None, count=None, done=None, eos_token_ids=(),
+                      status=None, debug=None, debug_w=None):
+    """The argument checks of sample() on any device (no library call): returns (ids_out, max_new, eos ids), ids_out allocated
+    when None.  Raises MagicPigError."""
+    if not isinstance(logits, torch.Tensor) or logits.dim() != 2:
+        raise N.MagicPigError("logits: expected a (B, V) tensor")
+    dev = logits.device
+    _sample_chk(logits, torch.float32, None, "logits", dev)
+    B, V = logits.shape
+    if B < 1 or V < 1:
+        raise N.MagicPigError(f"logits: empty shape {tuple(logits.shape)}")
+    if logits.stride(1) != 1 or logits.stride(0) < V:
+        raise N.MagicPigError(f"logits: rows must be contiguous with a stride >= V, got strides {logits.stride()}")
+    _sample_chk(temperature, torch.float32, (B,), "temperature", dev)
+    _sample_chk(top_p, torch.float32, (B,), "top_p", dev)
+    if not isinstance(offset, torch.Tensor) or offset.dtype not in (torch.int64, torch.uint64) or offset.numel() != 1:
+        raise N.MagicPigError("offset: expected a one-element int64 / uint64 tensor")
+    _sample_chk(offset, offset.dtype, None, "offset", dev)
+    for name, t in (("temperature", temperature), ("top_p", top_p)):
+        if not t.is_contiguous():
+            raise N.MagicPigError(f"{name}: must be contiguous")
+    eos = [int(e) for e in eos_token_ids]
+    if len(eos) > MAX_EOS_IDS:
+        raise N.MagicPigError(f"at most {MAX_EOS_IDS} EOS ids, got {len(eos)}")
+    if ids_out is None:
+        ids_out = torch.empty((B,), dtype=torch.int64, device=dev)
+    _sample_chk(ids_out, torch.int64, None, "ids_out", dev)
+    if ids_out.shape[0] != B or ids_out.dim() not in (1, 2):
+        raise N.MagicPigError(f"ids_out: expected (B={B},) or (B, n), got {tuple(ids_out.shape)}")
+    max_new = 0
+    if tokens_out is not None:
+        if count is None or done is None:
+            raise N.MagicPigError("tokens_out needs count and done")
+        _sample_chk(tokens_out, torch.int32, None, "tokens_out", dev)
+        if tokens_out.dim() != 2 or tokens_out.shape[0] != B or tokens_out.shape[1] < 1 or not tokens_out.is_contiguous():
+            raise N.MagicPigError(f"tokens_out: expected a contiguous (B={B}, max_new >= 1) tensor, got {tuple(tokens_out.shape)}")
+        max_new = tokens_out.shape[1]
+    elif count is not None or done is not None:
+        raise N.MagicPigError("count and done go with tokens_out")
+    for name, t, dt, shp in (("count", count, torch.int32, (B,)), ("done", done, torch.int32, (B,)),
+                             ("status", status, torch.int32, ((B + 31) // 32,)), ("debug", debug, torch.int64, (B, 5)),
+                             ("debug_w", debug_w, torch.float32, (B, V))):
+        if t is not None:
+            _sample_chk(t, dt, shp, name, dev)
+            if not t.is_contiguous():
+                raise N.MagicPigError(f"{name}: must be contiguous")
+    return ids_out, max_new, eos
+
+
+def sample(logits: torch.Tensor, temperature: torch.Tensor, top_p: torch.Tensor, seed: int, offset: torch.Tensor,
+           ids_out: Optional[torch.Tensor] = None, tokens_out: Optional[torch.Tensor] = None, count: Optional[torch.Tensor] = None,
+           done: Optional[torch.Tensor] = None, eos_token_ids: Sequence[int] = (), status: Optional[torch.Tensor] = None,
+           debug: Optional[torch.Tensor] = None, debug_w: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """One token per row of logits (B, V) fp32 (rows may be strided; elements contiguous) by temperature / top-p sampling on the
+    device (mpig_aux_sample, include/magicpig_b200_aux.h, states the exact rule): temperature (B,) fp32 (<= 0: greedy, the first
+    argmax), top_p (B,) fp32, offset a device uint64 (1,) tensor (int64 storage is accepted) read as the Philox counter and never
+    written.  ids_out: int64 tensor whose elements ids_out[b, 0] (or ids_out[b]) receive the tokens; None = a new int64 (B,)
+    tensor.  tokens_out int32 (B, max_new) with count / done int32 (B,): append the token unless done, done on an id in
+    eos_token_ids (at most 8) or when count reaches max_new.  status int32 ((B + 31) // 32,): bit b % 32 of word b // 32 is set
+    for a row with a NaN or +inf logit or none finite (its token is 0).  debug int64 (B, 5) / debug_w fp32 (B, V): the kernel's
+    integer stages and weights.  Every argument is checked here before the call; capturable.  Returns the tensor holding the
+    tokens (ids_out)."""
+    ids_out, max_new, eos = check_sample_args(logits, temperature, top_p, offset, ids_out, tokens_out, count, done, eos_token_ids,
+                                              status, debug, debug_w)
+    if logits.device.type != "cuda":
+        raise N.MagicPigError("sample runs on CUDA (sm_90a) only; there is no CPU path")
+    dev = logits.device
+    B, V = logits.shape
+    eos_arr = (ctypes.c_int32 * max(len(eos), 1))(*eos)
+    lib = N.load()
+    with torch.cuda.device(dev):
+        N.check(lib.mpig_aux_sample(_ptr(logits), B, V, logits.stride(0), _ptr(temperature), _ptr(top_p),
+                                    ctypes.c_uint64(int(seed) & (2 ** 64 - 1)), _ptr(offset), _ptr(ids_out), ids_out.stride(0),
+                                    _ptr(tokens_out), _ptr(count), _ptr(done), max_new, eos_arr, len(eos), _ptr(status), _ptr(debug),
+                                    _ptr(debug_w), _stream()), "mpig_aux_sample")
+    return ids_out
+
+
 # =================================================================================================
 # Reference-named facades
 # =================================================================================================
