@@ -75,6 +75,50 @@ int mpig_aux_sample(const float *logits, int B, int V, int64_t ld, const float *
 /* Clusters of mpig_aux_sample's kernel at vocabulary size V that the current device keeps resident at once. */
 int mpig_aux_sample_occupancy(int V, int *clusters);
 
+/* Speculative sampling: the acceptance of a verification step's draft tokens and the next token, for B requests in one call.
+ * logits: fp32 rows (b, t) at logits + b * ld_b + t * ld_t, t < T (1 <= T <= 8), the logits after each of the step's T input
+ * tokens; ids: int64 rows at ids + b * ids_stride, the step's inputs, so request b's drafts are ids[b, 1 .. T-1].  Row (b, t) is
+ * sampled with exactly mpig_aux_sample's rule (same w_i, W_i, nucleus, S_keep; temperature[b], top_p[b], seed, *offset).
+ * For t <= T - 2 let d = ids[b, t + 1] (an id outside [0, V) is never accepted):
+ *   - greedy (T <= 0): d is accepted iff it is the row's first argmax.
+ *   - sampled: d is accepted iff it is kept and umulhi64(r_acc, S_keep) < W_d, r_acc = the first 64 bits of Philox4x32-10 at
+ *     counter (*offset lo, *offset hi, b, t + 1) under mpig_aux_sample's key: probability p(d), the nucleus probability of d.
+ * k = the first row whose draft is rejected (T - 1 if all are accepted).  The request emits d_1 .. d_k, then one final token
+ * from row k: rejected there, greedy -> the row's argmax; sampled -> a draw from the residual, the kept set without d, of mass
+ * S_keep - W_d (S_keep when d is not kept), with mpig_aux_sample's counter (.., b, 0) and index-order scan skipping d; all
+ * accepted -> mpig_aux_sample's draw on row T - 1.  Each emitted token then follows the nucleus distribution of its row given its
+ * prefix (the standard rule for a deterministic, one-hot draft; it is NOT exact for drafts drawn from a draft distribution).
+ * At T = 1 the token is mpig_aux_sample's, bit for bit.  A row with a NaN or +inf logit, or no finite one, accepts nothing; if it
+ * is row k the final token is 0 and bit b % 32 of status[b / 32] is set (status may be NULL).
+ * Outputs: ids[b, 0] = the final token; drop[b] = T - 1 - k (int32 (B,), the mpig_rewind input; may be NULL; see below for a
+ * request that ends).  rows: int32
+ * (B, T, 2) scratch (each row's final token and flags).  Optional bookkeeping as mpig_aux_sample's, on a token history:
+ * history int32 (B, history_ld) with length / limit / done int32 (B,): the emitted tokens are appended in order at length[b]
+ * while length[b] < min(limit[b], history_ld); an EOS id (n_eos <= 8, host array; kept) or reaching the limit sets done[b] and ends
+ * the appending.  A request that ends in the call after appending j tokens gets drop[b] = T - j, so it keeps only the rows of the
+ * tokens it emitted before its last one.  A request with done[b] already set appends nothing, counts nothing and gets
+ * drop[b] = T (its whole step is rewound).  steps / accepted int32 (B,) (both or neither): += 1 and += k per call for requests not done.  debug int64 (B, T, 9):
+ * per row mpig_aux_sample's five integers (target = umulhi64(r, S_keep) of its draw), W_d, d's keep bit, umulhi64(r_acc, S_keep)
+ * and the residual mass (greedy rows: 0 0 0 1 0 0 accept 0 0; invalid rows: zeros); debug_w fp32 (B, T, V): the weights.
+ * Two launches: one cluster per row (mpig_aux_sample's kernel), then one thread per request.  Refused with MPIG_EINVAL: T outside
+ * [1, 8], V as for mpig_aux_sample, ld_t < V or ld_b < (T - 1) ld_t + V, null or misaligned logits / ids / rows / temperature /
+ * top_p / offset, ids_stride < T, n_eos > 8, history without length / limit / done, misaligned optional outputs.  Capturable. */
+int mpig_aux_verify_sample(const float *logits, int B, int T, int V, int64_t ld_b, int64_t ld_t, const float *temperature,
+                           const float *top_p, uint64_t seed, const uint64_t *offset, int64_t *ids, int64_t ids_stride,
+                           int32_t *rows, int32_t *drop, int32_t *history, int64_t history_ld, int32_t *length, const int32_t *limit,
+                           int32_t *done, int32_t *steps, int32_t *accepted, const int32_t *eos_ids, int n_eos, int32_t *status,
+                           int64_t *debug, float *debug_w, void *stream);
+
+/* Prompt-lookup drafts: for request b with history h = history[b, 0 .. n) (int32 (B, ld), n = min(length[b], ld), device), write
+ * T - 1 drafts into ids[b * ids_stride + 1 .. T - 1] (int64).  For each end e in [0, n - 2], m(e) = the largest m <= g_max with
+ * h[e - i] == h[n - 1 - i] for all i < m; e* maximises (m(e), e) among m(e) >= g_min (the longest match, then the most recent);
+ * draft i = h'[e* + 1 + i] with h' = h followed by the drafts (an overlapping copy: periodic text continues its period).  No
+ * match: every draft is h[n - 1] (0 when n = 0).  One cluster of 8 CTAs per request, a max of (m << 32 | e), so deterministic.
+ * Refused with MPIG_EINVAL: B < 1, T outside [1, 8], not 1 <= g_min <= g_max <= 8, null or misaligned pointers, ids_stride < T.
+ * Capturable. */
+int mpig_aux_ngram_draft(const int32_t *history, int B, int64_t ld, const int32_t *length, int64_t *ids, int64_t ids_stride, int T,
+                         int g_min, int g_max, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

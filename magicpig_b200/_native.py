@@ -129,6 +129,10 @@ _AUX_SIGNATURES = {
     "mpig_aux_sample": (_i, [_vp, _i, _i, ctypes.c_int64, _vp, _vp, ctypes.c_uint64, _vp, _vp, ctypes.c_int64, _vp, _vp, _vp, _i,
                              _vp, _i, _vp, _vp, _vp, _vp]),
     "mpig_aux_sample_occupancy": (_i, [_i, ctypes.POINTER(_i)]),
+    "mpig_aux_verify_sample": (_i, [_vp, _i, _i, _i, ctypes.c_int64, ctypes.c_int64, _vp, _vp, ctypes.c_uint64, _vp, _vp,
+                                    ctypes.c_int64, _vp, _vp, _vp, ctypes.c_int64, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp,
+                                    _vp]),
+    "mpig_aux_ngram_draft": (_i, [_vp, _i, ctypes.c_int64, _vp, _vp, ctypes.c_int64, _i, _i, _i, _vp]),
 }
 
 

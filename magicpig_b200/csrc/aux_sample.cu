@@ -31,6 +31,15 @@
 //
 // Radix key: key(W) = bits of (float)W.  (float)W is exact (W < 2^24, or W = w * 2^40 with w's 24-bit significand), and positive
 // floats order like their bits, so the 32-bit key orders the W and determines W; 4 passes of 8 bits decide it.
+//
+// Speculative sampling (mpig_aux_verify_sample) runs the same kernel as sample_kernel<true> over the B*T rows of a verification
+// step, row (b, t) checking the draft d = ids[b, t + 1] (t <= T - 2):
+//   * greedy: accept iff d is the first argmax; sampled: accept iff d is kept and umulhi64(r_acc, S_keep) < W_d, r_acc from
+//     Philox counter (offset lo, offset hi, b, t + 1) -- probability p(d);
+//   * the row's final token if acceptance ends here: the argmax (greedy), or the draw above with word (.., b, 0) over the kept set
+//     without d (mass S_keep - W_d if d is kept), scanned in index order with d's weight 0; with no draft it is the plain draw.
+// verify_resolve_kernel then takes k = the first rejected row (T - 1 if none): the request emits d_1 .. d_k and row k's final
+// token.  For a one-hot draft every emitted token follows the row's nucleus distribution; T = 1 is mpig_aux_sample bit for bit.
 #include <cooperative_groups.h>
 #include <curand_philox4x32_x.h>
 
@@ -48,6 +57,7 @@ constexpr int SMP_SLICE_ALIGN = 256;             // slice length granule (elemen
 constexpr int SMP_ROWS_PER_CTA_HINT = 4096;      // C = ceil(V / this), at most SMP_MAX_C
 constexpr int SMP_SMEM_CAP = 200 * 1024;         // dynamic shared memory of one slice (bytes)
 constexpr int SMP_MAX_EOS = 8;
+constexpr int SMP_MAX_VERIFY_T = 8;               // rows per request of mpig_aux_verify_sample
 
 struct SampleParams {
     const float *logits;
@@ -62,11 +72,27 @@ struct SampleParams {
     int max_new, n_eos;
     int eos[SMP_MAX_EOS];
     int *status;
-    long long *dbg;   // (B, 5): S, floor(p S), S_keep, kept count, target
-    float *dbg_w;     // (B, V): w_i
+    long long *dbg;   // (B, 5): S, floor(p S), S_keep, kept count, target; verification: (B, T, 9), see mpig_aux_verify_sample
+    float *dbg_w;     // (B, V): w_i; verification: (B, T, V)
+    // verification (sample_kernel<true> and verify_resolve_kernel): row (b, t) at logits + b * ld + t * ld_t, its draft at
+    // ids_out[b * ids_stride + t + 1]; rows (B, T, 2) receives each row's final token and flags
+    int T;
+    long long ld_t;
+    int *rows;
+    int *drop, *limit, *steps, *accepted;
+    long long hist_ld;
 };
 
+constexpr int ROW_ACCEPT = 1, ROW_INVALID = 2;   // flags of a verification row
+
 __device__ __forceinline__ unsigned long long key_weight(unsigned key) { return __float2ull_rz(__uint_as_float(key)); }
+__device__ __forceinline__ float row_weight(float l, float mx, float k) { return exp2f((l - mx) * k); }
+__device__ __forceinline__ unsigned long long fixed_weight(float w) { return __float2ull_rz(w * 0x1p40f); }
+__device__ __forceinline__ unsigned long long philox_word(unsigned long long off, int b, unsigned word, unsigned long long seed) {
+    const uint4 rnd = curand_Philox4x32_10(make_uint4((unsigned)off, (unsigned)(off >> 32), (unsigned)b, word),
+                                           make_uint2((unsigned)seed, (unsigned)(seed >> 32)));
+    return (unsigned long long)rnd.x | ((unsigned long long)rnd.y << 32);
+}
 
 __device__ __forceinline__ unsigned long long warp_sum_u64(unsigned long long v) {
 #pragma unroll
@@ -122,6 +148,11 @@ __device__ void sample_commit(const SampleParams &p, int b, int token) {
     }
 }
 
+// VERIFY = false: mpig_aux_sample, one row per request.  VERIFY = true: the rows of mpig_aux_verify_sample, row (b, t) with draft
+// d = ids[b, t + 1] (t < T - 1; none on the last row, and an id outside [0, V) is no token): the same stages decide whether d is
+// accepted and draw the row's final token from the kept set without d (the residual), scanning in index order with d's weight
+// taken as 0.  The row's accept bit and final token go to p.rows; verify_resolve_kernel does the bookkeeping.
+template <bool VERIFY>
 __global__ void __launch_bounds__(SMP_THREADS) sample_kernel(const __grid_constant__ SampleParams p) {
     extern __shared__ __align__(16) unsigned sbuf[];   // the slice: fp32 logits, then their keys
     // radix histograms (exchanged), alternating buffers.  The mass of a bin is kept as three u32 parts (bits 0-15, 16-31, 32-):
@@ -133,18 +164,25 @@ __global__ void __launch_bounds__(SMP_THREADS) sample_kernel(const __grid_consta
     __shared__ unsigned mcount[256];
     __shared__ unsigned long long scratch[SMP_WARPS], wscan[SMP_WARPS];
     __shared__ unsigned long long xb_s, xe_mass;       // exchanges B, E
-    __shared__ unsigned xe_count, xe_ties;
+    __shared__ unsigned xe_count, xe_ties, xe_ties_d;
     __shared__ float xa_max, red_max[SMP_WARPS];       // exchange A
     __shared__ int xa_idx, xa_bad, red_idx[SMP_WARPS];
     __shared__ int sel_bin, sel_warp;
     __shared__ unsigned long long sel_excl, sel_prefix, sel_tie_base;
 
     cg::cluster_group cl = cg::this_cluster();
-    const int C = p.C, rank = (int)cl.block_rank(), b = blockIdx.x / C;
+    const int C = p.C, rank = (int)cl.block_rank(), rw = blockIdx.x / C;
+    const int b = VERIFY ? rw / p.T : rw, t = VERIFY ? rw % p.T : 0;
     const int lo = rank * p.slice, n = max(0, min(p.slice, p.V - lo));
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     float *slf = reinterpret_cast<float *>(sbuf);
-    const float *src = p.logits + (size_t)b * p.ld + lo;
+    const float *row = p.logits + (size_t)b * p.ld + (VERIFY ? (size_t)t * p.ld_t : 0);
+    const float *src = row + lo;
+    int d = -1;   // the draft this row checks
+    if (VERIFY && t < p.T - 1) {
+        const long long id = p.ids_out[(size_t)b * p.ids_stride + t + 1];
+        d = id >= 0 && id < p.V ? (int)id : -1;
+    }
 
     // ---- A: stage the slice; max with its first index; invalid flag ----
     float mx = -INFINITY;
@@ -190,12 +228,24 @@ __global__ void __launch_bounds__(SMP_THREADS) sample_kernel(const __grid_consta
     if (bad || !(T > 0.f)) {
         if (rank == 0 && tid == 0) {
             const int token = bad ? 0 : mi;
-            if (bad && p.status) atomicOr(p.status + (b >> 5), 1 << (b & 31));
-            sample_commit(p, b, token);
-            if (p.dbg) {
-                long long *d = p.dbg + (size_t)b * 5;
-                d[0] = d[1] = d[2] = d[4] = 0;
-                d[3] = bad ? 0 : 1;
+            if constexpr (VERIFY) {
+                const bool acc = !bad && d == mi;
+                p.rows[2 * rw] = token;
+                p.rows[2 * rw + 1] = (bad ? ROW_INVALID : 0) | (acc ? ROW_ACCEPT : 0);
+                if (p.dbg) {
+                    long long *dd = p.dbg + (size_t)rw * 9;
+                    for (int j = 0; j < 9; ++j) dd[j] = 0;
+                    dd[3] = bad ? 0 : 1;
+                    dd[6] = acc;
+                }
+            } else {
+                if (bad && p.status) atomicOr(p.status + (b >> 5), 1 << (b & 31));
+                sample_commit(p, b, token);
+                if (p.dbg) {
+                    long long *d = p.dbg + (size_t)b * 5;
+                    d[0] = d[1] = d[2] = d[4] = 0;
+                    d[3] = bad ? 0 : 1;
+                }
             }
         }
         cl.sync();   // no CTA leaves while a peer may still read its exchange slot
@@ -206,11 +256,11 @@ __global__ void __launch_bounds__(SMP_THREADS) sample_kernel(const __grid_consta
     const float k = 1.44269504f / T;
     unsigned long long s_loc = 0;
     for (int i = tid; i < n; i += SMP_THREADS) {
-        const float w = exp2f((slf[i] - mx) * k);
-        const unsigned long long W = __float2ull_rz(w * 0x1p40f);
+        const float w = row_weight(slf[i], mx, k);
+        const unsigned long long W = fixed_weight(w);
         sbuf[i] = __float_as_uint(__ull2float_rn(W));
         s_loc += W;
-        if (p.dbg_w) p.dbg_w[(size_t)b * p.V + lo + i] = w;
+        if (p.dbg_w) p.dbg_w[(size_t)rw * p.V + lo + i] = w;
     }
     s_loc = block_sum_u64(s_loc, scratch);
     if (tid == 0) xb_s = s_loc;
@@ -289,24 +339,32 @@ __global__ void __launch_bounds__(SMP_THREADS) sample_kernel(const __grid_consta
 
     // ---- E: per CTA mass / count above v* and ties at v*; kept mass per CTA; target ----
     unsigned long long gmass = 0;
-    unsigned gcount = 0, ties = 0;
+    unsigned gcount = 0, ties = 0, ties_d = 0;
     for (int i = tid; i < n; i += SMP_THREADS) {
         const unsigned key = sbuf[i];
         if (key > vstar) { gmass += key_weight(key); ++gcount; }
-        else if (key == vstar) ++ties;
+        else if (key == vstar) {
+            ++ties;
+            if (VERIFY && lo + i < d) ++ties_d;   // ties ranked before the draft
+        }
     }
     gmass = block_sum_u64(gmass, scratch);
     gcount = (unsigned)block_sum_u64(gcount, scratch);
     ties = (unsigned)block_sum_u64(ties, scratch);
-    if (tid == 0) { xe_mass = gmass; xe_count = gcount; xe_ties = ties; }
+    if (VERIFY) ties_d = (unsigned)block_sum_u64(ties_d, scratch);
+    if (tid == 0) {
+        xe_mass = gmass; xe_count = gcount; xe_ties = ties;
+        if (VERIFY) xe_ties_d = ties_d;
+    }
     cl.sync();
     // lane r < C: rank r's numbers (every warp computes the same)
     unsigned long long r_mass = 0;
-    unsigned r_count = 0, r_ties = 0;
+    unsigned r_count = 0, r_ties = 0, r_ties_d = 0;
     if (lane < C) {
         r_mass = *cl.map_shared_rank(&xe_mass, lane);
         r_count = *cl.map_shared_rank(&xe_count, lane);
         r_ties = *cl.map_shared_rank(&xe_ties, lane);
+        if (VERIFY) r_ties_d = *cl.map_shared_rank(&xe_ties_d, lane);
     }
     const unsigned long long ties_total = warp_sum_u64(r_ties);
     const unsigned long long ties_before = warp_incl_scan_u64(r_ties, lane) - r_ties;
@@ -315,15 +373,36 @@ __global__ void __launch_bounds__(SMP_THREADS) sample_kernel(const __grid_consta
     const unsigned long long r_kept = r_mass + r_keep_ties * Wstar;
     const unsigned long long S_keep = warp_sum_u64(r_kept);
     const unsigned long long kept_count = warp_sum_u64(r_count + r_keep_ties);
-    const unsigned long long r_prefix = warp_incl_scan_u64(r_kept, lane) - r_kept;
+    // the draft's weight (recomputed from its logit by every thread, bitwise as staged) and keep bit; the residual mass per rank
+    unsigned long long W_d = 0;
+    bool kept_d = false;
+    if (VERIFY && d >= 0) {
+        W_d = fixed_weight(row_weight(__ldg(row + d), mx, k));
+        const unsigned key_d = __float_as_uint(__ull2float_rn(W_d));
+        kept_d = key_d > vstar || (key_d == vstar && warp_sum_u64(r_ties_d) < keep_ties);
+    }
+    const unsigned long long r_res = VERIFY && kept_d && lane == d / p.slice ? r_kept - W_d : r_kept;
+    const unsigned long long S_res = VERIFY && kept_d ? S_keep - W_d : S_keep;
+    const unsigned long long r_prefix = warp_incl_scan_u64(r_res, lane) - r_res;
     const unsigned long long off = *p.offset;
-    const uint4 rnd = curand_Philox4x32_10(make_uint4((unsigned)off, (unsigned)(off >> 32), (unsigned)b, 0u),
-                                           make_uint2((unsigned)p.seed, (unsigned)(p.seed >> 32)));
-    const unsigned long long r64 = (unsigned long long)rnd.x | ((unsigned long long)rnd.y << 32);
-    const unsigned long long target = __umul64hi(r64, S_keep);
-    const unsigned holder = __ballot_sync(0xffffffffu, lane < C && r_prefix <= target && target < r_prefix + r_kept);
+    const unsigned long long r64 = philox_word(off, b, 0u, p.seed);
+    const unsigned long long target = __umul64hi(r64, S_res);
+    const unsigned holder = __ballot_sync(0xffffffffu, lane < C && r_prefix <= target && target < r_prefix + r_res);
     const int sel_rank = __ffs(holder) - 1;
-    if (rank == 0 && tid == 0 && p.dbg) {
+    if constexpr (VERIFY) {
+        if (rank == 0 && tid == 0) {
+            const unsigned long long acc_target = d >= 0 ? __umul64hi(philox_word(off, b, (unsigned)t + 1u, p.seed), S_keep) : 0ull;
+            const bool acc = kept_d && acc_target < W_d;
+            p.rows[2 * rw + 1] = acc ? ROW_ACCEPT : 0;
+            if (!holder) p.rows[2 * rw] = mi;   // S_res = 0: d holds all the kept mass and is accepted for sure
+            if (p.dbg) {
+                long long *dd = p.dbg + (size_t)rw * 9;
+                dd[0] = (long long)S; dd[1] = (long long)thr; dd[2] = (long long)S_keep; dd[3] = (long long)kept_count;
+                dd[4] = (long long)__umul64hi(r64, S_keep);
+                dd[5] = (long long)W_d; dd[6] = kept_d; dd[7] = (long long)acc_target; dd[8] = (long long)S_res;
+            }
+        }
+    } else if (rank == 0 && tid == 0 && p.dbg) {
         long long *d = p.dbg + (size_t)b * 5;
         d[0] = (long long)S; d[1] = (long long)thr; d[2] = (long long)S_keep; d[3] = (long long)kept_count; d[4] = (long long)target;
     }
@@ -350,7 +429,8 @@ __global__ void __launch_bounds__(SMP_THREADS) sample_kernel(const __grid_consta
             sel_warp = -1;
             for (int w = 0; w < SMP_WARPS; ++w) {
                 const unsigned long long kt = my_keep_ties > tb ? min(my_keep_ties - tb, wscan[w]) : 0ull;
-                const unsigned long long kw = scratch[w] + kt * Wstar;
+                unsigned long long kw = scratch[w] + kt * Wstar;
+                if (VERIFY && kept_d && d - lo >= w * seg && d - lo < min(n, w * seg + seg)) kw -= W_d;   // the residual
                 if (sel_warp < 0 && tl < pre + kw) { sel_warp = w; sel_prefix = pre; sel_tie_base = tb; }
                 pre += kw;
                 tb += wscan[w];
@@ -368,10 +448,14 @@ __global__ void __launch_bounds__(SMP_THREADS) sample_kernel(const __grid_consta
                 unsigned long long kw = 0;
                 if (i < s1 && key > vstar) kw = key_weight(key);
                 else if (tie && my_rank < my_keep_ties) kw = Wstar;
+                if (VERIFY && lo + i == d) kw = 0;
                 const unsigned long long incl = warp_incl_scan_u64(kw, lane);
                 const unsigned hit = __ballot_sync(0xffffffffu, kw > 0 && run + incl > tl);
                 if (hit) {
-                    if (lane == __ffs(hit) - 1) sample_commit(p, b, lo + i);
+                    if (lane == __ffs(hit) - 1) {
+                        if constexpr (VERIFY) p.rows[2 * rw] = lo + i;
+                        else sample_commit(p, b, lo + i);
+                    }
                     break;
                 }
                 run += __shfl_sync(0xffffffffu, incl, 31);
@@ -380,6 +464,107 @@ __global__ void __launch_bounds__(SMP_THREADS) sample_kernel(const __grid_consta
         }
     }
     cl.sync();   // no CTA leaves while a peer may still read its exchange slots
+}
+
+// One thread per request after sample_kernel<true>: k = the first row whose draft was rejected (T - 1 if none), the final token
+// from row k, then drop, ids[b, 0], the history, done, the counters and the status bit (row k invalid).  drop = T - the rows that
+// stay: k + 1 (the input token and d_1 .. d_k) for a request that goes on; for one that ends in this step (EOS or its limit
+// after j appended tokens) only j, the rows of the tokens it emitted before its last one; for one already done none, so its
+// caches stay where they ended.  Every request then holds (prompt + emitted tokens - 1) rows.
+__device__ void history_append(const SampleParams &p, int b, int token, int lim) {
+    int c = p.count[b];
+    if (c < lim) {
+        p.tokens_out[(size_t)b * p.hist_ld + c] = token;
+        p.count[b] = ++c;
+    }
+    bool eos = false;
+    for (int k = 0; k < p.n_eos; ++k) eos |= token == p.eos[k];
+    if (eos || c >= lim) p.done[b] = 1;
+}
+
+__global__ void verify_resolve_kernel(const __grid_constant__ SampleParams p, int B) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= B) return;
+    const int T = p.T;
+    const int *row = p.rows + (size_t)b * T * 2;
+    int k = 0;
+    while (k < T - 1 && (row[2 * k + 1] & ROW_ACCEPT)) ++k;
+    const int token = row[2 * k];
+    if ((row[2 * k + 1] & ROW_INVALID) && p.status) atomicOr(p.status + (b >> 5), 1 << (b & 31));
+    long long *ids = p.ids_out + (size_t)b * p.ids_stride;
+    const bool was_done = p.done && p.done[b];
+    int keep = was_done ? 0 : k + 1;   // rows of the step that stay: the input token and the accepted drafts
+    if (!was_done) {
+        if (p.steps) { p.steps[b] += 1; p.accepted[b] += k; }
+        if (p.tokens_out) {
+            const int lim = (int)min((long long)p.limit[b], p.hist_ld), n0 = p.count[b];
+            for (int j = 1; j <= k + 1 && !p.done[b]; ++j) history_append(p, b, j <= k ? (int)ids[j] : token, lim);
+            // a request that ends here keeps only the rows of the tokens it emitted before its last one
+            if (p.done[b]) keep = p.count[b] - n0;
+        }
+    }
+    if (p.drop) p.drop[b] = T - keep;
+    ids[0] = token;
+}
+
+// Prompt-lookup drafts (mpig_aux_ngram_draft): one cluster of NGR_C CTAs per request.  Every CTA takes the ends e = rank * NGR_THREADS
+// + tid + j * NGR_C * NGR_THREADS and keeps the largest (m(e) << 32 | e) with m(e) >= g_min; the CTAs' maxima meet in rank 0, which
+// copies the drafts.  A max of integers, so the choice does not depend on the order in which threads finish.
+constexpr int NGR_THREADS = 512, NGR_C = 8, NGR_MAX_G = 8, NGR_UNROLL = 4;
+
+__global__ void __launch_bounds__(NGR_THREADS) ngram_draft_kernel(const int *hist, long long ld, const int *len, long long *ids,
+                                                                   long long ids_stride, int T, int g_min, int g_max) {
+    __shared__ int suf[NGR_MAX_G];
+    __shared__ unsigned long long red[NGR_THREADS / 32], best_s;
+    cg::cluster_group cl = cg::this_cluster();
+    const int rank = (int)cl.block_rank(), b = blockIdx.x / NGR_C, tid = threadIdx.x;
+    const int n = (int)min((long long)max(len[b], 0), ld);
+    const int *h = hist + (size_t)b * ld;
+    if (tid < g_max) suf[tid] = n - 1 - tid >= 0 ? h[n - 1 - tid] : 0;
+    __syncthreads();
+    unsigned long long best = 0;   // keys with m >= g_min >= 1 are >= 2^32
+    if (n >= 2) {
+        const int last = suf[0];
+        for (int e0 = rank * NGR_THREADS + tid; e0 <= n - 2; e0 += NGR_UNROLL * NGR_C * NGR_THREADS) {
+            int v[NGR_UNROLL];
+#pragma unroll
+            for (int u = 0; u < NGR_UNROLL; ++u) {
+                const int e = e0 + u * NGR_C * NGR_THREADS;
+                v[u] = e <= n - 2 ? __ldg(h + e) : ~last;
+            }
+#pragma unroll
+            for (int u = 0; u < NGR_UNROLL; ++u) {
+                if (v[u] != last) continue;
+                const int e = e0 + u * NGR_C * NGR_THREADS;
+                int m = 1;
+                while (m < g_max && e - m >= 0 && __ldg(h + e - m) == suf[m]) ++m;
+                if (m >= g_min) best = max(best, (unsigned long long)m << 32 | (unsigned)e);
+            }
+        }
+    }
+#pragma unroll
+    for (int o = 16; o; o >>= 1) best = max(best, __shfl_xor_sync(0xffffffffu, best, o));
+    if ((tid & 31) == 0) red[tid >> 5] = best;
+    __syncthreads();
+    if (tid == 0) {
+        for (int w = 1; w < NGR_THREADS / 32; ++w) best = max(best, red[w]);
+        best_s = best;
+    }
+    cl.sync();
+    if (rank == 0 && tid == 0) {
+        for (int r = 1; r < NGR_C; ++r) best = max(best, *cl.map_shared_rank(&best_s, r));
+        long long *out = ids + (size_t)b * ids_stride;
+        for (int i = 0; i < T - 1; ++i) {
+            long long tok;
+            if (best == 0) tok = n >= 1 ? h[n - 1] : 0;
+            else {
+                const int j = (int)(best & 0xffffffffu) + 1 + i;   // h' = h followed by the drafts: an overlapping copy
+                tok = j < n ? h[j] : out[1 + j - n];
+            }
+            out[1 + i] = tok;
+        }
+    }
+    cl.sync();   // rank 0 reads every peer's best_s
 }
 
 }  // namespace mpig
@@ -417,8 +602,9 @@ int mpig_aux_sample(const float *logits, int B, int V, int64_t ld, const float *
     prm.n_eos = n_eos;
     for (int i = 0; i < n_eos; ++i) prm.eos[i] = eos_ids[i];
     prm.status = status; prm.dbg = (long long *)debug; prm.dbg_w = debug_w;
+    prm.T = 1;
 
-    MPIG_FUNC_ATTR(sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMP_SMEM_CAP);
+    MPIG_FUNC_ATTR(sample_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMP_SMEM_CAP);
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(B * C);
     cfg.blockDim = dim3(SMP_THREADS);
@@ -431,7 +617,7 @@ int mpig_aux_sample(const float *logits, int B, int V, int64_t ld, const float *
     attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    MPIG_CUDA(cudaLaunchKernelEx(&cfg, sample_kernel, prm));
+    MPIG_CUDA(cudaLaunchKernelEx(&cfg, sample_kernel<false>, prm));
     return MPIG_OK;
 }
 
@@ -440,7 +626,7 @@ int mpig_aux_sample_occupancy(int V, int *clusters) {
     const int C = std::min(SMP_MAX_C, (V + SMP_ROWS_PER_CTA_HINT - 1) / SMP_ROWS_PER_CTA_HINT);
     const int slice = ((V + C - 1) / C + SMP_SLICE_ALIGN - 1) / SMP_SLICE_ALIGN * SMP_SLICE_ALIGN;
     MPIG_REQUIRE((size_t)slice * 4 <= (size_t)SMP_SMEM_CAP, MPIG_EINVAL, "mpig_aux_sample_occupancy: V=%d too large", V);
-    MPIG_FUNC_ATTR(sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMP_SMEM_CAP);
+    MPIG_FUNC_ATTR(sample_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMP_SMEM_CAP);
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(C);
     cfg.blockDim = dim3(SMP_THREADS);
@@ -452,7 +638,95 @@ int mpig_aux_sample_occupancy(int V, int *clusters) {
     attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    MPIG_CUDA(cudaOccupancyMaxActiveClusters(clusters, (const void *)sample_kernel, &cfg));
+    MPIG_CUDA(cudaOccupancyMaxActiveClusters(clusters, (const void *)sample_kernel<false>, &cfg));
+    return MPIG_OK;
+}
+
+int mpig_aux_verify_sample(const float *logits, int B, int T, int V, int64_t ld_b, int64_t ld_t, const float *temperature,
+                           const float *top_p, uint64_t seed, const uint64_t *offset, int64_t *ids, int64_t ids_stride,
+                           int32_t *rows, int32_t *drop, int32_t *history, int64_t history_ld, int32_t *length, const int32_t *limit,
+                           int32_t *done, int32_t *steps, int32_t *accepted, const int32_t *eos_ids, int n_eos, int32_t *status,
+                           int64_t *debug, float *debug_w, void *stream) {
+    MPIG_REQUIRE(B >= 1 && V >= 1, MPIG_EINVAL, "mpig_aux_verify_sample: B=%d and V=%d must be >= 1", B, V);
+    MPIG_REQUIRE(T >= 1 && T <= SMP_MAX_VERIFY_T, MPIG_EINVAL, "mpig_aux_verify_sample: T=%d outside [1, %d]", T, SMP_MAX_VERIFY_T);
+    const int C = std::min(SMP_MAX_C, (V + SMP_ROWS_PER_CTA_HINT - 1) / SMP_ROWS_PER_CTA_HINT);
+    const int slice = ((V + C - 1) / C + SMP_SLICE_ALIGN - 1) / SMP_SLICE_ALIGN * SMP_SLICE_ALIGN;
+    MPIG_REQUIRE((size_t)slice * 4 <= (size_t)SMP_SMEM_CAP, MPIG_EINVAL,
+                 "mpig_aux_verify_sample: V=%d exceeds what %d CTAs' shared memory holds (%d)", V, SMP_MAX_C, SMP_MAX_C * (SMP_SMEM_CAP / 4));
+    MPIG_REQUIRE(ld_t >= V && ld_b >= (T - 1) * ld_t + V, MPIG_EINVAL,
+                 "mpig_aux_verify_sample: strides ld_b=%lld, ld_t=%lld overlap rows of V=%d", (long long)ld_b, (long long)ld_t, V);
+    MPIG_REQUIRE(logits && ((uintptr_t)logits & 3) == 0, MPIG_EINVAL, "mpig_aux_verify_sample: logits null or misaligned");
+    MPIG_REQUIRE(temperature && top_p && offset, MPIG_EINVAL, "mpig_aux_verify_sample: temperature, top_p and offset are required");
+    MPIG_REQUIRE(((uintptr_t)temperature & 3) == 0 && ((uintptr_t)top_p & 3) == 0 && ((uintptr_t)offset & 7) == 0, MPIG_EINVAL,
+                 "mpig_aux_verify_sample: misaligned temperature, top_p or offset");
+    MPIG_REQUIRE(ids && ((uintptr_t)ids & 7) == 0 && ids_stride >= T, MPIG_EINVAL,
+                 "mpig_aux_verify_sample: ids null, misaligned or ids_stride=%lld < T=%d", (long long)ids_stride, T);
+    MPIG_REQUIRE(rows && ((uintptr_t)rows & 3) == 0, MPIG_EINVAL, "mpig_aux_verify_sample: rows (B, T, 2) null or misaligned");
+    MPIG_REQUIRE(n_eos >= 0 && n_eos <= SMP_MAX_EOS && (n_eos == 0 || eos_ids), MPIG_EINVAL,
+                 "mpig_aux_verify_sample: n_eos=%d outside [0, %d] (or eos_ids null)", n_eos, SMP_MAX_EOS);
+    MPIG_REQUIRE(!history || (length && limit && done && history_ld >= 1), MPIG_EINVAL,
+                 "mpig_aux_verify_sample: history needs length, limit, done and history_ld >= 1");
+    MPIG_REQUIRE(!steps == !accepted, MPIG_EINVAL, "mpig_aux_verify_sample: steps and accepted go together");
+    const void *aligned4[] = {drop, history, length, limit, done, steps, accepted, status, debug_w};
+    for (const void *q : aligned4)
+        MPIG_REQUIRE(((uintptr_t)q & 3) == 0, MPIG_EINVAL, "mpig_aux_verify_sample: misaligned int32 / fp32 argument");
+    MPIG_REQUIRE(((uintptr_t)debug & 7) == 0, MPIG_EINVAL, "mpig_aux_verify_sample: misaligned debug");
+    MPIG_REQUIRE((long long)B * T * C <= INT_MAX, MPIG_EINVAL, "mpig_aux_verify_sample: B=%d too large", B);
+
+    SampleParams prm = {};
+    prm.logits = logits; prm.ld = ld_b; prm.ld_t = ld_t; prm.V = V; prm.C = C; prm.slice = slice; prm.T = T;
+    prm.temperature = temperature; prm.top_p = top_p; prm.seed = seed; prm.offset = (const unsigned long long *)offset;
+    prm.ids_out = (long long *)ids; prm.ids_stride = ids_stride; prm.rows = rows; prm.drop = drop;
+    prm.tokens_out = history; prm.hist_ld = history_ld; prm.count = length; prm.limit = const_cast<int *>(limit); prm.done = done;
+    prm.steps = steps; prm.accepted = accepted;
+    prm.n_eos = n_eos;
+    for (int i = 0; i < n_eos; ++i) prm.eos[i] = eos_ids[i];
+    prm.status = status; prm.dbg = (long long *)debug; prm.dbg_w = debug_w;
+
+    MPIG_FUNC_ATTR(sample_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMP_SMEM_CAP);
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(B * T * C);
+    cfg.blockDim = dim3(SMP_THREADS);
+    cfg.dynamicSmemBytes = (size_t)slice * 4;
+    cfg.stream = as_stream(stream);
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = C;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    MPIG_CUDA(cudaLaunchKernelEx(&cfg, sample_kernel<true>, prm));
+    verify_resolve_kernel<<<(B + 127) / 128, 128, 0, as_stream(stream)>>>(prm, B);
+    MPIG_CUDA(cudaGetLastError());
+    return MPIG_OK;
+}
+
+int mpig_aux_ngram_draft(const int32_t *history, int B, int64_t ld, const int32_t *length, int64_t *ids, int64_t ids_stride, int T,
+                         int g_min, int g_max, void *stream) {
+    MPIG_REQUIRE(B >= 1 && ld >= 1, MPIG_EINVAL, "mpig_aux_ngram_draft: B=%d and ld=%lld must be >= 1", B, (long long)ld);
+    MPIG_REQUIRE(ld <= INT_MAX, MPIG_EINVAL, "mpig_aux_ngram_draft: ld=%lld too large", (long long)ld);
+    MPIG_REQUIRE(T >= 1 && T <= SMP_MAX_VERIFY_T, MPIG_EINVAL, "mpig_aux_ngram_draft: T=%d outside [1, %d]", T, SMP_MAX_VERIFY_T);
+    MPIG_REQUIRE(g_min >= 1 && g_min <= g_max && g_max <= NGR_MAX_G, MPIG_EINVAL,
+                 "mpig_aux_ngram_draft: need 1 <= g_min=%d <= g_max=%d <= %d", g_min, g_max, NGR_MAX_G);
+    MPIG_REQUIRE(history && length && ids, MPIG_EINVAL, "mpig_aux_ngram_draft: history, length and ids are required");
+    MPIG_REQUIRE(((uintptr_t)history & 3) == 0 && ((uintptr_t)length & 3) == 0 && ((uintptr_t)ids & 7) == 0, MPIG_EINVAL,
+                 "mpig_aux_ngram_draft: misaligned history, length or ids");
+    MPIG_REQUIRE(ids_stride >= T, MPIG_EINVAL, "mpig_aux_ngram_draft: ids_stride=%lld < T=%d", (long long)ids_stride, T);
+    MPIG_REQUIRE((long long)B * NGR_C <= INT_MAX, MPIG_EINVAL, "mpig_aux_ngram_draft: B=%d too large", B);
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(B * NGR_C);
+    cfg.blockDim = dim3(NGR_THREADS);
+    cfg.stream = as_stream(stream);
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = NGR_C;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    MPIG_CUDA(cudaLaunchKernelEx(&cfg, ngram_draft_kernel, (const int *)history, (long long)ld, (const int *)length, (long long *)ids,
+                                 (long long)ids_stride, T, g_min, g_max));
     return MPIG_OK;
 }
 

@@ -143,6 +143,42 @@ def check_generate_args(lengths, max_new_tokens: int, check_every: int, eos, max
                          "shared_spill")
 
 
+def check_spec_args(lengths, max_new_tokens: int, draft_tokens: int, ngram, max_query_tokens: int, generation_buffer: int,
+                    max_length: int, dense_tail_rows: int, can_spill: bool):
+    """generate(draft_tokens=k)'s refusals beyond check_generate_args' (ValueError): k + 1 verification rows must fit
+    max_query_tokens and the window (generation_buffer); P + max_new_tokens + k <= max_length for every prompt and, with
+    dense_tail_rows R > 0, max_new_tokens + k <= R (a request holds at most P + max_new_tokens - 1 rows, also after it ends,
+    and a step adds k + 1 before its rewind); no spill where the server cannot spill (requests sharing a context without
+    shared_spill): the max_new_tokens - 1 replays must fit spec_spill_every(generation_buffer, k); and ngram = (g_min, g_max)
+    needs 1 <= g_min <= g_max <= 8.  Pure host arithmetic."""
+    k = int(draft_tokens)
+    if k < 0:
+        raise ValueError(f"draft_tokens must be >= 0, got {draft_tokens}")
+    if k + 1 > max_query_tokens:
+        raise ValueError(f"draft_tokens={k} needs max_query_tokens >= {k + 1} (the runner has {max_query_tokens})")
+    if k + 1 > generation_buffer:
+        raise ValueError(f"draft_tokens={k} needs generation_buffer >= {k + 1} (got {generation_buffer})")
+    for P in lengths:
+        if P + int(max_new_tokens) + k > max_length:
+            raise ValueError(f"a prompt of {P} tokens + {max_new_tokens} new tokens + {k} drafts exceeds max_length {max_length}")
+    if dense_tail_rows and int(max_new_tokens) + k > dense_tail_rows:
+        raise ValueError(f"{max_new_tokens} new tokens with {k} drafts need {int(max_new_tokens) + k} dense tail rows "
+                         f"(dense_tail_rows={dense_tail_rows})")
+    if not can_spill and int(max_new_tokens) - 1 > spec_spill_every(generation_buffer, k):
+        raise ValueError(f"{max_new_tokens} new tokens with {k} drafts need window spills (every "
+                         f"{spec_spill_every(generation_buffer, k)} steps), which requests sharing a context cannot do without "
+                         "shared_spill")
+    g_min, g_max = (int(g) for g in ngram)
+    if not 1 <= g_min <= g_max <= ops.MAX_NGRAM:
+        raise ValueError(f"ngram=(g_min, g_max) needs 1 <= g_min <= g_max <= {ops.MAX_NGRAM}, got {tuple(ngram)}")
+
+
+def spec_spill_every(generation_buffer: int, draft_tokens: int) -> int:
+    """Replays of the speculative graph between window spills: each keeps at most k + 1 rows and holds k + 1 during its step, so
+    floor(generation_buffer / (k + 1)) replays fit the window with no device read to schedule the spill."""
+    return int(generation_buffer) // (int(draft_tokens) + 1)
+
+
 class LlamaDecodeRunner:
     # The CUDA-core GEMV issues 24*rows + 16 instructions per KB of weights per warp; at the HBM rate an SM has ~23 clocks per
     # KB (4 issue slots each), so it streams at the memory rate for rows <= 2 and is ALU-bound beyond (measured at rows = 8:
@@ -269,6 +305,16 @@ class LlamaDecodeRunner:
         self.eos_token_ids = tuple(shape.eos_token_ids)
         self._gen_graph = None
         self._gen_graph_key = None
+        # speculative decoding (spec_step(), capture(draft_tokens=k), generate(draft_tokens=k)): the token history (prompt, then
+        # generated tokens) the drafts are looked up in and verify_sample appends to, int32 (B, max_length), with device lengths,
+        # limits and done flags, and the per-request step / accepted-draft counters; allocated on first use
+        self.token_history = self.history_len = self.history_limit = None
+        self.spec_steps = self.spec_accepted = None
+        self.ngram = (1, 3)
+        self._spec_rows = self._spec_drop = None
+        self._spec_graph = None
+        self._spec_graph_key = None
+        self.last_generate_stats = None
 
     # ------------------------------------------------------------------------------------------
     def synthetic_prefill(self, P: int, seed: int = 100, dist: str = "gauss", shared: bool = False):
@@ -415,6 +461,47 @@ class LlamaDecodeRunner:
             self.gen_done = torch.zeros((self.B,), dtype=torch.int32, device=self.device)
         return self.gen_tokens, self.gen_count, self.gen_done
 
+    def _history(self):
+        if self.token_history is None:
+            B, M = self.B, self.server.max_length
+            z = lambda *shape: torch.zeros(shape, dtype=torch.int32, device=self.device)  # noqa: E731
+            self.token_history = z(B, M)
+            self.history_len, self.history_limit = z(B), z(B)
+            self.spec_steps, self.spec_accepted = z(B), z(B)
+            self._spec_rows, self._spec_drop = z(B * ops.MAX_VERIFY_TOKENS * 2), z(B)
+            self._gen_record()
+        return self.token_history, self.history_len, self.history_limit, self.gen_done
+
+    def _verify(self, logits: torch.Tensor, count: bool = True):
+        """verify_sample of logits (B, T, V) against self.ids_tok into the history, with drop into self._spec_drop."""
+        hist, length, limit, done = self._history()
+        T = logits.shape[1]
+        ops.verify_sample(logits, self.temperature, self.top_p, self.sample_seed, self.sample_offset, self.ids_tok,
+                          rows=self._spec_rows[:self.B * T * 2].view(self.B, T, 2), drop=self._spec_drop, history=hist, length=length,
+                          limit=limit, done=done, steps=self.spec_steps if count else None,
+                          accepted=self.spec_accepted if count else None, eos_token_ids=self.eos_token_ids, status=self.sample_status)
+
+    def spec_step(self, T: int, draft: str | None = "ngram"):
+        """One step of speculative decoding, all on the device (capturable; capture(draft_tokens=T - 1) puts it into one graph).
+        self.ids_tok[:, 0] holds each request's last emitted token.  draft="ngram": prompt-lookup drafts from self.token_history
+        (ops.ngram_draft with self.ngram = (g_min, g_max)) into self.ids_tok[:, 1:T]; draft=None: the caller's drafts already there.
+        Then step_tokens(T), verify_sample (the accepted drafts and one final token are appended to the history, the final token goes
+        to self.ids_tok[:, 0]), server.rewind(drop), self.pos -= drop, self.sample_offset += 1.  Each request advances by its
+        accepted drafts + 1; a request whose done flag is set rewinds its whole step."""
+        assert self.tp_world == 1, "speculative decoding is built for a single GPU"
+        assert 1 <= T <= self.max_query_tokens, f"T={T} outside [1, max_query_tokens={self.max_query_tokens}]"
+        hist, length, _, _ = self._history()
+        if draft == "ngram":
+            ops.ngram_draft(hist, length, self.ids_tok, T, *self.ngram)
+        elif draft is not None:
+            raise ValueError(f"draft must be 'ngram' or None, got {draft!r}")
+        self.step_tokens(T)
+        self._verify(self.logits_tok[:, :T])
+        self.server.rewind(self._spec_drop)
+        self.pos.sub_(self._spec_drop.long())
+        self.sample_offset.add_(1)
+        return self.ids_tok
+
     def sample(self, temperature=None, top_p=None):
         """The next token of every request from self.logits into self.ids[:, 0], on the device (one mpig_aux_sample launch: the
         rule is stated in include/magicpig_b200_aux.h), then self.sample_offset += 1.  The token is also appended to the request's
@@ -431,7 +518,7 @@ class LlamaDecodeRunner:
         return self.ids
 
     def generate(self, prompt, max_new_tokens: int, temperature=0.6, top_p=0.9, eos_token_ids=None, seed: int = 0,
-                 chunk_size: int = 8192, check_every: int = 16):
+                 chunk_size: int = 8192, check_every: int = 16, draft_tokens: int = 0, ngram=(1, 3)):
         """The reference's LLM.generate (llama.py:328-360) for the batch.  prompt: one (P,) tensor of token ids for every request
         (prefilled once and forked when the batch has fewer contexts than requests, prefilled into each request otherwise), or a
         list of B prompts, one per request (needs one context per request; lengths may differ).  temperature / top_p: scalars or
@@ -442,14 +529,31 @@ class LlamaDecodeRunner:
         spill_window() whenever the windows are full, and the requests' done flags are read every check_every replays.
         Refused before anything is written: P + max_new_tokens > max_length, prompts the prefill refuses, a generation that needs
         spills the server cannot do.  Returns B host lists of ints.  Single GPU; the runner's state stays as the generation
-        leaves it."""
+        leaves it.
+        draft_tokens = k >= 1: speculative decoding with k prompt-lookup drafts per step (ngram = (g_min, g_max), see
+        ops.ngram_draft), lossless: every token follows the same nucleus distribution as without drafts (not the same draws).  The
+        spec_step(k + 1) graph is captured once per (seed, EOS ids, k, ngram) on a short synthetic context, then cleared; the prompts
+        are prefilled and written into self.token_history; the first token comes from the prefill's logits through verify_sample
+        at T = 1 (which equals sample()); then the graph is replayed at most max_new_tokens - 1 times, with spill_window() every
+        spec_spill_every(generation_buffer, k) replays and the done flags read every check_every replays.  Also refused: k + 1 >
+        max_query_tokens or > generation_buffer, P + max_new_tokens + k > max_length, a dense tail too short, spills the server cannot
+        do (sharing a context without shared_spill, more than spec_spill_every(generation_buffer, k) replays), a bad ngram.  With
+        drafts accepted, requests may finish well before max_new_tokens - 1 replays; the replays until the next done read (at most
+        check_every - 1) change nothing but cost a step each, so a smaller check_every trades host reads for fewer idle steps.
+        self.last_generate_stats then holds the per-request steps, accepted drafts and tokens per step."""
         assert self.tp_world == 1, "generate is built for a single GPU"
         srv, B = self.server, self.B
         prompts, shared = generate_prompts(prompt, B, srv.ctx.num_contexts)
         eos = tuple(int(e) for e in (self.shape.eos_token_ids if eos_token_ids is None else eos_token_ids))
-        check_generate_args([int(p.numel()) for p in prompts], max_new_tokens, check_every, eos, srv.max_length,
-                            srv.num_sink_tokens, srv.num_local_tokens, chunk_size, self.generation_buffer,
-                            can_spill=srv.ctx.num_contexts == B or srv.ctx.shared_spill)
+        lengths = [int(p.numel()) for p in prompts]
+        can_spill = srv.ctx.num_contexts == B or srv.ctx.shared_spill
+        check_generate_args(lengths, max_new_tokens, check_every, eos, srv.max_length,
+                            srv.num_sink_tokens, srv.num_local_tokens, chunk_size, self.generation_buffer, can_spill=can_spill)
+        if draft_tokens:
+            check_spec_args(lengths, max_new_tokens, draft_tokens, ngram, self.max_query_tokens, self.generation_buffer,
+                            srv.max_length, srv.ctx.dense_tail_rows if srv.dense_layers else 0, can_spill)
+            return self._generate_spec(prompts, shared, max_new_tokens, temperature, top_p, eos, seed, chunk_size, check_every,
+                                       int(draft_tokens), tuple(int(g) for g in ngram))
         temps = per_request(temperature, B, "temperature")
         tops = per_request(top_p, B, "top_p")
         self.eos_token_ids = eos
@@ -464,12 +568,7 @@ class LlamaDecodeRunner:
             self.capture(sample=True)
             self._gen_graph, self.graph = self.graph, prev
             self._gen_graph_key = key
-        srv.clear()
-        if shared and srv.ctx.num_contexts < B:
-            self.prefill(prompts[0], chunk_size=chunk_size)
-        else:
-            for b, p in enumerate(prompts):
-                self.prefill(p, request=b, chunk_size=chunk_size)
+        self._prefill_prompts(prompts, shared, chunk_size)
         tokens, count, done = self._gen_record()
         count.zero_()
         done.zero_()
@@ -490,6 +589,67 @@ class LlamaDecodeRunner:
             raise N.MagicPigError("generate: a request's logits held NaN / +inf or no finite value (its token was set to 0)")
         rows = tokens[:, :max(n)].tolist() if max(n) else [[] for _ in range(B)]
         return [rows[b][:n[b]] for b in range(B)]
+
+    def _prefill_prompts(self, prompts, shared: bool, chunk_size: int):
+        srv = self.server
+        srv.clear()
+        if shared and srv.ctx.num_contexts < self.B:
+            self.prefill(prompts[0], chunk_size=chunk_size)
+        else:
+            for b, p in enumerate(prompts):
+                self.prefill(p, request=b, chunk_size=chunk_size)
+
+    def _generate_spec(self, prompts, shared, max_new_tokens, temperature, top_p, eos, seed, chunk_size, check_every, k, ngram):
+        """generate(draft_tokens=k) after its checks (see generate())."""
+        srv, B, T = self.server, self.B, k + 1
+        temps = per_request(temperature, B, "temperature")
+        tops = per_request(top_p, B, "top_p")
+        self.eos_token_ids = eos
+        hist, length, limit, done = self._history()
+        key = (int(seed), eos, k, ngram)
+        if self._spec_graph is None or self._spec_graph_key != key:
+            # the capture's warm-up steps advance the state: capture on a short synthetic context, then clear it
+            self.sample_seed, self.ngram = int(seed), ngram
+            self._spec_graph = None
+            srv.clear()
+            self.synthetic_prefill(srv.num_sink_tokens + srv.num_local_tokens + 64, shared=srv.ctx.num_contexts < B)
+            length.zero_()
+            limit.fill_(hist.shape[1])
+            done.zero_()
+            prev = self.graph
+            self.capture(warm=max(1, min(3, self.generation_buffer // T - 1)), draft_tokens=k)
+            self._spec_graph, self.graph = self.graph, prev
+            self._spec_graph_key = key
+        self._prefill_prompts(prompts, shared, chunk_size)
+        P = [int(p.numel()) for p in prompts]
+        for b, p in enumerate(prompts):
+            hist[b, :P[b]] = p.to(self.device, torch.int32)
+        length.copy_(torch.tensor(P, dtype=torch.int32))
+        limit.copy_(torch.tensor([n + int(max_new_tokens) for n in P], dtype=torch.int32))
+        done.zero_()
+        self.spec_steps.zero_()
+        self.spec_accepted.zero_()
+        self.sample_status.zero_()
+        self.set_sampling(temps, tops, seed=seed, offset=0)
+        self._verify(self.logits[:, None], count=False)   # the first token, from the prefill's logits: T = 1 is sample()
+        self.sample_offset.add_(1)
+        every = spec_spill_every(self.generation_buffer, k)
+        since = 0   # replays since the last spill
+        for i in range(max_new_tokens - 1):
+            if i % check_every == 0 and bool(done.all()):
+                break
+            if since == every:
+                srv.spill_window()
+                since = 0
+            self._spec_graph.replay()
+            since += 1
+        n = length.tolist()
+        if int(self.sample_status.any()):
+            raise N.MagicPigError("generate: a request's logits held NaN / +inf or no finite value (its token was set to 0)")
+        steps, acc = self.spec_steps.tolist(), self.spec_accepted.tolist()
+        self.last_generate_stats = dict(draft_tokens=k, steps=steps, accepted=acc, tokens=[n[b] - P[b] for b in range(B)],
+                                        tokens_per_step=(sum(n) - sum(P) - B) / max(sum(steps), 1))
+        return [hist[b, P[b]:n[b]].tolist() for b in range(B)]
 
     # ------------------------------------------------------------------------------------------
     def _rope(self, x: torch.Tensor, pos: torch.Tensor) -> torch.Tensor:
@@ -763,13 +923,18 @@ class LlamaDecodeRunner:
         x1, x2 = x[..., : self.d // 2], x[..., self.d // 2:]
         return x * cos + torch.cat([-x2, x1], dim=-1) * sin
 
-    def capture(self, warm: int = 3, beam_scores: torch.Tensor | None = None, sample: bool = False):
+    def capture(self, warm: int = 3, beam_scores: torch.Tensor | None = None, sample: bool = False, draft_tokens: int = 0):
         """Capture step() into a CUDA graph (launch-bound otherwise: ~600 small kernels per token).  With beam_scores (a device
         fp32 (B,) tensor that stays in place) the graph is step() followed by beam_step(beam_scores); the warm-up steps run it too,
         so reset the beams' state (clear and prefill) before the first replay.  With sample=True the graph is step() followed by
         sample(): each replay writes the next token into self.ids, appends it to the record and advances the Philox offset, with
-        the parameters on the device at replay time and the seed at capture time; the warm-up steps sample too."""
+        the parameters on the device at replay time and the seed at capture time; the warm-up steps sample too.  With
+        draft_tokens = k >= 1 the graph is spec_step(k + 1) (prompt-lookup drafts with self.ngram) instead of step(); the warm-up
+        steps run it too."""
         def body():
+            if draft_tokens:
+                self.spec_step(draft_tokens + 1)
+                return
             self.step()
             if beam_scores is not None:
                 self.beam_step(beam_scores)

@@ -592,6 +592,120 @@ def sample(logits: torch.Tensor, temperature: torch.Tensor, top_p: torch.Tensor,
     return ids_out
 
 
+MAX_VERIFY_TOKENS = 8   # rows per request of verify_sample and ngram_draft's T
+MAX_NGRAM = 8           # longest suffix ngram_draft matches
+
+
+def _ids_chk(ids, B, T, dev):
+    _sample_chk(ids, torch.int64, None, "ids", dev)
+    if ids.dim() != 2 or ids.shape[0] != B or ids.shape[1] < T or ids.stride(1) != 1:
+        raise N.MagicPigError(f"ids: expected int64 (B={B}, >= T={T}) with contiguous rows, got {tuple(ids.shape)} strides {ids.stride()}")
+
+
+def check_verify_args(logits, temperature, top_p, offset, ids, rows=None, drop=None, history=None, length=None, limit=None, done=None,
+                      steps=None, accepted=None, eos_token_ids=(), status=None, debug=None, debug_w=None):
+    """The argument checks of verify_sample() on any device (no library call): returns (rows, eos ids), rows allocated when None.
+    Raises MagicPigError."""
+    if not isinstance(logits, torch.Tensor) or logits.dim() != 3:
+        raise N.MagicPigError("logits: expected a (B, T, V) tensor")
+    B, T, V = logits.shape
+    if not 1 <= T <= MAX_VERIFY_TOKENS:
+        raise N.MagicPigError(f"logits: T={T} outside [1, {MAX_VERIFY_TOKENS}]")
+    if V >= 1 and (logits.stride(2) != 1 or logits.stride(1) < V or logits.stride(0) < (T - 1) * logits.stride(1) + V):
+        raise N.MagicPigError(f"logits: rows must be contiguous and must not overlap, got strides {logits.stride()}")
+    # the per-request checks are sample()'s, on row 0 of every request
+    _, _, eos = check_sample_args(logits[:, 0], temperature, top_p, offset, eos_token_ids=eos_token_ids, status=status)
+    dev = logits.device
+    _ids_chk(ids, B, T, dev)
+    if rows is None:
+        rows = torch.empty((B, T, 2), dtype=torch.int32, device=dev)
+    if history is not None:
+        if length is None or limit is None or done is None:
+            raise N.MagicPigError("history needs length, limit and done")
+        _sample_chk(history, torch.int32, None, "history", dev)
+        if history.dim() != 2 or history.shape[0] != B or history.shape[1] < 1 or not history.is_contiguous():
+            raise N.MagicPigError(f"history: expected a contiguous (B={B}, n >= 1) tensor, got {tuple(history.shape)}")
+    elif length is not None or limit is not None or done is not None:
+        raise N.MagicPigError("length, limit and done go with history")
+    if (steps is None) != (accepted is None):
+        raise N.MagicPigError("steps and accepted go together")
+    for name, t, dt, shp in (("rows", rows, torch.int32, (B, T, 2)), ("drop", drop, torch.int32, (B,)),
+                             ("length", length, torch.int32, (B,)), ("limit", limit, torch.int32, (B,)),
+                             ("done", done, torch.int32, (B,)), ("steps", steps, torch.int32, (B,)),
+                             ("accepted", accepted, torch.int32, (B,)), ("debug", debug, torch.int64, (B, T, 9)),
+                             ("debug_w", debug_w, torch.float32, (B, T, V))):
+        if t is not None:
+            _sample_chk(t, dt, shp, name, dev)
+            if not t.is_contiguous():
+                raise N.MagicPigError(f"{name}: must be contiguous")
+    return rows, eos
+
+
+def verify_sample(logits: torch.Tensor, temperature: torch.Tensor, top_p: torch.Tensor, seed: int, offset: torch.Tensor,
+                  ids: torch.Tensor, rows: Optional[torch.Tensor] = None, drop: Optional[torch.Tensor] = None,
+                  history: Optional[torch.Tensor] = None, length: Optional[torch.Tensor] = None, limit: Optional[torch.Tensor] = None,
+                  done: Optional[torch.Tensor] = None, steps: Optional[torch.Tensor] = None, accepted: Optional[torch.Tensor] = None,
+                  eos_token_ids: Sequence[int] = (), status: Optional[torch.Tensor] = None, debug: Optional[torch.Tensor] = None,
+                  debug_w: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Speculative sampling of a verification step on the device (mpig_aux_verify_sample, include/magicpig_b200_aux.h, states the
+    exact rule): logits (B, T, V) fp32 (the logits after each of the step's T inputs; rows may be strided, elements contiguous),
+    ids (B, >= T) int64 the step's inputs, so ids[b, 1:T] are request b's drafts.  Accepts a prefix of the drafts and draws the
+    final token, which goes to ids[b, 0].  temperature / top_p / seed / offset / status / eos_token_ids as in sample().  rows: int32
+    (B, T, 2) scratch (None = allocated).  drop int32 (B,): T - 1 - accepted drafts, the rewind() input.  history int32 (B, n) with
+    length / limit / done int32 (B,): the emitted tokens are appended at length[b] until an EOS id or limit[b] sets done[b]; a
+    request already done appends nothing and gets drop = T.  steps / accepted int32 (B,): += 1 and += accepted drafts per call.
+    debug int64 (B, T, 9) / debug_w fp32 (B, T, V): each row's integer stages and weights.  Every argument is checked here before the
+    call; capturable.  Returns ids."""
+    rows, eos = check_verify_args(logits, temperature, top_p, offset, ids, rows, drop, history, length, limit, done, steps, accepted,
+                                  eos_token_ids, status, debug, debug_w)
+    if logits.device.type != "cuda":
+        raise N.MagicPigError("verify_sample runs on CUDA (sm_90a) only; there is no CPU path")
+    B, T, V = logits.shape
+    eos_arr = (ctypes.c_int32 * max(len(eos), 1))(*eos)
+    lib = N.load()
+    with torch.cuda.device(logits.device):
+        N.check(lib.mpig_aux_verify_sample(_ptr(logits), B, T, V, logits.stride(0), logits.stride(1), _ptr(temperature), _ptr(top_p),
+                                           ctypes.c_uint64(int(seed) & (2 ** 64 - 1)), _ptr(offset), _ptr(ids), ids.stride(0),
+                                           _ptr(rows), _ptr(drop), _ptr(history), history.shape[1] if history is not None else 0,
+                                           _ptr(length), _ptr(limit), _ptr(done), _ptr(steps), _ptr(accepted), eos_arr, len(eos),
+                                           _ptr(status), _ptr(debug), _ptr(debug_w), _stream()), "mpig_aux_verify_sample")
+    return ids
+
+
+def check_ngram_args(history, length, ids, T, g_min, g_max):
+    """The argument checks of ngram_draft() on any device (no library call).  Raises MagicPigError."""
+    if not isinstance(history, torch.Tensor) or history.dim() != 2:
+        raise N.MagicPigError("history: expected a (B, n) tensor")
+    dev = history.device
+    _sample_chk(history, torch.int32, None, "history", dev)
+    B = history.shape[0]
+    if B < 1 or history.shape[1] < 1 or not history.is_contiguous():
+        raise N.MagicPigError(f"history: expected a contiguous non-empty (B, n) tensor, got {tuple(history.shape)}")
+    _sample_chk(length, torch.int32, (B,), "length", dev)
+    if not length.is_contiguous():
+        raise N.MagicPigError("length: must be contiguous")
+    if not 1 <= int(T) <= MAX_VERIFY_TOKENS:
+        raise N.MagicPigError(f"T={T} outside [1, {MAX_VERIFY_TOKENS}]")
+    if not 1 <= int(g_min) <= int(g_max) <= MAX_NGRAM:
+        raise N.MagicPigError(f"need 1 <= g_min <= g_max <= {MAX_NGRAM}, got g_min={g_min}, g_max={g_max}")
+    _ids_chk(ids, B, int(T), dev)
+
+
+def ngram_draft(history: torch.Tensor, length: torch.Tensor, ids: torch.Tensor, T: int, g_min: int = 1, g_max: int = 3) -> torch.Tensor:
+    """Prompt-lookup drafts on the device (mpig_aux_ngram_draft, include/magicpig_b200_aux.h, states the rule): from the token
+    history int32 (B, n) of device lengths int32 (B,), T - 1 drafts per request into ids[b, 1:T] (int64 (B, >= T)): the text after
+    the most recent of the longest earlier matches (g_min .. g_max tokens) of the history's suffix, copied with overlap; the last
+    token repeated when nothing matches.  Checked here before the call; capturable.  Returns ids."""
+    check_ngram_args(history, length, ids, T, g_min, g_max)
+    if history.device.type != "cuda":
+        raise N.MagicPigError("ngram_draft runs on CUDA (sm_90a) only; there is no CPU path")
+    lib = N.load()
+    with torch.cuda.device(history.device):
+        N.check(lib.mpig_aux_ngram_draft(_ptr(history), history.shape[0], history.shape[1], _ptr(length), _ptr(ids), ids.stride(0),
+                                         int(T), int(g_min), int(g_max), _stream()), "mpig_aux_ngram_draft")
+    return ids
+
+
 # =================================================================================================
 # Reference-named facades
 # =================================================================================================
