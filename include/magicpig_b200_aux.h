@@ -109,6 +109,59 @@ int mpig_aux_verify_sample(const float *logits, int B, int T, int V, int64_t ld_
                            int32_t *done, int32_t *steps, int32_t *accepted, const int32_t *eos_ids, int n_eos, int32_t *status,
                            int64_t *debug, float *debug_w, void *stream);
 
+/* Sampling filters: top-k, min-p and repetition / presence / frequency penalties, for the two calls below.  The arrays are device
+ * arrays of shape (B,), so a captured call picks up new values:
+ *   top_k              int32  off when <= 0
+ *   min_p              fp32   in [0, 1]; off when 0 (NaN or <= 0 is off, > 1 is taken as 1)
+ *   repetition_penalty fp32   r > 0; off when 1 (non-finite or <= 0 is taken as 1)
+ *   presence_penalty   fp32   pr in [-2, 2]; off when 0 (non-finite is taken as 0)
+ *   frequency_penalty  fp32   f in [-2, 2]; off when 0 (non-finite is taken as 0)
+ * table: uint32 (B, ld), ld >= V, row b for request b: the low 31 bits of entry i are c_i, the times request b has emitted token i;
+ * bit 31 is set when token i occurs in the request's prompt.  As in Hugging Face and vLLM, the repetition penalty applies to prompt
+ * and output tokens, the presence and frequency penalties to output tokens only.
+ * The rule for row b, raw logit l_i:
+ *   1. penalties, fp32, every operation rounded to nearest with no contraction: seen_i = prompt bit or c_i > 0;
+ *      l1 = seen_i ? (l > 0 ? l / r : l * r) : l;  l2 = l1 - f * (float)c_i;  l3 = c_i > 0 ? l2 - pr : l2.  A row whose three
+ *      penalties are all neutral skips them (l3 = l).  Verification row t counts the drafts d_1 .. d_t of its step in c_i and
+ *      seen_i: the tokens that row's prefix emits.  A NaN or +inf raw or penalised logit makes the row invalid (token 0, status).
+ *   2. greedy (temperature <= 0): the first argmax of l3; top_k, min_p and top_p do not apply.
+ *   3. w, W and S from l3 exactly as in mpig_aux_sample.
+ *   4. truncation, in Hugging Face's processor order, each set a prefix of the order (W descending, lower index first on ties):
+ *      top-k: n_k = min(top_k, V) if top_k > 0 else V, S_k = the mass of the first n_k tokens;  top-p over the top-k set: order
+ *      position j < n_k is kept iff the mass before it is <= floor(p * S_k) (computed as mpig_aux_sample computes floor(p * S));
+ *      min-p: W_i >= floor(min_p * 2^40), computed the same way (the max has W = 2^40, so it always stays).  The kept set is the
+ *      first K = max(1, min(n_k, n_p, n_m)) tokens of the order; S_keep, the draw, the draft acceptance and the residual work as in
+ *      the unfiltered calls on that set.  With every filter neutral the result equals the unfiltered call's bit for bit.
+ *   5. bookkeeping: the call increments the table entry of each token it appends (to tokens_out, or to the history), in the same
+ *      call.  Rejected drafts and requests already done count nothing, and a call that appends nothing leaves the table as it is.
+ * With one-hot drafts every token a verification step emits then follows the filtered distribution given the request's whole prefix. */
+typedef struct mpig_sample_filters {
+    const int32_t *top_k;
+    const float *min_p;
+    const float *repetition_penalty;
+    const float *presence_penalty;
+    const float *frequency_penalty;
+    uint32_t *table;
+    int64_t ld;
+} mpig_sample_filters;
+
+/* mpig_aux_sample with the filters above.  debug int64 (B, 8): mpig_aux_sample's five integers (floor(p * S_k) in place of
+ * floor(p * S), the kept count K), then n_k, S_k and n_m, the tokens with W >= floor(min_p * 2^40) (greedy and invalid rows: zeros
+ * there); debug_w: the weights of the penalised logits.  Refused with MPIG_EINVAL as mpig_aux_sample, and for a null filters, a
+ * null or misaligned member, ld < V.  Capturable. */
+int mpig_aux_sample_filtered(const float *logits, int B, int V, int64_t ld, const float *temperature, const float *top_p,
+                             uint64_t seed, const uint64_t *offset, int64_t *ids_out, int64_t ids_stride, int32_t *tokens_out,
+                             int32_t *count, int32_t *done, int max_new, const int32_t *eos_ids, int n_eos, int32_t *status,
+                             int64_t *debug, float *debug_w, const mpig_sample_filters *filters, void *stream);
+/* mpig_aux_verify_sample with the filters above; debug int64 (B, T, 12): the nine integers, then n_k, S_k and n_m.  Refused as
+ * mpig_aux_verify_sample and mpig_aux_sample_filtered.  Capturable. */
+int mpig_aux_verify_sample_filtered(const float *logits, int B, int T, int V, int64_t ld_b, int64_t ld_t, const float *temperature,
+                                    const float *top_p, uint64_t seed, const uint64_t *offset, int64_t *ids, int64_t ids_stride,
+                                    int32_t *rows, int32_t *drop, int32_t *history, int64_t history_ld, int32_t *length,
+                                    const int32_t *limit, int32_t *done, int32_t *steps, int32_t *accepted, const int32_t *eos_ids,
+                                    int n_eos, int32_t *status, int64_t *debug, float *debug_w, const mpig_sample_filters *filters,
+                                    void *stream);
+
 /* Prompt-lookup drafts: for request b with history h = history[b, 0 .. n) (int32 (B, ld), n = min(length[b], ld), device), write
  * T - 1 drafts into ids[b * ids_stride + 1 .. T - 1] (int64).  For each end e in [0, n - 2], m(e) = the largest m <= g_max with
  * h[e - i] == h[n - 1 - i] for all i < m; e* maximises (m(e), e) among m(e) >= g_min (the longest match, then the most recent);

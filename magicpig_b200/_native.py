@@ -43,6 +43,19 @@ class MpigConfig(ctypes.Structure):
     ]
 
 
+class MpigSampleFilters(ctypes.Structure):
+    """mpig_sample_filters (include/magicpig_b200_aux.h): five per-request device arrays and the penalty table."""
+    _fields_ = [
+        ("top_k", ctypes.c_void_p),
+        ("min_p", ctypes.c_void_p),
+        ("repetition_penalty", ctypes.c_void_p),
+        ("presence_penalty", ctypes.c_void_p),
+        ("frequency_penalty", ctypes.c_void_p),
+        ("table", ctypes.c_void_p),
+        ("ld", ctypes.c_int64),
+    ]
+
+
 class MagicPigError(RuntimeError):
     pass
 
@@ -132,6 +145,11 @@ _AUX_SIGNATURES = {
     "mpig_aux_verify_sample": (_i, [_vp, _i, _i, _i, ctypes.c_int64, ctypes.c_int64, _vp, _vp, ctypes.c_uint64, _vp, _vp,
                                     ctypes.c_int64, _vp, _vp, _vp, ctypes.c_int64, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp,
                                     _vp]),
+    "mpig_aux_sample_filtered": (_i, [_vp, _i, _i, ctypes.c_int64, _vp, _vp, ctypes.c_uint64, _vp, _vp, ctypes.c_int64, _vp, _vp, _vp,
+                                      _i, _vp, _i, _vp, _vp, _vp, ctypes.POINTER(MpigSampleFilters), _vp]),
+    "mpig_aux_verify_sample_filtered": (_i, [_vp, _i, _i, _i, ctypes.c_int64, ctypes.c_int64, _vp, _vp, ctypes.c_uint64, _vp, _vp,
+                                             ctypes.c_int64, _vp, _vp, _vp, ctypes.c_int64, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp,
+                                             _vp, ctypes.POINTER(MpigSampleFilters), _vp]),
     "mpig_aux_ngram_draft": (_i, [_vp, _i, ctypes.c_int64, _vp, _vp, ctypes.c_int64, _i, _i, _i, _vp]),
 }
 

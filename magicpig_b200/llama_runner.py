@@ -124,10 +124,14 @@ def generate_prompts(prompt, B: int, num_contexts: int):
 
 
 def check_generate_args(lengths, max_new_tokens: int, check_every: int, eos, max_length: int, num_sink: int, num_local: int,
-                        chunk_size: int, generation_buffer: int, can_spill: bool):
+                        chunk_size: int, generation_buffer: int, can_spill: bool, *, B: int = 1, filters=None):
     """generate()'s refusals before anything is written (ValueError): max_new_tokens and check_every >= 1, at most 8 EOS ids,
     every prompt one the prefill takes with P + max_new_tokens <= max_length, and no spill needed where the server cannot spill
-    (requests sharing a context without shared_spill).  Pure host arithmetic."""
+    (requests sharing a context without shared_spill).  filters: a dict of the sampling filters (top_k, min_p,
+    repetition_penalty, presence_penalty, frequency_penalty), each a scalar or B values, refused outside their ranges
+    (see filter_values).  Pure host arithmetic."""
+    if filters is not None:
+        filter_values(B, **filters)
     if int(max_new_tokens) < 1:
         raise ValueError(f"max_new_tokens must be >= 1, got {max_new_tokens}")
     if int(check_every) < 1:
@@ -171,6 +175,31 @@ def check_spec_args(lengths, max_new_tokens: int, draft_tokens: int, ngram, max_
     g_min, g_max = (int(g) for g in ngram)
     if not 1 <= g_min <= g_max <= ops.MAX_NGRAM:
         raise ValueError(f"ngram=(g_min, g_max) needs 1 <= g_min <= g_max <= {ops.MAX_NGRAM}, got {tuple(ngram)}")
+
+
+FILTER_NEUTRAL = dict(top_k=0, min_p=0.0, repetition_penalty=1.0, presence_penalty=0.0, frequency_penalty=0.0)
+
+
+def filter_values(B: int, **filters) -> dict:
+    """The sampling filters given (None: not given) as B host values each, checked against their ranges (ValueError): top_k
+    integers (<= 0: off), min_p in [0, 1], repetition_penalty finite and > 0, presence / frequency penalties in [-2, 2]."""
+    out = {}
+    for name, val in filters.items():
+        if name not in FILTER_NEUTRAL:
+            raise TypeError(f"unknown sampling filter {name!r}")
+        if val is None:
+            continue
+        vals = per_request(val, B, name)
+        if name == "top_k":
+            if any(not float(v).is_integer() for v in vals):
+                raise ValueError(f"top_k: expected integers, got {vals}")
+            vals = [int(v) for v in vals]
+        try:
+            ops.check_filter_values(**{name: vals})
+        except N.MagicPigError as e:
+            raise ValueError(str(e)) from None
+        out[name] = vals
+    return out
 
 
 def spec_spill_every(generation_buffer: int, draft_tokens: int) -> int:
@@ -315,6 +344,16 @@ class LlamaDecodeRunner:
         self._spec_graph = None
         self._spec_graph_key = None
         self.last_generate_stats = None
+        # sampling filters (set_sampling(top_k=.., ..)): per-request device values, the penalty table (allocated on first use) and
+        # whether any value is not neutral, which selects the filtered sampling calls
+        self.top_k = torch.zeros((batch_size,), dtype=torch.int32, device=self.device)
+        self.min_p = torch.zeros((batch_size,), dtype=torch.float32, device=self.device)
+        self.repetition_penalty = torch.ones((batch_size,), dtype=torch.float32, device=self.device)
+        self.presence_penalty = torch.zeros((batch_size,), dtype=torch.float32, device=self.device)
+        self.frequency_penalty = torch.zeros((batch_size,), dtype=torch.float32, device=self.device)
+        self.penalty_table = None
+        self._filter_host = {k: [v] * batch_size for k, v in FILTER_NEUTRAL.items()}
+        self.filters_active = False
 
     # ------------------------------------------------------------------------------------------
     def synthetic_prefill(self, P: int, seed: int = 100, dist: str = "gauss", shared: bool = False):
@@ -437,10 +476,22 @@ class LlamaDecodeRunner:
         return parents, tokens, request_of
 
     # ------------------------------------------------------------------------------------------
-    def set_sampling(self, temperature=None, top_p=None, seed: int | None = None, offset: int | None = None):
+    def set_sampling(self, temperature=None, top_p=None, seed: int | None = None, offset: int | None = None, *, top_k=None, min_p=None,
+                     repetition_penalty=None, presence_penalty=None, frequency_penalty=None):
         """Per-request sampling parameters for sample(): temperature / top_p scalars or length-B sequences (a temperature below 0.1
         is greedy, as in the reference's LLM.generate), the Philox seed (a host value a captured graph keeps) and the device
-        counter offset.  Not capturable (host -> device copies)."""
+        counter offset.  Not capturable (host -> device copies).
+        top_k, min_p, repetition_penalty, presence_penalty, frequency_penalty (keyword only; scalars or B values; None keeps the
+        current ones): the sampling filters (ops.SampleFilters states them), checked against their ranges (ValueError) before any
+        value is written.  While any of them is not neutral, sample(), spec_step() and the graphs captured then run the filtered
+        calls on self.penalty_table (ops.penalty_table() builds it from prompts; generate() does)."""
+        fv = filter_values(self.B, top_k=top_k, min_p=min_p, repetition_penalty=repetition_penalty,
+                           presence_penalty=presence_penalty, frequency_penalty=frequency_penalty)
+        for name, vals in fv.items():
+            buf = getattr(self, name)
+            buf.copy_(torch.tensor(vals, dtype=buf.dtype))
+            self._filter_host[name] = vals
+        self.filters_active = any(v != FILTER_NEUTRAL[k] for k, vals in self._filter_host.items() for v in vals)
         for name, val, buf in (("temperature", temperature, self.temperature), ("top_p", top_p, self.top_p)):
             if val is None:
                 continue
@@ -452,6 +503,18 @@ class LlamaDecodeRunner:
             self.sample_seed = int(seed)
         if offset is not None:
             self.sample_offset.fill_(int(offset))
+
+    def _penalty_table(self) -> torch.Tensor:
+        if self.penalty_table is None:
+            self.penalty_table = torch.zeros((self.B, self.shape.vocab_size), dtype=torch.int32, device=self.device)
+        return self.penalty_table
+
+    def sample_filters(self):
+        """The ops.SampleFilters of the runner's device values and penalty table while a filter is set, else None."""
+        if not self.filters_active:
+            return None
+        return ops.SampleFilters(self.top_k, self.min_p, self.repetition_penalty, self.presence_penalty, self.frequency_penalty,
+                                 self._penalty_table())
 
     def _gen_record(self):
         if self.gen_tokens is None:
@@ -479,7 +542,8 @@ class LlamaDecodeRunner:
         ops.verify_sample(logits, self.temperature, self.top_p, self.sample_seed, self.sample_offset, self.ids_tok,
                           rows=self._spec_rows[:self.B * T * 2].view(self.B, T, 2), drop=self._spec_drop, history=hist, length=length,
                           limit=limit, done=done, steps=self.spec_steps if count else None,
-                          accepted=self.spec_accepted if count else None, eos_token_ids=self.eos_token_ids, status=self.sample_status)
+                          accepted=self.spec_accepted if count else None, eos_token_ids=self.eos_token_ids, status=self.sample_status,
+                          filters=self.sample_filters())
 
     def spec_step(self, T: int, draft: str | None = "ngram"):
         """One step of speculative decoding, all on the device (capturable; capture(draft_tokens=T - 1) puts it into one graph).
@@ -513,12 +577,14 @@ class LlamaDecodeRunner:
             self.set_sampling(temperature, top_p)
         tokens, count, done = self._gen_record()
         ops.sample(self.logits, self.temperature, self.top_p, self.sample_seed, self.sample_offset, ids_out=self.ids,
-                   tokens_out=tokens, count=count, done=done, eos_token_ids=self.eos_token_ids, status=self.sample_status)
+                   tokens_out=tokens, count=count, done=done, eos_token_ids=self.eos_token_ids, status=self.sample_status,
+                   filters=self.sample_filters())
         self.sample_offset.add_(1)
         return self.ids
 
     def generate(self, prompt, max_new_tokens: int, temperature=0.6, top_p=0.9, eos_token_ids=None, seed: int = 0,
-                 chunk_size: int = 8192, check_every: int = 16, draft_tokens: int = 0, ngram=(1, 3)):
+                 chunk_size: int = 8192, check_every: int = 16, draft_tokens: int = 0, ngram=(1, 3), top_k=0, min_p=0.0,
+                 repetition_penalty=1.0, presence_penalty=0.0, frequency_penalty=0.0):
         """The reference's LLM.generate (llama.py:328-360) for the batch.  prompt: one (P,) tensor of token ids for every request
         (prefilled once and forked when the batch has fewer contexts than requests, prefilled into each request otherwise), or a
         list of B prompts, one per request (needs one context per request; lengths may differ).  temperature / top_p: scalars or
@@ -540,24 +606,38 @@ class LlamaDecodeRunner:
         do (sharing a context without shared_spill, more than spec_spill_every(generation_buffer, k) replays), a bad ngram.  With
         drafts accepted, requests may finish well before max_new_tokens - 1 replays; the replays until the next done read (at most
         check_every - 1) change nothing but cost a step each, so a smaller check_every trades host reads for fewer idle steps.
-        self.last_generate_stats then holds the per-request steps, accepted drafts and tokens per step."""
+        self.last_generate_stats then holds the per-request steps, accepted drafts and tokens per step.
+        top_k, min_p, repetition_penalty, presence_penalty, frequency_penalty: scalars or per-request sequences, the sampling filters
+        of set_sampling() (Hugging Face's and vLLM's names and conventions; refused outside their ranges before anything is
+        written).  With any of them set, self.penalty_table is built from the prompts before the first token and the graphs run
+        the filtered calls, with and without drafts (lossless: every token follows the filtered distribution given its prefix).
+        With all of them neutral, generate() runs the unfiltered graph and returns what it returns without them."""
         assert self.tp_world == 1, "generate is built for a single GPU"
         srv, B = self.server, self.B
         prompts, shared = generate_prompts(prompt, B, srv.ctx.num_contexts)
         eos = tuple(int(e) for e in (self.shape.eos_token_ids if eos_token_ids is None else eos_token_ids))
         lengths = [int(p.numel()) for p in prompts]
         can_spill = srv.ctx.num_contexts == B or srv.ctx.shared_spill
+        filters = dict(top_k=top_k, min_p=min_p, repetition_penalty=repetition_penalty, presence_penalty=presence_penalty,
+                       frequency_penalty=frequency_penalty)
         check_generate_args(lengths, max_new_tokens, check_every, eos, srv.max_length,
-                            srv.num_sink_tokens, srv.num_local_tokens, chunk_size, self.generation_buffer, can_spill=can_spill)
+                            srv.num_sink_tokens, srv.num_local_tokens, chunk_size, self.generation_buffer, can_spill=can_spill,
+                            B=B, filters=filters)
+        if filter_values(B, **filters) != {k: [v] * B for k, v in FILTER_NEUTRAL.items()}:   # the table will mark the prompts' ids
+            for p in prompts:
+                if p.numel() and (int(p.min()) < 0 or int(p.max()) >= self.shape.vocab_size):
+                    raise ValueError(f"prompt: token ids must lie in [0, {self.shape.vocab_size})")
         if draft_tokens:
             check_spec_args(lengths, max_new_tokens, draft_tokens, ngram, self.max_query_tokens, self.generation_buffer,
                             srv.max_length, srv.ctx.dense_tail_rows if srv.dense_layers else 0, can_spill)
+            self.set_sampling(**filters)
             return self._generate_spec(prompts, shared, max_new_tokens, temperature, top_p, eos, seed, chunk_size, check_every,
                                        int(draft_tokens), tuple(int(g) for g in ngram))
         temps = per_request(temperature, B, "temperature")
         tops = per_request(top_p, B, "top_p")
         self.eos_token_ids = eos
-        key = (int(seed), eos)
+        self.set_sampling(**filters)
+        key = (int(seed), eos, self.filters_active)
         if self._gen_graph is None or self._gen_graph_key != key:
             # the capture's warm-up steps advance the state: capture on a short synthetic context, then clear it
             self.sample_seed = int(seed)
@@ -569,6 +649,8 @@ class LlamaDecodeRunner:
             self._gen_graph, self.graph = self.graph, prev
             self._gen_graph_key = key
         self._prefill_prompts(prompts, shared, chunk_size)
+        if self.filters_active:
+            ops.penalty_table(prompts, self.shape.vocab_size, out=self._penalty_table())
         tokens, count, done = self._gen_record()
         count.zero_()
         done.zero_()
@@ -606,7 +688,7 @@ class LlamaDecodeRunner:
         tops = per_request(top_p, B, "top_p")
         self.eos_token_ids = eos
         hist, length, limit, done = self._history()
-        key = (int(seed), eos, k, ngram)
+        key = (int(seed), eos, k, ngram, self.filters_active)
         if self._spec_graph is None or self._spec_graph_key != key:
             # the capture's warm-up steps advance the state: capture on a short synthetic context, then clear it
             self.sample_seed, self.ngram = int(seed), ngram
@@ -621,6 +703,8 @@ class LlamaDecodeRunner:
             self._spec_graph, self.graph = self.graph, prev
             self._spec_graph_key = key
         self._prefill_prompts(prompts, shared, chunk_size)
+        if self.filters_active:
+            ops.penalty_table(prompts, self.shape.vocab_size, out=self._penalty_table())
         P = [int(p.numel()) for p in prompts]
         for b, p in enumerate(prompts):
             hist[b, :P[b]] = p.to(self.device, torch.int32)
@@ -930,7 +1014,8 @@ class LlamaDecodeRunner:
         sample(): each replay writes the next token into self.ids, appends it to the record and advances the Philox offset, with
         the parameters on the device at replay time and the seed at capture time; the warm-up steps sample too.  With
         draft_tokens = k >= 1 the graph is spec_step(k + 1) (prompt-lookup drafts with self.ngram) instead of step(); the warm-up
-        steps run it too."""
+        steps run it too.  While a sampling filter is set (set_sampling()), the graph's sampling runs the filtered calls on the
+        device values and table it finds at replay time."""
         def body():
             if draft_tokens:
                 self.spec_step(draft_tokens + 1)

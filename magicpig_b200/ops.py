@@ -13,7 +13,9 @@ instead of being undefined behaviour.  Nothing here computes on the CPU and noth
 from __future__ import annotations
 
 import ctypes
+import math
 import os
+from dataclasses import dataclass
 from typing import Optional, Sequence
 
 import torch
@@ -515,7 +517,7 @@ def _sample_chk(t, dtype, shape, name, device):
 
 
 def check_sample_args(logits, temperature, top_p, offset, ids_out=None, tokens_out=None, count=None, done=None, eos_token_ids=(),
-                      status=None, debug=None, debug_w=None):
+                      status=None, debug=None, debug_w=None, *, n_debug: int = 5):
     """The argument checks of sample() on any device (no library call): returns (ids_out, max_new, eos ids), ids_out allocated
     when None.  Raises MagicPigError."""
     if not isinstance(logits, torch.Tensor) or logits.dim() != 2:
@@ -554,7 +556,7 @@ def check_sample_args(logits, temperature, top_p, offset, ids_out=None, tokens_o
     elif count is not None or done is not None:
         raise N.MagicPigError("count and done go with tokens_out")
     for name, t, dt, shp in (("count", count, torch.int32, (B,)), ("done", done, torch.int32, (B,)),
-                             ("status", status, torch.int32, ((B + 31) // 32,)), ("debug", debug, torch.int64, (B, 5)),
+                             ("status", status, torch.int32, ((B + 31) // 32,)), ("debug", debug, torch.int64, (B, n_debug)),
                              ("debug_w", debug_w, torch.float32, (B, V))):
         if t is not None:
             _sample_chk(t, dt, shp, name, dev)
@@ -566,7 +568,8 @@ def check_sample_args(logits, temperature, top_p, offset, ids_out=None, tokens_o
 def sample(logits: torch.Tensor, temperature: torch.Tensor, top_p: torch.Tensor, seed: int, offset: torch.Tensor,
            ids_out: Optional[torch.Tensor] = None, tokens_out: Optional[torch.Tensor] = None, count: Optional[torch.Tensor] = None,
            done: Optional[torch.Tensor] = None, eos_token_ids: Sequence[int] = (), status: Optional[torch.Tensor] = None,
-           debug: Optional[torch.Tensor] = None, debug_w: Optional[torch.Tensor] = None) -> torch.Tensor:
+           debug: Optional[torch.Tensor] = None, debug_w: Optional[torch.Tensor] = None, *,
+           filters: Optional["SampleFilters"] = None) -> torch.Tensor:
     """One token per row of logits (B, V) fp32 (rows may be strided; elements contiguous) by temperature / top-p sampling on the
     device (mpig_aux_sample, include/magicpig_b200_aux.h, states the exact rule): temperature (B,) fp32 (<= 0: greedy, the first
     argmax), top_p (B,) fp32, offset a device uint64 (1,) tensor (int64 storage is accepted) read as the Philox counter and never
@@ -575,20 +578,29 @@ def sample(logits: torch.Tensor, temperature: torch.Tensor, top_p: torch.Tensor,
     eos_token_ids (at most 8) or when count reaches max_new.  status int32 ((B + 31) // 32,): bit b % 32 of word b // 32 is set
     for a row with a NaN or +inf logit or none finite (its token is 0).  debug int64 (B, 5) / debug_w fp32 (B, V): the kernel's
     integer stages and weights.  Every argument is checked here before the call; capturable.  Returns the tensor holding the
-    tokens (ids_out)."""
+    tokens (ids_out).
+    filters (keyword only): a SampleFilters adds top-k, min-p and the repetition / presence / frequency penalties
+    (mpig_aux_sample_filtered); debug is then (B, 8) and each appended token is counted in filters.table.  None is the call
+    above, unchanged."""
     ids_out, max_new, eos = check_sample_args(logits, temperature, top_p, offset, ids_out, tokens_out, count, done, eos_token_ids,
-                                              status, debug, debug_w)
+                                              status, debug, debug_w, n_debug=5 if filters is None else 8)
+    B, V = logits.shape
+    if filters is not None:
+        check_filters(filters, B, V, logits.device)
     if logits.device.type != "cuda":
         raise N.MagicPigError("sample runs on CUDA (sm_90a) only; there is no CPU path")
     dev = logits.device
-    B, V = logits.shape
     eos_arr = (ctypes.c_int32 * max(len(eos), 1))(*eos)
     lib = N.load()
+    args = (_ptr(logits), B, V, logits.stride(0), _ptr(temperature), _ptr(top_p), ctypes.c_uint64(int(seed) & (2 ** 64 - 1)),
+            _ptr(offset), _ptr(ids_out), ids_out.stride(0), _ptr(tokens_out), _ptr(count), _ptr(done), max_new, eos_arr, len(eos),
+            _ptr(status), _ptr(debug), _ptr(debug_w))
     with torch.cuda.device(dev):
-        N.check(lib.mpig_aux_sample(_ptr(logits), B, V, logits.stride(0), _ptr(temperature), _ptr(top_p),
-                                    ctypes.c_uint64(int(seed) & (2 ** 64 - 1)), _ptr(offset), _ptr(ids_out), ids_out.stride(0),
-                                    _ptr(tokens_out), _ptr(count), _ptr(done), max_new, eos_arr, len(eos), _ptr(status), _ptr(debug),
-                                    _ptr(debug_w), _stream()), "mpig_aux_sample")
+        if filters is None:
+            N.check(lib.mpig_aux_sample(*args, _stream()), "mpig_aux_sample")
+        else:
+            f = filters.native()
+            N.check(lib.mpig_aux_sample_filtered(*args, ctypes.byref(f), _stream()), "mpig_aux_sample_filtered")
     return ids_out
 
 
@@ -603,7 +615,7 @@ def _ids_chk(ids, B, T, dev):
 
 
 def check_verify_args(logits, temperature, top_p, offset, ids, rows=None, drop=None, history=None, length=None, limit=None, done=None,
-                      steps=None, accepted=None, eos_token_ids=(), status=None, debug=None, debug_w=None):
+                      steps=None, accepted=None, eos_token_ids=(), status=None, debug=None, debug_w=None, *, n_debug: int = 9):
     """The argument checks of verify_sample() on any device (no library call): returns (rows, eos ids), rows allocated when None.
     Raises MagicPigError."""
     if not isinstance(logits, torch.Tensor) or logits.dim() != 3:
@@ -632,7 +644,7 @@ def check_verify_args(logits, temperature, top_p, offset, ids, rows=None, drop=N
     for name, t, dt, shp in (("rows", rows, torch.int32, (B, T, 2)), ("drop", drop, torch.int32, (B,)),
                              ("length", length, torch.int32, (B,)), ("limit", limit, torch.int32, (B,)),
                              ("done", done, torch.int32, (B,)), ("steps", steps, torch.int32, (B,)),
-                             ("accepted", accepted, torch.int32, (B,)), ("debug", debug, torch.int64, (B, T, 9)),
+                             ("accepted", accepted, torch.int32, (B,)), ("debug", debug, torch.int64, (B, T, n_debug)),
                              ("debug_w", debug_w, torch.float32, (B, T, V))):
         if t is not None:
             _sample_chk(t, dt, shp, name, dev)
@@ -646,7 +658,7 @@ def verify_sample(logits: torch.Tensor, temperature: torch.Tensor, top_p: torch.
                   history: Optional[torch.Tensor] = None, length: Optional[torch.Tensor] = None, limit: Optional[torch.Tensor] = None,
                   done: Optional[torch.Tensor] = None, steps: Optional[torch.Tensor] = None, accepted: Optional[torch.Tensor] = None,
                   eos_token_ids: Sequence[int] = (), status: Optional[torch.Tensor] = None, debug: Optional[torch.Tensor] = None,
-                  debug_w: Optional[torch.Tensor] = None) -> torch.Tensor:
+                  debug_w: Optional[torch.Tensor] = None, *, filters: Optional["SampleFilters"] = None) -> torch.Tensor:
     """Speculative sampling of a verification step on the device (mpig_aux_verify_sample, include/magicpig_b200_aux.h, states the
     exact rule): logits (B, T, V) fp32 (the logits after each of the step's T inputs; rows may be strided, elements contiguous),
     ids (B, >= T) int64 the step's inputs, so ids[b, 1:T] are request b's drafts.  Accepts a prefix of the drafts and draws the
@@ -655,21 +667,133 @@ def verify_sample(logits: torch.Tensor, temperature: torch.Tensor, top_p: torch.
     length / limit / done int32 (B,): the emitted tokens are appended at length[b] until an EOS id or limit[b] sets done[b]; a
     request already done appends nothing and gets drop = T.  steps / accepted int32 (B,): += 1 and += accepted drafts per call.
     debug int64 (B, T, 9) / debug_w fp32 (B, T, V): each row's integer stages and weights.  Every argument is checked here before the
-    call; capturable.  Returns ids."""
+    call; capturable.  Returns ids.
+    filters (keyword only): a SampleFilters adds top-k, min-p and the penalties (mpig_aux_verify_sample_filtered): row t also counts
+    the drafts ids[b, 1 .. t] in the penalties, debug is (B, T, 12) and each token appended to history is counted in
+    filters.table.  None is the call above, unchanged."""
     rows, eos = check_verify_args(logits, temperature, top_p, offset, ids, rows, drop, history, length, limit, done, steps, accepted,
-                                  eos_token_ids, status, debug, debug_w)
+                                  eos_token_ids, status, debug, debug_w, n_debug=9 if filters is None else 12)
+    B, T, V = logits.shape
+    if filters is not None:
+        check_filters(filters, B, V, logits.device)
     if logits.device.type != "cuda":
         raise N.MagicPigError("verify_sample runs on CUDA (sm_90a) only; there is no CPU path")
-    B, T, V = logits.shape
     eos_arr = (ctypes.c_int32 * max(len(eos), 1))(*eos)
     lib = N.load()
+    args = (_ptr(logits), B, T, V, logits.stride(0), logits.stride(1), _ptr(temperature), _ptr(top_p),
+            ctypes.c_uint64(int(seed) & (2 ** 64 - 1)), _ptr(offset), _ptr(ids), ids.stride(0), _ptr(rows), _ptr(drop), _ptr(history),
+            history.shape[1] if history is not None else 0, _ptr(length), _ptr(limit), _ptr(done), _ptr(steps), _ptr(accepted), eos_arr,
+            len(eos), _ptr(status), _ptr(debug), _ptr(debug_w))
     with torch.cuda.device(logits.device):
-        N.check(lib.mpig_aux_verify_sample(_ptr(logits), B, T, V, logits.stride(0), logits.stride(1), _ptr(temperature), _ptr(top_p),
-                                           ctypes.c_uint64(int(seed) & (2 ** 64 - 1)), _ptr(offset), _ptr(ids), ids.stride(0),
-                                           _ptr(rows), _ptr(drop), _ptr(history), history.shape[1] if history is not None else 0,
-                                           _ptr(length), _ptr(limit), _ptr(done), _ptr(steps), _ptr(accepted), eos_arr, len(eos),
-                                           _ptr(status), _ptr(debug), _ptr(debug_w), _stream()), "mpig_aux_verify_sample")
+        if filters is None:
+            N.check(lib.mpig_aux_verify_sample(*args, _stream()), "mpig_aux_verify_sample")
+        else:
+            f = filters.native()
+            N.check(lib.mpig_aux_verify_sample_filtered(*args, ctypes.byref(f), _stream()), "mpig_aux_verify_sample_filtered")
     return ids
+
+
+PROMPT_BIT = -(1 << 31)   # bit 31 of a penalty-table entry, as int32
+
+
+@dataclass
+class SampleFilters:
+    """The sampling filters of sample(..., filters=) and verify_sample(..., filters=) (mpig_sample_filters in
+    include/magicpig_b200_aux.h states the rule): per-request device arrays of shape (B,) -- top_k int32 (<= 0: off), min_p fp32 in
+    [0, 1] (0: off), repetition_penalty fp32 > 0 (1: off), presence_penalty and frequency_penalty fp32 in [-2, 2] (0: off) -- and the
+    penalty table, (B, ld >= V) int32 or uint32 with contiguous rows: the low 31 bits of entry i count request b's emitted token i,
+    bit 31 marks a token of its prompt (penalty_table() builds it).  The filtered calls increment the entries of the tokens they
+    append."""
+    top_k: torch.Tensor
+    min_p: torch.Tensor
+    repetition_penalty: torch.Tensor
+    presence_penalty: torch.Tensor
+    frequency_penalty: torch.Tensor
+    table: torch.Tensor
+
+    @classmethod
+    def neutral(cls, B: int, V: int, device) -> "SampleFilters":
+        """Every filter off and an empty table: the filtered calls then compute what the unfiltered ones do."""
+        f32 = lambda v: torch.full((B,), v, dtype=torch.float32, device=device)  # noqa: E731
+        return cls(torch.zeros((B,), dtype=torch.int32, device=device), f32(0.0), f32(1.0), f32(0.0), f32(0.0),
+                   torch.zeros((B, V), dtype=torch.int32, device=device))
+
+    def native(self) -> N.MpigSampleFilters:
+        return N.MpigSampleFilters(self.top_k.data_ptr(), self.min_p.data_ptr(), self.repetition_penalty.data_ptr(),
+                                   self.presence_penalty.data_ptr(), self.frequency_penalty.data_ptr(), self.table.data_ptr(),
+                                   self.table.stride(0))
+
+
+def check_filter_values(top_k=None, min_p=None, repetition_penalty=None, presence_penalty=None, frequency_penalty=None):
+    """The value ranges of the filters, on host sequences (MagicPigError): min_p in [0, 1], repetition_penalty finite and > 0,
+    presence / frequency penalties in [-2, 2]; top_k any integer (<= 0 is off)."""
+    def floats(name, vals, ok, what):
+        for v in vals:
+            if not (isinstance(v, (int, float)) and math.isfinite(float(v)) and ok(float(v))):
+                raise N.MagicPigError(f"{name}: every value must be {what}, got {v!r}")
+    if top_k is not None:
+        for v in top_k:
+            if isinstance(v, bool) or not float(v).is_integer() or not -2 ** 31 <= int(v) < 2 ** 31:
+                raise N.MagicPigError(f"top_k: every value must be an int32 integer, got {v!r}")
+    if min_p is not None:
+        floats("min_p", min_p, lambda v: 0.0 <= v <= 1.0, "in [0, 1]")
+    if repetition_penalty is not None:
+        floats("repetition_penalty", repetition_penalty, lambda v: v > 0.0, "finite and > 0")
+    for name, vals in (("presence_penalty", presence_penalty), ("frequency_penalty", frequency_penalty)):
+        if vals is not None:
+            floats(name, vals, lambda v: -2.0 <= v <= 2.0, "in [-2, 2]")
+
+
+def check_filters(filters, B: int, V: int, device, values: Optional[bool] = None):
+    """The checks of a SampleFilters on any device (MagicPigError): types, dtypes, shapes, devices, the table's layout, and the
+    values' ranges.  values=None checks the values unless the current stream is capturing a graph (reading them then would break
+    the capture; the device takes a value outside its range as neutral)."""
+    if not isinstance(filters, SampleFilters):
+        raise N.MagicPigError(f"filters: expected a SampleFilters, got {type(filters).__name__}")
+    _sample_chk(filters.top_k, torch.int32, (B,), "top_k", device)
+    for name in ("min_p", "repetition_penalty", "presence_penalty", "frequency_penalty"):
+        _sample_chk(getattr(filters, name), torch.float32, (B,), name, device)
+    for name in ("top_k", "min_p", "repetition_penalty", "presence_penalty", "frequency_penalty"):
+        if not getattr(filters, name).is_contiguous():
+            raise N.MagicPigError(f"{name}: must be contiguous")
+    t = filters.table
+    if not isinstance(t, torch.Tensor) or t.dtype not in (torch.int32, torch.uint32):
+        raise N.MagicPigError("table: expected an int32 or uint32 tensor")
+    _sample_chk(t, t.dtype, None, "table", device)
+    if t.dim() != 2 or t.shape[0] != B or t.shape[1] < V or t.stride(1) != 1 or t.stride(0) < V:
+        raise N.MagicPigError(f"table: expected (B={B}, ld >= V={V}) with contiguous rows, got {tuple(t.shape)} strides {t.stride()}")
+    if values is None:
+        values = not (device.type == "cuda" and torch.cuda.is_current_stream_capturing())
+    if values:
+        check_filter_values(filters.top_k.tolist(), filters.min_p.tolist(), filters.repetition_penalty.tolist(),
+                            filters.presence_penalty.tolist(), filters.frequency_penalty.tolist())
+
+
+def penalty_table(prompts, V: int, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The penalty table at the start of a generation: zero counts and bit 31 set on each request's prompt tokens.  prompts: one
+    1-D tensor (or sequence) of token ids per request, or a (B, P) tensor.  out: int32 / uint32 (B, ld >= V) with contiguous rows,
+    written in place (None: a new int32 (B, V) tensor on the prompts' device).  Torch ops, once per generation.  Returns out."""
+    rows = list(prompts.unbind(0)) if isinstance(prompts, torch.Tensor) and prompts.dim() == 2 else list(prompts)
+    rows = [torch.as_tensor(p).reshape(-1) for p in rows]
+    B = len(rows)
+    if B < 1 or int(V) < 1:
+        raise N.MagicPigError(f"penalty_table: need at least one prompt and V >= 1, got {B} prompts and V={V}")
+    if out is None:
+        out = torch.zeros((B, int(V)), dtype=torch.int32, device=rows[0].device)
+    if not isinstance(out, torch.Tensor) or out.dtype not in (torch.int32, torch.uint32) or out.dim() != 2:
+        raise N.MagicPigError("penalty_table: out must be an int32 or uint32 (B, ld) tensor")
+    if out.shape[0] != B or out.shape[1] < V or out.stride(1) != 1:
+        raise N.MagicPigError(f"penalty_table: out must be (B={B}, ld >= V={V}) with contiguous rows, got {tuple(out.shape)}")
+    for b, p in enumerate(rows):
+        if p.numel() and (p.dtype.is_floating_point or p.dtype == torch.bool):
+            raise N.MagicPigError(f"penalty_table: prompt {b} must hold integer token ids, got {p.dtype}")
+        if p.numel() and (int(p.min()) < 0 or int(p.max()) >= V):
+            raise N.MagicPigError(f"penalty_table: prompt {b} holds ids outside [0, V={V})")
+    view = out.view(torch.int32)
+    view.zero_()
+    for b, p in enumerate(rows):
+        view[b].index_fill_(0, p.to(out.device, torch.int64), PROMPT_BIT)
+    return out
 
 
 def check_ngram_args(history, length, ids, T, g_min, g_max):
